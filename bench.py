@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""Benchmark of the tape-evaluation hot path on B200 (see DESIGN.md, "Measurement").
+"""Benchmark of the tape-evaluation hot path on H100 (see DESIGN.md, "Measurement").
 
 A step = one pass of the hot path over one frame of synthetic input.
 
@@ -19,7 +19,9 @@ A step = one pass of the hot path over one frame of synthetic input.
   python bench.py --gpus N --steps K --warmup W           # CUDA arm
   python bench.py --impl reference --gpus N --steps K ...  # CPU arm (oracle port, all host threads)
 
-Prints ONE JSON line (rank 0).
+Prints ONE JSON line (rank 0).  --dump-outputs DIR also writes, after the timed steps, what the last timed step
+computed as DIR/<name>.npy (a fixed, seeded sample of each image; see dump_outputs), so that two builds can be
+compared output for output on identical inputs.
 """
 from __future__ import annotations
 
@@ -138,17 +140,52 @@ def measured_peaks():
     if os.path.exists(p):
         with open(p) as f:
             return json.load(f).get("hbm_gbs"), "measured (MEASURED_PEAKS.json)"
-    return 6650.0, "fallback (B200_PROFILING.md)"
+    return 3350.0, "H100 SXM data sheet (HBM3, 3.35 TB/s at up to 700 W), not measured"
 
 
-def ncu_table():
-    """Per-kernel ncu figures of the committed capture (profiles/dram_traffic.json): DRAM bytes per launch,
-    issue-active %, fp32-pipe %."""
-    tp = os.path.join(ROOT, "profiles", "dram_traffic.json")
-    if os.path.exists(tp):
-        with open(tp) as f:
-            return json.load(f)
-    return {}
+DUMP_SEED = 20240606
+DUMP_PIXELS_2D = 1 << 22   # 2 x 16 MiB of float32, a quarter of the 4096^2 frame
+DUMP_PIXELS_3D = 1 << 20   # 16 MiB of float32, 1/16 of the 4096^2 heightmap + normals image
+
+
+def sample_pixels(image, n_pixels):
+    """A fixed, seeded sample of the pixels of `image` ([h, w, ...], numpy or torch): the same pixels on every run."""
+    n = image.shape[0] * image.shape[1]
+    idx = np.sort(np.random.default_rng(DUMP_SEED).choice(n, size=min(n_pixels, n), replace=False))
+    flat = image.reshape((n,) + tuple(image.shape[2:]))
+    if isinstance(flat, np.ndarray):
+        return flat[idx]
+    import torch
+    return flat[torch.from_numpy(idx).to(flat.device)].cpu().numpy()
+
+
+def outputs_2d(image):
+    """The 2D frame (RawDistancePixel bits, pixel.rs:163-241) decoded into finite float32 arrays: `distance_2d`
+    holds the distance of every evaluated pixel (0 where a tile fill wrote the pixel, and where an evaluated
+    distance is not finite), `fill_2d` is 0 for an evaluated pixel and -1 / +1 for a pixel filled inside /
+    outside, so that a float comparison sees every field of the pixel."""
+    from fidget_b200.shape import pixel_inside
+    px = sample_pixels(image, DUMP_PIXELS_2D).astype(np.float32, copy=False)
+    bits = px.view(np.uint32)
+    filled = np.isnan(px) & ((bits & np.uint32(0xFF << 9)) == np.uint32(0xF6 << 9))
+    fill = np.where(filled, np.where(pixel_inside(px), -1.0, 1.0), 0.0).astype(np.float32)
+    distance = np.where(filled | ~np.isfinite(px), 0.0, px).astype(np.float32)
+    return {"distance_2d": distance, "fill_2d": fill}
+
+
+def outputs_3d(image):
+    """The 3D frame ([h, w, 4] float32 holding GeometryPixel {normal[3], depth: u32}) as float32 arrays."""
+    px = sample_pixels(image, DUMP_PIXELS_3D)
+    return {"volume_normals": np.ascontiguousarray(px[:, :3], dtype=np.float32),
+            "volume_depth": px[:, 3].copy().view(np.uint32).astype(np.float32)}
+
+
+def dump_outputs(out_dir, arrays):
+    """Writes each array as out_dir/<name>.npy (48 MiB in all for the CUDA arm at N = 1)."""
+    os.makedirs(out_dir, exist_ok=True)
+    for name, a in arrays.items():
+        assert a.dtype in (np.float32, np.float64) and np.isfinite(a).all(), name
+        np.save(os.path.join(out_dir, name + ".npy"), a)
 
 
 # ---------------------------------------------------------------------------------------------------
@@ -193,8 +230,10 @@ def run_reference(args):
             orc.render2d(t, SIZE, SIZE, threads=threads)
         t0 = time.perf_counter()
         for _ in range(args.steps):
-            orc.render2d(t, SIZE, SIZE, threads=threads)
+            img, _ = orc.render2d(t, SIZE, SIZE, threads=threads)
         dt = (time.perf_counter() - t0) / args.steps
+        if args.dump_outputs:
+            dump_outputs(args.dump_outputs, outputs_2d(img))
         v = SIZE * SIZE / dt / 1e6
         metric = METRIC
         workload = WORKLOAD_2D
@@ -241,7 +280,7 @@ def time_steps(torch, stream, flush, step, n, sync_all):
     return sum(s.elapsed_time(e) for s, e in zip(starts, stops)) / n
 
 
-def volume_on_one_gpu(torch, fb, cuda, shape, stream, flush, steps=3):
+def volume_on_one_gpu(torch, fb, cuda, shape, stream, flush, steps):
     """The N > 1 workload rendered whole on this GPU: returns (image, ms per render, stats)."""
     cfg = fb.RenderConfig3D(SIZE, SIZE, SIZE)
     img = torch.zeros((SIZE, SIZE, 4), dtype=torch.float32, device=flush.device)
@@ -261,6 +300,8 @@ def main():
     ap.add_argument("--impl", default="cuda")
     ap.add_argument("--no-cpu-baseline", action="store_true")
     ap.add_argument("--no-volume", action="store_true", help="N = 1: skip the 4096^3 strong-scaling base")
+    ap.add_argument("--dump-outputs", metavar="DIR", help="write a seeded sample of the last timed step's images "
+                                                          "as DIR/<name>.npy (float32)")
     args = ap.parse_args()
     if args.impl == "reference":
         return run_reference(args)
@@ -286,7 +327,7 @@ def main():
     ctx, root = fb.Context.from_text(model_text())
     tape = ctx.tape(root)
     shape = fb.CudaShape(cuda, tape)
-    flush = torch.empty(512 << 20, dtype=torch.uint8, device=dev)  # > 126 MB L2
+    flush = torch.empty(512 << 20, dtype=torch.uint8, device=dev)  # > 50 MB L2
     peak, peak_src = measured_peaks()
     bc = tape.bytecode()
 
@@ -304,7 +345,10 @@ def main():
     if world == 1:
         line = bench_2d(args, torch, fb, cuda, shape, tape, bc, stream, flush, dev, peak, peak_src, sync_all)
         if not args.no_volume:
-            _, ms3, st3 = volume_on_one_gpu(torch, fb, cuda, shape, stream, flush)
+            img3, ms3, st3 = volume_on_one_gpu(torch, fb, cuda, shape, stream, flush, args.steps)
+            if args.dump_outputs:
+                dump_outputs(args.dump_outputs, outputs_3d(img3))
+            del img3
             line["strong_scaling_base"] = {
                 "workload": f"models/{MODEL} 3D render {SIZE}^3 (the N > 1 workload), whole volume on 1 GPU",
                 "value": SIZE ** 3 / (ms3 * 1e-3) / 1e6, "unit": "Mvoxels/s", "ms_per_step": ms3,
@@ -316,7 +360,7 @@ def main():
 
     # ---------------- N > 1: one 4096^3 volume sharded over the ranks, one all-gather per step ----------------
     cfg3 = fb.RenderConfig3D(SIZE, SIZE, SIZE)
-    full, base_ms, base_st = volume_on_one_gpu(torch, fb, cuda, shape, stream, flush)   # every rank: the single-GPU image
+    full, base_ms, base_st = volume_on_one_gpu(torch, fb, cuda, shape, stream, flush, args.steps)   # every rank: the single-GPU image
     image = torch.zeros((SIZE, SIZE, 4), dtype=torch.float32, device=dev)
     chunk, gathered = shard.tile_buffers(world, SIZE, SIZE, 4, dev)
 
@@ -336,6 +380,8 @@ def main():
     with ClockSampler(local) as clocks:
         ms_local = time_steps(torch, stream, flush, step, args.steps, sync_all)
     cuda.synchronize()
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, outputs_3d(image))
     ms_per_step = maxrank(ms_local)
     value = SIZE ** 3 / (ms_per_step * 1e-3) / 1e6
 
@@ -415,6 +461,8 @@ def bench_2d(args, torch, fb, cuda, shape, tape, bc, stream, flush, dev, peak, p
     with ClockSampler(dev.index or 0) as clocks:
         ms_per_step = time_steps(torch, stream, flush, step, args.steps, sync_all)
     cuda.synchronize()
+    if args.dump_outputs:
+        dump_outputs(args.dump_outputs, outputs_2d(image))
     value = SIZE * SIZE / (ms_per_step * 1e-3) / 1e6
 
     # ---- per-kernel timing of one step (CUDA events inside the library, on the launching stream) ----
@@ -439,24 +487,21 @@ def bench_2d(args, torch, fb, cuda, shape, tape, bc, stream, flush, dev, peak, p
     launches_per_step = int(stats["kernel_launches"])
     names = {0: "k_interval_root_coop_2d[L0,128px]", 1: "k_interval_level<2>[L1,32px]",
              2: "k_interval_level<2>[L2,8px]", 8: "k_fill_2d (x3)", 9: "k_pixels_2d"}
-    ncu = ncu_table()
     n_fill_px = SIZE * SIZE - int(stats["pixels"])
     written = {0: 0, 1: 0, 2: 0, 8: n_fill_px * 4, 9: int(stats["pixels"]) * 4}     # bytes of the frame each kernel writes
     kernels = {}
     for k, nm in names.items():
-        e = ncu.get(nm, {}) if isinstance(ncu.get(nm), dict) else {"dram_bytes": ncu.get(nm)}
         kernels[nm] = {"ms": float(stage[k]), "share": float(stage[k] / max(stage[15], 1e-9)),
-                       "frame_bytes_written": written[k], "dram_bytes": e.get("dram_bytes"),
-                       "issue_active_pct": e.get("issue_active_pct"), "pipe_fp32_pct": e.get("pipe_fp32_pct")}
+                       "frame_bytes_written": written[k]}
     dom = max(names, key=lambda k: stage[k])
     algo = SIZE * SIZE * ALGO_BYTES_PER_PIXEL
     achieved = algo / (ms_per_step * 1e-3) / 1e9
     roofline = {"bound": "hbm", "kernel": "whole frame (dominant kernel: " + names[dom] + ")",
                 "achieved": achieved, "peak": peak, "unit": "GB/s", "frac": achieved / peak,
-                "traffic": sum(v["dram_bytes"] or 0 for v in kernels.values()) or None, "peak_source": peak_src,
+                "traffic": None, "peak_source": peak_src,
                 "algorithmic_bytes": algo,
-                "definition": "SURVEY 8(d): 4 B per pixel WRITTEN per step / ms_per_step / measured HBM copy bandwidth; "
-                              "traffic = sum of the kernels' dram bytes (ncu --set full, profiles/)",
+                "definition": "SURVEY 8(d): 4 B per pixel WRITTEN per step / ms_per_step / HBM bandwidth (peak_source); "
+                              "traffic (DRAM bytes actually moved) is not measured",
                 "stage_total_ms": float(stage[15]),
                 "kernels": kernels,
                 "experimental_fused_tail_ms": {"k_interval_root_coop_2d[L0,128px]": float(fstage[0]),

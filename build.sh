@@ -1,11 +1,11 @@
 #!/bin/bash
-# Builds libfidget_cuda.so (sm_100a only) in-tree and the CPU oracle.
+# Builds libfidget_cuda.so (sm_90a, H100, only) in-tree and the CPU oracle.
 set -e
 cd "$(dirname "$0")"
 NVCC=${NVCC:-/usr/local/cuda/bin/nvcc}
 SRC=fidget_b200/csrc
 OUT=${OUT:-fidget_b200/libfidget_cuda.so}
-FLAGS="-gencode arch=compute_100a,code=sm_100a -lineinfo -O3 -std=c++17 \
+FLAGS="-gencode arch=compute_90a,code=sm_90a -lineinfo -O3 -std=c++17 \
   -fmad=false -prec-div=true -prec-sqrt=true -ftz=false \
   -Xcompiler -fPIC,-O2,-ffp-contract=off -shared"
 if [ "$1" = "-v" ]; then FLAGS="$FLAGS -Xptxas -v"; fi

@@ -1,4 +1,4 @@
-"""fidget_b200 -- B200-native (sm_100a CUDA) backend for Fidget's tape
+"""fidget_b200 -- H100-native (sm_90a CUDA) backend for Fidget's tape
 evaluation hot path: interval evaluation + tape simplification over tiles and
 bulk f32 / gradient evaluation of the surviving voxels.
 

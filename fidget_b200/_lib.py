@@ -21,7 +21,7 @@ def load() -> C.CDLL:
     if _LIB is None:
         if not os.path.exists(LIB_PATH):
             raise BackendMissing(
-                f"{LIB_PATH} not found: build it with ./build.sh (nvcc, sm_100a). "
+                f"{LIB_PATH} not found: build it with ./build.sh (nvcc, sm_90a). "
                 "fidget_b200 has no CPU fallback.")
         from .host import bind_host_api
         lib = C.CDLL(LIB_PATH)

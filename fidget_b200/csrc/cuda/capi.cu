@@ -95,9 +95,9 @@ int32_t fc_ctx_create(int32_t device, fc_ctx** out) {
     cudaDeviceProp prop;
     CU(cudaGetDeviceProperties(&prop, device));
     c->sm_count = prop.multiProcessorCount;
-    if (prop.major < 10) {
+    if (prop.major != 9 || prop.minor != 0) {   // sm_90a code loads on compute capability 9.0 and nothing else
         delete c;
-        return fail(FC_ERR_NO_DEVICE, "libfidget_cuda is built for sm_100a only; found sm_" +
+        return fail(FC_ERR_NO_DEVICE, "libfidget_cuda is built for sm_90a (H100) only; found sm_" +
                                           std::to_string(prop.major) + std::to_string(prop.minor));
     }
     CU(cudaStreamCreateWithFlags(&c->own_stream, cudaStreamNonBlocking));

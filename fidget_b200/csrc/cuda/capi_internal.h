@@ -61,8 +61,7 @@ inline bool is_device_ptr(const void* p) {
 }
 
 // Pinned (page-locked, mapped) host memory can be written by kernels directly over PCIe.
-// Measured on B200 (profiles/r01_prospero4096.md): SM stores over PCIe reach well under half the
-// bandwidth of a DMA copy (3.07 ms vs 2.07 ms end to end for a 67 MB image), so this is opt-in
+// Scattered SM stores over PCIe move an image more slowly than one DMA copy of it, so this is opt-in
 // (FIDGET_B200_ZEROCOPY=1); the default stages the image in HBM and copies it with the DMA engine.
 // Returns the device alias of `p` or null.
 inline void* pinned_device_alias(const void* p) {
@@ -100,7 +99,7 @@ inline int env_int(const char* name, int dflt) {
 
 struct fc_ctx {
     int device = 0;
-    int sm_count = 148;
+    int sm_count = 132;
     cudaStream_t own_stream = nullptr;
     cudaStream_t stream = nullptr;
     cudaStream_t aux_stream = nullptr;        // fills are painted here, concurrently with the next levels

@@ -40,8 +40,7 @@ __host__ __device__ inline uint32_t enc(uint32_t op, uint32_t form, uint32_t out
 }
 // Multi-GPU tile interleave: which rank renders root tile (tx, ty).  A spatial hash rather than a regular
 // pattern: per-tile cost is heavy-tailed and structured (text lines, silhouettes), and a pseudo-random spread keeps
-// the busiest rank within a few per cent of the mean where the diagonal (tx + ty) % N was 15 % above it at N = 8
-// (prospero, profiles/r02_scaling.md).
+// the busiest rank closer to the mean than a diagonal (tx + ty) % N, which lines such structure up on a few ranks.
 __host__ __device__ inline uint32_t tile_owner(uint32_t tx, uint32_t ty, uint32_t n_ranks) {
     return ((tx * 73856093u) ^ (ty * 19349663u)) % n_ranks;
 }

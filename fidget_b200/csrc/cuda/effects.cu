@@ -1,5 +1,5 @@
 // Post-processing effects of fidget-raster (fidget-raster/src/effects.rs:13-547,
-// GeometryPixel::to_color voxel.rs:136-153) as sm_100a kernels: one thread per pixel,
+// GeometryPixel::to_color voxel.rs:136-153) as sm_90a kernels: one thread per pixel,
 // images stay in HBM/L2 between the passes.
 //
 // Vector arithmetic keeps nalgebra's evaluation order for fixed 3-vectors

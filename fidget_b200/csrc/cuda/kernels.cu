@@ -1,4 +1,4 @@
-// sm_100a kernels for the tape-evaluation hot path.
+// sm_90a kernels for the tape-evaluation hot path.
 //
 //  k_interval_level  -- K1: one warp per parent tile, one lane per child tile;
 //                       walks the (warp-uniform) parent tape, classifies each
@@ -480,7 +480,7 @@ __global__ void __launch_bounds__(128) k_grad_slice(const __grid_constant__ Bulk
 
 static int bulk_blocks(uint64_t n) {
     uint64_t b = (n + 127) / 128;
-    return int(b < 1 ? 1 : (b > 148ull * 16 ? 148ull * 16 : b));
+    return int(b < 1 ? 1 : (b > 132ull * 16 ? 132ull * 16 : b));   // H100: 132 SMs x 16 blocks of 128 threads
 }
 void launch_float_slice(const BulkParams& p, cudaStream_t s) {
     if (p.n == 0) return;

@@ -1,4 +1,4 @@
-// Host-side tape front end for the B200 backend.
+// Host-side tape front end for the H100 backend.
 //
 // This is the part of Fidget that "stays on the host" for every backend
 // (SURVEY.md §1, "TAPE / COMPILER"): a hash-consed expression context with

@@ -1,4 +1,4 @@
-/* libfidget_cuda -- B200 (sm_100a) backend for Fidget's tape-evaluation hot path.
+/* libfidget_cuda -- H100 (sm_90a) backend for Fidget's tape-evaluation hot path.
  *
  * C ABI, plain pointers and sizes only.  Every entry point cites the reference
  * interface it replaces (paths relative to the mkeeter/fidget checkout);
@@ -145,7 +145,7 @@ int32_t fc_simplify(fc_eval* e, const fc_tape* parent, const uint8_t* choices, s
 #define FC_FLAG_TIMING 2u       /* record per-stage CUDA events (fc_render_stats.stage_ms) */
 #define FC_FLAG_FUSED_TAIL 8u   /* fc_render2d, EXPERIMENTAL: the levels after the root level, the leaf pixels and the fills as one
                                    persistent launch draining a job queue (tail2d.cu) instead of one launch per stage.
-                                   Same image and census; measured SLOWER on B200 (queue polling hot spot, profiles/), so off
+                                   Same image and census; measured SLOWER on H100 (0.32 vs 0.25 ms for prospero 4096², profiles/), so off
                                    by default */
 #define FC_FLAG_EXACT_CENSUS 16u /* fc_render3d with stats: report the tile census and voxel count of the reference's front-to-back
                                    walk (voxel.rs:244-357), computed from the final heightmap; without it the census counts what

@@ -14,7 +14,7 @@ import torch
 import fidget_b200 as fb
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-PEAK = 6570.0
+PEAK = 3350.0   # H100 SXM data sheet (HBM3), unless a measured copy bandwidth is supplied
 if os.path.exists(os.path.join(ROOT, "MEASURED_PEAKS.json")):
     PEAK = json.load(open(os.path.join(ROOT, "MEASURED_PEAKS.json"))).get("hbm_gbs", PEAK)
 

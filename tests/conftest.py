@@ -11,7 +11,7 @@ MODELS = os.path.join(ROOT, "models")
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: needs a CUDA device (run on the B200 box)")
+    config.addinivalue_line("markers", "gpu: needs a CUDA device (an H100, sm_90)")
 
 
 def model_text(name):

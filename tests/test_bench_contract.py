@@ -1,11 +1,15 @@
-"""The committed bench lines (profiles/r01_bench_*.json, produced by bench.py on a B200) carry every key the
-measurement contract asks for.  Guards the JSON shape; the numbers themselves are measured, not tested."""
+"""The committed bench lines (profiles/r0*_bench_*.json, produced by bench.py on an H100) carry every key the
+measurement contract asks for.  Guards the JSON shape; the numbers themselves are measured, not tested.  The
+sharded (N > 1) line is produced in the test itself, on N GPUs of the machine that runs it."""
 import json
 import os
+import subprocess
+import sys
 
 import pytest
 
-PROFILES = os.path.join(os.path.dirname(os.path.dirname(os.path.abspath(__file__))), "profiles")
+ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
+PROFILES = os.path.join(ROOT, "profiles")
 BASE = {"metric": str, "value": float, "unit": str, "n_gpus": int, "steps": int, "warmup": int, "ms_per_step": float,
         "higher_is_better": bool, "scaling": str, "dtype": str, "data": str, "config": dict, "e2e": dict,
         "gpu_launches": int}
@@ -16,7 +20,7 @@ def load(name):
         return json.load(f)
 
 
-@pytest.mark.parametrize("name", ["r01_bench_n1.json", "r01_bench_n2.json", "r01_bench_n8.json", "r01_bench_n2_strong.json"])
+@pytest.mark.parametrize("name", ["r01_bench_n1.json"])
 def test_cuda_arm_line(name):
     d = load(name)
     for k, ty in BASE.items():
@@ -51,13 +55,25 @@ def test_reference_arm_line():
 
 
 # ---- round 2 lines: N = 1 is the 2D headline (+ the strong-scaling base), N > 1 is the sharded 4096^3 volume ----
+def _last_line(text):
+    return json.loads([l for l in text.splitlines() if l.startswith("{")][-1])
+
+
 def _r02(name):
-    p = os.path.join(PROFILES, name)
-    if not os.path.exists(p):
-        pytest.skip(f"{name} not committed yet")
-    with open(p) as f:
-        lines = [l for l in f if l.startswith("{")]
-    return json.loads(lines[-1])
+    with open(os.path.join(PROFILES, name)) as f:
+        return _last_line(f.read())
+
+
+def _sharded_bench_line(n):
+    """Runs bench.py --gpus n (one process per GPU, NCCL) and returns rank 0's line."""
+    import torch
+    if torch.cuda.device_count() < n:
+        pytest.skip(f"the sharded bench needs {n} GPUs; this machine has {torch.cuda.device_count()}")
+    out = subprocess.run([sys.executable, "-m", "torch.distributed.run", "--standalone", f"--nproc-per-node={n}",
+                          os.path.join(ROOT, "bench.py"), "--gpus", str(n), "--steps", "10", "--warmup", "3"],
+                         cwd=ROOT, capture_output=True, text=True, timeout=1800)
+    assert out.returncode == 0, out.stderr[-4000:]
+    return _last_line(out.stdout)
 
 
 def _common(d):
@@ -88,9 +104,11 @@ def test_r02_n1_line():
     assert d["cpu_baseline"]["kind"] == "port" and d["cpu_baseline"]["cores"] >= 1
 
 
+@pytest.mark.gpu
 @pytest.mark.parametrize("n", [2, 4, 8])
-def test_r02_sharded_lines(n):
-    d = _r02(f"r02_bench_n{n}.json")
+def test_sharded_bench_line_on_n_gpus(n):
+    """bench.py --gpus n, run here: the sharded 4096^3 line carries the contract's keys and a strong-scaling speed-up."""
+    d = _sharded_bench_line(n)
     _common(d)
     assert d["n_gpus"] == n and d["scaling"] == "strong" and "3D render 4096^3" in d["config"]["workload"]
     assert "all-gather" in d["config"]["collective"].lower() or "allgather" in d["config"]["collective"].lower()

@@ -18,7 +18,7 @@ def tables(tmp_path_factory):
     if not os.path.exists(nvcc):
         pytest.skip("nvcc not available")
     exe = str(tmp_path_factory.mktemp("dop") / "dop_check")
-    subprocess.run([nvcc, "-gencode", "arch=compute_100a,code=sm_100a", "-std=c++17", "-O1",
+    subprocess.run([nvcc, "-gencode", "arch=compute_90a,code=sm_90a", "-std=c++17", "-O1",
                     "-I", os.path.join(ROOT, "fidget_b200", "csrc", "cuda"), "-o", exe,
                     os.path.join(ROOT, "tests", "csrc", "dop_table_check.cu")], check=True, capture_output=True)
     out = subprocess.run([exe], check=True, capture_output=True, text=True).stdout.splitlines()

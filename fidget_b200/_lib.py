@@ -101,6 +101,7 @@ FC_FLAG_NO_CLAMP = 4
 FC_FLAG_FUSED_TAIL = 8
 FC_FLAG_EXACT_CENSUS = 16
 FC_FLAG_FULL_LADDER = 32
+FC_FLAG_MESH_COLLAPSE = 64
 FC_OUT_F32, FC_OUT_MASK_U8, FC_OUT_BITMAP_1BIT, FC_OUT_RGBA8 = 0, 1, 2, 3
 
 # name -> (restype, argtypes); mirrors include/fidget_cuda.h one to one
@@ -139,6 +140,7 @@ CUDA_API = {
     "fc_octree_sample": (_i32, [_vp, _vp, _P(FcOctreeCfg), _vp, _u64, _P(_u64), _P(FcOctreeStats)]),
     "fc_mesh_build": (_i32, [_vp, _vp, _P(FcOctreeCfg), _P(FcMeshInfo)]),
     "fc_mesh_read": (_i32, [_vp, _vp, _vp]),
+    "fc_mesh_read_cells": (_i32, [_vp, _vp, _u64, _P(_u64)]),
     "fc_mesh_write_stl": (_i32, [_vp, _vp, C.c_size_t, _P(C.c_size_t)]),
     "fc_schedule_check": (_i32, [_P(_u32), C.c_size_t, _u8, _u32, _u32, _u32, _P(FcScheduleInfo)]),
     "fc_denoise_normals": (_i32, [_vp, _vp, _u32, _u32, _vp]),

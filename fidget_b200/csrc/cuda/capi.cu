@@ -130,6 +130,9 @@ void fc_ctx_destroy(fc_ctx* c) {
     c->mesh_scratch.release();
     c->mesh_verts.release();
     c->mesh_tris.release();
+    c->mesh_tree.release();
+    c->mesh_herm.release();
+    c->mesh_cells.release();
     c->tile_slots.release();
     c->fx_in.release();
     c->fx_out.release();

@@ -110,6 +110,8 @@ struct fc_ctx {
     DevBuf arena, jobs[MAX_LEVELS + 1], fills[MAX_LEVELS], choice_scratch, counters, stats, image, heightmap, leaf_tapes, zsort, census, occl;
     DevBuf mesh_leaves, mesh_scratch, mesh_verts, mesh_tris;   // fc_mesh_build: sampler output and the mesh, resident in HBM
     uint32_t mesh_n_verts = 0, mesh_n_tris = 0;
+    DevBuf mesh_tree, mesh_herm, mesh_cells;                    // FC_FLAG_MESH_COLLAPSE: cell tree, Hermite records, final leaves
+    uint32_t mesh_n_cells = 0;
     DevBuf fx_in, fx_out, fx_tmp, fx_tables;  // effects: staged host images, intermediate maps, SSAO tables
     // tile interleave: device list of this rank's XY root tiles (cached on its key), and the
     // tile -> gathered-slot table of fc_tiles_unpack

@@ -11,9 +11,12 @@
 //              around the edge's intersection vertex (taken from cell d), winding 3 or 1 by the sign at the
 //              edge's start;
 //   STL        Mesh::write_stl (fidget-mesh/src/output.rs:7-38).
-// Out of scope here: cell collapse (octree.rs:252-440).  The reference merges the eight children of a branch into
-// one leaf when the merged QEF error is small and the result stays manifold; without it the mesh is the
-// uniform-depth Manifold Dual Contouring mesh -- same surface, more triangles in flat regions.
+//   collapse   with FC_FLAG_MESH_COLLAPSE only (the default stays the uniform-depth mesh): Octree::check_done /
+//              collapsible / try_collapse (octree.rs:252-440) merge the eight children of a cell into one leaf when
+//              the topology stays manifold and the merged QEF error (LeafHermiteData::merge / solve,
+//              octree.rs:912-1033) is below twice the children's; one launch per depth, bottom-up, over a tree of
+//              the surface leaves' ancestors keyed by (depth, x, y, z); the dual is then walked over leaves of
+//              different depths (k_tree_faces: dc_cell / dc_face / dc_edge's result, one thread per leaf edge).
 //
 // The 3x3 symmetric eigen-problem is solved with cyclic Jacobi rotations in f32 (the reference calls nalgebra's
 // SVD, a third-party algorithm not under /root/reference); positions agree to ~1e-5 of a cell, not bit for bit.
@@ -297,11 +300,576 @@ __global__ void k_mesh_stl(const float3* verts, const uint3* tris, uint32_t n_tr
     dst[24] = 0;
 }
 
+// ---- cell collapse and the adaptive dual walk (FC_FLAG_MESH_COLLAPSE) ---------------------------------------------
+// The tree: node ids [0, n_leaves) are the sampler's surface leaves (depth D); the ids after them are their ancestors,
+// built level by level bottom-up, so every depth is one contiguous id range.  A cell that is not a node is Empty or
+// Full as a whole (it holds no surface leaf, and neighbouring cells share their corner samples); its sign is the sign
+// at its parent's centre, which every child of that parent shares and a node child knows from its corner mask.
+constexpr float QEF_ERR_EMPTY = -1.0f, QEF_ERR_INVALID = -2.0f;   // octree.rs:895-899
+enum : uint8_t { NODE_LEAF = 1, NODE_BRANCH = 2, NODE_FINAL = 4 };
+
+struct Qef { float ata[6], atb[3], btb, mp[4]; };   // QuadraticErrorSolver; ata = xx xy xz yy yz zz
+struct Hermite { float ipos[12][4], igrad[12][4]; Qef face[6], center; };   // LeafHermiteData (qef_err: node_err)
+
+struct TreeScratch {
+    const OctreeLeaf* leaves;
+    uint32_t n_leaves, depth;
+    unsigned long long* hkeys;   // (depth, x, y, z) -> node id
+    uint32_t* hvals;
+    uint32_t hmask;
+    unsigned long long* node_key;
+    uint32_t* node_mask;         // corner mask (leaves: CellMask; branches: the signs at their eight corners)
+    uint8_t* node_state;
+    float* node_err;             // LeafHermiteData::qef_err
+    float3* node_vert;           // vertex of a collapsed leaf
+    Hermite* herm;               // [node - n_leaves]
+    const float3* cell_verts;    // k_mesh_vertices' output for the surface leaves
+    const uint32_t* corner_vert;
+    uint32_t n_nodes;
+    uint32_t* remap;             // [n_nodes][16] as MeshScratch::remap
+    uint32_t* counts;            // [0] vertices [1] triangles [2] triangle cursor [3] open edges [4] nodes [5] final leaves
+    float3* out_verts;
+    uint32_t cap_verts;
+    uint3* out_tris;
+    uint32_t cap_tris;
+    fc_mesh_cell* out_cells;
+};
+
+__host__ __device__ __forceinline__ unsigned long long tree_key(uint32_t d, uint32_t x, uint32_t y, uint32_t z) {
+    return (unsigned long long)x | ((unsigned long long)y << 16) | ((unsigned long long)z << 32) | ((unsigned long long)d << 48);
+}
+__device__ __forceinline__ uint32_t key_x(unsigned long long k, int a) { return uint32_t(k >> (16 * a)) & 0xffffu; }
+__device__ __forceinline__ uint32_t key_depth(unsigned long long k) { return uint32_t(k >> 48); }
+__device__ __forceinline__ uint32_t tree_find(const TreeScratch& m, unsigned long long key) {
+    uint32_t h = hash_key(key) & m.hmask;
+    for (;;) {
+        const unsigned long long k = m.hkeys[h];
+        if (k == key) return m.hvals[h];
+        if (k == ~0ull) return ~0u;
+        h = (h + 1u) & m.hmask;
+    }
+}
+// returns true when `key` was new; the caller owns hvals[slot] then
+__device__ __forceinline__ bool tree_insert(const TreeScratch& m, unsigned long long key, uint32_t& slot) {
+    uint32_t h = hash_key(key) & m.hmask;
+    for (;;) {
+        const unsigned long long old = atomicCAS(&m.hkeys[h], ~0ull, key);
+        if (old == ~0ull) { slot = h; return true; }
+        if (old == key) return false;
+        h = (h + 1u) & m.hmask;
+    }
+}
+
+__device__ inline void qef_zero(Qef& q) {
+    for (int k = 0; k < 6; ++k) q.ata[k] = 0.0f;
+    for (int k = 0; k < 3; ++k) q.atb[k] = 0.0f;
+    q.btb = 0.0f;
+    for (int k = 0; k < 4; ++k) q.mp[k] = 0.0f;
+}
+__device__ inline void qef_add(Qef& q, const Qef& r) {   // AddAssign (qef.rs:19-26)
+    for (int k = 0; k < 6; ++k) q.ata[k] += r.ata[k];
+    for (int k = 0; k < 3; ++k) q.atb[k] += r.atb[k];
+    q.btb += r.btb;
+    for (int k = 0; k < 4; ++k) q.mp[k] += r.mp[k];
+}
+__device__ inline void qef_add_intersection(Qef& q, const float p[3], const float g[4]) {   // qef.rs:48-59
+    q.mp[0] += p[0]; q.mp[1] += p[1]; q.mp[2] += p[2]; q.mp[3] += 1.0f;
+    const float nl = sqrtf(g[0] * g[0] + g[1] * g[1] + g[2] * g[2]);
+    const float n[3] = {g[0] / nl, g[1] / nl, g[2] / nl};
+    const float d = n[0] * p[0] + n[1] * p[1] + n[2] * p[2];
+    q.ata[0] += n[0] * n[0]; q.ata[1] += n[0] * n[1]; q.ata[2] += n[0] * n[2];
+    q.ata[3] += n[1] * n[1]; q.ata[4] += n[1] * n[2]; q.ata[5] += n[2] * n[2];
+    for (int r = 0; r < 3; ++r) q.atb[r] += n[r] * d;
+    q.btb += d * d;
+}
+// QuadraticErrorSolver::solve (qef.rs:67-118): the vertex as k_mesh_vertices places it, and the clamped error
+__device__ inline float qef_solve(const Qef& q, float pos[3]) {
+    const float ata[3][3] = {{q.ata[0], q.ata[1], q.ata[2]}, {q.ata[1], q.ata[3], q.ata[4]}, {q.ata[2], q.ata[4], q.ata[5]}};
+    const float center[3] = {q.mp[0] / q.mp[3], q.mp[1] / q.mp[3], q.mp[2] / q.mp[3]};
+    float b[3];
+    for (int r = 0; r < 3; ++r) b[r] = q.atb[r] - (ata[r][0] * center[0] + ata[r][1] * center[1] + ata[r][2] * center[2]);
+    float w[3], V[3][3], a2[3][3];
+    for (int r = 0; r < 3; ++r) for (int c2 = 0; c2 < 3; ++c2) a2[r][c2] = ata[r][c2];
+    jacobi3(a2, w, V);
+    int order[3] = {0, 1, 2};
+    for (int x = 0; x < 2; ++x) for (int y = x + 1; y < 3; ++y)
+        if (fabsf(w[order[y]]) > fabsf(w[order[x]])) { const int tmp = order[x]; order[x] = order[y]; order[y] = tmp; }
+    const float cutoff = fabsf(w[order[0]]) * 1e-3f;
+    int rank = 3;
+    for (int k = 0; k < 3; ++k) if (fabsf(w[order[k]]) < cutoff) { rank = k; break; }
+    const float eps = rank < 3 ? fabsf(w[order[rank]]) : 0.0f;
+    float sol[3] = {0, 0, 0};
+    for (int k = 0; k < 3; ++k) {
+        const int j = order[k];
+        if (!(fabsf(w[j]) > eps)) continue;
+        const float coef = (V[0][j] * b[0] + V[1][j] * b[1] + V[2][j] * b[2]) / w[j];
+        sol[0] += coef * V[0][j]; sol[1] += coef * V[1][j]; sol[2] += coef * V[2][j];
+    }
+    for (int r = 0; r < 3; ++r) pos[r] = sol[r] + center[r];
+    if (!(pos[0] == pos[0] && pos[1] == pos[1] && pos[2] == pos[2])) for (int r = 0; r < 3; ++r) pos[r] = center[r];
+    // pos^T A^T A pos - 2 pos^T A^T b + b^T b, clamped to >= 1e-6 (qef.rs:111-115)
+    float row[3];
+    for (int c2 = 0; c2 < 3; ++c2) row[c2] = pos[0] * ata[0][c2] + pos[1] * ata[1][c2] + pos[2] * ata[2][c2];
+    const float quad = row[0] * pos[0] + row[1] * pos[1] + row[2] * pos[2];
+    const float lin = (2.0f * pos[0]) * q.atb[0] + (2.0f * pos[1]) * q.atb[1] + (2.0f * pos[2]) * q.atb[2];
+    const float err = (quad - lin) + q.btb;
+    return err > 1e-6f ? err : 1e-6f;   // f32::max: a NaN error becomes 1e-6
+}
+
+// Surface leaves enter the tree at depth D
+__global__ void k_tree_leaves(TreeScratch m) {
+    const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= m.n_leaves) return;
+    const OctreeLeaf& L = m.leaves[i];
+    const unsigned long long key = tree_key(m.depth, L.ix, L.iy, L.iz);
+    uint32_t slot;
+    if (tree_insert(m, key, slot)) m.hvals[slot] = i;
+    m.node_key[i] = key;
+    m.node_mask[i] = L.mask;
+    m.node_state[i] = NODE_LEAF;
+}
+// The parents of the nodes [lo, hi) (one depth), appended as new nodes
+__global__ void k_tree_parents(TreeScratch m, uint32_t lo, uint32_t hi) {
+    const uint32_t i = lo + blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= hi) return;
+    const unsigned long long k = m.node_key[i];
+    const unsigned long long pk = tree_key(key_depth(k) - 1u, key_x(k, 0) >> 1, key_x(k, 1) >> 1, key_x(k, 2) >> 1);
+    uint32_t slot;
+    if (!tree_insert(m, pk, slot)) return;
+    const uint32_t id = atomicAdd(&m.counts[4], 1u);
+    m.hvals[slot] = id;
+    m.node_key[id] = pk;
+}
+
+// LeafHermiteData::qef_err of every surface leaf (OctreeBuilder::leaf, octree.rs:810-851): one QEF per vertex group,
+// the last group's error wins; a NaN gradient marks the group QEF_ERR_INVALID
+__global__ void __launch_bounds__(128) k_tree_leaf_err(TreeScratch m) {
+    const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= m.n_leaves) return;
+    const OctreeLeaf& L = m.leaves[i];
+    const uint32_t mask = L.mask, cv = m.corner_vert[i], n_groups = cv >> 16;
+    float err = QEF_ERR_EMPTY;
+    for (uint32_t g = 0; g < n_groups && g < 4u; ++g) {
+        Qef q;
+        qef_zero(q);
+        bool invalid = false;
+        for (uint32_t s = 0; s < 8 && !invalid; ++s) {
+            if (!((mask >> s) & 1u) || ((cv >> (2u * s)) & 3u) != g) continue;
+            for (uint32_t t = 1; t < 8; t <<= 1) {
+                if ((mask >> (s ^ t)) & 1u) continue;
+                const uint32_t u = next_axis(t), v = next_axis(u);
+                const uint32_t ti = t == 1u ? 0u : (t == 2u ? 1u : 2u);
+                const uint32_t e = ti * 4u + ((s & u) ? 1u : 0u) + ((s & v) ? 2u : 0u);
+                const float p[3] = {L.pos[e][0], L.pos[e][1], L.pos[e][2]};
+                const float gr[4] = {L.grad[e][0], L.grad[e][1], L.grad[e][2], L.grad[e][3]};
+                if (gr[0] != gr[0] || gr[1] != gr[1] || gr[2] != gr[2] || gr[3] != gr[3]) { invalid = true; break; }
+                qef_add_intersection(q, p, gr);
+            }
+        }
+        if (invalid) { err = QEF_ERR_INVALID; continue; }
+        float pos[3];
+        err = qef_solve(q, pos);
+    }
+    m.node_err[i] = err;
+}
+
+// Hermite data of one child, as LeafHermiteData::merge reads it: a surface leaf's intersections, a collapsed leaf's
+// merged record, or the default record of an Empty / Full cell (no intersections, zero QEFs)
+__device__ __forceinline__ bool child_inter(const TreeScratch& m, uint32_t ch, uint32_t e, float p[3], float g[4]) {
+    if (ch == ~0u) return false;
+    if (ch < m.n_leaves) {
+        const OctreeLeaf& L = m.leaves[ch];
+        if (!((L.present >> e) & 1u)) return false;
+        for (int k = 0; k < 3; ++k) p[k] = L.pos[e][k];
+        for (int k = 0; k < 4; ++k) g[k] = L.grad[e][k];
+        return true;
+    }
+    const Hermite& H = m.herm[ch - m.n_leaves];
+    if (!(H.ipos[e][3] != 0.0f)) return false;
+    for (int k = 0; k < 3; ++k) p[k] = H.ipos[e][k];
+    for (int k = 0; k < 4; ++k) g[k] = H.igrad[e][k];
+    return true;
+}
+__device__ __forceinline__ void add_child_inter(const TreeScratch& m, uint32_t ch, uint32_t e, Qef& q) {   // From<LeafIntersection>
+    float p[3], g[4];
+    if (child_inter(m, ch, e, p, g)) qef_add_intersection(q, p, g);
+}
+__device__ __forceinline__ void add_child_face(const TreeScratch& m, uint32_t ch, uint32_t f, Qef& q) {
+    if (ch != ~0u && ch >= m.n_leaves) qef_add(q, m.herm[ch - m.n_leaves].face[f]);
+}
+__device__ __forceinline__ uint32_t axis_index(uint32_t a) { return a == 1u ? 0u : (a == 2u ? 1u : 2u); }
+
+// One thread per node of one depth: Octree::check_done / collapsible / try_collapse (octree.rs:252-440) with
+// LeafHermiteData::merge / solve (octree.rs:917-1033)
+__global__ void __launch_bounds__(128) k_tree_collapse(TreeScratch m, uint32_t lo, uint32_t hi) {
+    const uint32_t id = lo + blockIdx.x * blockDim.x + threadIdx.x;
+    if (id >= hi) return;
+    const unsigned long long key = m.node_key[id];
+    const uint32_t d = key_depth(key), x = key_x(key, 0), y = key_x(key, 1), z = key_x(key, 2);
+    uint32_t ch[8];
+    for (uint32_t c = 0; c < 8; ++c)
+        ch[c] = tree_find(m, tree_key(d + 1u, 2u * x + (c & 1u), 2u * y + ((c >> 1) & 1u), 2u * z + ((c >> 2) & 1u)));
+    uint32_t centre = 0;   // sign at this cell's centre: corner 7 ^ c of child c
+    for (uint32_t c = 0; c < 8; ++c)
+        if (ch[c] != ~0u) { centre = (m.node_mask[ch[c]] >> (7u ^ c)) & 1u; break; }
+    uint32_t cmask = 0, cm[8];   // cm[c]: corner mask of child c (Empty / Full: all corners alike)
+    bool branch = false, multi = false;
+    for (uint32_t c = 0; c < 8; ++c) {
+        if (ch[c] == ~0u) { cm[c] = centre ? 0xffu : 0u; }
+        else {
+            cm[c] = m.node_mask[ch[c]];
+            branch |= (m.node_state[ch[c]] & NODE_BRANCH) != 0;
+            multi |= ch[c] < m.n_leaves && (m.corner_vert[ch[c]] >> 16) > 1u;   // CELL_TO_VERT_TO_EDGES[mask].len() > 1
+        }
+        cmask |= ((cm[c] >> c) & 1u) << c;
+    }
+    m.node_mask[id] = cmask;
+    m.node_state[id] = NODE_BRANCH;
+    if (branch || multi) return;
+    // collapsible: the three predicates of Ju et al. 2002, section 4.1
+    const uint32_t frames[3][3] = {{1u, 2u, 4u}, {2u, 4u, 1u}, {4u, 1u, 2u}};
+    for (int f = 0; f < 3; ++f) {
+        const uint32_t t = frames[f][0], u = frames[f][1], v = frames[f][2];
+        for (uint32_t i = 0; i < 4; ++i) {
+            const uint32_t a = ((i & 1u) ? u : 0u) | ((i & 2u) ? v : 0u), b = a | t;
+            const uint32_t mid = (cm[a] >> b) & 1u;
+            if (((cmask >> a) & 1u) != mid && ((cmask >> b) & 1u) != mid) return;
+        }
+        for (uint32_t i = 0; i < 2; ++i) {
+            const uint32_t a = (i & 1u) == 0 ? t : 0u, q[4] = {a, a | u, a | v, a | u | v};
+            const uint32_t mid = (cm[a] >> (a | u | v)) & 1u;
+            bool agree = false;
+            for (int k = 0; k < 4; ++k) agree |= ((cmask >> q[k]) & 1u) == mid;
+            if (!agree) return;
+        }
+        const uint32_t mid = (cm[0] >> (t | u | v)) & 1u;
+        bool agree = false;
+        for (uint32_t k = 0; k < 8; ++k) agree |= ((cmask >> k) & 1u) == mid;
+        if (!agree) return;
+    }
+    if (cmask == 0u || cmask == 0xffu) return;
+    {   // one vertex group (the collapsed cell is manifold)
+        uint32_t label[8];
+        for (uint32_t c = 0; c < 8; ++c) label[c] = c;
+        for (int it = 0; it < 8; ++it)
+            for (uint32_t c = 0; c < 8; ++c)
+                for (uint32_t ax = 1; ax < 8; ax <<= 1) {
+                    const uint32_t g = c ^ ax;
+                    if (((cmask >> c) & 1u) && ((cmask >> g) & 1u)) { const uint32_t lo2 = min(label[c], label[g]); label[c] = label[g] = lo2; }
+                }
+        for (uint32_t c = 0; c < 8; ++c) if (((cmask >> c) & 1u) && label[c] != label[__ffs(cmask) - 1]) return;
+    }
+    // merge: any invalid child QEF stops the collapse
+    float child_err = INFINITY;
+    for (uint32_t c = 0; c < 8; ++c) {
+        const float e = ch[c] == ~0u ? QEF_ERR_EMPTY : m.node_err[ch[c]];
+        if (e == QEF_ERR_INVALID) return;
+        if (e >= 0.0f) child_err = fminf(child_err, e);
+    }
+    Hermite& out = m.herm[id - m.n_leaves];
+    for (uint32_t ti = 0; ti < 3; ++ti) {   // intersections along the coarse edges
+        const uint32_t t = 1u << ti, u = next_axis(t), v = next_axis(u);
+        for (uint32_t edge = 0; edge < 4; ++edge) {
+            const uint32_t start = ((edge & 1u) ? u : 0u) | ((edge & 2u) ? v : 0u), end = start | t, e = ti * 4u + edge;
+            float p[3], g[4];
+            bool have = child_inter(m, ch[start], e, p, g);
+            if (!have) have = child_inter(m, ch[end], e, p, g);
+            for (int k = 0; k < 3; ++k) out.ipos[e][k] = have ? p[k] : 0.0f;
+            out.ipos[e][3] = have ? 1.0f : 0.0f;
+            for (int k = 0; k < 4; ++k) out.igrad[e][k] = have ? g[k] : 0.0f;
+        }
+    }
+    // face QEFs, as written in the reference: `v` is `t.next()` like `u`, and the "u" edges use edge_index_v
+    for (uint32_t ti = 0; ti < 3; ++ti) {
+        const uint32_t t = 1u << ti, u = next_axis(t), v = u;
+        for (uint32_t face = 0; face < 2; ++face) {
+            const uint32_t a = face == 1 ? t : 0u, b = a | u, c = a | v, dd = a | u | v, f = ti * 2u + face;
+            Qef q;
+            qef_zero(q);
+            add_child_face(m, ch[a], f, q); add_child_face(m, ch[b], f, q); add_child_face(m, ch[c], f, q); add_child_face(m, ch[dd], f, q);
+            const uint32_t ev = axis_index(v) * 4u + face * 2u + 1u;
+            add_child_inter(m, ch[a], ev, q); add_child_inter(m, ch[b], ev, q);
+            add_child_inter(m, ch[a], ev, q); add_child_inter(m, ch[c], ev, q);
+            out.face[f] = q;
+        }
+    }
+    {   // centre QEF
+        Qef q;
+        qef_zero(q);
+        for (uint32_t ti = 0; ti < 3; ++ti) {
+            const uint32_t t = 1u << ti, u = next_axis(t), v = u;
+            const uint32_t a = 0u, b = a | u, c = a | v, dd = a | u | v;
+            add_child_face(m, ch[a], ti * 2u + 1u, q); add_child_face(m, ch[b], ti * 2u + 1u, q);
+            add_child_face(m, ch[c], ti * 2u + 1u, q); add_child_face(m, ch[dd], ti * 2u + 1u, q);
+            add_child_inter(m, ch[a], axis_index(u) * 4u + 3u, q);
+            add_child_inter(m, ch[b], axis_index(u) * 4u + 3u, q);
+        }
+        for (uint32_t c = 0; c < 8; ++c)
+            if (ch[c] != ~0u && ch[c] >= m.n_leaves) qef_add(q, m.herm[ch[c] - m.n_leaves].center);
+        out.center = q;
+    }
+    // LeafHermiteData::solve
+    Qef q = out.center;
+    for (uint32_t e = 0; e < 12; ++e)
+        if (out.ipos[e][3] != 0.0f) {
+            const float p[3] = {out.ipos[e][0], out.ipos[e][1], out.ipos[e][2]}, g[4] = {out.igrad[e][0], out.igrad[e][1], out.igrad[e][2], out.igrad[e][3]};
+            qef_add_intersection(q, p, g);
+        }
+    for (int f = 0; f < 6; ++f) qef_add(q, out.face[f]);
+    float pos[3];
+    const float err = qef_solve(q, pos);
+    // CellBounds::contains: closed intervals of the cell's bounds
+    const float size = 2.0f / float(1u << d), lo3[3] = {-1.0f + float(x) * size, -1.0f + float(y) * size, -1.0f + float(z) * size};
+    bool inside = true;
+    for (int k = 0; k < 3; ++k) inside &= pos[k] >= lo3[k] && pos[k] <= lo3[k] + size;
+    if (err >= child_err * 2.0f || !inside) return;
+    m.node_err[id] = err;
+    m.node_vert[id] = make_float3(pos[0], pos[1], pos[2]);
+    m.node_state[id] = NODE_LEAF;
+}
+
+// Final leaves: leaves whose parent stayed a branch (or the root); listed for fc_mesh_read_cells
+__global__ void k_tree_final(TreeScratch m) {
+    const uint32_t id = blockIdx.x * blockDim.x + threadIdx.x;
+    if (id >= m.n_nodes || !(m.node_state[id] & NODE_LEAF)) return;
+    const unsigned long long k = m.node_key[id];
+    const uint32_t d = key_depth(k);
+    if (d > 0) {
+        const uint32_t p = tree_find(m, tree_key(d - 1u, key_x(k, 0) >> 1, key_x(k, 1) >> 1, key_x(k, 2) >> 1));
+        if (!(m.node_state[p] & NODE_BRANCH)) return;
+    }
+    m.node_state[id] = NODE_LEAF | NODE_FINAL;
+    const uint32_t slot = atomicAdd(&m.counts[5], 1u);
+    fc_mesh_cell cell;
+    cell.ix = uint16_t(key_x(k, 0)); cell.iy = uint16_t(key_x(k, 1)); cell.iz = uint16_t(key_x(k, 2));
+    cell.depth = uint8_t(d);
+    cell.mask = uint8_t(m.node_mask[id]);
+    const float3 v = id < m.n_leaves ? m.cell_verts[size_t(id) * 4] : m.node_vert[id];
+    cell.vertex[0] = v.x; cell.vertex[1] = v.y; cell.vertex[2] = v.z;
+    m.out_cells[slot] = cell;
+}
+
+// The final leaf covering cell (d, p) of the domain: 0 = found (id, depth), 1 = smaller leaves own this spot (a branch
+// at depth d), 2 = an Empty / Full cell
+__device__ inline int tree_cover(const TreeScratch& m, uint32_t d, const uint32_t p[3], uint32_t& id, uint32_t& depth) {
+    for (uint32_t k = 0; k <= d; ++k) {
+        const uint32_t dk = d - k, n = tree_find(m, tree_key(dk, p[0] >> k, p[1] >> k, p[2] >> k));
+        if (n == ~0u) continue;
+        const uint8_t st = m.node_state[n];
+        if (st & NODE_FINAL) { id = n; depth = dk; return 0; }
+        if (st & NODE_BRANCH) return k == 0 ? 1 : 2;
+    }
+    return 2;
+}
+
+// dc_edge over the adaptive tree (dc.rs:104-213): one thread per (final leaf, edge).  The four cells around the edge
+// segment are looked up at the leaf's depth; the quad is emitted by the deepest of them (the last such in [a, b, c, d],
+// as Iterator::max_by_key picks), with the vertex of every shallower leaf being its single one, the intersection
+// vertex from the emitting leaf, and no triangle between two corners that are the same cell.
+template <int PASS>
+__global__ void __launch_bounds__(128) k_tree_faces(TreeScratch m) {
+    const uint32_t gid = blockIdx.x * blockDim.x + threadIdx.x;
+    if (gid >= m.n_nodes * 12u) return;
+    const uint32_t id = gid / 12u, e = gid % 12u;
+    if (!(m.node_state[id] & NODE_FINAL)) return;
+    const uint32_t mask = m.node_mask[id], ti = e / 4u, j = e % 4u, t = 1u << ti, u = next_axis(t), v = next_axis(u);
+    const uint32_t start = ((j & 1u) ? u : 0u) | ((j & 2u) ? v : 0u);
+    if (((mask >> start) & 1u) == ((mask >> (start | t)) & 1u)) return;
+    const unsigned long long key = m.node_key[id];
+    const uint32_t d = key_depth(key), side = 1u << d;
+    const uint32_t self = j == 3u ? 0u : (j == 2u ? 1u : (j == 0u ? 2u : 3u));   // position in [a, b, c, d]
+    int pos[4][3];
+    const int du[3] = {(u & 1u) ? 1 : 0, (u & 2u) ? 1 : 0, (u & 4u) ? 1 : 0}, dv[3] = {(v & 1u) ? 1 : 0, (v & 2u) ? 1 : 0, (v & 4u) ? 1 : 0};
+    const int offu[4] = {0, 1, 1, 0}, offv[4] = {0, 0, 1, 1};
+    bool boundary = false;
+    for (int k = 0; k < 4; ++k)
+        for (int a = 0; a < 3; ++a) {
+            pos[k][a] = int(key_x(key, a)) + (offu[k] - offu[self]) * du[a] + (offv[k] - offv[self]) * dv[a];
+            boundary |= pos[k][a] < 0 || pos[k][a] >= int(side);
+        }
+    uint32_t node[4], depth[4];
+    bool in_domain[4], empty = false;
+    for (int k = 0; k < 4; ++k) {
+        in_domain[k] = pos[k][0] >= 0 && pos[k][0] < int(side) && pos[k][1] >= 0 && pos[k][1] < int(side) && pos[k][2] >= 0 && pos[k][2] < int(side);
+        if (!in_domain[k]) { node[k] = ~0u; depth[k] = 0; continue; }
+        if (uint32_t(k) == self) { node[k] = id; depth[k] = d; continue; }
+        const uint32_t p[3] = {uint32_t(pos[k][0]), uint32_t(pos[k][1]), uint32_t(pos[k][2])};
+        const int r = tree_cover(m, d, p, node[k], depth[k]);
+        if (r == 1) return;
+        if (r == 2) { empty = true; node[k] = ~0u; depth[k] = 0; }
+    }
+    uint32_t deepest = self;
+    for (uint32_t k = 0; k < 4; ++k) if (node[k] != ~0u && depth[k] == d) deepest = k;
+    if (deepest != self) return;
+    if (boundary) {
+        if (PASS == 0) atomicAdd(&m.counts[3], 1u);
+        return;
+    }
+    if (empty) return;
+    const uint32_t edge_of[4] = {ti * 4u + 3u, ti * 4u + 2u, ti * 4u + 0u, ti * 4u + 1u};
+    uint32_t slot[4];
+    for (int k = 0; k < 4; ++k) {
+        uint32_t g = 0;
+        if (depth[k] == d && node[k] < m.n_leaves) {
+            const uint32_t ek = edge_of[k], s = ((ek & 1u) ? u : 0u) | ((ek & 2u) ? v : 0u), mk = m.node_mask[node[k]];
+            const uint32_t inside_corner = ((mk >> s) & 1u) ? s : (s | t);
+            g = (m.corner_vert[node[k]] >> (2u * inside_corner)) & 3u;
+        }
+        slot[k] = node[k] * 16u + g;
+    }
+    const uint32_t islot = id * 16u + 4u + e;
+    const uint32_t winding = ((mask >> start) & 1u) ? 1u : 3u;
+    if (PASS == 0) {   // MeshBuilder::vertex is called for all five vertices, whichever triangles are dropped
+        uint32_t n_tris = 0;
+        for (uint32_t k = 0; k < 4u; ++k) {
+            m.remap[slot[k]] = 1u;
+            n_tris += node[k] != node[(k + winding) & 3u];
+        }
+        m.remap[islot] = 1u;
+        atomicAdd(&m.counts[1], n_tris);
+        return;
+    }
+    uint32_t n_tris = 0;
+    for (uint32_t k = 0; k < 4u; ++k) n_tris += node[k] != node[(k + winding) & 3u];
+    const uint32_t base = atomicAdd(&m.counts[2], n_tris), iv = m.remap[islot];
+    uint32_t o = 0;
+    for (uint32_t k = 0; k < 4u; ++k)
+        if (node[k] != node[(k + winding) & 3u]) {
+            if (base + o < m.cap_tris) m.out_tris[base + o] = make_uint3(m.remap[slot[k]], m.remap[slot[(k + winding) & 3u]], iv);
+            ++o;
+        }
+}
+
+// compaction of the used vertex slots (MeshBuilder::vertex: one output vertex per octree vertex)
+__global__ void k_tree_assign(TreeScratch m) {
+    const uint64_t s = uint64_t(blockIdx.x) * blockDim.x + threadIdx.x;
+    if (s >= uint64_t(m.n_nodes) * 16u) return;
+    if (m.remap[s] != 1u) { m.remap[s] = ~0u; return; }
+    const uint32_t id = atomicAdd(&m.counts[0], 1u);
+    m.remap[s] = id;
+    if (id >= m.cap_verts) return;
+    const uint32_t node = uint32_t(s / 16u), k = uint32_t(s % 16u);
+    if (k < 4u) {
+        m.out_verts[id] = node < m.n_leaves ? m.cell_verts[size_t(node) * 4 + k] : m.node_vert[node];
+    } else if (node < m.n_leaves) {
+        const OctreeLeaf& L = m.leaves[node];
+        m.out_verts[id] = make_float3(L.pos[k - 4u][0], L.pos[k - 4u][1], L.pos[k - 4u][2]);
+    } else {
+        const Hermite& H = m.herm[node - m.n_leaves];
+        m.out_verts[id] = make_float3(H.ipos[k - 4u][0], H.ipos[k - 4u][1], H.ipos[k - 4u][2]);
+    }
+}
+
 }  // namespace fdev
 
 // fc_octree_sample's device half (octree_capi.cu)
 int32_t octree_sample_device(fc_ctx* c, const fc_tape* tape, const fc_octree_cfg* cfg, OctreeLeaf* dout, uint64_t cap,
                              uint32_t* n_out, fc_octree_stats* stats);
+
+// fc_mesh_build with FC_FLAG_MESH_COLLAPSE, after the sampler (n > 0 surface leaves in c->mesh_leaves; c->mu held)
+static int32_t mesh_build_collapse(fc_ctx* c, uint32_t n, uint32_t depth, fc_mesh_info* info) {
+    using namespace fdev;
+    cudaStream_t s = c->stream;
+    // nodes: the leaves plus at most min(n, 8^d) ancestors at every depth d < D
+    uint64_t cap_nodes = n;
+    for (uint32_t d = 0; d < depth; ++d) cap_nodes += std::min<uint64_t>(n, 1ull << (3 * d));
+    if (cap_nodes * 16 >= (1ull << 32)) return fail(FC_ERR_INVALID, "mesh too large for cell collapse");
+    uint64_t hsize = 1024;
+    while (hsize < 2 * cap_nodes) hsize <<= 1;
+    auto al = [](size_t x) { return (x + 255) & ~size_t(255); };
+    const size_t b_keys = hsize * 8, b_vals = hsize * 4, b_nkey = cap_nodes * 8, b_nmask = cap_nodes * 4, b_nstate = cap_nodes,
+                 b_nerr = cap_nodes * 4, b_nvert = cap_nodes * sizeof(float3), b_cv = size_t(n) * 4 * sizeof(float3), b_cn = size_t(n) * 4;
+    CU(c->mesh_tree.ensure(al(b_keys) + al(b_vals) + al(b_nkey) + al(b_nmask) + al(b_nstate) + al(b_nerr) + al(b_nvert) + al(b_cv) +
+                           al(b_cn) + 256));
+    TreeScratch m{};
+    char* q = c->mesh_tree.as<char>();
+    m.hkeys = reinterpret_cast<unsigned long long*>(q); q += al(b_keys);
+    m.hvals = reinterpret_cast<uint32_t*>(q); q += al(b_vals);
+    m.node_key = reinterpret_cast<unsigned long long*>(q); q += al(b_nkey);
+    m.node_mask = reinterpret_cast<uint32_t*>(q); q += al(b_nmask);
+    m.node_state = reinterpret_cast<uint8_t*>(q); q += al(b_nstate);
+    m.node_err = reinterpret_cast<float*>(q); q += al(b_nerr);
+    m.node_vert = reinterpret_cast<float3*>(q); q += al(b_nvert);
+    float3* cell_verts = reinterpret_cast<float3*>(q); q += al(b_cv);
+    uint32_t* corner_vert = reinterpret_cast<uint32_t*>(q); q += al(b_cn);
+    m.counts = reinterpret_cast<uint32_t*>(q);
+    m.leaves = c->mesh_leaves.as<OctreeLeaf>();
+    m.n_leaves = n;
+    m.depth = depth;
+    m.hmask = uint32_t(hsize - 1);
+    m.cell_verts = cell_verts;
+    m.corner_vert = corner_vert;
+    MeshScratch ms{};   // k_mesh_vertices: the surface leaves' vertices, exactly as the uniform mesh places them
+    ms.leaves = m.leaves;
+    ms.n_leaves = n;
+    ms.cell_verts = cell_verts;
+    ms.corner_vert = corner_vert;
+
+    cudaEvent_t e0 = get_event(c, 0), e1 = get_event(c, 1);
+    CU(cudaEventRecord(e0, s));
+    CU(cudaMemsetAsync(m.hkeys, 0xff, b_keys, s));
+    CU(cudaMemsetAsync(m.node_state, 0, b_nstate, s));
+    CU(cudaMemsetAsync(m.counts, 0, 64, s));
+    const uint32_t first_branch = n;
+    CU(cudaMemcpyAsync(m.counts + 4, &first_branch, 4, cudaMemcpyHostToDevice, s));
+    const unsigned bl = (n + 127) / 128;
+    k_mesh_vertices<<<bl, 128, 0, s>>>(ms);
+    k_tree_leaves<<<bl, 128, 0, s>>>(m);
+    // ancestors, one depth at a time: range[d] = ids of depth d
+    uint32_t range_lo[FC_MAX_OCTREE_DEPTH + 1], range_hi[FC_MAX_OCTREE_DEPTH + 1];
+    range_lo[depth] = 0;
+    range_hi[depth] = n;
+    for (int d = int(depth) - 1; d >= 0; --d) {
+        const uint32_t lo = range_lo[d + 1], hi = range_hi[d + 1];
+        k_tree_parents<<<(hi - lo + 127) / 128, 128, 0, s>>>(m, lo, hi);
+        uint32_t count = 0;
+        CU(cudaMemcpyAsync(&count, m.counts + 4, 4, cudaMemcpyDeviceToHost, s));
+        CU(cudaStreamSynchronize(s));
+        range_lo[d] = hi;
+        range_hi[d] = count;
+    }
+    const uint32_t n_nodes = range_hi[0];
+    m.n_nodes = n_nodes;
+    const size_t b_herm = std::max<size_t>(n_nodes - n, 1) * sizeof(Hermite), b_remap = size_t(n_nodes) * 16 * 4;
+    CU(c->mesh_herm.ensure(al(b_herm) + al(b_remap)));
+    m.herm = c->mesh_herm.as<Hermite>();
+    m.remap = reinterpret_cast<uint32_t*>(c->mesh_herm.as<char>() + al(b_herm));
+    CU(c->mesh_cells.ensure(size_t(n_nodes) * sizeof(fc_mesh_cell)));
+    m.out_cells = c->mesh_cells.as<fc_mesh_cell>();
+    CU(cudaMemsetAsync(m.remap, 0, b_remap, s));
+    k_tree_leaf_err<<<bl, 128, 0, s>>>(m);
+    for (int d = int(depth) - 1; d >= 0; --d)
+        k_tree_collapse<<<(range_hi[d] - range_lo[d] + 127) / 128, 128, 0, s>>>(m, range_lo[d], range_hi[d]);
+    k_tree_final<<<(n_nodes + 127) / 128, 128, 0, s>>>(m);
+    k_tree_faces<0><<<(n_nodes * 12u + 127) / 128, 128, 0, s>>>(m);
+    CU(cudaGetLastError());
+    uint32_t cnt[6];
+    CU(cudaMemcpyAsync(cnt, m.counts, sizeof cnt, cudaMemcpyDeviceToHost, s));
+    CU(cudaStreamSynchronize(s));
+    const uint32_t n_tris = cnt[1];
+    const uint64_t v_cap = std::min<uint64_t>(uint64_t(n_nodes) * 16, uint64_t(n_tris) * 5 + 16);
+    CU(c->mesh_verts.ensure(std::max<uint64_t>(v_cap, 1) * sizeof(float3)));
+    CU(c->mesh_tris.ensure(std::max<uint64_t>(n_tris, 1) * sizeof(uint3)));
+    m.out_verts = c->mesh_verts.as<float3>();
+    m.cap_verts = uint32_t(v_cap);
+    m.out_tris = c->mesh_tris.as<uint3>();
+    m.cap_tris = n_tris;
+    k_tree_assign<<<unsigned((uint64_t(n_nodes) * 16 + 255) / 256), 256, 0, s>>>(m);
+    k_tree_faces<1><<<(n_nodes * 12u + 127) / 128, 128, 0, s>>>(m);
+    CU(cudaEventRecord(e1, s));
+    CU(cudaGetLastError());
+    CU(cudaMemcpyAsync(cnt, m.counts, sizeof cnt, cudaMemcpyDeviceToHost, s));
+    CU(cudaStreamSynchronize(s));
+    if (cnt[0] > v_cap) return fail(FC_ERR_CUDA, "mesh vertex buffer overflow");
+    c->mesh_n_verts = cnt[0];
+    c->mesh_n_tris = n_tris;
+    c->mesh_n_cells = cnt[5];
+    info->n_vertices = cnt[0];
+    info->n_triangles = n_tris;
+    info->open_edges = cnt[3];
+    cudaEventElapsedTime(&info->mesh_ms, e0, e1);
+    return FC_OK;
+}
 
 extern "C" {
 
@@ -328,8 +896,9 @@ int32_t fc_mesh_build(fc_ctx* c, const fc_tape* tape, const fc_octree_cfg* cfg, 
     m.n_leaves = n;
     info->n_leaves = n;
     info->sampler_ms = ost.total_ms;
-    c->mesh_n_verts = c->mesh_n_tris = 0;
+    c->mesh_n_verts = c->mesh_n_tris = c->mesh_n_cells = 0;
     if (n == 0) return FC_OK;
+    if (cfg->flags & FC_FLAG_MESH_COLLAPSE) return mesh_build_collapse(c, n, cfg->depth, info);
     uint32_t hsize = 1024;
     while (hsize < 2u * n) hsize <<= 1;
     const size_t b_keys = size_t(hsize) * 8, b_vals = size_t(hsize) * 4, b_cv = size_t(n) * 4 * sizeof(float3), b_cn = size_t(n) * 4,
@@ -389,6 +958,19 @@ int32_t fc_mesh_read(fc_ctx* c, float* vertices, uint32_t* triangles) {
         CU(cudaMemcpyAsync(vertices, c->mesh_verts.p, size_t(c->mesh_n_verts) * 12, cudaMemcpyDefault, c->stream));
     if (triangles && c->mesh_n_tris)
         CU(cudaMemcpyAsync(triangles, c->mesh_tris.p, size_t(c->mesh_n_tris) * 12, cudaMemcpyDefault, c->stream));
+    CU(cudaStreamSynchronize(c->stream));
+    return FC_OK;
+}
+
+int32_t fc_mesh_read_cells(fc_ctx* c, fc_mesh_cell* out, uint64_t cap, uint64_t* n) {
+    if (!c) return fail(FC_ERR_INVALID, "null ctx");
+    std::lock_guard<std::mutex> guard(c->mu);
+    if (n) *n = c->mesh_n_cells;
+    if (!out) return FC_OK;
+    if (cap < c->mesh_n_cells) return fail(FC_ERR_INVALID, "buffer too small");
+    CU(cudaSetDevice(c->device));
+    if (c->mesh_n_cells)
+        CU(cudaMemcpyAsync(out, c->mesh_cells.p, size_t(c->mesh_n_cells) * sizeof(fc_mesh_cell), cudaMemcpyDefault, c->stream));
     CU(cudaStreamSynchronize(c->stream));
     return FC_OK;
 }

@@ -462,16 +462,18 @@ def octree_sample(shape: CudaShape, depth: int, world_to_model=None, capacity: i
     return (leaves, st.as_dict()) if stats else leaves
 
 
-def mesh(shape: CudaShape, depth: int, world_to_model=None, var_values=(), stl: bool = False):
-    """``Octree::build(...).walk_dual()`` without cell collapse (fidget-mesh): returns ``(vertices [n,3] float32,
-    triangles [m,3] uint32, info dict)`` -- plus the binary STL bytes (``Mesh::write_stl``) when ``stl``."""
+def mesh(shape: CudaShape, depth: int, world_to_model=None, var_values=(), stl: bool = False, collapse: bool = False):
+    """``Octree::build(...).walk_dual()`` (fidget-mesh): returns ``(vertices [n,3] float32, triangles [m,3] uint32,
+    info dict)`` -- plus the binary STL bytes (``Mesh::write_stl``) when ``stl``.  Without ``collapse`` the mesh is
+    the uniform-depth one (no cell collapse); with it, cells are collapsed as the reference's octree does and the
+    dual is walked over leaves of different depths (``mesh_cells`` then lists the final leaves)."""
     lib = shape._lib
     c = _lib.FcOctreeCfg()
     c.depth = depth
     if world_to_model is not None:
         c.has_transform = 1
         c.world_to_model[:] = np.ascontiguousarray(world_to_model, dtype=np.float32).reshape(16).tolist()
-    c.flags = _lib.FC_FLAG_TIMING
+    c.flags = _lib.FC_FLAG_TIMING | (_lib.FC_FLAG_MESH_COLLAPSE if collapse else 0)
     c.n_var_values = len(var_values)
     for i, v in enumerate(var_values):
         c.var_values[i] = float(v)
@@ -488,6 +490,21 @@ def mesh(shape: CudaShape, depth: int, world_to_model=None, var_values=(), stl: 
     buf = np.zeros(n.value, dtype=np.uint8)
     _ck(lib.fc_mesh_write_stl(shape.cuda._h, _ptr(buf), n.value, C.byref(n)))
     return verts, tris, d, buf.tobytes()
+
+
+MESH_CELL = np.dtype([("ix", np.uint16), ("iy", np.uint16), ("iz", np.uint16), ("depth", np.uint8), ("mask", np.uint8),
+                      ("vertex", np.float32, 3)])
+
+
+def mesh_cells(cuda) -> np.ndarray:
+    """Final leaves of the octree of the context's last ``mesh(..., collapse=True)``: depth, cell coordinates at
+    that depth, corner mask and first cell vertex, sorted by (depth, iz, iy, ix).  Empty after a uniform mesh."""
+    lib = cuda._lib
+    n = C.c_uint64()
+    _ck(lib.fc_mesh_read_cells(cuda._h, None, 0, C.byref(n)))
+    out = np.zeros(n.value, dtype=MESH_CELL)
+    _ck(lib.fc_mesh_read_cells(cuda._h, _ptr(out), n.value, C.byref(n)))
+    return out[np.lexsort((out["ix"], out["iy"], out["iz"], out["depth"]))]
 
 
 def pixel_inside(img: np.ndarray) -> np.ndarray:

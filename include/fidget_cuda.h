@@ -290,9 +290,13 @@ int32_t fc_octree_sample(fc_ctx* ctx, const fc_tape* tape, const fc_octree_cfg* 
 /* fc_mesh_build = fc_octree_sample + the rest of the Manifold Dual Contouring pipeline on the device, the mesh
  * staying in HBM until it is read: one vertex per connected group of inside corners of every surface leaf,
  * positioned by QuadraticErrorSolver::solve (fidget-mesh/src/qef.rs:67-168); four triangles around every
- * sign-changing cell edge as in dc_edge (fidget-mesh/src/dc.rs:104-213).  Cell collapse (octree.rs:252-440) is
- * not performed: the result is the uniform-depth mesh (same surface, more triangles in flat regions than the
- * reference's adaptive one).  Edges on the boundary of the [-1,1]^3 domain get no triangles (open_edges). */
+ * sign-changing cell edge as in dc_edge (fidget-mesh/src/dc.rs:104-213).  By default there is no cell collapse:
+ * the result is the uniform-depth mesh.  With FC_FLAG_MESH_COLLAPSE in fc_octree_cfg.flags the eight children of a
+ * cell are merged into one leaf as Octree::check_done / try_collapse do (octree.rs:252-440: manifold topology and a
+ * merged QEF error below twice the children's), and the dual is walked over leaves of different depths, as
+ * Octree::build(..).walk_dual() does: fewer triangles in flat regions.  Edges on the boundary of the [-1,1]^3 domain
+ * get no triangles (open_edges). */
+#define FC_FLAG_MESH_COLLAPSE 64u /* fc_mesh_build: cell collapse and the adaptive dual walk */
 typedef struct fc_mesh_info {
     uint64_t n_leaves, n_vertices, n_triangles, open_edges;
     float sampler_ms, mesh_ms;   /* device time of the sampler / of QEF + dual walk */
@@ -300,6 +304,16 @@ typedef struct fc_mesh_info {
 int32_t fc_mesh_build(fc_ctx* ctx, const fc_tape* tape, const fc_octree_cfg* cfg, fc_mesh_info* info);
 /* vertices: n_vertices * 3 floats, triangles: n_triangles * 3 vertex indices; host or device; either may be NULL */
 int32_t fc_mesh_read(fc_ctx* ctx, float* vertices, uint32_t* triangles);
+/* One final leaf of the octree of the last fc_mesh_build, when it ran with FC_FLAG_MESH_COLLAPSE */
+typedef struct fc_mesh_cell {
+    uint16_t ix, iy, iz;        /* cell coordinates at `depth` */
+    uint8_t depth;
+    uint8_t mask;               /* CellMask of the leaf */
+    float vertex[3];            /* the leaf's first cell vertex */
+} fc_mesh_cell;
+/* out: `cap` cells, host or device, in no particular order; *n receives the number of final leaves (0 after a build
+ * without FC_FLAG_MESH_COLLAPSE).  out == NULL queries the count. */
+int32_t fc_mesh_read_cells(fc_ctx* ctx, fc_mesh_cell* out, uint64_t cap, uint64_t* n);
 /* Mesh::write_stl (fidget-mesh/src/output.rs:7-38): binary STL of the last mesh, assembled on the device.
  * buf == NULL queries the size (84 + 50 * n_triangles). */
 int32_t fc_mesh_write_stl(fc_ctx* ctx, uint8_t* buf, size_t cap, size_t* n_bytes);

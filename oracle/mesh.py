@@ -79,6 +79,32 @@ def qef_vertex(points, grads):
 def build(leaves):
     """leaves: the structured array of ``oracle.octree_sample``.  Returns (cell_vertices dict (leaf, group) -> pos,
     triangles as a list of three positions each, open edge count)."""
+    verts, tri_slots, open_edges = _walk(leaves, qef_vertex)
+    tris = [tuple(_slot_pos(leaves, verts, k) for k in t) for t in tri_slots]
+    return verts, tris, open_edges
+
+
+def build_indexed(leaves, vertex=qef_vertex):
+    """build() indexed the way fc_mesh_build returns the mesh: one vertex per slot the triangles use (MeshBuilder's
+    dedup), ``(vertices [n,3] float32, triangles [m,3] int64, open edge count, slots)``, where a slot is
+    ('v', leaf, group) for a cell vertex or ('i', leaf, edge) for an intersection.  ``vertex(points, grads)``
+    places a cell vertex (qef_vertex by default); the triangles do not depend on it."""
+    verts, tri_slots, open_edges = _walk(leaves, vertex)
+    index = {}
+    for t in tri_slots:
+        for k in t:
+            index.setdefault(k, len(index))
+    pos = np.array([_slot_pos(leaves, verts, k) for k in index], dtype=np.float32).reshape(-1, 3)
+    tris = np.array([[index[k] for k in t] for t in tri_slots], dtype=np.int64).reshape(-1, 3)
+    return pos, tris, open_edges, list(index)
+
+
+def _slot_pos(leaves, verts, slot):
+    kind, i, j = slot
+    return verts[(i, j)] if kind == "v" else leaves[i]["pos"][j].astype(np.float32)
+
+
+def _walk(leaves, vertex):
     index = {(int(l["ix"]), int(l["iy"]), int(l["iz"])): i for i, l in enumerate(leaves)}
     groups = []
     verts = {}
@@ -97,7 +123,7 @@ def build(leaves):
                     e = edge_index(s, t)
                     pts.append(l["pos"][e].astype(np.float32))
                     grs.append(l["grad"][e].astype(np.float32))
-            verts[(i, g)] = qef_vertex(pts, grs)
+            verts[(i, g)] = vertex(pts, grs)
     tris = []
     open_edges = 0
     for ci, l in enumerate(leaves):
@@ -122,8 +148,8 @@ def build(leaves):
                 start = (u if e & 1 else 0) | (v if e & 2 else 0)
                 mk = int(leaves[ids[k]]["mask"])
                 inside = start if (mk >> start) & 1 else start | t
-                vs.append(verts[(ids[k], groups[ids[k]][inside])])
-            iv = leaves[ids[3]]["pos"][edges[3]].astype(np.float32)        # the deepest (= last) cell's intersection
+                vs.append(("v", ids[k], groups[ids[k]][inside]))
+            iv = ("i", ids[3], edges[3])                                            # the deepest (= last) cell's intersection
             start_d = (u if edges[3] & 1 else 0) | (v if edges[3] & 2 else 0)
             winding = 1 if (int(leaves[ids[3]]["mask"]) >> start_d) & 1 else 3
             for j in range(4):

@@ -10,8 +10,10 @@ output (``oracle.octree_sample``: the surface leaves at the maximum depth with t
 
 A cell the sampler left no surface leaf in is Empty or Full as a whole; the reference learns which from an interval
 evaluation, here it is the sample at the parent's centre, which every child of that parent shares (``sign_at``
-decides it for a tree without any surface leaf).  numpy's SVD stands in for nalgebra's, in float64, as in
-oracle/mesh.py; everything else is float32 like the reference.
+decides it for a tree without any surface leaf).  Everything is float32 like the reference; the eigen-solve inside
+QuadraticErrorSolver::solve is the device's float32 Jacobi (``jacobi3``), operation for operation, where the reference
+calls nalgebra's SVD.  So agreement with the device proves only that the two agree: tests/qef_f64.py solves the same
+QEFs in float64, and tests/test_qef_f64.py holds this solve against it (``Octree.qefs`` keeps every QEF solved).
 """
 from __future__ import annotations
 
@@ -66,7 +68,12 @@ class Qef:
         self.btb = f32(self.btb + f32(d * d))
 
     def solve(self):
-        """QuadraticErrorSolver::solve: (vertex, error clamped to >= 1e-6).  The truncated pseudo-inverse is the
+        """QuadraticErrorSolver::solve: (vertex, error clamped to >= 1e-6)."""
+        pos, err, _ = self.solve_rank()
+        return pos, err
+
+    def solve_rank(self):
+        """solve's (vertex, clamped error, rank of the truncated pseudo-inverse).  The truncated pseudo-inverse is the
         float32 Jacobi eigen-solve of the device, operation for operation (see jacobi3): the error term cancels
         down to the size of its rounding where the surface is flat, so a collapse decision near the 2x threshold
         depends on the last bit of the vertex."""
@@ -99,7 +106,7 @@ class Qef:
             quad = f32(f32(row[0] * p[0] + row[1] * p[1]) + row[2] * p[2])
             lin = f32(f32(f32(2 * p[0]) * self.atb[0] + f32(2 * p[1]) * self.atb[1]) + f32(2 * p[2]) * self.atb[2])
             err = f32(f32(quad - lin) + self.btb)
-        return pos, (err if err > f32(1e-6) else f32(1e-6))
+        return pos, (err if err > f32(1e-6) else f32(1e-6)), rank
 
 
 def jacobi3(a):
@@ -198,13 +205,16 @@ class Hermite:
                 out.err = min(out.err, h.err)
         return out
 
-    def solve(self):
+    def qef(self):                         # the QEF LeafHermiteData::solve solves
         q = self.center.copy()
         for e in range(12):
             q += self.qef_of(e)
         for f in self.face:
             q += f
-        return q.solve()
+        return q
+
+    def solve(self):
+        return self.qef().solve()
 
 
 def groups_of(mask):
@@ -217,10 +227,17 @@ def groups_of(mask):
 class Octree:
     """Octree::build over the sampler leaves.  ``cells`` maps (depth, x, y, z) to a dict with ``kind`` in
     'E' / 'F' / 'L' / 'B' (plus ``mask``, ``groups`` and the vertices ``verts`` {slot: pos} of a leaf: slots 0-3
-    are cell vertices, 4 + e the intersection on undirected edge e)."""
+    are cell vertices, 4 + e the intersection on undirected edge e).
+
+    ``qefs`` keeps the QEFs that were solved, by cell key: a surface leaf's list with one per vertex group (None for a
+    group forced to an intersection by a NaN gradient), and the merged QEF of every cell whose children were merged
+    (it became a Leaf or stayed a Branch); ``child_err`` holds the children's error that merged QEF was held
+    against.  They are records only: nothing reads them here."""
 
     def __init__(self, leaves, depth, sign_at=None):
         self.depth = depth
+        self.qefs = {}
+        self.child_err = {}
         self.leaves = {(depth, int(l["ix"]), int(l["iy"]), int(l["iz"])): l for l in leaves}
         self.anc = set()
         for (d, x, y, z) in self.leaves:
@@ -268,6 +285,7 @@ class Octree:
         g_of, n = groups_of(mask)
         h = Hermite()
         verts = {}
+        self.qefs[key] = [None] * n
         for e in range(12):
             if (int(l["present"]) >> e) & 1:
                 h.inter[e] = (l["pos"][e].astype(f32), l["grad"][e].astype(f32))
@@ -290,6 +308,7 @@ class Octree:
             if invalid:
                 h.err = QEF_ERR_INVALID
                 continue
+            self.qefs[key][g] = q
             verts[g], h.err = q.solve()                 # last writer wins (octree.rs:846-849)
         self.cells[key] = {"kind": "L", "mask": mask, "groups": g_of, "n_groups": n, "verts": verts}
         return h
@@ -308,7 +327,9 @@ class Octree:
         mask = self.collapsible(kids)
         merged = Hermite.merge(herm) if mask is not None else None
         if merged is not None:
-            pos, err = merged.solve()
+            q = merged.qef()
+            self.qefs[key], self.child_err[key] = q, merged.err
+            pos, err = q.solve()
             if not (err >= merged.err * 2) and self.contains(key, pos):
                 merged.err = err
                 verts = {0: pos}
@@ -438,12 +459,16 @@ class Octree:
         return n
 
     def _cover(self, d, p):
+        """The final leaf covering cell (d, p): (depth, key); "branch" when smaller leaves own it (a Branch at depth
+        d, reachable from the root or not); "empty" for an Empty / Full cell."""
         for k in range(d + 1):
             key = (d - k, int(p[0]) >> k, int(p[1]) >> k, int(p[2]) >> k)
             cell = self.cells.get(key)
-            if cell is None or not self._is_final(key):
-                if cell is not None and cell["kind"] == "B":
-                    return "branch" if k == 0 else "empty"
+            if cell is None:
+                continue
+            if cell["kind"] == "B":
+                return "branch" if k == 0 else "empty"
+            if not self._is_final(key):
                 continue
             return (d - k, key) if cell["kind"] == "L" else "empty"
         return "empty"

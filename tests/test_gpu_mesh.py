@@ -6,6 +6,7 @@ import pytest
 from scipy.spatial import cKDTree
 
 import fidget_b200 as fb
+import mesh_compare
 from conftest import model_text
 from oracle import mesh as om
 
@@ -69,6 +70,16 @@ def test_mesh_matches_numpy_oracle(orc, cuda, shape_fn, depth):
     a, b, c = body[:, 1], body[:, 2], body[:, 3]
     assert np.allclose(body[:, 0], np.cross(b - a, c - a), atol=1e-6)
     assert not rec[:, 48:].any()
+    # exactly the oracle's walk with the device's float32 solve, and every cell vertex within the float64 bound
+    print(mesh_compare.compare_uniform(g, leaves, depth))
+
+
+@pytest.mark.parametrize("name,depth", [("colonnade.vm", 6), ("bear.vm", 6), ("gyroid-sphere.vm", 6), ("colonnade.vm", 7)])
+def test_model_mesh_matches_oracle(cuda, name, depth):
+    """On the device sampler's leaves: vertices, triangles and open_edges exactly as oracle/mesh.py's walk with the
+    device's float32 vertex solve, and every cell vertex within the float64 bound of its QEF's solution."""
+    g = fb.CudaShape.from_vm(cuda, model_text(name))
+    print(f"{name} depth {depth}: {mesh_compare.compare_uniform(g, fb.octree_sample(g, depth), depth)}")
 
 
 def test_cube_mesh_has_sharp_corners(cuda):

@@ -4,7 +4,9 @@ import numpy as np
 import pytest
 
 import mesh_collapse_oracle as mco
+import mesh_shapes
 from conftest import model_text
+from oracle import mesh as om
 
 f32 = np.float32
 
@@ -189,3 +191,30 @@ def test_qef_near_planar(orc):
     v, _, _ = _build(orc, lambda c: sphere(c, (0, 0, 0), 0.75), 4).walk_dual()
     n = np.linalg.norm(v, axis=1)
     assert len(n) and (n > 0.7).all() and (n < 0.8).all()
+
+
+def test_fuzz_reaches_the_edge_cases(orc):
+    """The GPU mesh fuzz corpus (tests/test_gpu_mesh_fuzz.py) reaches what it is drawn for: leaves with several
+    vertex groups, NaN gradients (forced vertices), sign changes on the domain boundary, and shapes without a surface."""
+    multi = nan = boundary = empty = 0
+    for seed in mesh_shapes.FUZZ_SEEDS:
+        depth = mesh_shapes.fuzz_depth(seed)
+        _, o, _ = mesh_shapes.tape_pair(orc, None, seed, depth)
+        leaves, _ = orc.octree_sample(o, depth)
+        empty += len(leaves) == 0
+        for l in leaves:
+            multi += om.corner_groups(int(l["mask"]))[1] > 1
+            present = [e for e in range(12) if (int(l["present"]) >> e) & 1]
+            nan += bool(np.isnan(l["grad"][present]).any())
+            boundary += bool({int(l["ix"]), int(l["iy"]), int(l["iz"])} & {0, 2 ** depth - 1})
+    assert multi >= 100 and nan >= 8 and boundary >= 100 and empty >= 3, (multi, nan, boundary, empty)
+
+
+@pytest.mark.parametrize("seed,open_edges", [(5, 25), (43, 13)])
+def test_open_edges_skip_segments_smaller_leaves_own(orc, seed, open_edges):
+    """Regression: a sign-changing boundary edge of a coarse final leaf whose neighbour at its depth is a Branch
+    reachable from the root belongs to the smaller leaves there, not to the coarse leaf.  The oracle used to take such
+    a Branch for an Empty cell and counted the edge; the counts here are fc_mesh_build's on an H100."""
+    depth = mesh_shapes.fuzz_depth(seed)
+    _, tape, _ = mesh_shapes.tape_pair(orc, None, seed, depth)
+    assert mco.build(orc, tape, depth).open_edges() == open_edges

@@ -103,6 +103,7 @@ FC_FLAG_EXACT_CENSUS = 16
 FC_FLAG_FULL_LADDER = 32
 FC_FLAG_MESH_COLLAPSE = 64
 FC_OUT_F32, FC_OUT_MASK_U8, FC_OUT_BITMAP_1BIT, FC_OUT_RGBA8 = 0, 1, 2, 3
+FC_ERR_CANCELLED = -6
 
 # name -> (restype, argtypes); mirrors include/fidget_cuda.h one to one
 _vp, _u32, _i32, _u64, _u8 = C.c_void_p, C.c_uint32, C.c_int32, C.c_uint64, C.c_uint8
@@ -115,6 +116,7 @@ CUDA_API = {
     "fc_ctx_set_stream": (_i32, [_vp, _vp, _i32]),
     "fc_ctx_synchronize": (_i32, [_vp]),
     "fc_ctx_set_arena_bytes": (_i32, [_vp, _u64]),
+    "fc_ctx_set_cancel": (_i32, [_vp, _vp]),
     "fc_tape_create": (_i32, [_vp, _P(_u32), C.c_size_t, _u8, _u32, _u32, _u32, _u32, _P(_vp)]),
     "fc_tape_retain": (_i32, [_vp]),
     "fc_tape_release": (_i32, [_vp]),

@@ -1,6 +1,8 @@
 // C ABI of libfidget_cuda (include/fidget_cuda.h): contexts, tapes, the trait-level evaluators and
 // fc_simplify.  The renderers live in render.cu, the octree sampler in octree_capi.cu, the effects in
 // effects_capi.cu, the level-0 schedule in schedule.cu.
+#include <thread>
+
 #include "capi_internal.h"
 
 thread_local std::string g_err;
@@ -144,6 +146,10 @@ void fc_ctx_destroy(fc_ctx* c) {
     for (auto ev : c->events) cudaEventDestroy(ev);
     for (auto e : c->ev_fork) if (e) cudaEventDestroy(e);
     if (c->ev_join) cudaEventDestroy(c->ev_join);
+    if (c->cancel_word) cudaFree(c->cancel_word);
+    if (c->cancel_pin) cudaFreeHost(c->cancel_pin);
+    if (c->cancel_ev) cudaEventDestroy(c->cancel_ev);
+    if (c->cancel_stream) cudaStreamDestroy(c->cancel_stream);
     cudaStreamDestroy(c->aux_stream);
     cudaStreamDestroy(c->own_stream);
     delete c;
@@ -160,7 +166,103 @@ int32_t fc_ctx_set_stream(fc_ctx* c, void* s, int32_t use_own) {
     return FC_OK;
 }
 
+int32_t fc_ctx_set_cancel(fc_ctx* c, const uint8_t* flag) {
+    if (!c) return fail(FC_ERR_INVALID, "null ctx");
+    if (flag && !c->cancel_word) {
+        std::lock_guard<std::mutex> guard(c->mu);
+        CU(cudaSetDevice(c->device));
+        CU(cudaStreamCreateWithFlags(&c->cancel_stream, cudaStreamNonBlocking));
+        CU(cudaEventCreateWithFlags(&c->cancel_ev, cudaEventDisableTiming));
+        CU(cudaHostAlloc(reinterpret_cast<void**>(&c->cancel_pin), 4, cudaHostAllocDefault));
+        uint32_t* w = nullptr;
+        CU(cudaMalloc(&w, 4));
+        CU(cudaMemsetAsync(w, 0, 4, c->cancel_stream));   // 0 is no call's id
+        CU(cudaStreamSynchronize(c->cancel_stream));
+        c->cancel_word = w;
+    }
+    c->cancel_flag.store(flag);
+    return FC_OK;
+}
+
 }  // extern "C"
+
+// FIDGET_B200_CANCEL_AT=<site>:<n> names the poll sites of kernels.cuh (CancelSite)
+static int32_t cancel_site_of(const std::string& name) {
+    static const char* const names[] = {
+        "k_interval_root_coop", "k_fill_2d", "k_pixels_2d", "k_tail_2d", "k_voxels_3d", "k_normals_3d", "k_census_3d",
+        "k_octree_leaf", "k_octree_grads", "k_mesh_hash", "k_mesh_vertices", "k_mesh_faces0", "k_mesh_faces1",
+        "k_mesh_assign", "k_tree_leaves", "k_tree_parents", "k_tree_leaf_err", "k_tree_collapse", "k_tree_final",
+        "k_tree_faces0", "k_tree_faces1", "k_tree_assign"};
+    static_assert(sizeof(names) / sizeof(names[0]) == CS_WAIT - CS_ROOT_COOP, "one name per poll site");
+    for (int i = 0; i < MAX_LEVELS; ++i)
+        if (name == "k_interval_level" + std::to_string(i)) return CS_LEVEL0 + i;
+    for (int i = 0; i < CS_WAIT - CS_ROOT_COOP; ++i)
+        if (name == names[i]) return CS_ROOT_COOP + i;
+    return -1;
+}
+
+int32_t begin_call(fc_ctx* c, CallCancel& cc) {
+    cc = CallCancel{};
+    const uint8_t* flag = c->cancel_flag.load();
+    if (!flag) return FC_OK;
+    if (__atomic_load_n(flag, __ATOMIC_ACQUIRE)) return fail(FC_ERR_CANCELLED, "cancelled before the call started");
+    cc.flag = flag;
+    cc.ref.word = c->cancel_word;
+    {
+        std::lock_guard<std::mutex> guard(c->mu);
+        if (++c->call_id == 0) c->call_id = 1;
+        cc.ref.id = c->call_id;
+    }
+    // diagnostic: the poll at <site> that claims item <n> cancels this call, as the host would
+    const std::string at = env_str("FIDGET_B200_CANCEL_AT");
+    if (!at.empty()) {
+        const size_t colon = at.rfind(':');
+        const int32_t site = colon == std::string::npos ? -1 : cancel_site_of(at.substr(0, colon));
+        if (site < 0) return fail(FC_ERR_INVALID, "FIDGET_B200_CANCEL_AT: expected <kernel site>:<item>, got " + at);
+        cc.ref.site = site;
+        cc.ref.item = uint32_t(strtoul(at.c_str() + colon + 1, nullptr, 10));
+    }
+    return FC_OK;
+}
+
+int32_t wait_call(fc_ctx* c, cudaStream_t s, const CallCancel& cc) {
+    if (!cc.flag) {
+        CU(cudaStreamSynchronize(s));
+        return FC_OK;
+    }
+    CU(cudaEventRecord(c->cancel_ev, s));
+    bool written = false;
+    for (;;) {
+        const cudaError_t q = cudaEventQuery(c->cancel_ev);
+        if (q == cudaSuccess) break;
+        if (q != cudaErrorNotReady) return fail(FC_ERR_CUDA, std::string("cudaEventQuery: ") + cudaGetErrorString(q));
+        if (!written && __atomic_load_n(cc.flag, __ATOMIC_ACQUIRE)) {
+            // the kernels of this call read the word from L2 at their next claim; the copy engine runs beside them
+            *c->cancel_pin = cc.ref.id;
+            CU(cudaMemcpyAsync(c->cancel_word, c->cancel_pin, 4, cudaMemcpyHostToDevice, c->cancel_stream));
+            written = true;
+        }
+        std::this_thread::yield();
+    }
+    CU(cudaStreamSynchronize(s));
+    bool cancelled = written;
+    if (written) CU(cudaStreamSynchronize(c->cancel_stream));   // (the pinned word is reused by the next call)
+    else if (cc.ref.site >= 0) {                                 // FIDGET_B200_CANCEL_AT: did a poll cancel the call?
+        CU(cudaMemcpyAsync(c->cancel_pin, c->cancel_word, 4, cudaMemcpyDeviceToHost, c->cancel_stream));
+        CU(cudaStreamSynchronize(c->cancel_stream));
+        cancelled = *c->cancel_pin == cc.ref.id;
+    }
+    return cancelled ? fail(FC_ERR_CANCELLED, "cancelled") : FC_OK;
+}
+
+int32_t wait_read(fc_ctx* c, cudaStream_t s, const CallCancel& cc, void* dst, const void* src, size_t bytes) {
+    if (cc.flag)
+        if (int32_t rc = wait_call(c, s, cc)) return rc;
+    CU(cudaMemcpyAsync(dst, src, bytes, cudaMemcpyDeviceToHost, s));
+    CU(cudaStreamSynchronize(s));
+    return FC_OK;
+}
+
 int32_t check_device_errors(fc_ctx* c) {
     if (!c->counters.p) return FC_OK;
     Counters h;
@@ -175,7 +277,12 @@ extern "C" {
 int32_t fc_ctx_synchronize(fc_ctx* c) {
     if (!c) return fail(FC_ERR_INVALID, "null ctx");
     CU(cudaSetDevice(c->device));
-    CU(cudaStreamSynchronize(c->stream));
+    // a flag attached now applies to the last FC_FLAG_ASYNC render / sampler / mesh call still in flight
+    CallCancel cc = c->async_call;
+    c->async_call = CallCancel{};
+    cc.flag = cc.ref.word ? c->cancel_flag.load() : nullptr;
+    if (!cc.flag) cc = CallCancel{};
+    if (int32_t rc = wait_call(c, c->stream, cc)) return rc;
     return check_device_errors(c);
 }
 

@@ -96,6 +96,25 @@ inline int env_int(const char* name, int dflt) {
     }
     return read(dflt);
 }
+// String knobs, read like env_int: once per process, or on every call with FIDGET_B200_ENV_LIVE=1
+inline std::string env_str(const char* name) {
+    static std::mutex mu;
+    static std::vector<std::pair<const char*, std::string>> cache;
+    static const bool live = [] { const char* v = getenv("FIDGET_B200_ENV_LIVE"); return v && *v && atoi(v) != 0; }();
+    auto read = [&] { const char* v = getenv(name); return std::string(v ? v : ""); };
+    if (live) return read();
+    std::lock_guard<std::mutex> g(mu);
+    for (auto& kv : cache) if (kv.first == name) return kv.second;
+    cache.emplace_back(name, read());
+    return cache.back().second;
+}
+
+// Cancellation of one call (fc_ctx_set_cancel): the flag attached when the call began and the device side's view
+// (ref.word == null when no flag is attached)
+struct CallCancel {
+    const uint8_t* flag = nullptr;
+    CancelRef ref{nullptr, 0, -1, 0};
+};
 
 struct fc_ctx {
     int device = 0;
@@ -129,6 +148,15 @@ struct fc_ctx {
     struct { size_t smem; int per_sm, threads; } coop_memo[2] = {};   // level-0 launch shape per DIM (occupancy query cached)
     std::shared_ptr<struct Sched> sched_cache[4];
     unsigned sched_next = 0;
+    // cancellation (fc_ctx_set_cancel): the caller's flag; the device word kernels poll, written from pinned memory on
+    // a non-blocking side stream while the work stream runs; ids of the calls, so that a late write cancels nothing newer
+    std::atomic<const uint8_t*> cancel_flag{nullptr};
+    uint32_t* cancel_word = nullptr;
+    uint32_t* cancel_pin = nullptr;
+    cudaStream_t cancel_stream = nullptr;
+    cudaEvent_t cancel_ev = nullptr;
+    uint32_t call_id = 0;
+    CallCancel async_call;                    // the last FC_FLAG_ASYNC call that returned before its work was done
 };
 
 struct fc_tape {
@@ -172,6 +200,14 @@ void upload_schedule(fc_tape* t);
 int coop_blocks(fc_ctx* c, const fc_tape* tape, uint64_t n_roots, LevelParams& p, int dim, int& threads);
 // capi.cu
 int32_t check_device_errors(fc_ctx* c);
+// Start of a cancellable call: FC_ERR_CANCELLED if the attached flag is already set, else `cc` for its kernels
+int32_t begin_call(fc_ctx* c, CallCancel& cc);
+// cudaStreamSynchronize(s) of a cancellable call.  With a flag attached it polls the work and the flag, writes the
+// cancel word once it sees the flag, drains the stream and returns FC_ERR_CANCELLED if the call was cancelled.
+int32_t wait_call(fc_ctx* c, cudaStream_t s, const CallCancel& cc);
+// The readback of device counters that ends a wait: a copy to pageable memory would block the host until the stream
+// drains, so with a flag attached the (cancellable) wait comes first
+int32_t wait_read(fc_ctx* c, cudaStream_t s, const CallCancel& cc, void* dst, const void* src, size_t bytes);
 int32_t transcode(const uint32_t* words, size_t n_words, uint8_t reg_count, uint32_t mem_count, uint32_t n_vars,
                   uint32_t n_outputs, std::vector<uint2>& out, uint32_t& n_choices);
 // render.cu

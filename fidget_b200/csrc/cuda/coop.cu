@@ -66,6 +66,7 @@ k_interval_root_coop(const __grid_constant__ LevelParams p) {
     for (;;) {
         if (tid == 0) {
             s_tile = atomicAdd(&p.ctr->cursor[0], 1u);
+            if (s_tile < n_roots && cancel_poll(p.cancel, CS_ROOT_COOP, s_tile)) s_tile = ~0u;   // cancelled: claim nothing more
             s_nonboth = 0;
             s_ref = 0;
             s_nch = 0;

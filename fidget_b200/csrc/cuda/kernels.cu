@@ -46,7 +46,10 @@ k_interval_level(const __grid_constant__ LevelParams p) {
 
     for (;;) {
         uint32_t j = 0;
-        if (lane == 0) j = atomicAdd(&p.ctr->cursor[p.level], 1u);
+        if (lane == 0) {
+            j = atomicAdd(&p.ctr->cursor[p.level], 1u);
+            if (j < n_jobs && cancel_poll(p.cancel, CS_LEVEL0 + p.level, j)) j = ~0u;   // cancelled: claim nothing more
+        }
         j = __shfl_sync(FULL, j, 0);
         if (j >= n_jobs) break;
 
@@ -77,7 +80,10 @@ __global__ void __launch_bounds__(128) k_voxels_3d(const __grid_constant__ Voxel
     unsigned long long shaded = 0;
     for (;;) {
         uint32_t j = 0;
-        if (lane == 0) j = atomicAdd(&p.ctr->cursor[p.cursor], 1u);
+        if (lane == 0) {
+            j = atomicAdd(&p.ctr->cursor[p.cursor], 1u);
+            if (j < n_jobs && cancel_poll(p.cancel, CS_VOXELS_3D, j)) j = ~0u;
+        }
         j = __shfl_sync(FULL, j, 0);
         if (j >= n_jobs) break;
         if (p.order) j = p.order[j];   // front-to-back: tiles behind a finished column find it done and exit early
@@ -189,6 +195,7 @@ __global__ void __launch_bounds__(256) k_census_3d(const __grid_constant__ Censu
     const int lane = threadIdx.x & 31;
     const uint32_t warp = (blockIdx.x * blockDim.x + threadIdx.x) >> 5, n_warps = (gridDim.x * blockDim.x) >> 5;
     for (uint32_t i = warp; i < n; i += n_warps) {
+        if (cancel_poll(p.cancel, CS_CENSUS_3D, i)) break;   // (uniform over the warp)
         const CensusRec r = p.recs[i];
         const uint32_t T = p.tile[r.level], top = uint32_t(r.z) + T;
         uint32_t open_cols = 0;
@@ -222,6 +229,7 @@ __global__ void __launch_bounds__(128) k_normals_3d(const __grid_constant__ Norm
     const int lane = threadIdx.x & 31;
     // 8x4 pixel patch per warp
     const uint32_t warp = (blockIdx.x * blockDim.x + threadIdx.x) >> 5;
+    if (cancel_poll(p.cancel, CS_NORMALS_3D, warp)) return;   // one patch per warp: the claim is the launch itself
     uint32_t x, y;
     if (p.root_list) {   // patches of the listed root tiles only
         const uint32_t ppt = (p.root_tile / 8u) * (p.root_tile / 4u), ppr = p.root_tile / 8u;
@@ -337,7 +345,10 @@ __global__ void __launch_bounds__(128) k_pixels_2d(const __grid_constant__ Pixel
     unsigned long long shaded = 0;
     for (;;) {
         uint32_t j = 0;
-        if (lane == 0) j = atomicAdd(&p.ctr->cursor[p.cursor], 1u);
+        if (lane == 0) {
+            j = atomicAdd(&p.ctr->cursor[p.cursor], 1u);
+            if (j < n_jobs && cancel_poll(p.cancel, CS_PIXELS_2D, j)) j = ~0u;
+        }
         j = __shfl_sync(FULL, j, 0);
         if (j >= n_jobs) break;
         const TileJob* job = p.jobs + j;
@@ -389,6 +400,7 @@ __global__ void __launch_bounds__(256) k_fill_2d(const __grid_constant__ FillPar
     const bool vec_ok = (p.width % 4u == 0u) && ((reinterpret_cast<uintptr_t>(p.out) & 15u) == 0u) && (T % 4u == 0u);
     const unsigned long long total = (unsigned long long)n * units;
     for (unsigned long long w = warp; w < total; w += n_warps) {
+        if (cancel_poll(p.cancel, CS_FILL_2D, uint32_t(w))) break;
         const uint32_t rec = uint32_t(w / units), u = uint32_t(w % units);
         const FillRec fr = p.fills[rec];
         const float v = __uint_as_float(fr.value);

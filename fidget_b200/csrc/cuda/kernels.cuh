@@ -11,6 +11,39 @@ constexpr int MAX_LEVELS = 16;             // 3D renders use <= 8; the octree sa
 constexpr int WARPS_PER_BLOCK = 4;          // interval kernels
 constexpr int REG_SLOTS = 256;              // register slots of the fast interpreters
 
+// Cancellation (fc_ctx_set_cancel).  The context owns one device word; the host writes the id of a cancelled call into
+// it from a side stream while the call's kernels run.  Kernels poll it where a warp or CTA is about to claim new work
+// (cancel_poll) and stop claiming once it equals their own call's id; a claimed job always runs to its end, so every
+// record a producer has reserved is written.  word == null: no flag attached, the poll is one uniform predicate.
+// Poll sites, for the FIDGET_B200_CANCEL_AT diagnostic (the poll at `site` that claims item `item` cancels the call
+// itself, as the host would); the host maps their names (cancel_site_of, capi.cu) to these ids.
+enum CancelSite : int32_t {
+    CS_LEVEL0 = 0,                                        // k_interval_level, level l = CS_LEVEL0 + l (< MAX_LEVELS)
+    CS_ROOT_COOP = 16, CS_FILL_2D, CS_PIXELS_2D, CS_TAIL_2D, CS_VOXELS_3D, CS_NORMALS_3D, CS_CENSUS_3D,
+    CS_OCTREE_LEAF, CS_OCTREE_GRADS,
+    CS_MESH_HASH, CS_MESH_VERTICES, CS_MESH_FACES0, CS_MESH_FACES1, CS_MESH_ASSIGN,
+    CS_TREE_LEAVES, CS_TREE_PARENTS, CS_TREE_LEAF_ERR, CS_TREE_COLLAPSE, CS_TREE_FINAL, CS_TREE_FACES0, CS_TREE_FACES1,
+    CS_TREE_ASSIGN,
+    CS_WAIT,                                              // polls inside spin waits: not a claim, never a trigger site
+    CS_COUNT
+};
+struct CancelRef {
+    uint32_t* word;       // the context's cancel word, or null
+    uint32_t id;          // this call's id (never 0)
+    int32_t site;         // FIDGET_B200_CANCEL_AT: poll site that cancels (-1: none) ...
+    uint32_t item;        // ... when it claims this item
+};
+#ifdef __CUDACC__
+// true when the call is cancelled; `item` is the job / record / block being claimed (0xffffffff: not a claim)
+__device__ __forceinline__ bool cancel_poll(const CancelRef& c, int32_t site, uint32_t item) {
+    if (!c.word) return false;
+    if (site == c.site && item == c.item) { atomicExch(c.word, c.id); return true; }
+    uint32_t v;
+    asm volatile("ld.relaxed.gpu.global.u32 %0, [%1];" : "=r"(v) : "l"(c.word) : "memory");
+    return v == c.id;
+}
+#endif
+
 // A tape living in the device arena (units of uint2 clauses)
 struct TapeRef {
     const uint2* ptr;     // first clause (device memory: a root tape buffer or the arena)
@@ -158,6 +191,7 @@ struct LevelParams {
     CensusRec* census;              // exact 3D census records (or null)
     uint32_t cap_census;
     VarBind vb;
+    CancelRef cancel;
 };
 
 #ifdef __CUDACC__
@@ -189,6 +223,7 @@ struct PixelParams {
     int cursor;
     Stats* stats;
     VarBind vb;
+    CancelRef cancel;
 };
 
 struct FillParams {
@@ -196,6 +231,7 @@ struct FillParams {
     const FillRec* fills;
     const uint32_t* n_fills;
     float* out;
+    CancelRef cancel;
 };
 
 struct VoxelParams {
@@ -209,6 +245,7 @@ struct VoxelParams {
     int list, cursor;
     Stats* stats;
     VarBind vb;
+    CancelRef cancel;
 };
 struct NormalParams {
     uint32_t width, height, depth;
@@ -223,6 +260,7 @@ struct NormalParams {
     void* out;                  // GeometryPixel[width*height]
     Stats* stats;
     VarBind vb;
+    CancelRef cancel;
 };
 
 // One leaf of the Manifold-Dual-Contouring octree (LeafHermiteData, fidget-mesh/src/octree.rs:864-900)
@@ -247,6 +285,7 @@ struct OctreeLeafParams {
     uint32_t cap_out;
     uint32_t* n_out;            // device counter
     unsigned long long* stats;  // [0] leaf_empty [1] leaf_full [2] leaf_surface [3] float points [4] grad points
+    CancelRef cancel;
 };
 
 // launchers (kernels.cu)
@@ -267,6 +306,7 @@ struct CensusParams {
     const unsigned long long* heightmap;
     uint32_t width;
     Stats* stats;
+    CancelRef cancel;
 };
 void launch_census_3d(const CensusParams& p, int blocks, cudaStream_t s);
 void launch_merge_slabs(const void* const* d_slabs, uint32_t n_slabs, uint32_t n_pixels, uint32_t depth, void* out,
@@ -295,6 +335,7 @@ struct Tail2DParams {
     uint32_t fill_cap[TAIL_MAX_LEVELS + 1];
     uint32_t epoch;
     uint32_t paint_fills;              // 1: idle warps paint the fill records; 0: k_fill_2d launches do (after / beside this kernel)
+    CancelRef cancel;
 };
 cudaError_t launch_tail_2d(const Tail2DParams& p, int sm_count, cudaStream_t s);
 int tail_2d_blocks(int sm_count);

@@ -13,9 +13,13 @@ __device__ __forceinline__ uint32_t ld_volatile_u32(const uint32_t* p) { return 
 
 // Waits until job slot `j` carries this render's ready mark, then reads it from L2 (another SM wrote it
 // during this launch; L1 may hold a stale copy of the line).  Bounded: a lost job raises error bit 2.
-__device__ __forceinline__ TileJob load_job_ready(const TileJob* j, uint32_t epoch, Counters* ctr) {
+// A cancelled call leaves the wait with ok = false (and no error bit); the job is then skipped.
+__device__ __forceinline__ TileJob load_job_ready(const TileJob* j, uint32_t epoch, Counters* ctr, const CancelRef& cancel,
+                                                  bool& ok) {
     uint32_t spins = 0;
+    ok = true;
     while (ld_volatile_u32(&j->pad) != epoch) {
+        if (cancel_poll(cancel, CS_WAIT, ~0u)) { ok = false; return TileJob{}; }
         __nanosleep(64);
         if (++spins > (1u << 22)) { atomicOr(&ctr->error, 4u); break; }
     }
@@ -49,7 +53,9 @@ __device__ __forceinline__ void level_job(const LevelParams& p, uint32_t j, uint
         tr = p.root_tape;
         nchild = min(32u, n_roots - j * 32u);
     } else {
-        const TileJob jb = FUSED ? load_job_ready(p.jobs_in + j, epoch, p.ctr) : p.jobs_in[j];
+        bool ok = true;
+        const TileJob jb = FUSED ? load_job_ready(p.jobs_in + j, epoch, p.ctr, p.cancel, ok) : p.jobs_in[j];
+        if (FUSED && __any_sync(FULL, !ok)) return;   // cancelled while waiting for the record
         px = jb.x;
         py = jb.y;
         pz = jb.z;

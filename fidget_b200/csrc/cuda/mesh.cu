@@ -40,6 +40,7 @@ struct MeshScratch {
     uint32_t cap_verts;
     uint3* out_tris;
     uint32_t cap_tris;
+    CancelRef cancel;            // polled at block entry of every kernel (item = block index)
 };
 
 __device__ __forceinline__ unsigned long long cell_key(uint32_t x, uint32_t y, uint32_t z) {
@@ -50,6 +51,7 @@ __device__ __forceinline__ uint32_t hash_key(unsigned long long k) {
     return uint32_t(k);
 }
 __global__ void k_mesh_hash(MeshScratch m) {
+    if (cancel_poll(m.cancel, CS_MESH_HASH, blockIdx.x)) return;
     const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= m.n_leaves) return;
     const OctreeLeaf& L = m.leaves[i];
@@ -106,6 +108,7 @@ __device__ inline void jacobi3(float a[3][3], float w[3], float v[3][3]) {
 
 // One thread per leaf: groups of inside corners, one QEF vertex per group
 __global__ void __launch_bounds__(128) k_mesh_vertices(MeshScratch m) {
+    if (cancel_poll(m.cancel, CS_MESH_VERTICES, blockIdx.x)) return;
     const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= m.n_leaves) return;
     const OctreeLeaf& L = m.leaves[i];
@@ -219,6 +222,7 @@ __device__ __forceinline__ bool edge_cells(const MeshScratch& m, uint32_t ci, ui
 // pass 0: mark the vertex slots in use and count triangles; pass 1: emit
 template <int PASS>
 __global__ void __launch_bounds__(128) k_mesh_faces(MeshScratch m) {
+    if (cancel_poll(m.cancel, PASS == 0 ? CS_MESH_FACES0 : CS_MESH_FACES1, blockIdx.x)) return;
     const uint32_t gid = blockIdx.x * blockDim.x + threadIdx.x;
     if (gid >= m.n_leaves * 3u) return;
     const uint32_t ci = gid / 3u, ti = gid % 3u, t = 1u << ti;
@@ -263,6 +267,7 @@ __global__ void __launch_bounds__(128) k_mesh_faces(MeshScratch m) {
 
 // compaction of the used vertex slots
 __global__ void k_mesh_assign(MeshScratch m) {
+    if (cancel_poll(m.cancel, CS_MESH_ASSIGN, blockIdx.x)) return;
     const uint64_t s = uint64_t(blockIdx.x) * blockDim.x + threadIdx.x;
     if (s >= uint64_t(m.n_leaves) * 16u) return;
     if (m.remap[s] != 1u) { m.remap[s] = ~0u; return; }
@@ -333,6 +338,7 @@ struct TreeScratch {
     uint3* out_tris;
     uint32_t cap_tris;
     fc_mesh_cell* out_cells;
+    CancelRef cancel;            // as MeshScratch::cancel
 };
 
 __host__ __device__ __forceinline__ unsigned long long tree_key(uint32_t d, uint32_t x, uint32_t y, uint32_t z) {
@@ -418,6 +424,7 @@ __device__ inline float qef_solve(const Qef& q, float pos[3]) {
 
 // Surface leaves enter the tree at depth D
 __global__ void k_tree_leaves(TreeScratch m) {
+    if (cancel_poll(m.cancel, CS_TREE_LEAVES, blockIdx.x)) return;
     const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= m.n_leaves) return;
     const OctreeLeaf& L = m.leaves[i];
@@ -430,6 +437,7 @@ __global__ void k_tree_leaves(TreeScratch m) {
 }
 // The parents of the nodes [lo, hi) (one depth), appended as new nodes
 __global__ void k_tree_parents(TreeScratch m, uint32_t lo, uint32_t hi) {
+    if (cancel_poll(m.cancel, CS_TREE_PARENTS, blockIdx.x)) return;
     const uint32_t i = lo + blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= hi) return;
     const unsigned long long k = m.node_key[i];
@@ -444,6 +452,7 @@ __global__ void k_tree_parents(TreeScratch m, uint32_t lo, uint32_t hi) {
 // LeafHermiteData::qef_err of every surface leaf (OctreeBuilder::leaf, octree.rs:810-851): one QEF per vertex group,
 // the last group's error wins; a NaN gradient marks the group QEF_ERR_INVALID
 __global__ void __launch_bounds__(128) k_tree_leaf_err(TreeScratch m) {
+    if (cancel_poll(m.cancel, CS_TREE_LEAF_ERR, blockIdx.x)) return;
     const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= m.n_leaves) return;
     const OctreeLeaf& L = m.leaves[i];
@@ -502,6 +511,7 @@ __device__ __forceinline__ uint32_t axis_index(uint32_t a) { return a == 1u ? 0u
 // One thread per node of one depth: Octree::check_done / collapsible / try_collapse (octree.rs:252-440) with
 // LeafHermiteData::merge / solve (octree.rs:917-1033)
 __global__ void __launch_bounds__(128) k_tree_collapse(TreeScratch m, uint32_t lo, uint32_t hi) {
+    if (cancel_poll(m.cancel, CS_TREE_COLLAPSE, blockIdx.x)) return;
     const uint32_t id = lo + blockIdx.x * blockDim.x + threadIdx.x;
     if (id >= hi) return;
     const unsigned long long key = m.node_key[id];
@@ -630,6 +640,7 @@ __global__ void __launch_bounds__(128) k_tree_collapse(TreeScratch m, uint32_t l
 
 // Final leaves: leaves whose parent stayed a branch (or the root); listed for fc_mesh_read_cells
 __global__ void k_tree_final(TreeScratch m) {
+    if (cancel_poll(m.cancel, CS_TREE_FINAL, blockIdx.x)) return;
     const uint32_t id = blockIdx.x * blockDim.x + threadIdx.x;
     if (id >= m.n_nodes || !(m.node_state[id] & NODE_LEAF)) return;
     const unsigned long long k = m.node_key[id];
@@ -668,6 +679,7 @@ __device__ inline int tree_cover(const TreeScratch& m, uint32_t d, const uint32_
 // vertex from the emitting leaf, and no triangle between two corners that are the same cell.
 template <int PASS>
 __global__ void __launch_bounds__(128) k_tree_faces(TreeScratch m) {
+    if (cancel_poll(m.cancel, PASS == 0 ? CS_TREE_FACES0 : CS_TREE_FACES1, blockIdx.x)) return;
     const uint32_t gid = blockIdx.x * blockDim.x + threadIdx.x;
     if (gid >= m.n_nodes * 12u) return;
     const uint32_t id = gid / 12u, e = gid % 12u;
@@ -742,6 +754,7 @@ __global__ void __launch_bounds__(128) k_tree_faces(TreeScratch m) {
 
 // compaction of the used vertex slots (MeshBuilder::vertex: one output vertex per octree vertex)
 __global__ void k_tree_assign(TreeScratch m) {
+    if (cancel_poll(m.cancel, CS_TREE_ASSIGN, blockIdx.x)) return;
     const uint64_t s = uint64_t(blockIdx.x) * blockDim.x + threadIdx.x;
     if (s >= uint64_t(m.n_nodes) * 16u) return;
     if (m.remap[s] != 1u) { m.remap[s] = ~0u; return; }
@@ -764,10 +777,10 @@ __global__ void k_tree_assign(TreeScratch m) {
 
 // fc_octree_sample's device half (octree_capi.cu)
 int32_t octree_sample_device(fc_ctx* c, const fc_tape* tape, const fc_octree_cfg* cfg, OctreeLeaf* dout, uint64_t cap,
-                             uint32_t* n_out, fc_octree_stats* stats);
+                             uint32_t* n_out, fc_octree_stats* stats, const CallCancel& cc);
 
 // fc_mesh_build with FC_FLAG_MESH_COLLAPSE, after the sampler (n > 0 surface leaves in c->mesh_leaves; c->mu held)
-static int32_t mesh_build_collapse(fc_ctx* c, uint32_t n, uint32_t depth, fc_mesh_info* info) {
+static int32_t mesh_build_collapse(fc_ctx* c, uint32_t n, uint32_t depth, fc_mesh_info* info, const CallCancel& cc) {
     using namespace fdev;
     cudaStream_t s = c->stream;
     // nodes: the leaves plus at most min(n, 8^d) ancestors at every depth d < D
@@ -799,11 +812,13 @@ static int32_t mesh_build_collapse(fc_ctx* c, uint32_t n, uint32_t depth, fc_mes
     m.hmask = uint32_t(hsize - 1);
     m.cell_verts = cell_verts;
     m.corner_vert = corner_vert;
+    m.cancel = cc.ref;
     MeshScratch ms{};   // k_mesh_vertices: the surface leaves' vertices, exactly as the uniform mesh places them
     ms.leaves = m.leaves;
     ms.n_leaves = n;
     ms.cell_verts = cell_verts;
     ms.corner_vert = corner_vert;
+    ms.cancel = cc.ref;
 
     cudaEvent_t e0 = get_event(c, 0), e1 = get_event(c, 1);
     CU(cudaEventRecord(e0, s));
@@ -823,8 +838,7 @@ static int32_t mesh_build_collapse(fc_ctx* c, uint32_t n, uint32_t depth, fc_mes
         const uint32_t lo = range_lo[d + 1], hi = range_hi[d + 1];
         k_tree_parents<<<(hi - lo + 127) / 128, 128, 0, s>>>(m, lo, hi);
         uint32_t count = 0;
-        CU(cudaMemcpyAsync(&count, m.counts + 4, 4, cudaMemcpyDeviceToHost, s));
-        CU(cudaStreamSynchronize(s));
+        if (int32_t wrc = wait_read(c, s, cc, &count, m.counts + 4, 4)) return wrc;
         range_lo[d] = hi;
         range_hi[d] = count;
     }
@@ -844,8 +858,7 @@ static int32_t mesh_build_collapse(fc_ctx* c, uint32_t n, uint32_t depth, fc_mes
     k_tree_faces<0><<<(n_nodes * 12u + 127) / 128, 128, 0, s>>>(m);
     CU(cudaGetLastError());
     uint32_t cnt[6];
-    CU(cudaMemcpyAsync(cnt, m.counts, sizeof cnt, cudaMemcpyDeviceToHost, s));
-    CU(cudaStreamSynchronize(s));
+    if (int32_t wrc = wait_read(c, s, cc, cnt, m.counts, sizeof cnt)) return wrc;
     const uint32_t n_tris = cnt[1];
     const uint64_t v_cap = std::min<uint64_t>(uint64_t(n_nodes) * 16, uint64_t(n_tris) * 5 + 16);
     CU(c->mesh_verts.ensure(std::max<uint64_t>(v_cap, 1) * sizeof(float3)));
@@ -858,8 +871,7 @@ static int32_t mesh_build_collapse(fc_ctx* c, uint32_t n, uint32_t depth, fc_mes
     k_tree_faces<1><<<(n_nodes * 12u + 127) / 128, 128, 0, s>>>(m);
     CU(cudaEventRecord(e1, s));
     CU(cudaGetLastError());
-    CU(cudaMemcpyAsync(cnt, m.counts, sizeof cnt, cudaMemcpyDeviceToHost, s));
-    CU(cudaStreamSynchronize(s));
+    if (int32_t wrc = wait_read(c, s, cc, cnt, m.counts, sizeof cnt)) return wrc;
     if (cnt[0] > v_cap) return fail(FC_ERR_CUDA, "mesh vertex buffer overflow");
     c->mesh_n_verts = cnt[0];
     c->mesh_n_tris = n_tris;
@@ -876,6 +888,14 @@ extern "C" {
 int32_t fc_mesh_build(fc_ctx* c, const fc_tape* tape, const fc_octree_cfg* cfg, fc_mesh_info* info) {
     if (!c || !tape || !cfg || !info) return fail(FC_ERR_INVALID, "null argument");
     memset(info, 0, sizeof *info);
+    CallCancel cc;
+    auto no_mesh = [&](int32_t rc) {   // a cancelled build leaves no mesh (a failed one keeps the previous)
+        std::lock_guard<std::mutex> guard(c->mu);
+        c->mesh_n_verts = c->mesh_n_tris = c->mesh_n_cells = 0;
+        memset(info, 0, sizeof *info);
+        return rc;
+    };
+    if (int32_t crc = begin_call(c, cc)) return crc == FC_ERR_CANCELLED ? no_mesh(crc) : crc;
     // ---- sampler: leaves stay in HBM ----
     uint64_t cap = c->mesh_leaves.cap / sizeof(OctreeLeaf);
     if (cap < 1024) cap = std::max<uint64_t>(1024, std::min<uint64_t>(1ull << (3 * cfg->depth), 6ull << (2 * cfg->depth)));
@@ -884,12 +904,17 @@ int32_t fc_mesh_build(fc_ctx* c, const fc_tape* tape, const fc_octree_cfg* cfg, 
     for (int attempt = 0; attempt < 2; ++attempt) {
         CU(cudaSetDevice(c->device));
         CU(c->mesh_leaves.ensure(cap * sizeof(OctreeLeaf)));
-        int32_t rc = octree_sample_device(c, tape, cfg, c->mesh_leaves.as<OctreeLeaf>(), cap, &n, &ost);
+        int32_t rc = octree_sample_device(c, tape, cfg, c->mesh_leaves.as<OctreeLeaf>(), cap, &n, &ost, cc);
         if (rc == FC_OK) break;
+        if (rc == FC_ERR_CANCELLED) return no_mesh(rc);
         if (n > cap && attempt == 0) { cap = n; continue; }   // retry once with the exact count
         return rc;
     }
-    std::lock_guard<std::mutex> guard(c->mu);
+    std::unique_lock<std::mutex> guard(c->mu);
+    auto cancelled = [&](int32_t rc) {
+        guard.unlock();
+        return rc == FC_ERR_CANCELLED ? no_mesh(rc) : rc;
+    };
     cudaStream_t s = c->stream;
     MeshScratch m{};
     m.leaves = c->mesh_leaves.as<OctreeLeaf>();
@@ -898,7 +923,7 @@ int32_t fc_mesh_build(fc_ctx* c, const fc_tape* tape, const fc_octree_cfg* cfg, 
     info->sampler_ms = ost.total_ms;
     c->mesh_n_verts = c->mesh_n_tris = c->mesh_n_cells = 0;
     if (n == 0) return FC_OK;
-    if (cfg->flags & FC_FLAG_MESH_COLLAPSE) return mesh_build_collapse(c, n, cfg->depth, info);
+    if (cfg->flags & FC_FLAG_MESH_COLLAPSE) return cancelled(mesh_build_collapse(c, n, cfg->depth, info, cc));
     uint32_t hsize = 1024;
     while (hsize < 2u * n) hsize <<= 1;
     const size_t b_keys = size_t(hsize) * 8, b_vals = size_t(hsize) * 4, b_cv = size_t(n) * 4 * sizeof(float3), b_cn = size_t(n) * 4,
@@ -913,6 +938,7 @@ int32_t fc_mesh_build(fc_ctx* c, const fc_tape* tape, const fc_octree_cfg* cfg, 
     m.remap = reinterpret_cast<uint32_t*>(q); q += al(b_remap);
     m.counts = reinterpret_cast<uint32_t*>(q);
     m.hmask = hsize - 1;
+    m.cancel = cc.ref;
     cudaEvent_t e0 = get_event(c, 0), e1 = get_event(c, 1);
     CU(cudaEventRecord(e0, s));
     CU(cudaMemsetAsync(m.hkeys, 0xff, b_keys, s));
@@ -923,8 +949,7 @@ int32_t fc_mesh_build(fc_ctx* c, const fc_tape* tape, const fc_octree_cfg* cfg, 
     k_mesh_vertices<<<bl, 128, 0, s>>>(m);
     k_mesh_faces<0><<<(n * 3u + 127) / 128, 128, 0, s>>>(m);
     uint32_t cnt[4];
-    CU(cudaMemcpyAsync(cnt, m.counts, sizeof cnt, cudaMemcpyDeviceToHost, s));
-    CU(cudaStreamSynchronize(s));
+    if (int32_t wrc = wait_read(c, s, cc, cnt, m.counts, sizeof cnt)) return cancelled(wrc);
     const uint32_t n_tris = cnt[1];
     // every used slot becomes a vertex: count them on the device, sized by the worst case (5 slots per triangle fan)
     const uint64_t v_cap = std::min<uint64_t>(uint64_t(n) * 16, uint64_t(n_tris) * 5 / 4 + 16);
@@ -938,8 +963,7 @@ int32_t fc_mesh_build(fc_ctx* c, const fc_tape* tape, const fc_octree_cfg* cfg, 
     k_mesh_faces<1><<<(n * 3u + 127) / 128, 128, 0, s>>>(m);
     CU(cudaEventRecord(e1, s));
     CU(cudaGetLastError());
-    CU(cudaMemcpyAsync(cnt, m.counts, sizeof cnt, cudaMemcpyDeviceToHost, s));
-    CU(cudaStreamSynchronize(s));
+    if (int32_t wrc = wait_read(c, s, cc, cnt, m.counts, sizeof cnt)) return cancelled(wrc);
     if (cnt[0] > v_cap) return fail(FC_ERR_CUDA, "mesh vertex buffer overflow");
     c->mesh_n_verts = cnt[0];
     c->mesh_n_tris = n_tris;

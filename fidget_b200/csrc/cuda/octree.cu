@@ -37,7 +37,10 @@ __global__ void __launch_bounds__(128) k_octree_leaf(const __grid_constant__ Oct
     unsigned long long n_empty = 0, n_full = 0, n_surf = 0, n_pts = 0;
     for (;;) {
         uint32_t j = 0;
-        if (lane == 0) j = atomicAdd(&p.ctr->cursor[p.cursor], 1u);
+        if (lane == 0) {
+            j = atomicAdd(&p.ctr->cursor[p.cursor], 1u);
+            if (j < n_jobs && cancel_poll(p.cancel, CS_OCTREE_LEAF, j)) j = ~0u;
+        }
         j = __shfl_sync(FULL, j, 0);
         if (j >= n_jobs) break;
         const TileJob* job = p.jobs + j;
@@ -153,6 +156,7 @@ __global__ void __launch_bounds__(128) k_octree_grads(const __grid_constant__ Oc
     const uint32_t n = min(*p.n_out, p.cap_out);
     unsigned long long n_pts = 0;
     for (uint32_t i = warp; i < n; i += n_warps) {
+        if (cancel_poll(p.cancel, CS_OCTREE_GRADS, i)) break;   // (uniform over the warp)
         OctreeLeaf* L = p.out + i;
         const TapeRef tr = p.out_tapes[i];
         const uint32_t active = L->present;

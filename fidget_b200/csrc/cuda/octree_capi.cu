@@ -2,9 +2,9 @@
 #include "capi_internal.h"
 
 // Device half: runs the sampler into `dout` (device memory, `cap` leaves); *n_out = surface leaves found
-// (FC_ERR_INVALID when it exceeds cap).  Takes the context lock.
+// (FC_ERR_INVALID when it exceeds cap).  Takes the context lock.  `cc`: the call's cancellation (begin_call).
 int32_t octree_sample_device(fc_ctx* c, const fc_tape* tape, const fc_octree_cfg* cfg, OctreeLeaf* dout, uint64_t cap,
-                             uint32_t* n_out_p, fc_octree_stats* stats) {
+                             uint32_t* n_out_p, fc_octree_stats* stats, const CallCancel& cc) {
     static_assert(sizeof(fc_octree_leaf) == sizeof(OctreeLeaf) && sizeof(OctreeLeaf) == 348, "leaf layout");
     if (!c || !tape || !cfg || !n_out_p) return fail(FC_ERR_INVALID, "null argument");
     if (cfg->depth > FC_MAX_OCTREE_DEPTH) return fail(FC_ERR_INVALID, "octree depth too large");
@@ -69,6 +69,7 @@ int32_t octree_sample_device(fc_ctx* c, const fc_tape* tape, const fc_octree_cfg
         p.has_transform = cfg->has_transform;
         p.cell_h = 2.0f / float(1u << D);
         p.vb = vb;
+        p.cancel = cc.ref;
         uint64_t cells = 1ull << (3 * l);
         uint64_t warps = l ? std::max<uint64_t>(1, cells / 8) : 1;
         int blocks = int(std::min<uint64_t>((warps + WARPS_PER_BLOCK - 1) / WARPS_PER_BLOCK, uint64_t(grid_blocks)));
@@ -89,14 +90,18 @@ int32_t octree_sample_device(fc_ctx* c, const fc_tape* tape, const fc_octree_cfg
     q.cap_out = uint32_t(cap);
     q.n_out = d_n_out;
     q.stats = d_leaf_stats;
+    q.cancel = cc.ref;
     launch_octree_leaf(q, c->sm_count * 8, s);
     launch_octree_grads(q, c->sm_count * 8, s);
     launches += 2;
     if (timing) CU(cudaEventRecord(get_event(c, 1), s));
     CU(cudaGetLastError());
     uint32_t n_out = 0;
-    CU(cudaMemcpyAsync(&n_out, d_n_out, 4, cudaMemcpyDeviceToHost, s));
-    CU(cudaStreamSynchronize(s));
+    if (int32_t wrc = wait_read(c, s, cc, &n_out, d_n_out, 4)) {
+        *n_out_p = 0;
+        if (stats) memset(stats, 0, sizeof *stats);
+        return wrc;
+    }
     *n_out_p = n_out;
     int32_t rc = check_device_errors(c);
     if (n_out > cap) rc = fail(FC_ERR_INVALID, "leaf buffer too small: " + std::to_string(n_out) + " surface leaves");
@@ -128,6 +133,9 @@ extern "C" {
 int32_t fc_octree_sample(fc_ctx* c, const fc_tape* tape, const fc_octree_cfg* cfg, fc_octree_leaf* out, uint64_t cap,
                          uint64_t* n_leaves, fc_octree_stats* stats) {
     if (!c || !tape || !cfg || !n_leaves || (!out && cap)) return fail(FC_ERR_INVALID, "null argument");
+    *n_leaves = 0;
+    CallCancel cc;
+    if (int32_t crc = begin_call(c, cc)) return crc;
     const bool out_dev = is_device_ptr(out);
     OctreeLeaf* dout = reinterpret_cast<OctreeLeaf*>(out);
     if (!out_dev) {
@@ -137,7 +145,7 @@ int32_t fc_octree_sample(fc_ctx* c, const fc_tape* tape, const fc_octree_cfg* cf
         dout = c->image.as<OctreeLeaf>();
     }
     uint32_t n_out = 0;
-    int32_t rc = octree_sample_device(c, tape, cfg, dout, cap, &n_out, stats);
+    int32_t rc = octree_sample_device(c, tape, cfg, dout, cap, &n_out, stats, cc);
     *n_leaves = n_out;
     if (!rc && !out_dev && n_out) CU(cudaMemcpy(out, dout, size_t(n_out) * sizeof(OctreeLeaf), cudaMemcpyDeviceToHost));
     return rc;

@@ -79,6 +79,8 @@ int32_t fc_render2d(fc_ctx* c, const fc_tape* tape, const fc_render2d_cfg* cfg, 
     if (cfg->width == 0 || cfg->height == 0) return fail(FC_ERR_INVALID, "empty image");
     if (tape->info.mem_count) return fail(FC_ERR_UNSUPPORTED, "renderers need a tape without memory spills (<= 255 registers)");
     if (tape->info.n_outputs != 1) return fail(FC_ERR_INVALID, "ShapeTape has multiple outputs");
+    CallCancel cc;
+    if (int32_t crc = begin_call(c, cc)) return crc;
     std::lock_guard<std::mutex> guard(c->mu);
     CU(cudaSetDevice(c->device));
     static const uint32_t DFLT[3] = {128, 32, 8};
@@ -190,6 +192,7 @@ int32_t fc_render2d(fc_ctx* c, const fc_tape* tape, const fc_render2d_cfg* cfg, 
         p.ctr = c->counters.as<Counters>();
         p.stats = want_stats ? c->stats.as<Stats>() : nullptr;
         p.vb = vb;
+        p.cancel = cc.ref;
         if (fused) {
             tail.fill_tile[l] = ts[l];
             tail.fills[l] = c->fills[l].as<FillRec>();
@@ -222,6 +225,7 @@ int32_t fc_render2d(fc_ctx* c, const fc_tape* tape, const fc_render2d_cfg* cfg, 
             f.fills = c->fills[l].as<FillRec>();
             f.n_fills = &c->counters.as<Counters>()->n_fills[l];
             f.out = dimg;
+            f.cancel = cc.ref;
             cudaStream_t fs = serial_fill ? s : c->aux_stream;
             if (!serial_fill) {
                 CU(cudaEventRecord(c->ev_fork[l], s));
@@ -245,10 +249,12 @@ int32_t fc_render2d(fc_ctx* c, const fc_tape* tape, const fc_render2d_cfg* cfg, 
         q.cursor = L;
         q.stats = want_stats ? c->stats.as<Stats>() : nullptr;
         q.vb = vb;
+        q.cancel = cc.ref;
         if (fused) {
             tail.n_levels = L - 1;
             tail.px = q;
             tail.epoch = c->epoch;
+            tail.cancel = cc.ref;
             tail.paint_fills = env_int("FIDGET_B200_TAIL_PAINTS", 0) ? 1 : 0;
             auto paint = [&](int l, cudaStream_t fs) {
                 FillParams f{};
@@ -257,6 +263,7 @@ int32_t fc_render2d(fc_ctx* c, const fc_tape* tape, const fc_render2d_cfg* cfg, 
                 f.fills = c->fills[l].as<FillRec>();
                 f.n_fills = &c->counters.as<Counters>()->n_fills[l];
                 f.out = dimg;
+                f.cancel = cc.ref;
                 launch_fill_2d(f, c->sm_count * 2, fs);
                 ++launches;
             };
@@ -282,6 +289,13 @@ int32_t fc_render2d(fc_ctx* c, const fc_tape* tape, const fc_render2d_cfg* cfg, 
     }
     if (timing) CU(cudaEventRecord(get_event(c, ev++), s));
     CU(cudaGetLastError());
+    const bool early_return = async && out_dev && !want_stats;
+    if (cc.flag && !early_return) {   // a cancelled render derives no format and copies nothing to the host
+        if (int32_t wrc = wait_call(c, s, cc)) {
+            if (stats) memset(stats, 0, sizeof *stats);
+            return wrc;
+        }
+    }
     if (fmt != FC_OUT_F32) {
         const size_t fb = fmt == FC_OUT_MASK_U8 ? size_t(cfg->width) * cfg->height
                         : fmt == FC_OUT_BITMAP_1BIT ? size_t((cfg->width + 7) / 8) * cfg->height : img_bytes;
@@ -301,7 +315,10 @@ int32_t fc_render2d(fc_ctx* c, const fc_tape* tape, const fc_render2d_cfg* cfg, 
             CU(cudaMemcpyAsync(out + size_t(by0) * cfg->width, dimg + size_t(by0) * cfg->width,
                                size_t(by1 - by0) * cfg->width * 4, cudaMemcpyDeviceToHost, s));
     }
-    if (async && out_dev && !want_stats) return FC_OK;
+    if (early_return) {
+        c->async_call = cc;
+        return FC_OK;
+    }
     CU(cudaStreamSynchronize(s));
     rc = check_device_errors(c);
     if (stats) {
@@ -363,6 +380,8 @@ int32_t fc_render3d(fc_ctx* c, const fc_tape* tape, const fc_render3d_cfg* cfg, 
     if (cfg->width == 0 || cfg->height == 0 || cfg->depth == 0) return fail(FC_ERR_INVALID, "empty volume");
     if (tape->info.mem_count) return fail(FC_ERR_UNSUPPORTED, "renderers need a tape without memory spills (<= 255 registers)");
     if (tape->info.n_outputs != 1) return fail(FC_ERR_INVALID, "ShapeTape has multiple outputs");
+    CallCancel cc;
+    if (int32_t crc = begin_call(c, cc)) return crc;
     std::lock_guard<std::mutex> guard(c->mu);
     CU(cudaSetDevice(c->device));
     static const uint32_t DFLT[5] = {128, 64, 32, 16, 8};
@@ -506,6 +525,7 @@ int32_t fc_render3d(fc_ctx* c, const fc_tape* tape, const fc_render3d_cfg* cfg, 
         p.census = exact_census ? c->census.as<CensusRec>() : nullptr;
         p.cap_census = uint32_t(cap_census);
         p.vb = vb;
+        p.cancel = cc.ref;
         int blocks = (l == L - 1 && l > 0) ? grid_blocks_last : grid_blocks;
         if (l == 0) {
             uint64_t warps = (n_roots + 31) / 32;
@@ -546,6 +566,7 @@ int32_t fc_render3d(fc_ctx* c, const fc_tape* tape, const fc_render3d_cfg* cfg, 
         q.list = L; q.cursor = L;
         q.stats = want_stats ? c->stats.as<Stats>() : nullptr;
         q.vb = vb;
+        q.cancel = cc.ref;
         launch_voxels_3d(q, c->sm_count * env_int("FIDGET_B200_VOXEL_BLOCKS_PER_SM", 12), s);
         ++launches;
     }
@@ -563,6 +584,7 @@ int32_t fc_render3d(fc_ctx* c, const fc_tape* tape, const fc_render3d_cfg* cfg, 
         cp.heightmap = c->heightmap.as<unsigned long long>();
         cp.width = cfg->width;
         cp.stats = ds;
+        cp.cancel = cc.ref;
         launch_census_3d(cp, c->sm_count * 8, s);
         ++launches;
     }
@@ -579,16 +601,27 @@ int32_t fc_render3d(fc_ctx* c, const fc_tape* tape, const fc_render3d_cfg* cfg, 
         q.out = dimg;
         q.stats = want_stats ? c->stats.as<Stats>() : nullptr;
         q.vb = vb;
+        q.cancel = cc.ref;
         launch_normals_3d(q, s);
         ++launches;
     }
     if (timing) CU(cudaEventRecord(get_event(c, ev++), s));
     CU(cudaGetLastError());
+    const bool early_return = async && out_dev && !want_stats;
+    if (cc.flag && !early_return) {   // a cancelled render copies nothing to the host
+        if (int32_t wrc = wait_call(c, s, cc)) {
+            if (stats) memset(stats, 0, sizeof *stats);
+            return wrc;
+        }
+    }
     if (!out_dev && band_y1 > band_y0)
         CU(cudaMemcpyAsync(reinterpret_cast<char*>(out) + size_t(band_y0) * cfg->width * 16,
                            static_cast<char*>(dimg) + size_t(band_y0) * cfg->width * 16, size_t(band_y1 - band_y0) * cfg->width * 16,
                            cudaMemcpyDeviceToHost, s));
-    if (async && out_dev && !want_stats) return FC_OK;
+    if (early_return) {
+        c->async_call = cc;
+        return FC_OK;
+    }
     CU(cudaStreamSynchronize(s));
     rc = check_device_errors(c);
     if (stats) {

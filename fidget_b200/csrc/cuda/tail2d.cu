@@ -18,7 +18,8 @@
 //     of the interpreters can never hit a line that an SM cached before another SM filled it;
 //   * outstanding = jobs queued or running; a producer adds its children BEFORE retiring itself, so the count
 //     reaches zero exactly when no interval / pixel work is left; fills are drained after that.
-// Every spin is bounded (error bit 2) -- a logic error must not hang the device.
+// Every spin is bounded (error bit 2) -- a logic error must not hang the device.  A cancelled call (fc_ctx_set_cancel)
+// ends every spin and every warp at its next poll, without an error bit.
 #include <algorithm>
 
 #include "level_job.cuh"
@@ -135,8 +136,12 @@ __global__ void __launch_bounds__(WARPS_PER_BLOCK * 32) k_tail_2d(const __grid_c
                 const uint32_t e = sch.ring[h % RING];     // read before the claim: the slot may be reused right after it
                 if (atomicCAS(&sch.head, h, h + 1u) == h) { entry = e; break; }
             }
+            // a cancelled call claims nothing more: the warp leaves (entries still in the ring are dropped; `outstanding`
+            // then never reaches zero, so no warp may wait for it)
+            if (cancel_poll(p.cancel, entry == 0xffffffffu ? CS_WAIT : CS_TAIL_2D, entry & 0x0fffffffu)) entry = 0xfffffffeu;
         }
         entry = __shfl_sync(FULL, entry, 0);
+        if (entry == 0xfffffffeu) break;
         if (entry == 0xffffffffu) {
             if (*v_done) break;
             // ---- 2. become the CTA's scout, or wait for the one that is ----
@@ -215,8 +220,9 @@ __global__ void __launch_bounds__(WARPS_PER_BLOCK * 32) k_tail_2d(const __grid_c
             __syncwarp();
             if (lane == 0) { __threadfence(); atomicSub(&ctr->outstanding, 1u); }   // children were added before
         } else if (kind == L) {
-            const TileJob job = load_job_ready(p.px.jobs + idx, p.epoch, ctr);
-            pixel_job(p.px, job, reinterpret_cast<float2*>(slots), lane, shaded);
+            bool ok = true;
+            const TileJob job = load_job_ready(p.px.jobs + idx, p.epoch, ctr, p.cancel, ok);
+            if (!__any_sync(FULL, !ok)) pixel_job(p.px, job, reinterpret_cast<float2*>(slots), lane, shaded);
             __syncwarp();
             if (lane == 0) atomicSub(&ctr->outstanding, 1u);
         } else {
@@ -225,6 +231,7 @@ __global__ void __launch_bounds__(WARPS_PER_BLOCK * 32) k_tail_2d(const __grid_c
             uint4 rec = __ldcg(rp);
             uint32_t spins = 0;
             while (rec.w != p.epoch) {   // reserved but not written yet
+                if (cancel_poll(p.cancel, CS_WAIT, ~0u)) break;
                 __nanosleep(64);
                 rec = __ldcg(rp);
                 if (++spins > (1u << 22)) { atomicOr(&ctr->error, 4u); break; }

@@ -6,6 +6,7 @@
   RenderConfig2D/3D    <-> pixel::RenderConfig / voxel::RenderConfig
                            (fidget-raster/src/pixel.rs:27-39, voxel.rs:26-36)
   render2d / render3d  <-> pixel::render / voxel::render (pixel.rs:452, voxel.rs:500)
+  CancelToken          <-> fidget_core::render::CancelToken (render/config.rs:59-80)
 
 Everything here calls through the C ABI in include/fidget_cuda.h; there is no
 CPU implementation behind it.
@@ -13,6 +14,7 @@ CPU implementation behind it.
 from __future__ import annotations
 
 import ctypes as C
+import threading
 from dataclasses import dataclass, field
 
 import numpy as np
@@ -54,6 +56,23 @@ def schedule_check(tape: TapeData) -> dict:
     return {n: getattr(info, n) for n, _ in info._fields_}
 
 
+class CancelToken:
+    """``CancelToken``: a flag another thread sets to stop a render, ``octree_sample`` or ``mesh`` in flight (the call
+    then returns ``None``).  One byte, read by the library with an acquire load (``fc_ctx_set_cancel``)."""
+
+    def __init__(self):
+        self._flag = C.c_uint8(0)
+
+    def cancel(self):
+        self._flag.value = 1
+
+    def is_cancelled(self) -> bool:
+        return bool(self._flag.value)
+
+    def _address(self):
+        return C.c_void_p(C.addressof(self._flag))
+
+
 class CudaContext:
     """One GPU: stream + scratch arenas (``fc_ctx``)."""
 
@@ -64,6 +83,22 @@ class CudaContext:
         self._h = h
         self.device = device
         self._stream = None
+        # the cancel flag is context-wide: a call attaches its token (or none), runs and detaches it under this lock, so
+        # that two threads sharing the context cannot run under each other's token
+        self._cancel_lock = threading.Lock()
+        self._async_cancel = None      # token of the last asynchronous call, re-attached by synchronize()
+
+    def _cancellable(self, token, fn, asynchronous=False):
+        """fn() with ``token``'s flag attached; returns fn's status."""
+        with self._cancel_lock:
+            _ck(self._lib.fc_ctx_set_cancel(self._h, token._address() if token is not None else None))
+            try:
+                rc = fn()
+            finally:
+                self._lib.fc_ctx_set_cancel(self._h, None)
+            if asynchronous:
+                self._async_cancel = token
+            return rc
 
     def close(self):
         if getattr(self, "_h", None):
@@ -102,7 +137,16 @@ class CudaContext:
         return _Bound()
 
     def synchronize(self):
-        _ck(self._lib.fc_ctx_synchronize(self._h))
+        """Waits for the enqueued work; raises CudaError (code -6, FC_ERR_CANCELLED) when the token of the last
+        ``asynchronous=True`` call cancelled it."""
+        with self._cancel_lock:
+            token, self._async_cancel = self._async_cancel, None
+            _ck(self._lib.fc_ctx_set_cancel(self._h, token._address() if token is not None else None))
+            try:
+                rc = self._lib.fc_ctx_synchronize(self._h)
+            finally:
+                self._lib.fc_ctx_set_cancel(self._h, None)
+        _ck(rc)
 
     def set_arena_bytes(self, n: int):
         _ck(self._lib.fc_ctx_set_arena_bytes(self._h, n))
@@ -337,6 +381,7 @@ class RenderConfig2D:
     interleave: tuple = (0, 0)                  # (N, r): only the root tiles rank r of N owns (shard.tile_owner)
     out_format: str = "f32"                     # "f32" | "mask_u8" | "bitmap_1bit" | "rgba8"
     fused_tail: bool = False                    # experimental: levels 1.., leaf pixels, fills as one persistent launch
+    cancel: CancelToken | None = None           # EvalConfig::cancel: render2d returns None once it is cancelled
 
     def matrix(self):
         return self.mat if self.mat is not None else pixel_mat(self.width, self.height, self.world_to_model)
@@ -358,6 +403,7 @@ class RenderConfig3D:
     interleave: tuple = (0, 0)                  # (N, r): only the root-tile columns rank r of N owns
     exact_census: bool = False                  # stats = the reference's front-to-back census (voxel.rs:244-357)
     full_ladder: bool = False                   # default tile sizes: evaluate all of (128,64,32,16,8), not the device's (128,32,8)
+    cancel: CancelToken | None = None           # EvalConfig::cancel: render3d returns None once it is cancelled
 
     def matrix(self):
         return self.mat if self.mat is not None else voxel_mat(self.width, self.height, self.depth,
@@ -370,7 +416,7 @@ OUT_FORMATS = {"f32": _lib.FC_OUT_F32, "mask_u8": _lib.FC_OUT_MASK_U8, "bitmap_1
 
 def render2d(shape: CudaShape, cfg: RenderConfig2D, out=None, stats: bool = False, asynchronous: bool = False):
     """pixel::render.  ``out``: None (returns a numpy float32 [h,w] of
-    RawDistancePixel bits), a numpy array, or a CUDA torch tensor."""
+    RawDistancePixel bits), a numpy array, or a CUDA torch tensor.  None when ``cfg.cancel`` cancelled it."""
     lib = shape._lib
     c = _lib.FcRender2dCfg()
     c.width, c.height = cfg.width, cfg.height
@@ -398,12 +444,17 @@ def render2d(shape: CudaShape, cfg: RenderConfig2D, out=None, stats: bool = Fals
         else:
             out = np.zeros((cfg.height, cfg.width, 4), dtype=np.uint8)
     st = _lib.FcRenderStats() if stats else None
-    _ck(lib.fc_render2d(shape.cuda._h, shape._h, C.byref(c), _ptr(out), C.byref(st) if stats else None))
+    rc = shape.cuda._cancellable(cfg.cancel, lambda: lib.fc_render2d(shape.cuda._h, shape._h, C.byref(c), _ptr(out),
+                                                                     C.byref(st) if stats else None), asynchronous)
+    if rc == _lib.FC_ERR_CANCELLED:
+        return None
+    _ck(rc)
     return (out, st.as_dict()) if stats else out
 
 
 def render3d(shape: CudaShape, cfg: RenderConfig3D, out=None, stats: bool = False, asynchronous: bool = False):
-    """voxel::render -> numpy structured array [h,w] of GEOMETRY_PIXEL (or fills ``out``)."""
+    """voxel::render -> numpy structured array [h,w] of GEOMETRY_PIXEL (or fills ``out``); None when ``cfg.cancel``
+    cancelled it."""
     lib = shape._lib
     c = _lib.FcRender3dCfg()
     c.width, c.height, c.depth = cfg.width, cfg.height, cfg.depth
@@ -423,7 +474,11 @@ def render3d(shape: CudaShape, cfg: RenderConfig3D, out=None, stats: bool = Fals
     if out is None:
         out = np.zeros((cfg.height, cfg.width), dtype=GEOMETRY_PIXEL)
     st = _lib.FcRenderStats() if stats else None
-    _ck(lib.fc_render3d(shape.cuda._h, shape._h, C.byref(c), _ptr(out), C.byref(st) if stats else None))
+    rc = shape.cuda._cancellable(cfg.cancel, lambda: lib.fc_render3d(shape.cuda._h, shape._h, C.byref(c), _ptr(out),
+                                                                     C.byref(st) if stats else None), asynchronous)
+    if rc == _lib.FC_ERR_CANCELLED:
+        return None
+    _ck(rc)
     return (out, st.as_dict()) if stats else out
 
 
@@ -433,9 +488,9 @@ OCTREE_LEAF = np.dtype([("ix", np.uint16), ("iy", np.uint16), ("iz", np.uint16),
 
 
 def octree_sample(shape: CudaShape, depth: int, world_to_model=None, capacity: int | None = None,
-                  stats: bool = False, timing: bool = False, var_values=()):
+                  stats: bool = False, timing: bool = False, var_values=(), cancel: CancelToken | None = None):
     """Sampler half of ``fidget_mesh::Octree::build`` (octree.rs:521-808): surface leaves with their
-    corner mask and per-edge Hermite data, sorted by (iz, iy, ix)."""
+    corner mask and per-edge Hermite data, sorted by (iz, iy, ix).  None when ``cancel`` cancelled it."""
     lib = shape._lib
     c = _lib.FcOctreeCfg()
     c.depth = depth
@@ -451,7 +506,10 @@ def octree_sample(shape: CudaShape, depth: int, world_to_model=None, capacity: i
     while True:
         out = np.zeros(cap, dtype=OCTREE_LEAF)
         n = C.c_uint64()
-        rc = lib.fc_octree_sample(shape.cuda._h, shape._h, C.byref(c), _ptr(out), cap, C.byref(n), C.byref(st))
+        rc = shape.cuda._cancellable(cancel, lambda: lib.fc_octree_sample(shape.cuda._h, shape._h, C.byref(c), _ptr(out),
+                                                                          cap, C.byref(n), C.byref(st)))
+        if rc == _lib.FC_ERR_CANCELLED:
+            return None
         if rc != 0 and n.value > cap and capacity is None:
             cap = int(n.value)          # retry once with the exact count
             continue
@@ -462,11 +520,13 @@ def octree_sample(shape: CudaShape, depth: int, world_to_model=None, capacity: i
     return (leaves, st.as_dict()) if stats else leaves
 
 
-def mesh(shape: CudaShape, depth: int, world_to_model=None, var_values=(), stl: bool = False, collapse: bool = False):
+def mesh(shape: CudaShape, depth: int, world_to_model=None, var_values=(), stl: bool = False, collapse: bool = False,
+         cancel: CancelToken | None = None):
     """``Octree::build(...).walk_dual()`` (fidget-mesh): returns ``(vertices [n,3] float32, triangles [m,3] uint32,
     info dict)`` -- plus the binary STL bytes (``Mesh::write_stl``) when ``stl``.  Without ``collapse`` the mesh is
     the uniform-depth one (no cell collapse); with it, cells are collapsed as the reference's octree does and the
-    dual is walked over leaves of different depths (``mesh_cells`` then lists the final leaves)."""
+    dual is walked over leaves of different depths (``mesh_cells`` then lists the final leaves).  None when
+    ``cancel`` cancelled the build (the context then holds no mesh)."""
     lib = shape._lib
     c = _lib.FcOctreeCfg()
     c.depth = depth
@@ -478,7 +538,10 @@ def mesh(shape: CudaShape, depth: int, world_to_model=None, var_values=(), stl: 
     for i, v in enumerate(var_values):
         c.var_values[i] = float(v)
     info = _lib.FcMeshInfo()
-    _ck(lib.fc_mesh_build(shape.cuda._h, shape._h, C.byref(c), C.byref(info)))
+    rc = shape.cuda._cancellable(cancel, lambda: lib.fc_mesh_build(shape.cuda._h, shape._h, C.byref(c), C.byref(info)))
+    if rc == _lib.FC_ERR_CANCELLED:
+        return None
+    _ck(rc)
     verts = np.zeros((info.n_vertices, 3), dtype=np.float32)
     tris = np.zeros((info.n_triangles, 3), dtype=np.uint32)
     _ck(lib.fc_mesh_read(shape.cuda._h, _ptr(verts), _ptr(tris)))

@@ -36,7 +36,8 @@ typedef enum fc_status {
     FC_ERR_CUDA = -2,         /* CUDA runtime error (message has the detail) */
     FC_ERR_UNSUPPORTED = -3,  /* valid input the device path cannot take (e.g. spilled tape in a renderer) */
     FC_ERR_ARENA = -4,        /* tape arena exhausted during on-device simplification */
-    FC_ERR_NO_DEVICE = -5     /* no usable CUDA device; there is NO CPU fallback */
+    FC_ERR_NO_DEVICE = -5,    /* no usable CUDA device; there is NO CPU fallback */
+    FC_ERR_CANCELLED = -6     /* the cancel flag attached with fc_ctx_set_cancel was set (never returned without one) */
 } fc_status;
 
 typedef struct fc_ctx fc_ctx;    /* one GPU + stream + scratch arenas */
@@ -60,6 +61,18 @@ int32_t fc_ctx_synchronize(fc_ctx* ctx);
 /* Size of the tape arena used by on-device simplification (bytes; default
  * 1 GiB).  Takes effect at the next render call. */
 int32_t fc_ctx_set_arena_bytes(fc_ctx* ctx, uint64_t bytes);
+/* Cancellation (CancelToken, fidget-core/src/render/config.rs:59-80).  `flag` points to a caller-owned byte with the
+ * layout of Rust's AtomicBool (CancelToken::into_raw() as *const u8): nonzero = cancelled.  The library reads it with
+ * an acquire load, from any thread; NULL detaches it.  Context-wide, like fc_ctx_set_stream, and consulted only by
+ * fc_render2d, fc_render3d, fc_octree_sample, fc_mesh_build, and fc_ctx_synchronize after the most recent
+ * FC_FLAG_ASYNC call of those.  With a flag attached:
+ *  - set on entry: the call returns FC_ERR_CANCELLED before it allocates or launches anything;
+ *  - set while the call runs: the kernels stop claiming work and the call returns FC_ERR_CANCELLED ("cancelled" in
+ *    fc_last_error); `out` is unspecified (a host `out` receives no copy), stats / info are zeroed, and the context
+ *    stays usable.  A cancelled fc_mesh_build leaves no mesh (fc_mesh_read copies nothing, fc_mesh_read_cells
+ *    reports 0, fc_mesh_write_stl 84 bytes);
+ *  - FC_OK: the result, stats included, is exactly that of the same call without a flag. */
+int32_t fc_ctx_set_cancel(fc_ctx* ctx, const uint8_t* flag);
 
 /* ---- tapes -------------------------------------------------------------- */
 /* `words` is exactly what fidget_bytecode::Bytecode::new emits

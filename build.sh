@@ -11,6 +11,10 @@ FLAGS="-gencode arch=compute_90a,code=sm_90a -lineinfo -O3 -std=c++17 \
 if [ "$1" = "-v" ]; then FLAGS="$FLAGS -Xptxas -v"; fi
 # EXTRA="-DSOME_SWITCH" OUT=fidget_b200/libfidget_cuda_variant.so ./build.sh builds a variant for FIDGET_B200_LIB
 FLAGS="$FLAGS $EXTRA"
-$NVCC $FLAGS -o $OUT $SRC/cuda/kernels.cu $SRC/cuda/coop.cu $SRC/cuda/bulk.cu $SRC/cuda/tail2d.cu $SRC/cuda/octree.cu $SRC/cuda/effects.cu $SRC/cuda/capi.cu $SRC/cuda/schedule.cu $SRC/cuda/render.cu $SRC/cuda/octree_capi.cu $SRC/cuda/mesh.cu $SRC/cuda/effects_capi.cu $SRC/host/tape.cc $SRC/host/host_capi.cc
+$NVCC $FLAGS -o $OUT $SRC/cuda/kernels.cu $SRC/cuda/coop.cu $SRC/cuda/bulk.cu $SRC/cuda/tail2d.cu $SRC/cuda/octree.cu $SRC/cuda/effects.cu $SRC/cuda/capi.cu $SRC/cuda/schedule.cu $SRC/cuda/render.cu $SRC/cuda/octree_capi.cu $SRC/cuda/mesh.cu $SRC/cuda/effects_capi.cu $SRC/cuda/solve.cu $SRC/cuda/solve_capi.cu $SRC/host/tape.cc $SRC/host/host_capi.cc
 make -s -C oracle liboracle.so
-echo "built $OUT and oracle/liboracle.so"
+# the solver's CPU oracle (oracle/solve.cc) on top of liboracle's point and gradient VM
+CXX=$([ -x /usr/bin/g++ ] && echo /usr/bin/g++ || echo g++)
+$CXX -std=c++17 -O2 -fPIC -ffp-contract=off -fno-fast-math -Wall -Wno-unused-function -pthread -shared \
+  -o oracle/libsolve_oracle.so oracle/solve.cc -Loracle -l:liboracle.so -Wl,-rpath,'$ORIGIN'
+echo "built $OUT, oracle/liboracle.so and oracle/libsolve_oracle.so"

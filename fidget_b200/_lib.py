@@ -95,6 +95,21 @@ class FcMeshInfo(C.Structure):
                [("sampler_ms", C.c_float), ("mesh_ms", C.c_float)]
 
 
+class FcSolveCfg(C.Structure):
+    _fields_ = [("n_params", C.c_uint32), ("n_free", C.c_uint32), ("max_iters", C.c_uint32)]
+
+
+class FcSolveResult(C.Structure):
+    _fields_ = [("status", C.c_uint32), ("iterations", C.c_uint32), ("err", C.c_float), ("pad", C.c_uint32)]
+
+
+FC_SOLVE_MAX_FREE, FC_SOLVE_MAX_CONSTRAINTS, FC_SOLVE_MAX_PARAMS = 64, 256, 1024
+FC_SOLVE_ZERO_RESIDUAL = 0
+FC_SOLVE_UNCHANGED = 1
+FC_SOLVE_ZERO_ERR = 2
+FC_SOLVE_ZERO_DAMPING = 3
+FC_SOLVE_STALLED = 4
+FC_SOLVE_MAX_ITERS = 5
 FC_FLAG_ASYNC = 1
 FC_FLAG_TIMING = 2
 FC_FLAG_NO_CLAMP = 4
@@ -144,6 +159,7 @@ CUDA_API = {
     "fc_mesh_read": (_i32, [_vp, _vp, _vp]),
     "fc_mesh_read_cells": (_i32, [_vp, _vp, _u64, _P(_u64)]),
     "fc_mesh_write_stl": (_i32, [_vp, _vp, C.c_size_t, _P(C.c_size_t)]),
+    "fc_solve_batch": (_i32, [_vp, _P(_vp), _u32, _P(_P(_i32)), _P(FcSolveCfg), _vp, _u64, _vp]),
     "fc_schedule_check": (_i32, [_P(_u32), C.c_size_t, _u8, _u32, _u32, _u32, _P(FcScheduleInfo)]),
     "fc_denoise_normals": (_i32, [_vp, _vp, _u32, _u32, _vp]),
     "fc_compute_ssao": (_i32, [_vp, _vp, _u32, _u32, _u32, _vp, _u32, _vp, _u32, _vp]),

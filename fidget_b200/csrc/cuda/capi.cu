@@ -140,6 +140,9 @@ void fc_ctx_destroy(fc_ctx* c) {
     c->fx_out.release();
     c->fx_tmp.release();
     c->fx_tables.release();
+    c->solve_meta.release();
+    c->solve_vals.release();
+    c->solve_res.release();
     for (auto& pb : c->tape_pool) cudaFree(pb.second);
     if (c->stage) cudaFreeHost(c->stage);
     if (c->stage_ev) cudaEventDestroy(c->stage_ev);

@@ -132,6 +132,7 @@ struct fc_ctx {
     DevBuf mesh_tree, mesh_herm, mesh_cells;                    // FC_FLAG_MESH_COLLAPSE: cell tree, Hermite records, final leaves
     uint32_t mesh_n_cells = 0;
     DevBuf fx_in, fx_out, fx_tmp, fx_tables;  // effects: staged host images, intermediate maps, SSAO tables
+    DevBuf solve_meta, solve_vals, solve_res; // fc_solve_batch: tape table + slot maps, staged host values / results
     // tile interleave: device list of this rank's XY root tiles (cached on its key), and the
     // tile -> gathered-slot table of fc_tiles_unpack
     DevBuf root_list, tile_slots;

@@ -167,9 +167,12 @@ class CudaShape:
             self._h = h
             self._axes = tape.var_slots()
             _ck(self._lib.fc_tape_set_axes(h, *self._axes))
+            # input slot -> ("x" | "y" | "z" | "v", var id): what fb.solve binds parameters by
+            self._vars = tape.vars()
         else:
             self._h = _handle
             self._axes = _axes
+            self._vars = None
         info = _lib.FcTapeInfo()
         _ck(self._lib.fc_tape_get_info(self._h, C.byref(info)))
         self.info = info
@@ -300,7 +303,23 @@ class CudaShape:
         c = np.ascontiguousarray(choices, dtype=np.uint8)
         h = C.c_void_p()
         _ck(self._lib.fc_simplify(self._ev(), self._h, _ptr(c), len(c), C.byref(h)))
-        return CudaShape(self.cuda, _handle=h, _axes=self._axes)
+        child = CudaShape(self.cuda, _handle=h, _axes=self._axes)
+        child._vars = self._vars
+        return child
+
+    def slot_keys(self) -> list:
+        """The variable behind each tape input slot: "x", "y", "z" or the var id of ``Context.var()``.  A shape
+        loaded from a blob knows only its axis slots, so another input raises ValueError."""
+        if self._vars is not None:
+            return [kind if kind in "xyz" else vid for kind, vid in self._vars]
+        keys = []
+        for s in range(self.n_vars):
+            if s in self._axes:
+                keys.append("xyz"[self._axes.index(s)])
+            else:
+                raise ValueError(f"input slot {s} is not an axis, and a shape loaded from a blob does not know which "
+                                 "Var it is; build the shape from its TapeData to solve with it")
+        return keys
 
 
 # ---------------------------------------------------------------------------
@@ -568,6 +587,72 @@ def mesh_cells(cuda) -> np.ndarray:
     out = np.zeros(n.value, dtype=MESH_CELL)
     _ck(lib.fc_mesh_read_cells(cuda._h, _ptr(out), n.value, C.byref(n)))
     return out[np.lexsort((out["ix"], out["iy"], out["iz"], out["depth"]))]
+
+
+# ---------------------------------------------------------------------------
+# Constraint solver (fidget-solver/src/lib.rs): fc_solve_batch
+@dataclass(frozen=True)
+class Free:
+    """``Parameter::Free``: a variable the solver moves, starting at ``value``."""
+    value: float
+
+
+@dataclass(frozen=True)
+class Fixed:
+    """``Parameter::Fixed``: a variable held at ``value``."""
+    value: float
+
+
+def solve_batch(constraints, free, fixed, values, max_iters=None):
+    """Levenberg-Marquardt least squares on the constraints' output 0, for many problems at once
+    (``fc_solve_batch``).  ``free`` / ``fixed``: the variable keys ("x", "y", "z" or ``Context.var()`` ids); the free
+    ones are the Jacobian's columns, in this order.  ``values``: [n_problems, len(free) + len(fixed)] starting values
+    of the free variables followed by the fixed ones -- a numpy array, or a CUDA torch tensor (the work and the
+    results then stay on the device).  ``max_iters``: step cap (default 1000).
+    Returns ``(values, status, iterations, err)``: a copy of ``values`` with the free entries solved, and per problem
+    the exit (``FC_SOLVE_*``), the number of steps and the final squared error."""
+    constraints = list(constraints)
+    if not constraints:
+        raise ValueError("solve_batch needs at least one constraint")
+    cuda = constraints[0].cuda
+    lib = cuda._lib
+    free, fixed = list(free), list(fixed)
+    keys = free + fixed
+    index = {k: i for i, k in enumerate(keys)}
+    if len(index) != len(keys):
+        raise ValueError("a variable is listed twice")
+    maps = [np.array([index.get(k, -1) for k in c.slot_keys()], dtype=np.int32) for c in constraints]
+    device = hasattr(values, "data_ptr") and values.is_cuda
+    if device:
+        import torch
+        vals = values.to(torch.float32).reshape(-1, len(keys)).contiguous().clone()
+        res = torch.zeros((vals.shape[0], 4), dtype=torch.int32, device=vals.device)
+        torch.cuda.current_stream(vals.device).synchronize()   # the library works on its own stream
+    else:
+        vals = np.array(values, dtype=np.float32, order="C", copy=True).reshape(-1, len(keys))
+        res = np.zeros((vals.shape[0], 4), dtype=np.int32)
+    tapes = (C.c_void_p * len(constraints))(*[c._h for c in constraints])
+    sp = (C.POINTER(C.c_int32) * len(maps))(*[m.ctypes.data_as(C.POINTER(C.c_int32)) for m in maps])
+    cfg = _lib.FcSolveCfg(len(keys), len(free), 0 if max_iters is None else int(max_iters))
+    _ck(lib.fc_solve_batch(cuda._h, tapes, len(constraints), sp, C.byref(cfg), _ptr(vals), int(vals.shape[0]),
+                           _ptr(res)))
+    if device:
+        import torch
+        return vals, res[:, 0].clone(), res[:, 1].clone(), res.view(torch.float32)[:, 2].clone()
+    return vals, res[:, 0].astype(np.uint32), res[:, 1].astype(np.uint32), res.view(np.float32)[:, 2].copy()
+
+
+def solve(constraints, params: dict, max_iters=None) -> dict:
+    """``fidget_solver::solve``: ``params`` maps variable keys ("x", "y", "z" or ``Context.var()`` ids) to
+    ``Free(start)`` / ``Fixed(value)``; returns {key: solved value} for the free ones."""
+    for k, p in params.items():
+        if not isinstance(p, (Free, Fixed)):
+            raise TypeError(f"parameter {k!r} must be Free(..) or Fixed(..), not {p!r}")
+    free = [k for k, p in params.items() if isinstance(p, Free)]
+    fixed = [k for k, p in params.items() if isinstance(p, Fixed)]
+    row = [params[k].value for k in free] + [params[k].value for k in fixed]
+    vals, _, _, _ = solve_batch(constraints, free, fixed, np.array([row], dtype=np.float32), max_iters)
+    return {k: float(vals[0, i]) for i, k in enumerate(free)}
 
 
 def pixel_inside(img: np.ndarray) -> np.ndarray:

@@ -331,6 +331,44 @@ int32_t fc_mesh_read_cells(fc_ctx* ctx, fc_mesh_cell* out, uint64_t cap, uint64_
  * buf == NULL queries the size (84 + 50 * n_triangles). */
 int32_t fc_mesh_write_stl(fc_ctx* ctx, uint8_t* buf, size_t cap, size_t* n_bytes);
 
+/* ---- constraint solver (fidget-solver) ----------------------------------------------------------------------- */
+/* fidget_solver::solve (fidget-solver/src/lib.rs:191-289) for a batch of independent problems that share their
+ * constraint tapes (multi-start solves, parameter sweeps, one sketch re-solved for many drag positions), the whole
+ * Levenberg-Marquardt loop of every problem in one launch.  Per problem exactly the reference's loop: the Jacobian
+ * from the gradient of output 0 of each constraint, damping 1.0 (x1.5 per rejected step, /3 per accepted one),
+ * delta = pinv(JtJ + damping diag(JtJ)) Jtr with eigenvalues |w| <= f32::EPSILON dropped, err = the sum of the
+ * squared constraint values in constraint order, and the reference's exits (FC_SOLVE_*).  Differences:
+ *  - the loop stops after max_iters steps (FC_SOLVE_MAX_ITERS); the reference's has no cap;
+ *  - every tape input slot must be bound to a parameter (FC_ERR_INVALID otherwise): the reference shares one input
+ *    buffer across its tapes, so an unbound slot would read whatever another tape last wrote there;
+ *  - Jacobian columns follow the caller's parameter order (the reference's come from HashMap iteration order);
+ *  - the pseudo-inverse is a cyclic Jacobi eigen-solve in f32 with a fixed operation order (the reference calls
+ *    nalgebra's SVD): results agree with the reference to rounding, and bit for bit with the project's CPU oracle.
+ * Limits (FC_ERR_UNSUPPORTED beyond them): n_free <= 64, n_constraints <= 256, n_params <= 1024, constraint tapes
+ * without memory slots.  n_free == 0 is FC_ERR_INVALID (the reference indexes an empty Jacobian).  Not cancellable. */
+#define FC_SOLVE_MAX_FREE 64
+#define FC_SOLVE_MAX_CONSTRAINTS 256
+#define FC_SOLVE_MAX_PARAMS 1024
+/* problem parameters: indices [0, n_free) are free (Parameter::Free), [n_free, n_params) fixed (Parameter::Fixed) */
+typedef struct fc_solve_cfg {
+    uint32_t n_params, n_free;
+    uint32_t max_iters;          /* 0 => 1000 */
+} fc_solve_cfg;
+#define FC_SOLVE_ZERO_RESIDUAL 0u /* every residual == 0 before a step */
+#define FC_SOLVE_UNCHANGED 1u     /* the step changed no free value */
+#define FC_SOLVE_ZERO_ERR 2u      /* the accepted step's error is 0 */
+#define FC_SOLVE_ZERO_DAMPING 3u  /* damping underflowed to 0 */
+#define FC_SOLVE_STALLED 4u       /* four equal errors in a row */
+#define FC_SOLVE_MAX_ITERS 5u     /* max_iters steps taken without another exit */
+/* iterations: steps applied to the free values; err: the last accepted step's error (0 for FC_SOLVE_ZERO_RESIDUAL) */
+typedef struct fc_solve_result { uint32_t status, iterations; float err; uint32_t pad; } fc_solve_result;
+/* slot_param[k]: n_vars(constraints[k]) entries, tape input slot -> parameter index (host arrays).
+ * values: [n_problems][n_params], host or device; free entries are overwritten with the solution.
+ * results: [n_problems], host or device, or NULL.  n_problems == 0 launches nothing. */
+int32_t fc_solve_batch(fc_ctx* ctx, const fc_tape* const* constraints, uint32_t n_constraints,
+                       const int32_t* const* slot_param, const fc_solve_cfg* cfg, float* values, uint64_t n_problems,
+                       fc_solve_result* results);
+
 /* ---- diagnostics ---------------------------------------------------------- */
 /* Host-only (no device needed): builds the level-0 schedule fc_tape_create would build for this
  * bytecode -- dependency waves, serial / chain tail segments, slot colouring -- and replays it

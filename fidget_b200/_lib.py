@@ -44,6 +44,10 @@ class FcRender2dCfg(C.Structure):
                 ("root_stride", C.c_uint32), ("root_offset", C.c_uint32), ("out_format", C.c_uint32)]
 
 
+class FcFrame2d(C.Structure):
+    _fields_ = [("mat", C.c_float * 16), ("z", C.c_float), ("n_var_values", C.c_uint32), ("var_values", C.c_float * 16)]
+
+
 class FcScheduleInfo(C.Structure):
     _fields_ = [(n, C.c_uint32) for n in ("suitable", "n_clauses", "n_waves", "widest_wave", "n_tail", "n_segments",
                                           "n_chain_clauses", "n_slots")]
@@ -119,6 +123,8 @@ FC_FLAG_FULL_LADDER = 32
 FC_FLAG_MESH_COLLAPSE = 64
 FC_OUT_F32, FC_OUT_MASK_U8, FC_OUT_BITMAP_1BIT, FC_OUT_RGBA8 = 0, 1, 2, 3
 FC_ERR_CANCELLED = -6
+FC_FRAMES_PASS_BYTES = 512 << 20
+FC_MAX_VARS = 16
 
 # name -> (restype, argtypes); mirrors include/fidget_cuda.h one to one
 _vp, _u32, _i32, _u64, _u8 = C.c_void_p, C.c_uint32, C.c_int32, C.c_uint64, C.c_uint8
@@ -149,6 +155,7 @@ CUDA_API = {
     "fc_grad_slice_eval": (_i32, [_vp, _vp, _P(_vp), _P(_vp), _u64]),
     "fc_simplify": (_i32, [_vp, _vp, _vp, C.c_size_t, _P(_vp)]),
     "fc_render2d": (_i32, [_vp, _vp, _P(FcRender2dCfg), _vp, _P(FcRenderStats)]),
+    "fc_render2d_frames": (_i32, [_vp, _vp, _P(FcRender2dCfg), _P(FcFrame2d), _u32, _vp, _P(FcRenderStats)]),
     "fc_render3d": (_i32, [_vp, _vp, _P(FcRender3dCfg), _vp, _P(FcRenderStats)]),
     "fc_merge_slabs": (_i32, [_vp, _P(_vp), _u32, _u32, _u32, _u32, _vp]),
     "fc_tiles_per_rank": (_u32, [_u32, _u32, _u32, _u32]),

@@ -143,6 +143,16 @@ void fc_ctx_destroy(fc_ctx* c) {
     c->solve_meta.release();
     c->solve_vals.release();
     c->solve_res.release();
+    c->frame_table.release();
+    c->frame_tops.release();
+    if (c->copy_stream) {
+        cudaStreamSynchronize(c->copy_stream);
+        cudaStreamDestroy(c->copy_stream);
+    }
+    for (int i = 0; i < 2; ++i) {
+        if (c->ev_pass[i]) cudaEventDestroy(c->ev_pass[i]);
+        if (c->ev_copied[i]) cudaEventDestroy(c->ev_copied[i]);
+    }
     for (auto& pb : c->tape_pool) cudaFree(pb.second);
     if (c->stage) cudaFreeHost(c->stage);
     if (c->stage_ev) cudaEventDestroy(c->stage_ev);

@@ -133,6 +133,11 @@ struct fc_ctx {
     uint32_t mesh_n_cells = 0;
     DevBuf fx_in, fx_out, fx_tmp, fx_tables;  // effects: staged host images, intermediate maps, SSAO tables
     DevBuf solve_meta, solve_vals, solve_res; // fc_solve_batch: tape table + slot maps, staged host values / results
+    // fc_render2d_frames: the frame table, each pass's arena high-water mark, and the copy stream that returns a pass's
+    // images to a host `out` while the next pass runs (ev_pass: pass k's images are complete; ev_copied: copied back)
+    DevBuf frame_table, frame_tops;
+    cudaStream_t copy_stream = nullptr;
+    cudaEvent_t ev_pass[2] = {}, ev_copied[2] = {};
     // tile interleave: device list of this rank's XY root tiles (cached on its key), and the
     // tile -> gathered-slot table of fc_tiles_unpack
     DevBuf root_list, tile_slots;
@@ -146,7 +151,8 @@ struct fc_ctx {
     void* stage = nullptr;
     size_t stage_cap = 0;
     cudaEvent_t stage_ev = nullptr;
-    struct { size_t smem; int per_sm, threads; } coop_memo[2] = {};   // level-0 launch shape per DIM (occupancy query cached)
+    // level-0 launch shape (occupancy query cached) per instantiation: 2D, 2D frame batch, 3D
+    struct { size_t smem; int per_sm, threads; } coop_memo[3] = {};
     std::shared_ptr<struct Sched> sched_cache[4];
     unsigned sched_next = 0;
     // cancellation (fc_ctx_set_cancel): the caller's flag; the device word kernels poll, written from pinned memory on

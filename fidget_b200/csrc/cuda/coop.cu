@@ -38,7 +38,7 @@ __device__ __forceinline__ Rec load_rec(const CoopRec* recs, uint32_t i) {
     return Rec(__ldg(reinterpret_cast<const uint4*>(recs) + i));
 }
 
-template <int DIM>
+template <int DIM, bool FRAMES = false>
 __global__ void __launch_bounds__(COOP_THREADS)
 k_interval_root_coop(const __grid_constant__ LevelParams p) {
     extern __shared__ __align__(16) unsigned char smem_raw[];
@@ -79,9 +79,12 @@ k_interval_root_coop(const __grid_constant__ LevelParams p) {
         uint32_t cx, cy, cz;
         root_corner(p, tile, T, cx, cy, cz);
         if (DIM != 3) cz = 0u;
+        const FrameView fv = frame_of<DIM == 2 && FRAMES>(p, cy);   // 2D frame batch
+        const VarBind& vb = *fv.vb;
         itv vx, vy, vz;
-        xform_iv(p.mat, iv(float(cx), float(cx) + float(T)), iv(float(cy), float(cy) + float(T)),
-                 DIM == 3 ? iv(float(cz), float(cz) + float(T)) : iv(p.z2d, p.z2d), vx, vy, vz);
+        xform_iv(*fv.mat, iv(float(cx), float(cx) + float(T)),
+                 iv(float(cy - fv.y0), float(cy - fv.y0) + float(T)),
+                 DIM == 3 ? iv(float(cz), float(cz) + float(T)) : iv(fv.z, fv.z), vx, vy, vz);
         auto put_choice = [&](uint32_t cidx, uint32_t c) {
             atomicOr(&chs[cidx >> 4], c << ((cidx & 15u) * 2u));
             if (c != 3u) s_nonboth = 1u;
@@ -120,7 +123,7 @@ k_interval_root_coop(const __grid_constant__ LevelParams p) {
                     } else if (d.op == OP_COPY) {
                         r = d.form == F_RI ? iv1(imm) : sl;
                     } else if (d.op == OP_INPUT) {
-                        r = pick_input(p.vb, rc.y, vx, vy, vz, [](float f) { return iv1(f); });
+                        r = pick_input(vb, rc.y, vx, vy, vz, [](float f) { return iv1(f); });
                     } else {
                         if (rc.y == 0) s_res = sl;
                         r = sl;
@@ -489,37 +492,44 @@ k_interval_root_coop(const __grid_constant__ LevelParams p) {
     }
 }
 
-template <int DIM>
+template <int DIM, bool FRAMES>
 static cudaError_t launch_coop(const LevelParams& p, int blocks, int threads, cudaStream_t s) {
     size_t smem = coop_smem_bytes(p.root_tape.n_ops, p.root_tape.n_choices, p.sched.n_slots);
-    static size_t configured = 0;
+    static size_t configured = 0;   // (per instantiation)
     if (smem > configured) {
-        cudaError_t e = cudaFuncSetAttribute(k_interval_root_coop<DIM>, cudaFuncAttributeMaxDynamicSharedMemorySize, int(smem));
+        cudaError_t e = cudaFuncSetAttribute(k_interval_root_coop<DIM, FRAMES>, cudaFuncAttributeMaxDynamicSharedMemorySize, int(smem));
         if (e != cudaSuccess) return e;
         // many small CTAs per SM: ask for the largest shared-memory carve-out
-        cudaFuncSetAttribute(k_interval_root_coop<DIM>, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared);
+        cudaFuncSetAttribute(k_interval_root_coop<DIM, FRAMES>, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared);
         configured = smem;
     }
-    k_interval_root_coop<DIM><<<blocks, threads, smem, s>>>(p);
+    k_interval_root_coop<DIM, FRAMES><<<blocks, threads, smem, s>>>(p);
     return cudaGetLastError();
 }
-int coop_occupancy(int dim, int threads, size_t smem) {
+// the instantiation a launch takes: DIM, and for 2D whether it renders a frame batch (its register count differs)
+static void (*coop_kernel(int dim, bool frames))(LevelParams) {
+    if (dim == 3) return k_interval_root_coop<3, false>;
+    return frames ? k_interval_root_coop<2, true> : k_interval_root_coop<2, false>;
+}
+int coop_occupancy(int dim, bool frames, int threads, size_t smem) {
     int n = 0;
-    if (dim == 3) cudaOccupancyMaxActiveBlocksPerMultiprocessor(&n, k_interval_root_coop<3>, threads, smem);
-    else cudaOccupancyMaxActiveBlocksPerMultiprocessor(&n, k_interval_root_coop<2>, threads, smem);
+    cudaOccupancyMaxActiveBlocksPerMultiprocessor(&n, coop_kernel(dim, frames), threads, smem);
     return n;
 }
-int coop_regs_per_thread(int dim) {
-    static int regs[2] = {0, 0};
-    int& r = regs[dim == 3];
+int coop_regs_per_thread(int dim, bool frames) {
+    static int regs[3] = {0, 0, 0};
+    int& r = regs[dim == 3 ? 2 : int(frames)];
     if (!r) {
         cudaFuncAttributes a{};
-        cudaError_t e = dim == 3 ? cudaFuncGetAttributes(&a, k_interval_root_coop<3>) : cudaFuncGetAttributes(&a, k_interval_root_coop<2>);
+        cudaError_t e = cudaFuncGetAttributes(&a, coop_kernel(dim, frames));
         r = e == cudaSuccess ? a.numRegs : 64;
     }
     return r;
 }
-cudaError_t launch_interval_root_coop_2d(const LevelParams& p, int blocks, int threads, cudaStream_t s) { return launch_coop<2>(p, blocks, threads, s); }
-cudaError_t launch_interval_root_coop_3d(const LevelParams& p, int blocks, int threads, cudaStream_t s) { return launch_coop<3>(p, blocks, threads, s); }
+// (a frame batch, p.frames != null, takes the instantiation that reads its frames from the table)
+cudaError_t launch_interval_root_coop_2d(const LevelParams& p, int blocks, int threads, cudaStream_t s) {
+    return p.frames ? launch_coop<2, true>(p, blocks, threads, s) : launch_coop<2, false>(p, blocks, threads, s);
+}
+cudaError_t launch_interval_root_coop_3d(const LevelParams& p, int blocks, int threads, cudaStream_t s) { return launch_coop<3, false>(p, blocks, threads, s); }
 
 }  // namespace fdev

@@ -31,7 +31,7 @@ namespace fdev {
 // painted later by k_fill_2d).  DIM = 3: voxel::render tiles; an
 // interval-proven-inside tile raises the heightmap to its top + 1
 // (voxel.rs:310-317), heightmap entries are (depth << 32 | leaf job id + 1).
-template <int DIM, bool FUSED_PATH = false>
+template <int DIM, bool FUSED_PATH = false, bool FRAMES = false>
 __global__ void __launch_bounds__(WARPS_PER_BLOCK * 32)
 k_interval_level(const __grid_constant__ LevelParams p) {
     __shared__ uint32_t live_s[WARPS_PER_BLOCK][8][32];
@@ -53,7 +53,7 @@ k_interval_level(const __grid_constant__ LevelParams p) {
         j = __shfl_sync(FULL, j, 0);
         if (j >= n_jobs) break;
 
-        level_job<DIM, FUSED_PATH>(p, j, n_roots, slots, cs, live_s[wib], lane, p.epoch);
+        level_job<DIM, FUSED_PATH, FRAMES>(p, j, n_roots, slots, cs, live_s[wib], lane, p.epoch);
     }
 }
 
@@ -61,7 +61,8 @@ void launch_interval_level_2d(const LevelParams& p, int blocks, cudaStream_t s) 
     // (diagnostic: FIDGET_B200_LEVEL_FUSED_PATH=1 runs the per-level launch with the code path of the fused tail --
     //  plain tape loads, published jobs, line-aligned arena slots -- to tell code-path cost from scheduling cost)
     static const bool fused_path = getenv("FIDGET_B200_LEVEL_FUSED_PATH") && atoi(getenv("FIDGET_B200_LEVEL_FUSED_PATH"));
-    if (fused_path && !p.root_mode) k_interval_level<2, true><<<blocks, WARPS_PER_BLOCK * 32, 0, s>>>(p);
+    if (p.frames) k_interval_level<2, false, true><<<blocks, WARPS_PER_BLOCK * 32, 0, s>>>(p);   // a frame batch
+    else if (fused_path && !p.root_mode) k_interval_level<2, true><<<blocks, WARPS_PER_BLOCK * 32, 0, s>>>(p);
     else k_interval_level<2><<<blocks, WARPS_PER_BLOCK * 32, 0, s>>>(p);
 }
 void launch_interval_level_3d(const LevelParams& p, int blocks, cudaStream_t s) {
@@ -336,7 +337,8 @@ void launch_tiles_copy(const void* src, void* dst, uint32_t width, uint32_t heig
 }
 
 // ---------------------------------------------------------------------------
-// K2: leaf pixels (2D)
+// K2: leaf pixels (2D); FRAMES: a frame batch (kernels.cuh, Frame2D)
+template <bool FRAMES>
 __global__ void __launch_bounds__(128) k_pixels_2d(const __grid_constant__ PixelParams p) {
     const int lane = threadIdx.x & 31;
     float2 slots[REG_SLOTS];
@@ -352,27 +354,29 @@ __global__ void __launch_bounds__(128) k_pixels_2d(const __grid_constant__ Pixel
         j = __shfl_sync(FULL, j, 0);
         if (j >= n_jobs) break;
         const TileJob* job = p.jobs + j;
-        const uint32_t cx = job->x, cy = job->y;
         const TapeRef tr = job->tape;
         const uint2* tape = tr.ptr;
+        const FrameView fv = frame_of<FRAMES>(p, job->y);   // (uniform over the warp: one tile, one frame)
+        const uint32_t cx = job->x, cy = job->y - fv.y0;
+        float* const out = p.out + size_t(fv.out_row0) * p.width;
         for (uint32_t base = 0; base < npix; base += 64u) {
             uint32_t p0 = base + lane, p1 = p0 + 32u;
             bool v0 = p0 < npix, v1 = p1 < npix;
             uint32_t i0 = (v0 ? p0 : 0u) % T, j0 = (v0 ? p0 : 0u) / T;
             uint32_t i1 = (v1 ? p1 : 0u) % T, j1 = (v1 ? p1 : 0u) / T;
             float x0, y0, z0, x1, y1, z1;
-            xform_f32(p.mat, float(cx + i0), float(cy + j0), p.z2d, x0, y0, z0);
-            xform_f32(p.mat, float(cx + i1), float(cy + j1), p.z2d, x1, y1, z1);
+            xform_f32(*fv.mat, float(cx + i0), float(cy + j0), fv.z, x0, y0, z0);
+            xform_f32(*fv.mat, float(cx + i1), float(cy + j1), fv.z, x1, y1, z1);
             const float2 X = make_float2(x0, x1), Y = make_float2(y0, y1), Z = make_float2(z0, z1);
             float2 r = run_f32x2(tape, tr.n_ops, slots, [&](uint32_t i) {
-                return pick_input(p.vb, i, X, Y, Z, [](float f) { return make_float2(f, f); });
+                return pick_input(*fv.vb, i, X, Y, Z, [](float f) { return make_float2(f, f); });
             });
             // RawDistancePixel::from(f32): canonical NaN (pixel.rs:234-240)
             if (r.x != r.x) r.x = nanf_();
             if (r.y != r.y) r.y = nanf_();
             uint32_t gx0 = cx + i0, gy0 = cy + j0, gx1 = cx + i1, gy1 = cy + j1;
-            if (v0 && gx0 < p.width && gy0 < p.height) p.out[size_t(gy0) * p.width + gx0] = r.x;
-            if (v1 && gx1 < p.width && gy1 < p.height) p.out[size_t(gy1) * p.width + gx1] = r.y;
+            if (v0 && gx0 < p.width && gy0 < p.height) out[size_t(gy0) * p.width + gx0] = r.x;
+            if (v1 && gx1 < p.width && gy1 < p.height) out[size_t(gy1) * p.width + gx1] = r.y;
             shaded += (v0 ? 1 : 0) + (v1 ? 1 : 0);
         }
     }
@@ -382,12 +386,16 @@ __global__ void __launch_bounds__(128) k_pixels_2d(const __grid_constant__ Pixel
     }
 }
 
-void launch_pixels_2d(const PixelParams& p, int blocks, cudaStream_t s) { k_pixels_2d<<<blocks, 128, 0, s>>>(p); }
+void launch_pixels_2d(const PixelParams& p, int blocks, cudaStream_t s) {
+    if (p.frames) k_pixels_2d<true><<<blocks, 128, 0, s>>>(p);
+    else k_pixels_2d<false><<<blocks, 128, 0, s>>>(p);
+}
 
 // ---------------------------------------------------------------------------
 // Fill painter: one warp per (record, unit of <= 1024 pixels).  Any tile edge T works: the last
 // unit of a tile may be partial, and tiles whose edge is not a multiple of four (a 4-pixel group
 // would straddle two rows) take the per-pixel path.
+template <bool FRAMES>
 __global__ void __launch_bounds__(256) k_fill_2d(const __grid_constant__ FillParams p) {
     const uint32_t n = *p.n_fills;
     const uint32_t T = p.tile;
@@ -405,24 +413,30 @@ __global__ void __launch_bounds__(256) k_fill_2d(const __grid_constant__ FillPar
         const FillRec fr = p.fills[rec];
         const float v = __uint_as_float(fr.value);
         const uint32_t first = u * unit_px;
+        // frame batch: the record's frame, its row inside the frame, and where that frame's rows start in `out`
+        const uint32_t f = FRAMES ? fr.y / p.frame_rows : 0u, fy = fr.y - f * p.frame_rows;
+        float* const out = p.out + size_t(f) * p.height * p.width;
         for (uint32_t q = lane * 4u; q < unit_px; q += 128u) {
             const uint32_t pix = first + q;
             if (pix >= tile_px) break;
             if (vec_ok) {   // T % 4 == 0: the group lies in one row, 16-byte aligned
-                const uint32_t x = fr.x + pix % T, y = fr.y + pix / T;
+                const uint32_t x = fr.x + pix % T, y = fy + pix / T;
                 if (y >= p.height || x >= p.width) continue;
-                *reinterpret_cast<float4*>(p.out + size_t(y) * p.width + x) = make_float4(v, v, v, v);   // width % 4 == 0
+                *reinterpret_cast<float4*>(out + size_t(y) * p.width + x) = make_float4(v, v, v, v);   // width % 4 == 0
             } else {
                 for (uint32_t k = 0; k < 4u && pix + k < tile_px; ++k) {
-                    const uint32_t x = fr.x + (pix + k) % T, y = fr.y + (pix + k) / T;
-                    if (x < p.width && y < p.height) p.out[size_t(y) * p.width + x] = v;
+                    const uint32_t x = fr.x + (pix + k) % T, y = fy + (pix + k) / T;
+                    if (x < p.width && y < p.height) out[size_t(y) * p.width + x] = v;
                 }
             }
         }
     }
 }
 
-void launch_fill_2d(const FillParams& p, int blocks, cudaStream_t s) { k_fill_2d<<<blocks, 256, 0, s>>>(p); }
+void launch_fill_2d(const FillParams& p, int blocks, cudaStream_t s) {
+    if (p.frame_rows != 0xffffffffu) k_fill_2d<true><<<blocks, 256, 0, s>>>(p);
+    else k_fill_2d<false><<<blocks, 256, 0, s>>>(p);
+}
 
 // ---------------------------------------------------------------------------
 // Trait-level evaluators

@@ -140,6 +140,17 @@ struct VarBind {
     float values[MAX_RENDER_VARS];
 };
 
+// One frame of a 2D frame batch (fc_render2d_frames): what fc_render2d takes from its cfg per call.  The batch's
+// tile grid stacks its frames vertically: frame k owns the grid rows [k * frame_rows, (k + 1) * frame_rows), where
+// frame_rows is the frame's height rounded up to whole root tiles, so no tile straddles two frames.  A tile's screen
+// coordinates are taken relative to its frame, and its frame's pixel rows land at k * height in the output.  A
+// single render is the batch of one frame with frame_rows = 0xffffffff and the frame in the launch parameters.
+struct Frame2D {
+    Mat4 mat;
+    float z;
+    VarBind vb;
+};
+
 struct LevelParams {
     CoopSched sched;
     int level;                 // index into tile sizes
@@ -192,6 +203,9 @@ struct LevelParams {
     uint32_t cap_census;
     VarBind vb;
     CancelRef cancel;
+    // 2D frame batch: the frame table (null: the one frame is mat / z2d / vb above) and the grid rows per frame
+    const Frame2D* frames;
+    uint32_t frame_rows;
 };
 
 #ifdef __CUDACC__
@@ -224,7 +238,29 @@ struct PixelParams {
     Stats* stats;
     VarBind vb;
     CancelRef cancel;
+    const Frame2D* frames;     // 2D frame batch, as in LevelParams
+    uint32_t frame_rows;
 };
+
+// The frame a 2D tile at grid row `y` belongs to: its parameters (in the launch parameters or the frame table),
+// the first grid row of its frame and the first output row of its frame
+struct FrameView {
+    const Mat4* mat;
+    float z;
+    const VarBind* vb;
+    uint32_t y0, out_row0;
+};
+#ifdef __CUDACC__
+// FRAMES is a compile-time switch: the kernels of a single fc_render2d (FRAMES = false) read their one frame from the
+// launch parameters exactly as before the frame dimension existed (a runtime choice cost 2.7 % on prospero 4096^2)
+template <bool FRAMES, class P>
+__device__ __forceinline__ FrameView frame_of(const P& p, uint32_t y) {
+    if (!FRAMES) return FrameView{&p.mat, p.z2d, &p.vb, 0u, 0u};
+    const uint32_t f = y / p.frame_rows;
+    const Frame2D* fr = p.frames + f;
+    return FrameView{&fr->mat, fr->z, &fr->vb, f * p.frame_rows, f * p.height};
+}
+#endif
 
 struct FillParams {
     uint32_t tile, width, height;
@@ -232,6 +268,7 @@ struct FillParams {
     const uint32_t* n_fills;
     float* out;
     CancelRef cancel;
+    uint32_t frame_rows;       // 2D frame batch: grid rows per frame (0xffffffff: one frame)
 };
 
 struct VoxelParams {
@@ -317,8 +354,9 @@ void launch_tiles_copy(const void* src, void* dst, uint32_t width, uint32_t heig
                        uint32_t roots_x, uint32_t roots_y, const uint32_t* slots, uint32_t n_ranks, uint32_t per_rank, int rank,
                        cudaStream_t s);
 void launch_interval_level_2d(const LevelParams& p, int blocks, cudaStream_t s);
-int coop_regs_per_thread(int dim);
-int coop_occupancy(int dim, int threads, size_t smem);
+// occupancy of the level-0 kernel instantiation a launch takes (frames: a 2D frame batch)
+int coop_regs_per_thread(int dim, bool frames);
+int coop_occupancy(int dim, bool frames, int threads, size_t smem);
 size_t coop_smem_bytes(uint32_t n_ops, uint32_t n_choices, uint32_t n_slots);
 cudaError_t launch_interval_root_coop_2d(const LevelParams& p, int blocks, int threads, cudaStream_t s);
 cudaError_t launch_interval_root_coop_3d(const LevelParams& p, int blocks, int threads, cudaStream_t s);

@@ -42,7 +42,7 @@ __device__ __forceinline__ void store_fill(FillRec* dst, const FillRec& fr) {
     *reinterpret_cast<uint4*>(dst) = make_uint4(fr.x, fr.y, fr.value, fr.ready);
 }
 
-template <int DIM, bool FUSED>
+template <int DIM, bool FUSED, bool FRAMES = false>
 __device__ __forceinline__ void level_job(const LevelParams& p, uint32_t j, uint32_t n_roots, itv* slots, uint32_t* cs,
                                           uint32_t (*live)[32], int lane, uint32_t epoch) {
     const uint32_t T = p.tile;
@@ -88,10 +88,14 @@ __device__ __forceinline__ void level_job(const LevelParams& p, uint32_t j, uint
             cy = py + ((cc / p.n_axis) % p.n_axis) * T;
             if (DIM == 3) cz = pz + (cc / (p.n_axis * p.n_axis)) * T;
         }
-        // Region in screen coordinates -> model space (pixel.rs:325-342, voxel.rs:291-306)
+        // Region in screen coordinates -> model space (pixel.rs:325-342, voxel.rs:291-306); a 2D tile's
+        // coordinates are relative to its frame (per lane at level 0, whose 32 roots may span frames)
+        const FrameView fv = frame_of<DIM == 2 && FRAMES>(p, cy);
+        const Mat4& M = *fv.mat;
+        const VarBind& vb = *fv.vb;
         itv X = iv(float(cx), float(cx) + float(T));
-        itv Y = iv(float(cy), float(cy) + float(T));
-        itv Z = DIM == 3 ? iv(float(cz), float(cz) + float(T)) : iv(p.z2d, p.z2d);
+        itv Y = iv(float(cy - fv.y0), float(cy - fv.y0) + float(T));
+        itv Z = DIM == 3 ? iv(float(cz), float(cz) + float(T)) : iv(fv.z, fv.z);
         itv vx, vy, vz;
         if (DIM == 3 && p.mode == 1u) {
             // octree cell bounds in world space (CellBounds::child, cell.rs:155-166): dyadic, exact in f32
@@ -102,7 +106,7 @@ __device__ __forceinline__ void level_job(const LevelParams& p, uint32_t j, uint
             if (p.has_transform) xform_iv(p.mat, X, Y, Z, vx, vy, vz);
             else { vx = X; vy = Y; vz = Z; }
         } else {
-            xform_iv(p.mat, X, Y, Z, vx, vy, vz);
+            xform_iv(M, X, Y, Z, vx, vy, vz);
         }
 
         if (DIM == 3 && cull_check && chunk == 0) {
@@ -116,7 +120,7 @@ __device__ __forceinline__ void level_job(const LevelParams& p, uint32_t j, uint
         itv r = iv_nan();
         run_interval<!FUSED>(
             tape, tr.n_ops, slots,
-            [&](uint32_t i) { return pick_input(p.vb, i, vx, vy, vz, [](float f) { return iv1(f); }); }, pk,
+            [&](uint32_t i) { return pick_input(vb, i, vx, vy, vz, [](float f) { return iv1(f); }); }, pk,
             [&](uint32_t oi, itv v) { if (oi == 0) r = v; });
         pk.finish();
 

@@ -72,24 +72,293 @@ int32_t root_subset(fc_ctx* c, uint32_t roots_x, uint32_t row0, uint32_t row1, u
     return FC_OK;
 }
 
+// Job and fill lists of a 2D render whose tile grid has n_roots root tiles: level_tiles[l] = worst-case jobs queued for
+// level l (tiles of edge ts[l - 1]), which is also the worst case of the fill records level l - 1 writes
+static int32_t size_lists_2d(const std::vector<uint32_t>& ts, uint64_t n_roots, std::vector<uint64_t>& level_tiles) {
+    const int L = int(ts.size());
+    level_tiles.assign(L + 1, 0);
+    for (int l = 1; l <= L; ++l) {
+        uint64_t per_root = uint64_t(ts[0] / ts[l - 1]) * (ts[0] / ts[l - 1]);
+        level_tiles[l] = n_roots * per_root;
+        if (level_tiles[l] > 0xfffffff0ull) return fail(FC_ERR_UNSUPPORTED, "image too large for 32-bit tile lists");
+    }
+    return FC_OK;
+}
+
+// The tile pipeline of fc_render2d (pixel::render), enqueued on `s`: the interval levels, the fills of every level
+// (on the auxiliary stream, joined back into `s`) and the leaf pixels, into the distance image `dimg`.  The grid is
+// roots_x x roots_y root tiles from root row row0 (or the listed ones, d_roots); with a frame table it stacks the
+// frames of a batch (frame_rows grid rows each), else it is the one frame of vb / cfg->mat / cfg->z.  The caller has
+// sized the scratch and zeroed the counters (and stats).
+struct Tiles2D {
+    std::vector<uint32_t> ts;
+    uint32_t roots_x = 0, roots_y = 0, row0 = 0;
+    const uint32_t* d_roots = nullptr;
+    uint32_t n_list = 0;
+    uint64_t n_roots = 0;
+    std::vector<uint64_t> level_tiles;
+    uint32_t choice_words = 0;
+    int grid_blocks = 0;
+    const Frame2D* frames = nullptr;
+    uint32_t frame_rows = 0xffffffffu;
+};
+static int32_t enqueue_tiles_2d(fc_ctx* c, const fc_tape* tape, const fc_render2d_cfg* cfg, const Tiles2D& g,
+                                const VarBind& vb, float* dimg, bool want_stats, bool timing, const CallCancel& cc,
+                                cudaStream_t s, size_t& ev, uint32_t& launches, bool& fused_out) {
+    const std::vector<uint32_t>& ts = g.ts;
+    const int L = int(ts.size());
+    const bool serial_fill = env_int("FIDGET_B200_SERIAL_FILL", 0) != 0;
+    if (timing) CU(cudaEventRecord(get_event(c, ev++), s));
+    if (++c->epoch == 0) c->epoch = 1;
+    // experimental (FC_FLAG_FUSED_TAIL): every level after the root level, the leaf pixels and the fills as ONE
+    // persistent launch draining a job queue (tail2d.cu); the default is one launch per stage
+    const bool fused = !g.frames && L >= 2 && L - 1 <= TAIL_MAX_LEVELS &&
+                       ((cfg->flags & FC_FLAG_FUSED_TAIL) || env_int("FIDGET_B200_FUSE", 0));
+    fused_out = fused;
+    Tail2DParams tail{};
+    for (int l = 0; l < L; ++l) {
+        LevelParams p{};
+        p.level = l;
+        p.epoch = c->epoch;
+        p.tile = ts[l];
+        p.n_axis = l ? ts[l - 1] / ts[l] : 0;
+        p.is_last = (l == L - 1);
+        p.pixel_perfect = cfg->pixel_perfect;
+        p.root_mode = (l == 0);
+        p.roots_x = g.roots_x; p.roots_y = g.roots_y; p.roots_z = 1;
+        p.root_x0 = 0; p.root_y0 = g.row0 * ts[0]; p.root_z0 = 0;
+        p.root_list = g.d_roots; p.n_root_list = g.n_list;
+        p.root_tape.ptr = tape->dev;
+        p.root_tape.n_ops = tape->info.n_ops;
+        p.root_tape.ref_len = tape->info.ref_len;
+        p.root_tape.n_choices = tape->info.choice_count;
+        p.width = cfg->width; p.height = cfg->height; p.depth = 1;
+        p.z2d = cfg->z;
+        memcpy(p.mat.m, cfg->mat, sizeof p.mat.m);
+        p.jobs_in = l ? c->jobs[l].as<TileJob>() : nullptr;
+        p.cap_in = l ? uint32_t(g.level_tiles[l]) : 0;
+        p.jobs_out = c->jobs[l + 1].as<TileJob>();
+        p.cap_out = uint32_t(g.level_tiles[l + 1]);
+        p.fills = c->fills[l].as<FillRec>();
+        p.cap_fills = uint32_t(g.level_tiles[l + 1]);
+        p.arena = c->arena.as<uint2>();
+        p.arena_cap = std::min<uint64_t>(c->arena.cap, c->arena_bytes) / sizeof(uint2);
+        p.choice_scratch = c->choice_scratch.as<uint32_t>();
+        p.choice_words = g.choice_words;
+        p.ctr = c->counters.as<Counters>();
+        p.stats = want_stats ? c->stats.as<Stats>() : nullptr;
+        p.vb = vb;
+        p.cancel = cc.ref;
+        p.frames = g.frames;
+        p.frame_rows = g.frame_rows;
+        if (fused) {
+            tail.fill_tile[l] = ts[l];
+            tail.fills[l] = c->fills[l].as<FillRec>();
+            tail.fill_cap[l] = uint32_t(g.level_tiles[l + 1]);
+            if (l) { tail.lv[l - 1] = p; continue; }
+        }
+        int blocks = g.grid_blocks;
+        if (l == 0) {
+            uint64_t warps = (g.n_roots + 31) / 32;
+            blocks = int(std::min<uint64_t>((warps + WARPS_PER_BLOCK - 1) / WARPS_PER_BLOCK, uint64_t(g.grid_blocks)));
+        }
+        bool coop = false;
+        if (l == 0) {
+            int ct = COOP_THREADS;
+            int cb = coop_blocks(c, tape, g.n_roots, p, 2, ct);
+            if (cb > 0) {
+                CU(launch_interval_root_coop_2d(p, cb, ct, s));
+                coop = true;
+            }
+        }
+        if (!coop) launch_interval_level_2d(p, std::max(blocks, 1), s);
+        ++launches;
+        if (timing) CU(cudaEventRecord(get_event(c, ev++), s));
+        if (!fused) {
+            // the tiles this level proved inside/outside are painted on a second stream while the
+            // next (latency-bound) levels run: fills and leaf pixels never touch the same pixel
+            FillParams f{};
+            f.tile = ts[l];
+            f.width = cfg->width; f.height = cfg->height;
+            f.fills = c->fills[l].as<FillRec>();
+            f.n_fills = &c->counters.as<Counters>()->n_fills[l];
+            f.out = dimg;
+            f.cancel = cc.ref;
+            f.frame_rows = g.frame_rows;
+            cudaStream_t fs = serial_fill ? s : c->aux_stream;
+            if (!serial_fill) {
+                CU(cudaEventRecord(c->ev_fork[l], s));
+                CU(cudaStreamWaitEvent(c->aux_stream, c->ev_fork[l], 0));
+            }
+            launch_fill_2d(f, c->sm_count * 2, fs);
+            ++launches;
+        }
+    }
+    if (timing) CU(cudaEventRecord(get_event(c, ev++), s));
+    {
+        PixelParams q{};
+        q.tile = ts[L - 1];
+        q.width = cfg->width; q.height = cfg->height;
+        q.z2d = cfg->z;
+        memcpy(q.mat.m, cfg->mat, sizeof q.mat.m);
+        q.jobs = c->jobs[L].as<TileJob>();
+        q.out = dimg;
+        q.ctr = c->counters.as<Counters>();
+        q.list = L;
+        q.cursor = L;
+        q.stats = want_stats ? c->stats.as<Stats>() : nullptr;
+        q.vb = vb;
+        q.cancel = cc.ref;
+        q.frames = g.frames;
+        q.frame_rows = g.frame_rows;
+        if (fused) {
+            tail.n_levels = L - 1;
+            tail.px = q;
+            tail.epoch = c->epoch;
+            tail.cancel = cc.ref;
+            tail.paint_fills = env_int("FIDGET_B200_TAIL_PAINTS", 0) ? 1 : 0;
+            auto paint = [&](int l, cudaStream_t fs) {
+                FillParams f{};
+                f.tile = ts[l];
+                f.width = cfg->width; f.height = cfg->height;
+                f.fills = c->fills[l].as<FillRec>();
+                f.n_fills = &c->counters.as<Counters>()->n_fills[l];
+                f.out = dimg;
+                f.cancel = cc.ref;
+                f.frame_rows = g.frame_rows;
+                launch_fill_2d(f, c->sm_count * 2, fs);
+                ++launches;
+            };
+            if (!tail.paint_fills) {   // level-0 fills are final already: paint them beside the tail
+                CU(cudaEventRecord(c->ev_fork[0], s));
+                CU(cudaStreamWaitEvent(c->aux_stream, c->ev_fork[0], 0));
+                paint(0, c->aux_stream);
+            }
+            CU(launch_tail_2d(tail, c->sm_count, s));
+            if (!tail.paint_fills) {
+                for (int l = 1; l < L; ++l) paint(l, s);
+                CU(cudaEventRecord(c->ev_join, c->aux_stream));
+                CU(cudaStreamWaitEvent(s, c->ev_join, 0));
+            }
+        } else {
+            launch_pixels_2d(q, c->sm_count * env_int("FIDGET_B200_PIXEL_BLOCKS_PER_SM", 8), s);
+        }
+        ++launches;
+    }
+    if (!serial_fill && !fused) {
+        CU(cudaEventRecord(c->ev_join, c->aux_stream));
+        CU(cudaStreamWaitEvent(s, c->ev_join, 0));
+    }
+    if (timing) CU(cudaEventRecord(get_event(c, ev++), s));
+    CU(cudaGetLastError());
+    return FC_OK;
+}
+
+// FC_FLAG_TIMING: stage times of the passes whose events start at `first` (L + 3 events per pass), added to `stage_ms`
+static void add_stage_ms_2d(fc_ctx* c, size_t first, int L, bool fused, const Stats& h, float* stage_ms) {
+    float ms = 0;
+    const cudaEvent_t* e = c->events.data() + first;
+    if (fused) {   // [0] = root level, [12] = the fused tail (levels 1.., leaf pixels, fills)
+        cudaEventElapsedTime(&ms, e[0], e[1]);
+        stage_ms[0] += ms;
+        cudaEventElapsedTime(&ms, e[1], e[3]);
+        stage_ms[12] += ms;
+        // when the last job of each list finished inside the fused launch (device clock, ms after its first warp):
+        // [1 .. L-1] interval levels, [L] leaf tiles, [13] level-0 fills .. (statistics of the experiment)
+        if (h.culled[0]) {
+            for (int k = 1; k <= 2 * (L - 1) + 2 && k < 8; ++k)
+                stage_ms[k] = h.culled[k] > h.culled[0] ? float(double(h.culled[k] - h.culled[0]) * 1e-6) : 0.0f;
+            // [8], [9]: latest start of a level-1 / level-2 job; [10], [11]: the longest such job
+            for (int k = 8; k <= 9; ++k)
+                stage_ms[k] = h.culled[k] > h.culled[0] ? float(double(h.culled[k] - h.culled[0]) * 1e-6) : 0.0f;
+            stage_ms[10] = float(double(h.culled[10]) * 1e-6);
+            stage_ms[11] = float(double(h.culled[11]) * 1e-6);
+        }
+        cudaEventElapsedTime(&ms, e[0], e[3]);
+        stage_ms[15] += ms;
+    } else {
+        for (int l = 0; l < L; ++l) {
+            cudaEventElapsedTime(&ms, e[l], e[l + 1]);
+            stage_ms[l] += ms;
+        }
+        cudaEventElapsedTime(&ms, e[L], e[L + 1]);
+        stage_ms[8] += ms;
+        cudaEventElapsedTime(&ms, e[L + 1], e[L + 2]);
+        stage_ms[9] += ms;
+        cudaEventElapsedTime(&ms, e[0], e[L + 2]);
+        stage_ms[15] += ms;
+    }
+}
+
+static void copy_census(const Stats& h, fc_render_stats* stats) {
+    for (int l = 0; l < FC_MAX_TILE_LEVELS; ++l) {
+        stats->evaluated[l] = h.evaluated[l];
+        stats->filled_inside[l] = h.filled_inside[l];
+        stats->filled_outside[l] = h.filled_outside[l];
+        stats->ambiguous[l] = h.ambiguous[l];
+        stats->simplified[l] = h.simplified[l];
+    }
+    stats->pixels = h.pixels;
+}
+
+// Validation and tile grid shared by fc_render2d and fc_render2d_frames
+static int32_t check_2d(const fc_tape* tape, const fc_render2d_cfg* cfg) {
+    if (cfg->width == 0 || cfg->height == 0) return fail(FC_ERR_INVALID, "empty image");
+    if (tape->info.mem_count) return fail(FC_ERR_UNSUPPORTED, "renderers need a tape without memory spills (<= 255 registers)");
+    if (tape->info.n_outputs != 1) return fail(FC_ERR_INVALID, "ShapeTape has multiple outputs");
+    return FC_OK;
+}
+static int32_t prepare_2d(fc_ctx* c, const fc_tape* tape, const fc_render2d_cfg* cfg, Tiles2D& g) {
+    static const uint32_t DFLT[3] = {128, 32, 8};
+    if (int32_t rc = pick_tile_sizes(cfg->tile_sizes, cfg->n_tile_sizes, DFLT, 3, std::max(cfg->width, cfg->height), g.ts))
+        return rc;
+    g.roots_x = (cfg->width + g.ts[0] - 1) / g.ts[0];
+    const int bps = env_int("FIDGET_B200_BLOCKS_PER_SM", 6);
+    g.grid_blocks = c->sm_count * bps;
+    g.choice_words = (tape->info.choice_count + 15) / 16 + 1;
+    return FC_OK;
+}
+// scratch of a pipeline over n_roots root tiles (level_tiles sized by the caller)
+static int32_t ensure_scratch_2d(fc_ctx* c, const Tiles2D& g) {
+    const int L = int(g.ts.size());
+    CU(c->choice_scratch.ensure(size_t(std::max(g.grid_blocks, tail_2d_blocks(c->sm_count))) * WARPS_PER_BLOCK * g.choice_words * 32 * 4));
+    CU(c->arena.ensure(c->arena_bytes));
+    CU(c->counters.ensure(sizeof(Counters)));
+    CU(c->stats.ensure(sizeof(Stats)));
+    for (int l = 1; l <= L; ++l) {
+        CU(c->jobs[l].ensure(g.level_tiles[l] * sizeof(TileJob)));
+        CU(c->fills[l - 1].ensure(g.level_tiles[l] * sizeof(FillRec)));
+    }
+    return FC_OK;
+}
+
+// bytes of one image of `fmt` (FC_OUT_*)
+static size_t format_bytes(uint32_t fmt, uint32_t width, uint32_t height) {
+    return fmt == FC_OUT_MASK_U8 ? size_t(width) * height
+         : fmt == FC_OUT_BITMAP_1BIT ? size_t((width + 7) / 8) * height
+         : size_t(width) * height * 4;
+}
+// the small formats, derived on the device from `rows` rows of distance image
+static void derive_format(uint32_t fmt, const float* dimg, uint32_t width, uint32_t rows, uint8_t* dst, cudaStream_t s) {
+    if (fmt == FC_OUT_RGBA8) launch_to_rgba(0, dimg, uint64_t(width) * rows, dst, s);
+    else launch_to_mask(dimg, width, rows, dst, fmt == FC_OUT_BITMAP_1BIT, s);
+}
+
 extern "C" {
 
 int32_t fc_render2d(fc_ctx* c, const fc_tape* tape, const fc_render2d_cfg* cfg, float* out, fc_render_stats* stats) {
     if (!c || !tape || !cfg || !out) return fail(FC_ERR_INVALID, "null argument");
-    if (cfg->width == 0 || cfg->height == 0) return fail(FC_ERR_INVALID, "empty image");
-    if (tape->info.mem_count) return fail(FC_ERR_UNSUPPORTED, "renderers need a tape without memory spills (<= 255 registers)");
-    if (tape->info.n_outputs != 1) return fail(FC_ERR_INVALID, "ShapeTape has multiple outputs");
+    if (int32_t vrc = check_2d(tape, cfg)) return vrc;
     CallCancel cc;
     if (int32_t crc = begin_call(c, cc)) return crc;
     std::lock_guard<std::mutex> guard(c->mu);
     CU(cudaSetDevice(c->device));
-    static const uint32_t DFLT[3] = {128, 32, 8};
-    std::vector<uint32_t> ts;
-    int32_t rc = pick_tile_sizes(cfg->tile_sizes, cfg->n_tile_sizes, DFLT, 3, std::max(cfg->width, cfg->height), ts);
+    Tiles2D g;
+    int32_t rc = prepare_2d(c, tape, cfg, g);
     if (rc) return rc;
-    const int L = int(ts.size());
-    const uint32_t T0 = ts[0];
-    const uint32_t roots_x = (cfg->width + T0 - 1) / T0;
+    const int L = int(g.ts.size());
+    const uint32_t T0 = g.ts[0];
+    const uint32_t roots_x = g.roots_x;
     uint32_t roots_y_all = (cfg->height + T0 - 1) / T0;
     uint32_t row0 = cfg->root_row_begin, row1 = cfg->root_row_end ? cfg->root_row_end : roots_y_all;
     if (row0 > row1 || row1 > roots_y_all) return fail(FC_ERR_INVALID, "bad root row band");
@@ -105,26 +374,13 @@ int32_t fc_render2d(fc_ctx* c, const fc_tape* tape, const fc_render2d_cfg* cfg, 
         if (!is_device_ptr(out)) return fail(FC_ERR_UNSUPPORTED, "tile-interleaved renders need a device image");
         if (int32_t lrc = root_subset(c, roots_x, row0, row1, cfg->root_stride, cfg->root_offset, s, &d_roots, &n_list)) return lrc;
     }
-    const uint64_t n_roots = d_roots ? uint64_t(n_list) : uint64_t(roots_x) * roots_y;
-    const bool serial_fill = env_int("FIDGET_B200_SERIAL_FILL", 0) != 0;
-
-    // ---- scratch ----
-    const int bps = env_int("FIDGET_B200_BLOCKS_PER_SM", 6);
-    const int grid_blocks = c->sm_count * bps;
-    const uint32_t choice_words = (tape->info.choice_count + 15) / 16 + 1;
-    CU(c->choice_scratch.ensure(size_t(std::max(grid_blocks, tail_2d_blocks(c->sm_count))) * WARPS_PER_BLOCK * choice_words * 32 * 4));
-    CU(c->arena.ensure(c->arena_bytes));
-    CU(c->counters.ensure(sizeof(Counters)));
-    CU(c->stats.ensure(sizeof(Stats)));
-    std::vector<uint64_t> level_tiles(L + 1);
-    for (int l = 1; l <= L; ++l) {
-        // jobs queued for level l are tiles of size ts[l-1]
-        uint64_t per_root = uint64_t(T0 / ts[l - 1]) * (T0 / ts[l - 1]);
-        level_tiles[l] = n_roots * per_root;
-        if (level_tiles[l] > 0xfffffff0ull) return fail(FC_ERR_UNSUPPORTED, "image too large for 32-bit tile lists");
-        CU(c->jobs[l].ensure(level_tiles[l] * sizeof(TileJob)));
-        CU(c->fills[l - 1].ensure(level_tiles[l] * sizeof(FillRec)));
-    }
+    g.roots_y = roots_y;
+    g.row0 = row0;
+    g.d_roots = d_roots;
+    g.n_list = n_list;
+    g.n_roots = d_roots ? uint64_t(n_list) : uint64_t(roots_x) * roots_y;
+    if (int32_t src = size_lists_2d(g.ts, g.n_roots, g.level_tiles)) return src;
+    if (int32_t erc = ensure_scratch_2d(c, g)) return erc;
     bool out_dev = is_device_ptr(out);
     float* dimg = out;
     const size_t img_bytes = size_t(cfg->width) * cfg->height * 4;
@@ -153,141 +409,9 @@ int32_t fc_render2d(fc_ctx* c, const fc_tape* tape, const fc_render2d_cfg* cfg, 
     VarBind vb;
     if (int32_t vrc = bind_vars(tape, cfg->var_values, cfg->n_var_values, vb)) return vrc;
     size_t ev = 0;
-    if (timing) CU(cudaEventRecord(get_event(c, ev++), s));
     uint32_t launches = 0;
-    if (++c->epoch == 0) c->epoch = 1;
-    // experimental (FC_FLAG_FUSED_TAIL): every level after the root level, the leaf pixels and the fills as ONE
-    // persistent launch draining a job queue (tail2d.cu); the default is one launch per stage
-    const bool fused = L >= 2 && L - 1 <= TAIL_MAX_LEVELS && ((cfg->flags & FC_FLAG_FUSED_TAIL) || env_int("FIDGET_B200_FUSE", 0));
-    Tail2DParams tail{};
-    for (int l = 0; l < L; ++l) {
-        LevelParams p{};
-        p.level = l;
-        p.epoch = c->epoch;
-        p.tile = ts[l];
-        p.n_axis = l ? ts[l - 1] / ts[l] : 0;
-        p.is_last = (l == L - 1);
-        p.pixel_perfect = cfg->pixel_perfect;
-        p.root_mode = (l == 0);
-        p.roots_x = roots_x; p.roots_y = roots_y; p.roots_z = 1;
-        p.root_x0 = 0; p.root_y0 = row0 * T0; p.root_z0 = 0;
-        p.root_list = d_roots; p.n_root_list = n_list;
-        p.root_tape.ptr = tape->dev;
-        p.root_tape.n_ops = tape->info.n_ops;
-        p.root_tape.ref_len = tape->info.ref_len;
-        p.root_tape.n_choices = tape->info.choice_count;
-        p.width = cfg->width; p.height = cfg->height; p.depth = 1;
-        p.z2d = cfg->z;
-        memcpy(p.mat.m, cfg->mat, sizeof p.mat.m);
-        p.jobs_in = l ? c->jobs[l].as<TileJob>() : nullptr;
-        p.cap_in = l ? uint32_t(level_tiles[l]) : 0;
-        p.jobs_out = c->jobs[l + 1].as<TileJob>();
-        p.cap_out = uint32_t(level_tiles[l + 1]);
-        p.fills = c->fills[l].as<FillRec>();
-        p.cap_fills = uint32_t(level_tiles[l + 1]);
-        p.arena = c->arena.as<uint2>();
-        p.arena_cap = std::min<uint64_t>(c->arena.cap, c->arena_bytes) / sizeof(uint2);
-        p.choice_scratch = c->choice_scratch.as<uint32_t>();
-        p.choice_words = choice_words;
-        p.ctr = c->counters.as<Counters>();
-        p.stats = want_stats ? c->stats.as<Stats>() : nullptr;
-        p.vb = vb;
-        p.cancel = cc.ref;
-        if (fused) {
-            tail.fill_tile[l] = ts[l];
-            tail.fills[l] = c->fills[l].as<FillRec>();
-            tail.fill_cap[l] = uint32_t(level_tiles[l + 1]);
-            if (l) { tail.lv[l - 1] = p; continue; }
-        }
-        int blocks = grid_blocks;
-        if (l == 0) {
-            uint64_t warps = (n_roots + 31) / 32;
-            blocks = int(std::min<uint64_t>((warps + WARPS_PER_BLOCK - 1) / WARPS_PER_BLOCK, uint64_t(grid_blocks)));
-        }
-        bool coop = false;
-        if (l == 0) {
-            int ct = COOP_THREADS;
-            int cb = coop_blocks(c, tape, n_roots, p, 2, ct);
-            if (cb > 0) {
-                CU(launch_interval_root_coop_2d(p, cb, ct, s));
-                coop = true;
-            }
-        }
-        if (!coop) launch_interval_level_2d(p, std::max(blocks, 1), s);
-        ++launches;
-        if (timing) CU(cudaEventRecord(get_event(c, ev++), s));
-        if (!fused) {
-            // the tiles this level proved inside/outside are painted on a second stream while the
-            // next (latency-bound) levels run: fills and leaf pixels never touch the same pixel
-            FillParams f{};
-            f.tile = ts[l];
-            f.width = cfg->width; f.height = cfg->height;
-            f.fills = c->fills[l].as<FillRec>();
-            f.n_fills = &c->counters.as<Counters>()->n_fills[l];
-            f.out = dimg;
-            f.cancel = cc.ref;
-            cudaStream_t fs = serial_fill ? s : c->aux_stream;
-            if (!serial_fill) {
-                CU(cudaEventRecord(c->ev_fork[l], s));
-                CU(cudaStreamWaitEvent(c->aux_stream, c->ev_fork[l], 0));
-            }
-            launch_fill_2d(f, c->sm_count * 2, fs);
-            ++launches;
-        }
-    }
-    if (timing) CU(cudaEventRecord(get_event(c, ev++), s));
-    {
-        PixelParams q{};
-        q.tile = ts[L - 1];
-        q.width = cfg->width; q.height = cfg->height;
-        q.z2d = cfg->z;
-        memcpy(q.mat.m, cfg->mat, sizeof q.mat.m);
-        q.jobs = c->jobs[L].as<TileJob>();
-        q.out = dimg;
-        q.ctr = c->counters.as<Counters>();
-        q.list = L;
-        q.cursor = L;
-        q.stats = want_stats ? c->stats.as<Stats>() : nullptr;
-        q.vb = vb;
-        q.cancel = cc.ref;
-        if (fused) {
-            tail.n_levels = L - 1;
-            tail.px = q;
-            tail.epoch = c->epoch;
-            tail.cancel = cc.ref;
-            tail.paint_fills = env_int("FIDGET_B200_TAIL_PAINTS", 0) ? 1 : 0;
-            auto paint = [&](int l, cudaStream_t fs) {
-                FillParams f{};
-                f.tile = ts[l];
-                f.width = cfg->width; f.height = cfg->height;
-                f.fills = c->fills[l].as<FillRec>();
-                f.n_fills = &c->counters.as<Counters>()->n_fills[l];
-                f.out = dimg;
-                f.cancel = cc.ref;
-                launch_fill_2d(f, c->sm_count * 2, fs);
-                ++launches;
-            };
-            if (!tail.paint_fills) {   // level-0 fills are final already: paint them beside the tail
-                CU(cudaEventRecord(c->ev_fork[0], s));
-                CU(cudaStreamWaitEvent(c->aux_stream, c->ev_fork[0], 0));
-                paint(0, c->aux_stream);
-            }
-            CU(launch_tail_2d(tail, c->sm_count, s));
-            if (!tail.paint_fills) {
-                for (int l = 1; l < L; ++l) paint(l, s);
-                CU(cudaEventRecord(c->ev_join, c->aux_stream));
-                CU(cudaStreamWaitEvent(s, c->ev_join, 0));
-            }
-        } else {
-            launch_pixels_2d(q, c->sm_count * env_int("FIDGET_B200_PIXEL_BLOCKS_PER_SM", 8), s);
-        }
-        ++launches;
-    }
-    if (!serial_fill && !fused) {
-        CU(cudaEventRecord(c->ev_join, c->aux_stream));
-        CU(cudaStreamWaitEvent(s, c->ev_join, 0));
-    }
-    if (timing) CU(cudaEventRecord(get_event(c, ev++), s));
+    bool fused = false;
+    if (int32_t erc = enqueue_tiles_2d(c, tape, cfg, g, vb, dimg, want_stats, timing, cc, s, ev, launches, fused)) return erc;
     CU(cudaGetLastError());
     const bool early_return = async && out_dev && !want_stats;
     if (cc.flag && !early_return) {   // a cancelled render derives no format and copies nothing to the host
@@ -297,15 +421,13 @@ int32_t fc_render2d(fc_ctx* c, const fc_tape* tape, const fc_render2d_cfg* cfg, 
         }
     }
     if (fmt != FC_OUT_F32) {
-        const size_t fb = fmt == FC_OUT_MASK_U8 ? size_t(cfg->width) * cfg->height
-                        : fmt == FC_OUT_BITMAP_1BIT ? size_t((cfg->width + 7) / 8) * cfg->height : img_bytes;
+        const size_t fb = format_bytes(fmt, cfg->width, cfg->height);
         uint8_t* dfmt = reinterpret_cast<uint8_t*>(out);
         if (!out_dev) {
             CU(c->fx_out.ensure(fb));
             dfmt = c->fx_out.as<uint8_t>();
         }
-        if (fmt == FC_OUT_RGBA8) launch_to_rgba(0, dimg, uint64_t(cfg->width) * cfg->height, dfmt, s);
-        else launch_to_mask(dimg, cfg->width, cfg->height, dfmt, fmt == FC_OUT_BITMAP_1BIT, s);
+        derive_format(fmt, dimg, cfg->width, cfg->height, dfmt, s);
         ++launches;
         CU(cudaGetLastError());
         if (!out_dev) CU(cudaMemcpyAsync(out, dfmt, fb, cudaMemcpyDeviceToHost, s));
@@ -327,49 +449,181 @@ int32_t fc_render2d(fc_ctx* c, const fc_tape* tape, const fc_render2d_cfg* cfg, 
         Counters hc;
         CU(cudaMemcpy(&h, c->stats.p, sizeof h, cudaMemcpyDeviceToHost));
         CU(cudaMemcpy(&hc, c->counters.p, sizeof hc, cudaMemcpyDeviceToHost));
-        for (int l = 0; l < FC_MAX_TILE_LEVELS; ++l) {
-            stats->evaluated[l] = h.evaluated[l];
-            stats->filled_inside[l] = h.filled_inside[l];
-            stats->filled_outside[l] = h.filled_outside[l];
-            stats->ambiguous[l] = h.ambiguous[l];
-            stats->simplified[l] = h.simplified[l];
-        }
-        stats->pixels = h.pixels;
+        copy_census(h, stats);
         stats->arena_bytes_used = hc.arena_top * sizeof(uint2);
         stats->kernel_launches = launches;
-        if (timing) {
-            float ms = 0;
-            if (fused) {   // [0] = root level, [12] = the fused tail (levels 1.., leaf pixels, fills)
-                cudaEventElapsedTime(&ms, c->events[0], c->events[1]);
-                stats->stage_ms[0] = ms;
-                cudaEventElapsedTime(&ms, c->events[1], c->events[3]);
-                stats->stage_ms[12] = ms;
-                // when the last job of each list finished inside the fused launch (device clock, ms after its first warp):
-                // [1 .. L-1] interval levels, [L] leaf tiles, [13] level-0 fills .. (statistics of the experiment)
-                if (h.culled[0]) {
-                    for (int k = 1; k <= 2 * (L - 1) + 2 && k < 8; ++k)
-                        stats->stage_ms[k] = h.culled[k] > h.culled[0] ? float(double(h.culled[k] - h.culled[0]) * 1e-6) : 0.0f;
-                    // [8], [9]: latest start of a level-1 / level-2 job; [10], [11]: the longest such job
-                    for (int k = 8; k <= 9; ++k)
-                        stats->stage_ms[k] = h.culled[k] > h.culled[0] ? float(double(h.culled[k] - h.culled[0]) * 1e-6) : 0.0f;
-                    stats->stage_ms[10] = float(double(h.culled[10]) * 1e-6);
-                    stats->stage_ms[11] = float(double(h.culled[11]) * 1e-6);
-                }
-                cudaEventElapsedTime(&ms, c->events[0], c->events[3]);
-                stats->stage_ms[15] = ms;
-            } else {
-                for (int l = 0; l < L; ++l) {
-                    cudaEventElapsedTime(&ms, c->events[l], c->events[l + 1]);
-                    stats->stage_ms[l] = ms;
-                }
-                cudaEventElapsedTime(&ms, c->events[L], c->events[L + 1]);
-                stats->stage_ms[8] = ms;
-                cudaEventElapsedTime(&ms, c->events[L + 1], c->events[L + 2]);
-                stats->stage_ms[9] = ms;
-                cudaEventElapsedTime(&ms, c->events[0], c->events[L + 2]);
-                stats->stage_ms[15] = ms;
-            }
+        if (timing) add_stage_ms_2d(c, 0, L, fused, h, stats->stage_ms);
+    }
+    return rc;
+}
+
+int32_t fc_render2d_frames(fc_ctx* c, const fc_tape* tape, const fc_render2d_cfg* cfg, const fc_frame2d* frames,
+                           uint32_t n_frames, void* out, fc_render_stats* stats) {
+    if (!c || !tape || !cfg || !out || (n_frames && !frames)) return fail(FC_ERR_INVALID, "null argument");
+    if (int32_t vrc = check_2d(tape, cfg)) return vrc;
+    if (cfg->flags & FC_FLAG_FUSED_TAIL) return fail(FC_ERR_UNSUPPORTED, "FC_FLAG_FUSED_TAIL is not supported by frame batches");
+    if (cfg->root_row_begin || cfg->root_row_end) return fail(FC_ERR_UNSUPPORTED, "root row bands are not supported by frame batches");
+    if (cfg->root_stride > 1) return fail(FC_ERR_UNSUPPORTED, "the tile interleave is not supported by frame batches");
+    const uint32_t fmt = cfg->out_format;
+    if (fmt > FC_OUT_RGBA8) return fail(FC_ERR_INVALID, "unknown out_format");
+    // every frame's ShapeVars binding, before anything is allocated or launched
+    std::vector<Frame2D> table(n_frames);
+    for (uint32_t k = 0; k < n_frames; ++k) {
+        if (frames[k].n_var_values > FC_MAX_VARS) return fail(FC_ERR_INVALID, "n_var_values above FC_MAX_VARS");
+        memcpy(table[k].mat.m, frames[k].mat, sizeof table[k].mat.m);
+        table[k].z = frames[k].z;
+        if (int32_t brc = bind_vars(tape, frames[k].var_values, frames[k].n_var_values, table[k].vb)) return brc;
+    }
+    CallCancel cc;
+    if (int32_t crc = begin_call(c, cc)) return crc;
+    if (stats) memset(stats, 0, sizeof *stats);
+    if (n_frames == 0) return FC_OK;
+    std::lock_guard<std::mutex> guard(c->mu);
+    CU(cudaSetDevice(c->device));
+    Tiles2D g;
+    if (int32_t rc = prepare_2d(c, tape, cfg, g)) return rc;
+    const int L = int(g.ts.size());
+    const uint32_t T0 = g.ts[0];
+    const uint32_t W = cfg->width, H = cfg->height;
+    const uint32_t roots_y = (H + T0 - 1) / T0;
+    const bool timing = (cfg->flags & FC_FLAG_TIMING) != 0;
+    const bool async = (cfg->flags & FC_FLAG_ASYNC) != 0;
+    const bool want_stats = stats != nullptr;
+    const bool out_dev = is_device_ptr(out);
+    cudaStream_t s = c->stream;
+
+    // ---- frames per pass: the worst-case lists of a frame plus its staged images, within FC_FRAMES_PASS_BYTES ----
+    std::vector<uint64_t> frame_tiles;
+    if (int32_t src = size_lists_2d(g.ts, uint64_t(g.roots_x) * roots_y, frame_tiles)) return src;
+    uint64_t per_frame = 0;
+    for (int l = 1; l <= L; ++l) per_frame += frame_tiles[l] * (sizeof(TileJob) + sizeof(FillRec));
+    const size_t img_f32 = size_t(W) * H * 4, img_fmt = format_bytes(fmt, W, H);
+    const bool stage_f32 = fmt != FC_OUT_F32 || !out_dev;             // the distance images live in the context
+    const int f32_bufs = fmt == FC_OUT_F32 ? 2 : 1;                    // (a host F32 copy-back is double-buffered)
+    if (stage_f32) per_frame += uint64_t(img_f32) * f32_bufs;
+    if (fmt != FC_OUT_F32 && !out_dev) per_frame += 2ull * img_fmt;    // double-buffered derived images
+    uint32_t per_pass = uint32_t(std::min<uint64_t>(n_frames, std::max<uint64_t>(1, FC_FRAMES_PASS_BYTES / per_frame)));
+    if (const int forced = env_int("FIDGET_B200_FRAMES_PER_PASS", 0); forced > 0) per_pass = std::min<uint32_t>(n_frames, forced);
+    const uint32_t n_passes = (n_frames + per_pass - 1) / per_pass;
+
+    g.roots_y = roots_y * per_pass;
+    g.n_roots = uint64_t(g.roots_x) * g.roots_y;
+    g.frame_rows = roots_y * T0;
+    if (int32_t src = size_lists_2d(g.ts, g.n_roots, g.level_tiles)) return src;
+    if (int32_t erc = ensure_scratch_2d(c, g)) return erc;
+    CU(c->frame_table.ensure(size_t(n_frames) * sizeof(Frame2D)));
+    CU(c->frame_tops.ensure(size_t(n_passes) * sizeof(unsigned long long)));
+    float* stage[2] = {nullptr, nullptr};
+    uint8_t* fstage[2] = {nullptr, nullptr};
+    if (stage_f32) {
+        CU(c->image.ensure(img_f32 * per_pass * f32_bufs));
+        stage[0] = c->image.as<float>();
+        stage[1] = stage[0] + (f32_bufs == 2 ? size_t(W) * H * per_pass : 0);
+    }
+    if (fmt != FC_OUT_F32 && !out_dev) {
+        CU(c->fx_out.ensure(img_fmt * per_pass * 2));
+        fstage[0] = c->fx_out.as<uint8_t>();
+        fstage[1] = fstage[0] + img_fmt * per_pass;
+    }
+    if (!out_dev && !c->copy_stream) {
+        CU(cudaStreamCreateWithFlags(&c->copy_stream, cudaStreamNonBlocking));
+        for (int i = 0; i < 2; ++i) {
+            CU(cudaEventCreateWithFlags(&c->ev_pass[i], cudaEventDisableTiming));
+            CU(cudaEventCreateWithFlags(&c->ev_copied[i], cudaEventDisableTiming));
         }
+    }
+    CU(cudaMemcpyAsync(c->frame_table.p, table.data(), table.size() * sizeof(Frame2D), cudaMemcpyHostToDevice, s));
+    CU(cudaMemsetAsync(c->counters.p, 0, sizeof(Counters), s));
+    if (want_stats) CU(cudaMemsetAsync(c->stats.p, 0, sizeof(Stats), s));
+
+    // host `out`: pass k's images go back on the copy stream while pass k + 1 runs (issued after pass k + 1 is
+    // enqueued, so that a copy into pageable memory, which blocks the host, still overlaps the next pass)
+    auto copy_back = [&](uint32_t k) -> int32_t {
+        const uint32_t f0 = k * per_pass, n = std::min(per_pass, n_frames - f0);
+        const size_t fb = fmt == FC_OUT_F32 ? img_f32 : img_fmt;
+        const void* src = fmt == FC_OUT_F32 ? static_cast<const void*>(stage[k & 1]) : static_cast<const void*>(fstage[k & 1]);
+        CU(cudaStreamWaitEvent(c->copy_stream, c->ev_pass[k & 1], 0));
+        // With a flag attached the host waits for pass k here, watching the flag (wait_call writes the cancel word the
+        // kernels of passes k and k + 1 poll), before it issues the copy: a copy into pageable memory blocks the host
+        // until it is done, and a blocked host could not cancel anything.  A cancelled pass copies nothing.
+        if (cc.flag)
+            if (int32_t wrc = wait_call(c, c->copy_stream, cc)) return wrc;
+        CU(cudaMemcpyAsync(static_cast<uint8_t*>(out) + size_t(f0) * fb, src, size_t(n) * fb, cudaMemcpyDeviceToHost, c->copy_stream));
+        CU(cudaEventRecord(c->ev_copied[k & 1], c->copy_stream));
+        return FC_OK;
+    };
+    // a call that stops early (cancelled, or a CUDA error) returns once its launched work has drained, stats zeroed
+    auto abandon = [&](int32_t rc) -> int32_t {
+        cudaStreamSynchronize(s);
+        cudaStreamSynchronize(c->copy_stream);
+        if (stats) memset(stats, 0, sizeof *stats);
+        return rc;
+    };
+    VarBind vb0 = table[0].vb;   // (unused by the kernels: every frame comes from the table)
+    size_t ev = 0;
+    uint32_t launches = 0, passes_run = 0;
+    for (uint32_t k = 0; k < n_passes; ++k) {
+        if (k && cc.flag && __atomic_load_n(cc.flag, __ATOMIC_ACQUIRE)) break;   // cancelled: enqueue no further pass
+        const uint32_t f0 = k * per_pass, n = std::min(per_pass, n_frames - f0);
+        Tiles2D gp = g;
+        gp.roots_y = roots_y * n;
+        gp.n_roots = uint64_t(g.roots_x) * gp.roots_y;
+        gp.frames = c->frame_table.as<Frame2D>() + f0;
+        if (k) {   // a new pass: fresh lists, cursors and arena; error bits accumulate over the call
+            CU(cudaMemsetAsync(c->counters.p, 0, offsetof(Counters, error), s));
+            CU(cudaMemsetAsync(&c->counters.as<Counters>()->arena_top, 0, sizeof(unsigned long long), s));
+        }
+        if (!out_dev && k >= 2) CU(cudaStreamWaitEvent(s, c->ev_copied[k & 1], 0));   // staging buffer k & 1 is free again
+        float* dimg = stage_f32 ? stage[k & 1] : static_cast<float*>(out) + size_t(f0) * W * H;
+        bool fused = false;
+        if (int32_t erc = enqueue_tiles_2d(c, tape, cfg, gp, vb0, dimg, want_stats, timing, cc, s, ev, launches, fused))
+            return erc;
+        if (fmt != FC_OUT_F32) {
+            uint8_t* dfmt = out_dev ? static_cast<uint8_t*>(out) + size_t(f0) * img_fmt : fstage[k & 1];
+            derive_format(fmt, dimg, W, H * n, dfmt, s);   // the pass's frames are one image of n * H rows
+            ++launches;
+            CU(cudaGetLastError());
+        }
+        if (want_stats)
+            CU(cudaMemcpyAsync(c->frame_tops.as<unsigned long long>() + k, &c->counters.as<Counters>()->arena_top,
+                               sizeof(unsigned long long), cudaMemcpyDeviceToDevice, s));
+        ++passes_run;
+        if (!out_dev) {
+            CU(cudaEventRecord(c->ev_pass[k & 1], s));
+            if (k) if (int32_t crc = copy_back(k - 1)) return abandon(crc);
+        }
+    }
+    if (!out_dev) {
+        if (int32_t crc = copy_back(passes_run - 1)) return abandon(crc);
+        CU(cudaStreamWaitEvent(s, c->ev_copied[(passes_run - 1) & 1], 0));   // the call ends when its last copy does
+    }
+    const bool early_return = async && out_dev && !want_stats;
+    if (early_return) {
+        c->async_call = cc;
+        return FC_OK;
+    }
+    if (cc.flag) {
+        if (int32_t wrc = wait_call(c, s, cc)) {
+            if (stats) memset(stats, 0, sizeof *stats);
+            return wrc;
+        }
+        if (passes_run < n_passes) {   // the flag stopped the passes, but was cleared before the wait saw it
+            if (stats) memset(stats, 0, sizeof *stats);
+            return fail(FC_ERR_CANCELLED, "cancelled");
+        }
+    }
+    CU(cudaStreamSynchronize(s));
+    int32_t rc = check_device_errors(c);
+    if (stats) {
+        Stats h;
+        std::vector<unsigned long long> tops(n_passes);
+        CU(cudaMemcpy(&h, c->stats.p, sizeof h, cudaMemcpyDeviceToHost));
+        CU(cudaMemcpy(tops.data(), c->frame_tops.p, tops.size() * sizeof(unsigned long long), cudaMemcpyDeviceToHost));
+        copy_census(h, stats);
+        stats->arena_bytes_used = *std::max_element(tops.begin(), tops.end()) * sizeof(uint2);
+        stats->kernel_launches = launches;
+        if (timing)
+            for (uint32_t k = 0; k < n_passes; ++k) add_stage_ms_2d(c, size_t(k) * (L + 3), L, false, h, stats->stage_ms);
     }
     return rc;
 }

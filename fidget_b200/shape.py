@@ -433,10 +433,7 @@ OUT_FORMATS = {"f32": _lib.FC_OUT_F32, "mask_u8": _lib.FC_OUT_MASK_U8, "bitmap_1
                "rgba8": _lib.FC_OUT_RGBA8}
 
 
-def render2d(shape: CudaShape, cfg: RenderConfig2D, out=None, stats: bool = False, asynchronous: bool = False):
-    """pixel::render.  ``out``: None (returns a numpy float32 [h,w] of
-    RawDistancePixel bits), a numpy array, or a CUDA torch tensor.  None when ``cfg.cancel`` cancelled it."""
-    lib = shape._lib
+def _render2d_cfg(cfg: RenderConfig2D, asynchronous: bool) -> _lib.FcRender2dCfg:
     c = _lib.FcRender2dCfg()
     c.width, c.height = cfg.width, cfg.height
     c.mat[:] = np.ascontiguousarray(cfg.matrix(), dtype=np.float32).reshape(16).tolist()
@@ -453,18 +450,116 @@ def render2d(shape: CudaShape, cfg: RenderConfig2D, out=None, stats: bool = Fals
     for i, v in enumerate(cfg.var_values):
         c.var_values[i] = float(v)
     c.out_format = OUT_FORMATS[cfg.out_format]
+    return c
+
+
+def _image_shape_2d(cfg: RenderConfig2D) -> tuple:
+    """Shape and dtype of one image of ``cfg.out_format``."""
+    if cfg.out_format == "f32":
+        return (cfg.height, cfg.width), np.float32
+    if cfg.out_format == "mask_u8":
+        return (cfg.height, cfg.width), np.uint8
+    if cfg.out_format == "bitmap_1bit":
+        return (cfg.height, (cfg.width + 7) // 8), np.uint8
+    return (cfg.height, cfg.width, 4), np.uint8
+
+
+def _check_out(out, need: int):
+    """A caller-given ``out`` must be one contiguous buffer of at least ``need`` bytes: the library writes that many."""
+    if hasattr(out, "data_ptr"):   # torch
+        contiguous, nbytes = out.is_contiguous(), out.numel() * out.element_size()
+    else:
+        contiguous, nbytes = out.flags["C_CONTIGUOUS"], out.nbytes
+    if not contiguous:
+        raise ValueError("out must be contiguous")
+    if nbytes < need:
+        raise ValueError(f"out holds {nbytes} bytes, the call writes {need}")
+
+
+def render2d(shape: CudaShape, cfg: RenderConfig2D, out=None, stats: bool = False, asynchronous: bool = False):
+    """pixel::render.  ``out``: None (returns a numpy float32 [h,w] of
+    RawDistancePixel bits), a numpy array, or a CUDA torch tensor.  None when ``cfg.cancel`` cancelled it."""
+    lib = shape._lib
+    c = _render2d_cfg(cfg, asynchronous)
     if out is None:
-        if cfg.out_format == "f32":
-            out = np.zeros((cfg.height, cfg.width), dtype=np.float32)
-        elif cfg.out_format == "mask_u8":
-            out = np.zeros((cfg.height, cfg.width), dtype=np.uint8)
-        elif cfg.out_format == "bitmap_1bit":
-            out = np.zeros((cfg.height, (cfg.width + 7) // 8), dtype=np.uint8)
-        else:
-            out = np.zeros((cfg.height, cfg.width, 4), dtype=np.uint8)
+        dims, dtype = _image_shape_2d(cfg)
+        out = np.zeros(dims, dtype=dtype)
     st = _lib.FcRenderStats() if stats else None
     rc = shape.cuda._cancellable(cfg.cancel, lambda: lib.fc_render2d(shape.cuda._h, shape._h, C.byref(c), _ptr(out),
                                                                      C.byref(st) if stats else None), asynchronous)
+    if rc == _lib.FC_ERR_CANCELLED:
+        return None
+    _ck(rc)
+    return (out, st.as_dict()) if stats else out
+
+
+def frame_table(cfg: RenderConfig2D, z=None, var_values=None, world_to_model=None, mats=None):
+    """The ``fc_frame2d`` table of ``render2d_frames``: frame k's matrix, Z and ShapeVars, each exactly what
+    ``render2d`` puts into ``fc_render2d_cfg`` for the config ``cfg`` with that frame's values.  Every argument
+    given is per frame (leading dimension n: ``z`` [n], ``var_values`` [n, k], ``world_to_model`` [n, 3, 3],
+    ``mats`` [n, 4, 4]); the others come from ``cfg``.  Lengths that disagree raise ValueError; with no per-frame
+    argument at all there is one frame.  ``mats`` and ``world_to_model`` are exclusive."""
+    if mats is not None and world_to_model is not None:
+        raise ValueError("give mats or world_to_model, not both")
+    per = {}
+    if z is not None:
+        per["z"] = np.asarray(z, dtype=np.float32).reshape(-1)
+    if var_values is not None:
+        vv = np.asarray(var_values, dtype=np.float32)
+        if vv.ndim != 2 or vv.shape[1] > _lib.FC_MAX_VARS:
+            raise ValueError(f"var_values must be [n, k] with k <= {_lib.FC_MAX_VARS}")
+        per["var_values"] = vv
+    if world_to_model is not None:
+        wm = np.asarray(world_to_model, dtype=np.float32)
+        if wm.ndim != 3 or wm.shape[1:] != (3, 3):
+            raise ValueError("world_to_model must be [n, 3, 3]")
+        per["world_to_model"] = wm
+    if mats is not None:
+        m = np.asarray(mats, dtype=np.float32)
+        if m.ndim != 3 or m.shape[1:] != (4, 4):
+            raise ValueError("mats must be [n, 4, 4]")
+        per["mats"] = m
+    lengths = {k: len(v) for k, v in per.items()}
+    if len(set(lengths.values())) > 1:
+        raise ValueError(f"per-frame arguments disagree in length: {lengths}")
+    n = next(iter(lengths.values())) if lengths else 1
+    table = (_lib.FcFrame2d * n)()
+    base = None if ("mats" in per or "world_to_model" in per) else \
+        np.ascontiguousarray(cfg.matrix(), dtype=np.float32).reshape(16).tolist()
+    for k in range(n):
+        f = table[k]
+        if "mats" in per:
+            f.mat[:] = per["mats"][k].reshape(16).tolist()
+        elif "world_to_model" in per:
+            f.mat[:] = pixel_mat(cfg.width, cfg.height, per["world_to_model"][k]).reshape(16).tolist()
+        else:
+            f.mat[:] = base
+        f.z = float(per["z"][k]) if "z" in per else cfg.z
+        values = per["var_values"][k] if "var_values" in per else cfg.var_values
+        f.n_var_values = len(values)
+        for i, v in enumerate(values):
+            f.var_values[i] = float(v)
+    return table
+
+
+def render2d_frames(shape: CudaShape, cfg: RenderConfig2D, z=None, var_values=None, world_to_model=None, mats=None,
+                    out=None, stats: bool = False, asynchronous: bool = False):
+    """Many frames of ``shape`` in one call (``fc_render2d_frames``): frame k is bit for bit ``render2d`` of ``cfg``
+    with frame k's ``z`` / ``var_values`` / ``world_to_model`` / ``mats`` (see ``frame_table``).  Returns a numpy
+    array [n, h, w] (f32, mask_u8), [n, h, (w + 7) // 8] (bitmap_1bit) or [n, h, w, 4] (rgba8), or fills ``out``
+    (a numpy array or CUDA tensor of that many bytes).  None when ``cfg.cancel`` cancelled it."""
+    lib = shape._lib
+    table = frame_table(cfg, z=z, var_values=var_values, world_to_model=world_to_model, mats=mats)
+    n = len(table)
+    c = _render2d_cfg(cfg, asynchronous)
+    dims, dtype = _image_shape_2d(cfg)
+    if out is None:
+        out = np.zeros((n,) + dims, dtype=dtype)
+    else:   # n frames of the format, back to back
+        _check_out(out, n * int(np.prod(dims)) * np.dtype(dtype).itemsize)
+    st = _lib.FcRenderStats() if stats else None
+    rc = shape.cuda._cancellable(cfg.cancel, lambda: lib.fc_render2d_frames(
+        shape.cuda._h, shape._h, C.byref(c), table, n, _ptr(out), C.byref(st) if stats else None), asynchronous)
     if rc == _lib.FC_ERR_CANCELLED:
         return None
     _ck(rc)

@@ -64,7 +64,7 @@ int32_t fc_ctx_set_arena_bytes(fc_ctx* ctx, uint64_t bytes);
 /* Cancellation (CancelToken, fidget-core/src/render/config.rs:59-80).  `flag` points to a caller-owned byte with the
  * layout of Rust's AtomicBool (CancelToken::into_raw() as *const u8): nonzero = cancelled.  The library reads it with
  * an acquire load, from any thread; NULL detaches it.  Context-wide, like fc_ctx_set_stream, and consulted only by
- * fc_render2d, fc_render3d, fc_octree_sample, fc_mesh_build, and fc_ctx_synchronize after the most recent
+ * fc_render2d, fc_render2d_frames, fc_render3d, fc_octree_sample, fc_mesh_build, and fc_ctx_synchronize after the most recent
  * FC_FLAG_ASYNC call of those.  With a flag attached:
  *  - set on entry: the call returns FC_ERR_CANCELLED before it allocates or launches anything;
  *  - set while the call runs: the kernels stop claiming work and the call returns FC_ERR_CANCELLED ("cancelled" in
@@ -242,6 +242,40 @@ typedef struct fc_render_stats {
  * RawDistancePixel bit patterns as f32, row-major; host or device. */
 int32_t fc_render2d(fc_ctx* ctx, const fc_tape* tape, const fc_render2d_cfg* cfg, float* out,
                     fc_render_stats* stats /* may be NULL */);
+
+/* Many 2D frames of one tape in one call: Z-slice stacks, ShapeVars sweeps, view sequences.  The reference has no
+ * batched call: frame k is pixel::render of its own RenderConfig, and here it is bit-identical to fc_render2d called
+ * with `cfg` plus frame k's mat, z and var_values (same device arithmetic, libm operations included), for every
+ * out_format and for pixel_perfect.  The frames of a pass share each launch of the tile pipeline, so every level
+ * launch holds the ambiguous tiles of all of them.
+ *  - cfg supplies what the frames share: width, height, pixel_perfect, tile_sizes, flags, out_format; its mat, z and
+ *    var_values are ignored.
+ *  - out (host or device) receives n_frames images back to back in fc_render2d's layout for out_format: frame k
+ *    starts at k * (one image's bytes).  A host out gets each pass's images while the next pass runs.
+ *  - stats: the per-level census and pixels summed over all frames (the sum of the per-frame fc_render2d stats),
+ *    arena_bytes_used the largest of any pass, stage_ms summed over passes.
+ *  - frames run in passes of as many as fit FC_FRAMES_PASS_BYTES of device memory: the worst-case job and fill lists
+ *    of a frame (4096^2 with {128,32,8}: 15.7 MB), plus its distance image (two with a host F32 out) when out_format
+ *    is not FC_OUT_F32 or out is on the host, plus two images of out_format with a host out.  The tape arena is
+ *    reset per pass; FC_ERR_ARENA if a pass exhausts it.
+ *  - n_frames == 0 launches nothing and returns FC_OK.  Errors follow fc_render2d (a spilled tape or more than 16
+ *    inputs: FC_ERR_UNSUPPORTED; a frame without a value for a bound variable: FC_ERR_INVALID).  FC_ERR_UNSUPPORTED
+ *    also for FC_FLAG_FUSED_TAIL, root row bands (root_row_begin / root_row_end) and the tile interleave
+ *    (root_stride > 1).
+ *  - FC_FLAG_ASYNC and the cancel flag (fc_ctx_set_cancel) behave as in fc_render2d; a cancelled call leaves `out`
+ *    unspecified.  With a flag attached and a host `out`, the host waits for each pass while watching the flag before
+ *    it copies that pass back (a copy into pageable memory would block it), so a flag set mid-call always stops the
+ *    work in flight. */
+#define FC_FRAMES_PASS_BYTES 536870912u   /* 512 MiB */
+typedef struct fc_frame2d {
+    float mat[16];                  /* row-major 4x4 screen -> model, as fc_render2d_cfg.mat */
+    float z;                        /* pixel::RenderConfig::z */
+    uint32_t n_var_values;          /* ShapeVars of this frame, as in fc_render2d_cfg */
+    float var_values[FC_MAX_VARS];
+} fc_frame2d;
+int32_t fc_render2d_frames(fc_ctx* ctx, const fc_tape* tape, const fc_render2d_cfg* cfg,
+                           const fc_frame2d* frames /* host */, uint32_t n_frames, void* out,
+                           fc_render_stats* stats /* may be NULL */);
 /* voxel::render (fidget-raster/src/voxel.rs:500-553).  out: width*height
  * GeometryPixel; host or device. */
 int32_t fc_render3d(fc_ctx* ctx, const fc_tape* tape, const fc_render3d_cfg* cfg, fc_geometry_pixel* out,

@@ -48,6 +48,10 @@ class FcFrame2d(C.Structure):
     _fields_ = [("mat", C.c_float * 16), ("z", C.c_float), ("n_var_values", C.c_uint32), ("var_values", C.c_float * 16)]
 
 
+class FcFrame3d(C.Structure):
+    _fields_ = [("mat", C.c_float * 16), ("n_var_values", C.c_uint32), ("var_values", C.c_float * 16)]
+
+
 class FcScheduleInfo(C.Structure):
     _fields_ = [(n, C.c_uint32) for n in ("suitable", "n_clauses", "n_waves", "widest_wave", "n_tail", "n_segments",
                                           "n_chain_clauses", "n_slots")]
@@ -157,6 +161,7 @@ CUDA_API = {
     "fc_render2d": (_i32, [_vp, _vp, _P(FcRender2dCfg), _vp, _P(FcRenderStats)]),
     "fc_render2d_frames": (_i32, [_vp, _vp, _P(FcRender2dCfg), _P(FcFrame2d), _u32, _vp, _P(FcRenderStats)]),
     "fc_render3d": (_i32, [_vp, _vp, _P(FcRender3dCfg), _vp, _P(FcRenderStats)]),
+    "fc_render3d_frames": (_i32, [_vp, _vp, _P(FcRender3dCfg), _P(FcFrame3d), _u32, _vp, _P(FcRenderStats)]),
     "fc_merge_slabs": (_i32, [_vp, _P(_vp), _u32, _u32, _u32, _u32, _vp]),
     "fc_tiles_per_rank": (_u32, [_u32, _u32, _u32, _u32]),
     "fc_tiles_pack": (_i32, [_vp, _vp, _u32, _u32, _u32, _u32, _u32, _u32, _vp]),

@@ -145,6 +145,7 @@ void fc_ctx_destroy(fc_ctx* c) {
     c->solve_res.release();
     c->frame_table.release();
     c->frame_tops.release();
+    if (c->pass_pin) cudaFreeHost(c->pass_pin);
     if (c->copy_stream) {
         cudaStreamSynchronize(c->copy_stream);
         cudaStreamDestroy(c->copy_stream);
@@ -280,9 +281,12 @@ int32_t check_device_errors(fc_ctx* c) {
     if (!c->counters.p) return FC_OK;
     Counters h;
     CU(cudaMemcpy(&h, c->counters.p, sizeof h, cudaMemcpyDeviceToHost));
-    if (h.error & 1u) return fail(FC_ERR_ARENA, "tape arena exhausted during on-device simplification; raise it with fc_ctx_set_arena_bytes");
-    if (h.error & 2u) return fail(FC_ERR_CUDA, "internal work list overflow");
-    if (h.error & 4u) return fail(FC_ERR_CUDA, "fused 2D kernel: a queued job never became ready (watchdog)");
+    return device_error(h.error);
+}
+int32_t device_error(uint32_t bits) {
+    if (bits & 1u) return fail(FC_ERR_ARENA, "tape arena exhausted during on-device simplification; raise it with fc_ctx_set_arena_bytes");
+    if (bits & 2u) return fail(FC_ERR_CUDA, "internal work list overflow");
+    if (bits & 4u) return fail(FC_ERR_CUDA, "fused 2D kernel: a queued job never became ready (watchdog)");
     return FC_OK;
 }
 extern "C" {

@@ -136,6 +136,8 @@ struct fc_ctx {
     // fc_render2d_frames: the frame table, each pass's arena high-water mark, and the copy stream that returns a pass's
     // images to a host `out` while the next pass runs (ev_pass: pass k's images are complete; ev_copied: copied back)
     DevBuf frame_table, frame_tops;
+    // fc_render3d_frames: each in-flight pass's counters and stats (two pinned host slots, one per staging buffer)
+    struct PassStatus* pass_pin = nullptr;
     cudaStream_t copy_stream = nullptr;
     cudaEvent_t ev_pass[2] = {}, ev_copied[2] = {};
     // tile interleave: device list of this rank's XY root tiles (cached on its key), and the
@@ -151,8 +153,8 @@ struct fc_ctx {
     void* stage = nullptr;
     size_t stage_cap = 0;
     cudaEvent_t stage_ev = nullptr;
-    // level-0 launch shape (occupancy query cached) per instantiation: 2D, 2D frame batch, 3D
-    struct { size_t smem; int per_sm, threads; } coop_memo[3] = {};
+    // level-0 launch shape (occupancy query cached) per instantiation: 2D, 2D frame batch, 3D, 3D frame batch
+    struct { size_t smem; int per_sm, threads; } coop_memo[4] = {};
     std::shared_ptr<struct Sched> sched_cache[4];
     unsigned sched_next = 0;
     // cancellation (fc_ctx_set_cancel): the caller's flag; the device word kernels poll, written from pinned memory on
@@ -164,6 +166,12 @@ struct fc_ctx {
     cudaEvent_t cancel_ev = nullptr;
     uint32_t call_id = 0;
     CallCancel async_call;                    // the last FC_FLAG_ASYNC call that returned before its work was done
+};
+
+// What the host reads of a finished pass of fc_render3d_frames: its counters (error bits, list and arena use) and stats
+struct PassStatus {
+    Counters ctr;
+    Stats st;
 };
 
 struct fc_tape {
@@ -207,6 +215,8 @@ void upload_schedule(fc_tape* t);
 int coop_blocks(fc_ctx* c, const fc_tape* tape, uint64_t n_roots, LevelParams& p, int dim, int& threads);
 // capi.cu
 int32_t check_device_errors(fc_ctx* c);
+// the error of a render's Counters::error bits (FC_OK for none)
+int32_t device_error(uint32_t bits);
 // Start of a cancellable call: FC_ERR_CANCELLED if the attached flag is already set, else `cc` for its kernels
 int32_t begin_call(fc_ctx* c, CallCancel& cc);
 // cudaStreamSynchronize(s) of a cancellable call.  With a flag attached it polls the work and the flag, writes the

@@ -79,7 +79,7 @@ k_interval_root_coop(const __grid_constant__ LevelParams p) {
         uint32_t cx, cy, cz;
         root_corner(p, tile, T, cx, cy, cz);
         if (DIM != 3) cz = 0u;
-        const FrameView fv = frame_of<DIM == 2 && FRAMES>(p, cy);   // 2D frame batch
+        const FrameView fv = frame_of<FRAMES>(p, cy);   // frame batch
         const VarBind& vb = *fv.vb;
         itv vx, vy, vz;
         xform_iv(*fv.mat, iv(float(cx), float(cx) + float(T)),
@@ -259,14 +259,14 @@ k_interval_root_coop(const __grid_constant__ LevelParams p) {
         const bool amb = !fill_in && !fill_out;
         if (DIM == 3 && fill_in) {   // voxel.rs:310-317
             const unsigned long long key = (unsigned long long)(cz + T + 1u) << 32;
-            for (uint32_t q = tid; q < T * T; q += NT) {
+            for (uint32_t q = tid; q < T * T; q += NT) {   // (frame batch: rows below the frame are its padding)
                 const uint32_t x = cx + q % T, y = cy + q / T;
-                if (x < p.width && y < p.height) atomicMax(&p.heightmap[size_t(y) * p.width + x], key);
+                if (x < p.width && y - fv.y0 < p.height) atomicMax(&p.heightmap[size_t(y) * p.width + x], key);
             }
             if (p.occl && T % 16u == 0u)
                 for (uint32_t q = tid; q < (T / 16u) * (T / 16u); q += NT) {
                     const uint32_t bx = cx / 16u + q % (T / 16u), by = cy / 16u + q / (T / 16u);
-                    if (bx < p.occl_w && by < p.occl_h) atomicMax(p.occl + size_t(by) * p.occl_w + bx, cz + T + 1u);
+                    if (bx < p.occl_w && by - fv.y0 / 16u < p.occl_h) atomicMax(p.occl + size_t(by) * p.occl_w + bx, cz + T + 1u);
                 }
         }
         if (tid == 0) {
@@ -506,9 +506,9 @@ static cudaError_t launch_coop(const LevelParams& p, int blocks, int threads, cu
     k_interval_root_coop<DIM, FRAMES><<<blocks, threads, smem, s>>>(p);
     return cudaGetLastError();
 }
-// the instantiation a launch takes: DIM, and for 2D whether it renders a frame batch (its register count differs)
+// the instantiation a launch takes: DIM, and whether it renders a frame batch (its register count differs)
 static void (*coop_kernel(int dim, bool frames))(LevelParams) {
-    if (dim == 3) return k_interval_root_coop<3, false>;
+    if (dim == 3) return frames ? k_interval_root_coop<3, true> : k_interval_root_coop<3, false>;
     return frames ? k_interval_root_coop<2, true> : k_interval_root_coop<2, false>;
 }
 int coop_occupancy(int dim, bool frames, int threads, size_t smem) {
@@ -517,8 +517,8 @@ int coop_occupancy(int dim, bool frames, int threads, size_t smem) {
     return n;
 }
 int coop_regs_per_thread(int dim, bool frames) {
-    static int regs[3] = {0, 0, 0};
-    int& r = regs[dim == 3 ? 2 : int(frames)];
+    static int regs[4] = {0, 0, 0, 0};
+    int& r = regs[(dim == 3 ? 2 : 0) + int(frames)];
     if (!r) {
         cudaFuncAttributes a{};
         cudaError_t e = cudaFuncGetAttributes(&a, coop_kernel(dim, frames));
@@ -530,6 +530,8 @@ int coop_regs_per_thread(int dim, bool frames) {
 cudaError_t launch_interval_root_coop_2d(const LevelParams& p, int blocks, int threads, cudaStream_t s) {
     return p.frames ? launch_coop<2, true>(p, blocks, threads, s) : launch_coop<2, false>(p, blocks, threads, s);
 }
-cudaError_t launch_interval_root_coop_3d(const LevelParams& p, int blocks, int threads, cudaStream_t s) { return launch_coop<3, false>(p, blocks, threads, s); }
+cudaError_t launch_interval_root_coop_3d(const LevelParams& p, int blocks, int threads, cudaStream_t s) {
+    return p.frames ? launch_coop<3, true>(p, blocks, threads, s) : launch_coop<3, false>(p, blocks, threads, s);
+}
 
 }  // namespace fdev

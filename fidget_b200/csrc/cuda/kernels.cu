@@ -66,13 +66,16 @@ void launch_interval_level_2d(const LevelParams& p, int blocks, cudaStream_t s) 
     else k_interval_level<2><<<blocks, WARPS_PER_BLOCK * 32, 0, s>>>(p);
 }
 void launch_interval_level_3d(const LevelParams& p, int blocks, cudaStream_t s) {
-    k_interval_level<3><<<blocks, WARPS_PER_BLOCK * 32, 0, s>>>(p);
+    if (p.frames) k_interval_level<3, false, true><<<blocks, WARPS_PER_BLOCK * 32, 0, s>>>(p);   // a frame batch
+    else k_interval_level<3><<<blocks, WARPS_PER_BLOCK * 32, 0, s>>>(p);
 }
 
 // ---------------------------------------------------------------------------
 // K2 (3D): leaf voxels.  One warp per leaf tile; each lane owns two XY columns
 // and walks Z front to back (k descending), two points per tape pass; the
-// warp stops as soon as every column has hit the surface (voxel.rs:359-447).
+// warp stops as soon as every column has hit the surface (voxel.rs:359-447).  FRAMES: a frame batch (the tile's
+// frame supplies matrix and vars; its screen rows are relative to the frame, its heightmap rows are grid rows).
+template <bool FRAMES>
 __global__ void __launch_bounds__(128) k_voxels_3d(const __grid_constant__ VoxelParams p) {
     const int lane = threadIdx.x & 31;
     float4 slots[REG_SLOTS];
@@ -93,13 +96,16 @@ __global__ void __launch_bounds__(128) k_voxels_3d(const __grid_constant__ Voxel
         const TapeRef tr = job->tape;
         const uint2* tape = tr.ptr;
         const unsigned long long id = (unsigned long long)(j + 1u);
+        const FrameView fv = frame_of<FRAMES>(p, cy);   // (uniform over the warp: one tile, one frame)
+        const Mat4& M = *fv.mat;
         for (uint32_t base = 0; base < ncol; base += 64u) {
             const uint32_t c0 = base + lane, c1 = c0 + 32u;
             const bool v0 = c0 < ncol, v1 = c1 < ncol;
             const uint32_t i0 = (v0 ? c0 : 0u) % T, j0 = (v0 ? c0 : 0u) / T;
             const uint32_t i1 = (v1 ? c1 : 0u) % T, j1 = (v1 ? c1 : 0u) / T;
             const uint32_t gx0 = cx + i0, gy0 = cy + j0, gx1 = cx + i1, gy1 = cy + j1;
-            const bool in0 = v0 && gx0 < p.width && gy0 < p.height, in1 = v1 && gx1 < p.width && gy1 < p.height;
+            const uint32_t sy0 = gy0 - fv.y0, sy1 = gy1 - fv.y0;   // rows inside the frame
+            const bool in0 = v0 && gx0 < p.width && sy0 < p.height, in1 = v1 && gx1 < p.width && sy1 < p.height;
             // columns already at or above this tile's top are skipped (voxel.rs:376-381)
             const uint32_t zmax = cz + T;
             bool done0 = !in0 || uint32_t(p.heightmap[size_t(gy0) * p.width + gx0] >> 32) >= zmax;
@@ -109,13 +115,13 @@ __global__ void __launch_bounds__(128) k_voxels_3d(const __grid_constant__ Voxel
                 if (__all_sync(FULL, done0 && done1)) break;
                 const int k2 = k > 0 ? k - 1 : 0;
                 float xa, ya, za, xb, yb, zb, xc, yc, zc, xd, yd, zd;
-                xform_f32(p.mat, float(gx0), float(gy0), float(cz + uint32_t(k)), xa, ya, za);
-                xform_f32(p.mat, float(gx1), float(gy1), float(cz + uint32_t(k)), xb, yb, zb);
-                xform_f32(p.mat, float(gx0), float(gy0), float(cz + uint32_t(k2)), xc, yc, zc);
-                xform_f32(p.mat, float(gx1), float(gy1), float(cz + uint32_t(k2)), xd, yd, zd);
+                xform_f32(M, float(gx0), float(sy0), float(cz + uint32_t(k)), xa, ya, za);
+                xform_f32(M, float(gx1), float(sy1), float(cz + uint32_t(k)), xb, yb, zb);
+                xform_f32(M, float(gx0), float(sy0), float(cz + uint32_t(k2)), xc, yc, zc);
+                xform_f32(M, float(gx1), float(sy1), float(cz + uint32_t(k2)), xd, yd, zd);
                 const float4 X = make_float4(xa, xb, xc, xd), Y = make_float4(ya, yb, yc, yd), Z = make_float4(za, zb, zc, zd);
                 const float4 r = run_f32x4(tape, tr.n_ops, slots, [&](uint32_t i) {
-                    return pick_input(p.vb, i, X, Y, Z, [](float f) { return make_float4(f, f, f, f); });
+                    return pick_input(*fv.vb, i, X, Y, Z, [](float f) { return make_float4(f, f, f, f); });
                 });
                 const unsigned long long key_hi = ((unsigned long long)(cz + uint32_t(k) + 1u) << 32) | id;
                 const unsigned long long key_lo = ((unsigned long long)(cz + uint32_t(k2) + 1u) << 32) | id;
@@ -138,7 +144,10 @@ __global__ void __launch_bounds__(128) k_voxels_3d(const __grid_constant__ Voxel
         if (lane == 0 && shaded) atomicAdd(&p.stats->pixels, shaded);
     }
 }
-void launch_voxels_3d(const VoxelParams& p, int blocks, cudaStream_t s) { k_voxels_3d<<<blocks, 128, 0, s>>>(p); }
+void launch_voxels_3d(const VoxelParams& p, int blocks, cudaStream_t s) {
+    if (p.frames) k_voxels_3d<true><<<blocks, 128, 0, s>>>(p);
+    else k_voxels_3d<false><<<blocks, 128, 0, s>>>(p);
+}
 
 // Front-to-back ordering of the leaf tiles (the reference walks Z descending, voxel.rs:244-263,
 // 335-351): a counting sort by Z layer, front layer first.
@@ -224,7 +233,9 @@ void launch_census_3d(const CensusParams& p, int blocks, cudaStream_t s) { k_cen
 // K3: normals + final image.  One thread per pixel; the gradient is evaluated
 // at the surface voxel (x, y, depth - 1) with the tape of the
 // leaf tile that found it (voxel.rs:449-481); lanes of a warp that share a
-// leaf tile run its tape together.
+// leaf tile run its tape together.  FRAMES: a frame batch, whose output row y is row y % height of frame
+// y / height (a patch may straddle two frames: each lane takes its own frame's matrix and vars).
+template <bool FRAMES>
 __global__ void __launch_bounds__(128) k_normals_3d(const __grid_constant__ NormalParams p) {
     grd slots[REG_SLOTS];
     const int lane = threadIdx.x & 31;
@@ -245,7 +256,17 @@ __global__ void __launch_bounds__(128) k_normals_3d(const __grid_constant__ Norm
         y = p.y0 + (warp / patches_x) * 4u + (lane >> 3);
     }
     const bool inb = x < p.width && y < p.y1;
-    const unsigned long long key = inb ? p.heightmap[size_t(y) * p.width + x] : 0ull;
+    uint32_t sy = y, hy = y;   // row inside the frame, heightmap row
+    const Mat4* M = &p.mat;
+    const VarBind* vb = &p.vb;
+    if (FRAMES) {
+        const uint32_t f = inb ? y / p.height : 0u;
+        sy = y - f * p.height;
+        hy = f * p.frame_rows + sy;
+        M = &p.frames[f].mat;
+        vb = &p.frames[f].vb;
+    }
+    const unsigned long long key = inb ? p.heightmap[size_t(hy) * p.width + x] : 0ull;
     const uint32_t depth = uint32_t(key >> 32), id = uint32_t(key);
     grd g = gr(0.0f, 0.0f, 0.0f, 0.0f);
     bool pending = inb && id != 0u;
@@ -258,10 +279,10 @@ __global__ void __launch_bounds__(128) k_normals_3d(const __grid_constant__ Norm
         const TileJob* job = p.jobs + (lead_id - 1u);
         const TapeRef tr = job->tape;
         grd gx, gy, gz;
-        xform_gr(p.mat, gr(float(x), 1.0f, 0.0f, 0.0f), gr(float(y), 0.0f, 1.0f, 0.0f),
+        xform_gr(*M, gr(float(x), 1.0f, 0.0f, 0.0f), gr(float(sy), 0.0f, 1.0f, 0.0f),
                  gr(float(depth - 1u), 0.0f, 0.0f, 1.0f), gx, gy, gz);
         const grd r = run_grad(tr.ptr, tr.n_ops, slots, [&](uint32_t i) {
-            return pick_input(p.vb, i, gx, gy, gz, [](float f) { return gr1(f); });
+            return pick_input(*vb, i, gx, gy, gz, [](float f) { return gr1(f); });
         });
         if (mine) { g = r; pending = false; ++n; }
     }
@@ -283,7 +304,8 @@ void launch_normals_3d(const NormalParams& p, cudaStream_t s) {
     const uint64_t warps = p.root_list ? uint64_t(p.n_root_list) * (p.root_tile / 8u) * (p.root_tile / 4u)
                                        : uint64_t((p.width + 7u) / 8u) * ((p.y1 - p.y0 + 3u) / 4u);
     if (!warps) return;
-    k_normals_3d<<<unsigned((warps + 3) / 4), 128, 0, s>>>(p);
+    if (p.frames) k_normals_3d<true><<<unsigned((warps + 3) / 4), 128, 0, s>>>(p);
+    else k_normals_3d<false><<<unsigned((warps + 3) / 4), 128, 0, s>>>(p);
 }
 
 // Multi-GPU: per-pixel merge of Z-ordered slab images; the highest slab with

@@ -145,6 +145,8 @@ struct VarBind {
 // frame_rows is the frame's height rounded up to whole root tiles, so no tile straddles two frames.  A tile's screen
 // coordinates are taken relative to its frame, and its frame's pixel rows land at k * height in the output.  A
 // single render is the batch of one frame with frame_rows = 0xffffffff and the frame in the launch parameters.
+// A 3D frame batch (fc_render3d_frames) uses the same table with z unused: its frames stack their XY root rows the
+// same way (the Z layers are shared), and its heightmap and occlusion map hold frame_rows rows per frame.
 struct Frame2D {
     Mat4 mat;
     float z;
@@ -203,7 +205,8 @@ struct LevelParams {
     uint32_t cap_census;
     VarBind vb;
     CancelRef cancel;
-    // 2D frame batch: the frame table (null: the one frame is mat / z2d / vb above) and the grid rows per frame
+    // frame batch (2D or 3D): the frame table (null: the one frame is mat / z2d / vb above) and the grid rows per
+    // frame; 3D: occl_h counts the block rows of one frame, and frame k's blocks start at row k * frame_rows / 16
     const Frame2D* frames;
     uint32_t frame_rows;
 };
@@ -251,11 +254,15 @@ struct FrameView {
     uint32_t y0, out_row0;
 };
 #ifdef __CUDACC__
-// FRAMES is a compile-time switch: the kernels of a single fc_render2d (FRAMES = false) read their one frame from the
-// launch parameters exactly as before the frame dimension existed (a runtime choice cost 2.7 % on prospero 4096^2)
+// FRAMES is a compile-time switch: the kernels of a single fc_render2d / fc_render3d (FRAMES = false) read their one
+// frame from the launch parameters exactly as before the frame dimension existed (a runtime choice cost 2.7 % on
+// prospero 4096^2).  (3D launch parameters have no z2d: their FrameView.z is 0 and unused.)
+template <class P> __device__ __forceinline__ float single_z(const P&) { return 0.0f; }
+__device__ __forceinline__ float single_z(const LevelParams& p) { return p.z2d; }
+__device__ __forceinline__ float single_z(const PixelParams& p) { return p.z2d; }
 template <bool FRAMES, class P>
 __device__ __forceinline__ FrameView frame_of(const P& p, uint32_t y) {
-    if (!FRAMES) return FrameView{&p.mat, p.z2d, &p.vb, 0u, 0u};
+    if (!FRAMES) return FrameView{&p.mat, single_z(p), &p.vb, 0u, 0u};
     const uint32_t f = y / p.frame_rows;
     const Frame2D* fr = p.frames + f;
     return FrameView{&fr->mat, fr->z, &fr->vb, f * p.frame_rows, f * p.height};
@@ -283,6 +290,8 @@ struct VoxelParams {
     Stats* stats;
     VarBind vb;
     CancelRef cancel;
+    const Frame2D* frames;      // 3D frame batch, as in LevelParams (job y is a grid row; the heightmap has its rows)
+    uint32_t frame_rows;
 };
 struct NormalParams {
     uint32_t width, height, depth;
@@ -298,6 +307,10 @@ struct NormalParams {
     Stats* stats;
     VarBind vb;
     CancelRef cancel;
+    // 3D frame batch: rows y0 .. y1 are output rows of the stacked frames (frame k's row y is k * height + y, its
+    // heightmap row k * frame_rows + y), each frame with its matrix and vars from the table
+    const Frame2D* frames;
+    uint32_t frame_rows;
 };
 
 // One leaf of the Manifold-Dual-Contouring octree (LeafHermiteData, fidget-mesh/src/octree.rs:864-900)

@@ -67,9 +67,10 @@ __device__ __forceinline__ void level_job(const LevelParams& p, uint32_t j, uint
             // tiles in its front-to-back walk (voxel.rs:283-293) -- and more, since it also knows the voxel hits in
             // front, which arrive last here.  One small read of the occlusion map per lane, not the heightmap itself.
             const uint32_t nb = (T * p.n_axis) / 16u, need = pz + T * p.n_axis + 1u;   // blocks per side of the parent
+            const uint32_t fb0 = frame_of<FRAMES>(p, py).y0 / 16u;                      // (frame batch: its first block row)
             for (uint32_t q = lane; q < nb * nb; q += 32u) {
                 const uint32_t bx = px / 16u + q % nb, by = py / 16u + q / nb;
-                if (bx < p.occl_w && by < p.occl_h) cull_open |= __ldcg(p.occl + size_t(by) * p.occl_w + bx) < need;
+                if (bx < p.occl_w && by - fb0 < p.occl_h) cull_open |= __ldcg(p.occl + size_t(by) * p.occl_w + bx) < need;
             }
             cull_check = true;
         }
@@ -88,9 +89,9 @@ __device__ __forceinline__ void level_job(const LevelParams& p, uint32_t j, uint
             cy = py + ((cc / p.n_axis) % p.n_axis) * T;
             if (DIM == 3) cz = pz + (cc / (p.n_axis * p.n_axis)) * T;
         }
-        // Region in screen coordinates -> model space (pixel.rs:325-342, voxel.rs:291-306); a 2D tile's
-        // coordinates are relative to its frame (per lane at level 0, whose 32 roots may span frames)
-        const FrameView fv = frame_of<DIM == 2 && FRAMES>(p, cy);
+        // Region in screen coordinates -> model space (pixel.rs:325-342, voxel.rs:291-306); in a frame batch a
+        // tile's coordinates are relative to its frame (per lane at level 0, whose 32 roots may span frames)
+        const FrameView fv = frame_of<FRAMES>(p, cy);
         const Mat4& M = *fv.mat;
         const VarBind& vb = *fv.vb;
         itv X = iv(float(cx), float(cx) + float(T));
@@ -137,14 +138,16 @@ __device__ __forceinline__ void level_job(const LevelParams& p, uint32_t j, uint
                 const uint32_t fx = __shfl_sync(FULL, cx, src), fy = __shfl_sync(FULL, cy, src),
                                fz = __shfl_sync(FULL, cz, src);
                 const unsigned long long key = (unsigned long long)(fz + T + 1u) << 32;
+                // (frame batch: rows past the bottom of the tile's frame are its padding, not the next frame's image)
+                const uint32_t fy0 = frame_of<FRAMES>(p, fy).y0;
                 for (uint32_t q = lane; q < T * T; q += 32u) {
                     const uint32_t x = fx + q % T, y = fy + q / T;
-                    if (x < p.width && y < p.height) atomicMax(&p.heightmap[size_t(y) * p.width + x], key);
+                    if (x < p.width && y - fy0 < p.height) atomicMax(&p.heightmap[size_t(y) * p.width + x], key);
                 }
                 if (p.occl && T % 16u == 0u)   // the whole blocks this tile covers now hold its depth (the same value the heightmap gets)
                     for (uint32_t q = lane; q < (T / 16u) * (T / 16u); q += 32u) {
                         const uint32_t bx = fx / 16u + q % (T / 16u), by = fy / 16u + q / (T / 16u);
-                        if (bx < p.occl_w && by < p.occl_h) atomicMax(p.occl + size_t(by) * p.occl_w + bx, fz + T + 1u);
+                        if (bx < p.occl_w && by - fy0 / 16u < p.occl_h) atomicMax(p.occl + size_t(by) * p.occl_w + bx, fz + T + 1u);
                     }
             }
             if (p.stats) {

@@ -1,4 +1,5 @@
-// The fused tile renderers: fc_render2d (pixel::render), fc_render3d (voxel::render), fc_merge_slabs.
+// The fused tile renderers: fc_render2d (pixel::render), fc_render3d (voxel::render), their frame batches
+// (fc_render2d_frames, fc_render3d_frames), fc_merge_slabs.
 #include <cstddef>
 
 #include "capi_internal.h"
@@ -338,10 +339,296 @@ static size_t format_bytes(uint32_t fmt, uint32_t width, uint32_t height) {
          : fmt == FC_OUT_BITMAP_1BIT ? size_t((width + 7) / 8) * height
          : size_t(width) * height * 4;
 }
+// ---- passes of the frame batches (fc_render2d_frames, fc_render3d_frames) ----
+// The copy stream that returns a pass's images to a host `out` while the next pass runs, with two event pairs
+// (ev_pass[b]: the pass in staging buffer b is complete; ev_copied[b]: its images are copied back)
+static int32_t ensure_copy_stream(fc_ctx* c) {
+    if (c->copy_stream) return FC_OK;
+    CU(cudaStreamCreateWithFlags(&c->copy_stream, cudaStreamNonBlocking));
+    for (int i = 0; i < 2; ++i) {
+        CU(cudaEventCreateWithFlags(&c->ev_pass[i], cudaEventDisableTiming));
+        CU(cudaEventCreateWithFlags(&c->ev_copied[i], cudaEventDisableTiming));
+    }
+    return FC_OK;
+}
+// Orders the copy stream after the pass in buffer b.  With a flag attached the host waits for that pass here, watching
+// the flag (wait_call writes the cancel word the kernels of this pass and the next one poll): a copy into pageable
+// memory blocks the host until it is done, and a blocked host could not cancel anything.  `host_wait`: the host waits
+// without a flag too (it reads the pass's status next).  A cancelled pass returns FC_ERR_CANCELLED.
+static int32_t wait_pass(fc_ctx* c, int b, const CallCancel& cc, bool host_wait) {
+    CU(cudaStreamWaitEvent(c->copy_stream, c->ev_pass[b], 0));
+    if (cc.flag) return wait_call(c, c->copy_stream, cc);
+    if (host_wait) CU(cudaStreamSynchronize(c->copy_stream));
+    return FC_OK;
+}
+// the images of the pass in staging buffer b back to the host, on the copy stream; ev_copied[b] marks b free again
+static int32_t copy_pass_back(fc_ctx* c, int b, void* dst, const void* src, size_t bytes) {
+    CU(cudaMemcpyAsync(dst, src, bytes, cudaMemcpyDeviceToHost, c->copy_stream));
+    CU(cudaEventRecord(c->ev_copied[b], c->copy_stream));
+    return FC_OK;
+}
+// a batch that stops early (cancelled, or an error) returns once its launched work has drained, stats zeroed
+static int32_t abandon_frames(fc_ctx* c, cudaStream_t s, fc_render_stats* stats, int32_t rc) {
+    cudaStreamSynchronize(s);
+    if (c->copy_stream) cudaStreamSynchronize(c->copy_stream);
+    if (stats) memset(stats, 0, sizeof *stats);
+    return rc;
+}
+
 // the small formats, derived on the device from `rows` rows of distance image
 static void derive_format(uint32_t fmt, const float* dimg, uint32_t width, uint32_t rows, uint8_t* dst, cudaStream_t s) {
     if (fmt == FC_OUT_RGBA8) launch_to_rgba(0, dimg, uint64_t(width) * rows, dst, s);
     else launch_to_mask(dimg, width, rows, dst, fmt == FC_OUT_BITMAP_1BIT, s);
+}
+
+// The tile grid of a 3D render (fc_render3d, fc_render3d_frames): the device's tile ladder, roots_x x roots_y x
+// roots_z root tiles from root row row0 and Z z_begin (or the listed XY ones, d_roots), the capped work lists, the
+// occlusion map and the exact census.  With a frame table the grid stacks the frames of a batch (frame_rows grid rows
+// each; heightmap and occlusion map hold frame_rows rows per frame), else it is the one frame of vb / cfg->mat.
+struct Tiles3D {
+    std::vector<uint32_t> ts;
+    uint32_t roots_x = 0, roots_y = 0, roots_z = 0, row0 = 0, z_begin = 0;
+    const uint32_t* d_roots = nullptr;
+    uint32_t n_list = 0;
+    uint64_t n_roots = 0;
+    std::vector<uint64_t> level_cap;
+    uint64_t cap_census = 0;
+    uint32_t choice_words = 0;
+    int grid_blocks = 0, grid_blocks_last = 0;
+    bool use_occl = false, exact_census = false;
+    uint32_t occl_w = 0, occl_h = 0;    // occlusion blocks per row, block rows of one frame
+    const Frame2D* frames = nullptr;
+    uint32_t frame_rows = 0xffffffffu;
+};
+
+static int32_t check_3d(const fc_tape* tape, const fc_render3d_cfg* cfg) {
+    if (cfg->width == 0 || cfg->height == 0 || cfg->depth == 0) return fail(FC_ERR_INVALID, "empty volume");
+    if (tape->info.mem_count) return fail(FC_ERR_UNSUPPORTED, "renderers need a tape without memory spills (<= 255 registers)");
+    if (tape->info.n_outputs != 1) return fail(FC_ERR_INVALID, "ShapeTape has multiple outputs");
+    return FC_OK;
+}
+// tile ladder, launch widths, choice scratch words and the occlusion map's shape
+static int32_t prepare_3d(fc_ctx* c, const fc_tape* tape, const fc_render3d_cfg* cfg, Tiles3D& g) {
+    static const uint32_t DFLT[5] = {128, 64, 32, 16, 8};
+    std::vector<uint32_t>& ts = g.ts;
+    if (int32_t rc = pick_tile_sizes(cfg->tile_sizes, cfg->n_tile_sizes, DFLT, 5, std::max(cfg->width, cfg->height), ts))
+        return rc;
+    if (cfg->n_tile_sizes == 0 && !(cfg->flags & (FC_FLAG_FULL_LADDER | FC_FLAG_EXACT_CENSUS)) &&
+        !env_int("FIDGET_B200_FULL_LADDER", 0)) {
+        // Device ladder: every other size of the default one.  A warp then carries 32 children per pass instead of 8
+        // and a whole level of launches, job records and tape writes disappears; the image cannot change, because a
+        // child's interval result on its grandparent's tape equals the one on its parent's simplified tape (a choice
+        // the parent's region decided is decided the same way on any sub-region, and the pruned branch never
+        // contributed to the value) -- tests/test_gpu_parity.py compares the two ladders bit for bit.
+        std::vector<uint32_t> fused(1, ts[0]);
+        for (size_t i = 0; i + 1 < ts.size();) {
+            const size_t nx = std::min(i + 2, ts.size() - 1);
+            fused.push_back(ts[nx]);
+            i = nx;
+        }
+        ts.swap(fused);
+    }
+    g.roots_x = (cfg->width + ts[0] - 1) / ts[0];
+    // persistent CTAs per SM: 6 for the upper levels, 8 for the last one (many short jobs; measured on prospero and bear:
+    // last level 1.10 -> 0.97 ms and 0.72 -> 0.61 ms, the level before it is fastest at 6)
+    const int bps = env_int("FIDGET_B200_BLOCKS_PER_SM", 6);
+    const int bps_last = std::max(bps, env_int("FIDGET_B200_LAST_LEVEL_BLOCKS_PER_SM", 8));
+    g.grid_blocks = c->sm_count * bps;
+    g.grid_blocks_last = c->sm_count * bps_last;
+    g.choice_words = (tape->info.choice_count + 15) / 16 + 1;
+    // occlusion map (16 x 16 pixel blocks); used when every tile size down to 16 is a multiple of 16
+    g.occl_w = (cfg->width + 15) / 16;
+    g.occl_h = (cfg->height + 15) / 16;
+    g.use_occl = !env_int("FIDGET_B200_NO_CULL", 0);
+    for (uint32_t t : ts) if (t >= 16 && t % 16) g.use_occl = false;
+    g.exact_census = (cfg->flags & FC_FLAG_EXACT_CENSUS) != 0;
+    return FC_OK;
+}
+// Work lists hold only ambiguous tiles (a surface-like set), so they are capped well below the N^3 tile count
+// (FIDGET_B200_MAX_TILES_M, 16 Mi jobs); overflow is reported, not ignored.  The exact census is capped at 64 Mi records.
+static uint64_t list_cap_limit() { return uint64_t(env_int("FIDGET_B200_MAX_TILES_M", 16)) << 20; }
+static void size_lists_3d(Tiles3D& g) {
+    const std::vector<uint32_t>& ts = g.ts;
+    const int L = int(ts.size());
+    const uint64_t cap_limit = list_cap_limit();
+    g.level_cap.assign(L + 1, 0);
+    for (int l = 1; l <= L; ++l) {
+        const uint64_t r = ts[0] / ts[l - 1];
+        g.level_cap[l] = std::min<uint64_t>(g.n_roots * r * r * r, cap_limit);
+    }
+    g.cap_census = 0;
+    if (g.exact_census) {
+        g.cap_census = g.n_roots;
+        for (int l = 1; l < L; ++l) { const uint64_t r = ts[l - 1] / ts[l]; g.cap_census += g.level_cap[l] * r * r * r; }
+        g.cap_census = std::min<uint64_t>(g.cap_census, 64ull << 20);
+    }
+}
+// scratch of a pipeline over g's lists, with heightmap pixels and occlusion blocks for hm_pixels / occl_blocks
+static int32_t ensure_scratch_3d(fc_ctx* c, const Tiles3D& g, size_t hm_pixels, size_t occl_blocks) {
+    const int L = int(g.ts.size());
+    CU(c->choice_scratch.ensure(size_t(g.grid_blocks_last) * WARPS_PER_BLOCK * g.choice_words * 32 * 4));
+    CU(c->arena.ensure(c->arena_bytes));
+    CU(c->counters.ensure(sizeof(Counters)));
+    CU(c->stats.ensure(sizeof(Stats)));
+    for (int l = 1; l <= L; ++l) CU(c->jobs[l].ensure(g.level_cap[l] * sizeof(TileJob)));
+    CU(c->heightmap.ensure(hm_pixels * 8));
+    if (g.exact_census) CU(c->census.ensure(g.cap_census * sizeof(CensusRec)));
+    if (g.use_occl) CU(c->occl.ensure(occl_blocks * 4));
+    return FC_OK;
+}
+static uint32_t zsort_layers(const Tiles3D& g) { return (g.roots_z * g.ts[0]) / g.ts.back(); }
+
+// The tile pipeline of fc_render3d (voxel::render), enqueued on `s`: the interval levels, the front-to-back sort of
+// the leaf tiles, the leaf voxels, the exact census and the normals of output rows y0 .. y1 into `dimg`.  The caller
+// has sized the scratch and zeroed the counters, the heightmap rows, the occlusion map and the stats.
+static int32_t enqueue_tiles_3d(fc_ctx* c, const fc_tape* tape, const fc_render3d_cfg* cfg, const Tiles3D& g,
+                                const VarBind& vb, void* dimg, uint32_t y0, uint32_t y1, bool want_stats, bool timing,
+                                const CallCancel& cc, cudaStream_t s, size_t& ev, uint32_t& launches) {
+    const std::vector<uint32_t>& ts = g.ts;
+    const int L = int(ts.size());
+    const uint32_t T0 = ts[0];
+    if (timing) CU(cudaEventRecord(get_event(c, ev++), s));
+    for (int l = 0; l < L; ++l) {
+        LevelParams p{};
+        p.level = l;
+        p.tile = ts[l];
+        p.n_axis = l ? ts[l - 1] / ts[l] : 0;
+        p.is_last = (l == L - 1);
+        p.pixel_perfect = 0;
+        p.root_mode = (l == 0);
+        p.roots_x = g.roots_x; p.roots_y = g.roots_y; p.roots_z = g.roots_z;
+        p.root_x0 = 0; p.root_y0 = g.row0 * T0; p.root_z0 = g.z_begin;
+        p.root_list = g.d_roots; p.n_root_list = g.n_list;
+        p.root_tape.ptr = tape->dev;
+        p.root_tape.n_ops = tape->info.n_ops;
+        p.root_tape.ref_len = tape->info.ref_len;
+        p.root_tape.n_choices = tape->info.choice_count;
+        p.width = cfg->width; p.height = cfg->height; p.depth = cfg->depth;
+        memcpy(p.mat.m, cfg->mat, sizeof p.mat.m);
+        p.jobs_in = l ? c->jobs[l].as<TileJob>() : nullptr;
+        p.cap_in = l ? uint32_t(g.level_cap[l]) : 0;
+        p.jobs_out = c->jobs[l + 1].as<TileJob>();
+        p.cap_out = uint32_t(g.level_cap[l + 1]);
+        p.arena = c->arena.as<uint2>();
+        p.arena_cap = std::min<uint64_t>(c->arena.cap, c->arena_bytes) / sizeof(uint2);
+        p.choice_scratch = c->choice_scratch.as<uint32_t>();
+        p.choice_words = g.choice_words;
+        p.ctr = c->counters.as<Counters>();
+        p.stats = want_stats ? c->stats.as<Stats>() : nullptr;
+        p.heightmap = c->heightmap.as<unsigned long long>();
+        p.occl = g.use_occl ? c->occl.as<uint32_t>() : nullptr;
+        p.occl_w = g.occl_w;
+        p.occl_h = g.occl_h;
+        p.cull = (g.use_occl && l >= 1 && ts[l - 1] >= 16u && ts[l - 1] <= 64u) ? 1u : 0u;   // parents made of 1, 4 or 16 blocks
+        p.census = g.exact_census ? c->census.as<CensusRec>() : nullptr;
+        p.cap_census = uint32_t(g.cap_census);
+        p.vb = vb;
+        p.cancel = cc.ref;
+        p.frames = g.frames;
+        p.frame_rows = g.frame_rows;
+        int blocks = (l == L - 1 && l > 0) ? g.grid_blocks_last : g.grid_blocks;
+        if (l == 0) {
+            uint64_t warps = (g.n_roots + 31) / 32;
+            blocks = int(std::min<uint64_t>((warps + WARPS_PER_BLOCK - 1) / WARPS_PER_BLOCK, uint64_t(g.grid_blocks)));
+        }
+        bool coop = false;
+        if (l == 0) {
+            int ct = COOP_THREADS;
+            int cb = coop_blocks(c, tape, g.n_roots, p, 3, ct);
+            if (cb > 0) {
+                CU(launch_interval_root_coop_3d(p, cb, ct, s));
+                coop = true;
+            }
+        }
+        if (!coop) launch_interval_level_3d(p, std::max(blocks, 1), s);
+        ++launches;
+        if (timing) CU(cudaEventRecord(get_event(c, ev++), s));
+    }
+    {
+        VoxelParams q{};
+        q.tile = ts[L - 1];
+        if (!env_int("FIDGET_B200_NO_ZSORT", 0)) {
+            const uint32_t n_layers = zsort_layers(g);
+            CU(c->zsort.ensure(size_t(n_layers + 1) * 4 + g.level_cap[L] * 4));
+            uint32_t* hist = c->zsort.as<uint32_t>();
+            uint32_t* order = hist + n_layers + 1;
+            launch_leaf_zsort(c->jobs[L].as<TileJob>(), &c->counters.as<Counters>()->n_jobs[L], uint32_t(g.level_cap[L]),
+                              g.z_begin, ts[L - 1], n_layers, hist, order, s);
+            launches += 3;
+            q.order = order;
+        }
+        q.width = cfg->width; q.height = cfg->height;
+        memcpy(q.mat.m, cfg->mat, sizeof q.mat.m);
+        q.jobs = c->jobs[L].as<TileJob>();
+        q.cap_jobs = uint32_t(g.level_cap[L]);
+        q.heightmap = c->heightmap.as<unsigned long long>();
+        q.ctr = c->counters.as<Counters>();
+        q.list = L; q.cursor = L;
+        q.stats = want_stats ? c->stats.as<Stats>() : nullptr;
+        q.vb = vb;
+        q.cancel = cc.ref;
+        q.frames = g.frames;
+        q.frame_rows = g.frame_rows;
+        launch_voxels_3d(q, c->sm_count * env_int("FIDGET_B200_VOXEL_BLOCKS_PER_SM", 12), s);
+        ++launches;
+    }
+    if (g.exact_census) {
+        // the counts collected so far describe what the device evaluated; replace them by the reference's census,
+        // judged against the final heightmap (k_census_3d).  (A frame batch's census needs no frame: its sides are
+        // multiples of the root tile, so the frames are stacked without padding rows.)
+        Stats* ds = c->stats.as<Stats>();
+        CU(cudaMemsetAsync(ds, 0, offsetof(Stats, grads), s));                        // evaluated .. simplified, pixels
+        CensusParams cp{};
+        cp.recs = c->census.as<CensusRec>();
+        cp.n_recs = &c->counters.as<Counters>()->n_census;
+        cp.cap = uint32_t(g.cap_census);
+        for (int l = 0; l < L; ++l) cp.tile[l] = ts[l];
+        cp.last_level = L - 1;
+        cp.heightmap = c->heightmap.as<unsigned long long>();
+        cp.width = cfg->width;
+        cp.stats = ds;
+        cp.cancel = cc.ref;
+        launch_census_3d(cp, c->sm_count * 8, s);
+        ++launches;
+    }
+    if (timing) CU(cudaEventRecord(get_event(c, ev++), s));
+    {
+        NormalParams q{};
+        q.width = cfg->width; q.height = cfg->height; q.depth = cfg->depth;
+        q.y0 = y0; q.y1 = y1;
+        q.root_list = g.d_roots; q.n_root_list = g.n_list; q.roots_x = g.roots_x; q.root_tile = T0;
+        q.clamp = (cfg->flags & FC_FLAG_NO_CLAMP) ? 0 : 1;
+        memcpy(q.mat.m, cfg->mat, sizeof q.mat.m);
+        q.jobs = c->jobs[L].as<TileJob>();
+        q.heightmap = c->heightmap.as<unsigned long long>();
+        q.out = dimg;
+        q.stats = want_stats ? c->stats.as<Stats>() : nullptr;
+        q.vb = vb;
+        q.cancel = cc.ref;
+        q.frames = g.frames;
+        q.frame_rows = g.frame_rows;
+        launch_normals_3d(q, s);
+        ++launches;
+    }
+    if (timing) CU(cudaEventRecord(get_event(c, ev++), s));
+    CU(cudaGetLastError());
+    return FC_OK;
+}
+
+// FC_FLAG_TIMING: stage times of the pass whose events start at `first` (L + 3 events), added to `stage_ms`
+static void add_stage_ms_3d(fc_ctx* c, size_t first, int L, float* stage_ms) {
+    float ms = 0;
+    const cudaEvent_t* e = c->events.data() + first;
+    for (int l = 0; l < L; ++l) {
+        cudaEventElapsedTime(&ms, e[l], e[l + 1]);
+        stage_ms[l] += ms;
+    }
+    cudaEventElapsedTime(&ms, e[L], e[L + 1]);
+    stage_ms[9] += ms;
+    cudaEventElapsedTime(&ms, e[L + 1], e[L + 2]);
+    stage_ms[10] += ms;
+    cudaEventElapsedTime(&ms, e[0], e[L + 2]);
+    stage_ms[15] += ms;
 }
 
 extern "C" {
@@ -525,13 +812,7 @@ int32_t fc_render2d_frames(fc_ctx* c, const fc_tape* tape, const fc_render2d_cfg
         fstage[0] = c->fx_out.as<uint8_t>();
         fstage[1] = fstage[0] + img_fmt * per_pass;
     }
-    if (!out_dev && !c->copy_stream) {
-        CU(cudaStreamCreateWithFlags(&c->copy_stream, cudaStreamNonBlocking));
-        for (int i = 0; i < 2; ++i) {
-            CU(cudaEventCreateWithFlags(&c->ev_pass[i], cudaEventDisableTiming));
-            CU(cudaEventCreateWithFlags(&c->ev_copied[i], cudaEventDisableTiming));
-        }
-    }
+    if (!out_dev) if (int32_t src = ensure_copy_stream(c)) return src;
     CU(cudaMemcpyAsync(c->frame_table.p, table.data(), table.size() * sizeof(Frame2D), cudaMemcpyHostToDevice, s));
     CU(cudaMemsetAsync(c->counters.p, 0, sizeof(Counters), s));
     if (want_stats) CU(cudaMemsetAsync(c->stats.p, 0, sizeof(Stats), s));
@@ -542,23 +823,10 @@ int32_t fc_render2d_frames(fc_ctx* c, const fc_tape* tape, const fc_render2d_cfg
         const uint32_t f0 = k * per_pass, n = std::min(per_pass, n_frames - f0);
         const size_t fb = fmt == FC_OUT_F32 ? img_f32 : img_fmt;
         const void* src = fmt == FC_OUT_F32 ? static_cast<const void*>(stage[k & 1]) : static_cast<const void*>(fstage[k & 1]);
-        CU(cudaStreamWaitEvent(c->copy_stream, c->ev_pass[k & 1], 0));
-        // With a flag attached the host waits for pass k here, watching the flag (wait_call writes the cancel word the
-        // kernels of passes k and k + 1 poll), before it issues the copy: a copy into pageable memory blocks the host
-        // until it is done, and a blocked host could not cancel anything.  A cancelled pass copies nothing.
-        if (cc.flag)
-            if (int32_t wrc = wait_call(c, c->copy_stream, cc)) return wrc;
-        CU(cudaMemcpyAsync(static_cast<uint8_t*>(out) + size_t(f0) * fb, src, size_t(n) * fb, cudaMemcpyDeviceToHost, c->copy_stream));
-        CU(cudaEventRecord(c->ev_copied[k & 1], c->copy_stream));
-        return FC_OK;
+        if (int32_t wrc = wait_pass(c, int(k & 1), cc, false)) return wrc;   // (a cancelled pass copies nothing)
+        return copy_pass_back(c, int(k & 1), static_cast<uint8_t*>(out) + size_t(f0) * fb, src, size_t(n) * fb);
     };
-    // a call that stops early (cancelled, or a CUDA error) returns once its launched work has drained, stats zeroed
-    auto abandon = [&](int32_t rc) -> int32_t {
-        cudaStreamSynchronize(s);
-        cudaStreamSynchronize(c->copy_stream);
-        if (stats) memset(stats, 0, sizeof *stats);
-        return rc;
-    };
+    auto abandon = [&](int32_t rc) { return abandon_frames(c, s, stats, rc); };
     VarBind vb0 = table[0].vb;   // (unused by the kernels: every frame comes from the table)
     size_t ev = 0;
     uint32_t launches = 0, passes_run = 0;
@@ -631,35 +899,17 @@ int32_t fc_render2d_frames(fc_ctx* c, const fc_tape* tape, const fc_render2d_cfg
 int32_t fc_render3d(fc_ctx* c, const fc_tape* tape, const fc_render3d_cfg* cfg, fc_geometry_pixel* out,
                     fc_render_stats* stats) {
     if (!c || !tape || !cfg || !out) return fail(FC_ERR_INVALID, "null argument");
-    if (cfg->width == 0 || cfg->height == 0 || cfg->depth == 0) return fail(FC_ERR_INVALID, "empty volume");
-    if (tape->info.mem_count) return fail(FC_ERR_UNSUPPORTED, "renderers need a tape without memory spills (<= 255 registers)");
-    if (tape->info.n_outputs != 1) return fail(FC_ERR_INVALID, "ShapeTape has multiple outputs");
+    if (int32_t vrc = check_3d(tape, cfg)) return vrc;
     CallCancel cc;
     if (int32_t crc = begin_call(c, cc)) return crc;
     std::lock_guard<std::mutex> guard(c->mu);
     CU(cudaSetDevice(c->device));
-    static const uint32_t DFLT[5] = {128, 64, 32, 16, 8};
-    std::vector<uint32_t> ts;
-    int32_t rc = pick_tile_sizes(cfg->tile_sizes, cfg->n_tile_sizes, DFLT, 5, std::max(cfg->width, cfg->height), ts);
+    Tiles3D g;
+    int32_t rc = prepare_3d(c, tape, cfg, g);
     if (rc) return rc;
-    if (cfg->n_tile_sizes == 0 && !(cfg->flags & (FC_FLAG_FULL_LADDER | FC_FLAG_EXACT_CENSUS)) &&
-        !env_int("FIDGET_B200_FULL_LADDER", 0)) {
-        // Device ladder: every other size of the default one.  A warp then carries 32 children per pass instead of 8
-        // and a whole level of launches, job records and tape writes disappears; the image cannot change, because a
-        // child's interval result on its grandparent's tape equals the one on its parent's simplified tape (a choice
-        // the parent's region decided is decided the same way on any sub-region, and the pruned branch never
-        // contributed to the value) -- tests/test_gpu_parity.py compares the two ladders bit for bit.
-        std::vector<uint32_t> fused(1, ts[0]);
-        for (size_t i = 0; i + 1 < ts.size();) {
-            const size_t nx = std::min(i + 2, ts.size() - 1);
-            fused.push_back(ts[nx]);
-            i = nx;
-        }
-        ts.swap(fused);
-    }
-    const int L = int(ts.size());
-    const uint32_t T0 = ts[0];
-    const uint32_t roots_x = (cfg->width + T0 - 1) / T0, roots_y_all = (cfg->height + T0 - 1) / T0;
+    const int L = int(g.ts.size());
+    const uint32_t T0 = g.ts[0];
+    const uint32_t roots_x = g.roots_x, roots_y_all = (cfg->height + T0 - 1) / T0;
     const uint32_t row0 = cfg->root_row_begin, row1 = cfg->root_row_end ? cfg->root_row_end : roots_y_all;
     if (row0 > row1 || row1 > roots_y_all) return fail(FC_ERR_INVALID, "bad root row band");
     const uint32_t roots_y = row1 - row0;
@@ -680,41 +930,18 @@ int32_t fc_render3d(fc_ctx* c, const fc_tape* tape, const fc_render3d_cfg* cfg, 
         if (T0 % 8) return fail(FC_ERR_UNSUPPORTED, "tile-interleaved renders need a root tile edge that is a multiple of 8");
         if (int32_t lrc = root_subset(c, roots_x, row0, row1, cfg->root_stride, cfg->root_offset, s, &d_roots, &n_list)) return lrc;
     }
-    const uint64_t n_roots = (d_roots ? uint64_t(n_list) : uint64_t(roots_x) * roots_y) * roots_z;
-    if (n_roots > 0xfffffff0ull) return fail(FC_ERR_UNSUPPORTED, "volume too large");
-
-    // persistent CTAs per SM: 6 for the upper levels, 8 for the last one (many short jobs; measured on prospero and bear:
-    // last level 1.10 -> 0.97 ms and 0.72 -> 0.61 ms, the level before it is fastest at 6)
-    const int bps = env_int("FIDGET_B200_BLOCKS_PER_SM", 6);
-    const int bps_last = std::max(bps, env_int("FIDGET_B200_LAST_LEVEL_BLOCKS_PER_SM", 8));
-    const int grid_blocks = c->sm_count * bps, grid_blocks_last = c->sm_count * bps_last;
-    const uint32_t choice_words = (tape->info.choice_count + 15) / 16 + 1;
-    CU(c->choice_scratch.ensure(size_t(grid_blocks_last) * WARPS_PER_BLOCK * choice_words * 32 * 4));
-    CU(c->arena.ensure(c->arena_bytes));
-    CU(c->counters.ensure(sizeof(Counters)));
-    CU(c->stats.ensure(sizeof(Stats)));
-    // Work lists hold only ambiguous tiles (a surface-like set), so they are
-    // capped well below the N^3 tile count; overflow is reported, not ignored.
-    const uint64_t cap_limit = uint64_t(env_int("FIDGET_B200_MAX_TILES_M", 16)) << 20;
-    std::vector<uint64_t> level_cap(L + 1);
-    for (int l = 1; l <= L; ++l) {
-        uint64_t r = T0 / ts[l - 1];
-        level_cap[l] = std::min<uint64_t>(n_roots * r * r * r, cap_limit);
-        CU(c->jobs[l].ensure(level_cap[l] * sizeof(TileJob)));
-    }
-    const size_t npix = size_t(cfg->width) * cfg->height;
-    CU(c->heightmap.ensure(npix * 8));
-    const bool exact_census = (cfg->flags & FC_FLAG_EXACT_CENSUS) != 0;
-    uint64_t cap_census = 0;
-    if (exact_census) {
+    g.roots_y = roots_y; g.roots_z = roots_z; g.row0 = row0; g.z_begin = z_begin;
+    g.d_roots = d_roots; g.n_list = n_list;
+    g.n_roots = (d_roots ? uint64_t(n_list) : uint64_t(roots_x) * roots_y) * roots_z;
+    if (g.n_roots > 0xfffffff0ull) return fail(FC_ERR_UNSUPPORTED, "volume too large");
+    if (g.exact_census) {
         if (!stats) return fail(FC_ERR_INVALID, "FC_FLAG_EXACT_CENSUS needs a stats struct");
         if (cfg->width % T0 || cfg->height % T0 || d_roots || row0 || row1 != roots_y_all || z_begin || z_end < cfg->depth)
             return fail(FC_ERR_UNSUPPORTED, "the exact census needs a whole-volume render of an image whose sides are multiples of the root tile");
-        cap_census = n_roots;
-        for (int l = 1; l < L; ++l) { const uint64_t r = ts[l - 1] / ts[l]; cap_census += level_cap[l] * r * r * r; }
-        cap_census = std::min<uint64_t>(cap_census, 64ull << 20);
-        CU(c->census.ensure(cap_census * sizeof(CensusRec)));
     }
+    size_lists_3d(g);
+    const size_t npix = size_t(cfg->width) * cfg->height;
+    if (int32_t erc = ensure_scratch_3d(c, g, npix, size_t(g.occl_w) * g.occl_h)) return erc;
     bool out_dev = is_device_ptr(out);
     void* dimg = out;
     if (!out_dev) {
@@ -729,138 +956,15 @@ int32_t fc_render3d(fc_ctx* c, const fc_tape* tape, const fc_render3d_cfg* cfg, 
     }
     CU(cudaMemsetAsync(c->counters.p, 0, sizeof(Counters), s));
     CU(cudaMemsetAsync(c->heightmap.as<char>() + size_t(band_y0) * cfg->width * 8, 0, size_t(band_y1 - band_y0) * cfg->width * 8, s));
-    // occlusion map (16 x 16 pixel blocks); used when every tile size down to 16 is a multiple of 16
-    const uint32_t occl_w = (cfg->width + 15) / 16, occl_h = (cfg->height + 15) / 16;
-    bool use_occl = !env_int("FIDGET_B200_NO_CULL", 0);
-    for (int l = 0; l < L; ++l) if (ts[l] >= 16 && ts[l] % 16) use_occl = false;
-    if (use_occl) {
-        CU(c->occl.ensure(size_t(occl_w) * occl_h * 4));
-        CU(cudaMemsetAsync(c->occl.p, 0, size_t(occl_w) * occl_h * 4, s));
-    }
+    if (g.use_occl) CU(cudaMemsetAsync(c->occl.p, 0, size_t(g.occl_w) * g.occl_h * 4, s));
     if (want_stats) CU(cudaMemsetAsync(c->stats.p, 0, sizeof(Stats), s));
 
     VarBind vb;
     if (int32_t vrc = bind_vars(tape, cfg->var_values, cfg->n_var_values, vb)) return vrc;
     size_t ev = 0;
-    if (timing) CU(cudaEventRecord(get_event(c, ev++), s));
     uint32_t launches = 0;
-    for (int l = 0; l < L; ++l) {
-        LevelParams p{};
-        p.level = l;
-        p.tile = ts[l];
-        p.n_axis = l ? ts[l - 1] / ts[l] : 0;
-        p.is_last = (l == L - 1);
-        p.pixel_perfect = 0;
-        p.root_mode = (l == 0);
-        p.roots_x = roots_x; p.roots_y = roots_y; p.roots_z = roots_z;
-        p.root_x0 = 0; p.root_y0 = row0 * T0; p.root_z0 = z_begin;
-        p.root_list = d_roots; p.n_root_list = n_list;
-        p.root_tape.ptr = tape->dev;
-        p.root_tape.n_ops = tape->info.n_ops;
-        p.root_tape.ref_len = tape->info.ref_len;
-        p.root_tape.n_choices = tape->info.choice_count;
-        p.width = cfg->width; p.height = cfg->height; p.depth = cfg->depth;
-        memcpy(p.mat.m, cfg->mat, sizeof p.mat.m);
-        p.jobs_in = l ? c->jobs[l].as<TileJob>() : nullptr;
-        p.cap_in = l ? uint32_t(level_cap[l]) : 0;
-        p.jobs_out = c->jobs[l + 1].as<TileJob>();
-        p.cap_out = uint32_t(level_cap[l + 1]);
-        p.arena = c->arena.as<uint2>();
-        p.arena_cap = std::min<uint64_t>(c->arena.cap, c->arena_bytes) / sizeof(uint2);
-        p.choice_scratch = c->choice_scratch.as<uint32_t>();
-        p.choice_words = choice_words;
-        p.ctr = c->counters.as<Counters>();
-        p.stats = want_stats ? c->stats.as<Stats>() : nullptr;
-        p.heightmap = c->heightmap.as<unsigned long long>();
-        p.occl = use_occl ? c->occl.as<uint32_t>() : nullptr;
-        p.occl_w = occl_w;
-        p.occl_h = occl_h;
-        p.cull = (use_occl && l >= 1 && ts[l - 1] >= 16u && ts[l - 1] <= 64u) ? 1u : 0u;   // parents made of 1, 4 or 16 blocks
-        p.census = exact_census ? c->census.as<CensusRec>() : nullptr;
-        p.cap_census = uint32_t(cap_census);
-        p.vb = vb;
-        p.cancel = cc.ref;
-        int blocks = (l == L - 1 && l > 0) ? grid_blocks_last : grid_blocks;
-        if (l == 0) {
-            uint64_t warps = (n_roots + 31) / 32;
-            blocks = int(std::min<uint64_t>((warps + WARPS_PER_BLOCK - 1) / WARPS_PER_BLOCK, uint64_t(grid_blocks)));
-        }
-        bool coop = false;
-        if (l == 0) {
-            int ct = COOP_THREADS;
-            int cb = coop_blocks(c, tape, n_roots, p, 3, ct);
-            if (cb > 0) {
-                CU(launch_interval_root_coop_3d(p, cb, ct, s));
-                coop = true;
-            }
-        }
-        if (!coop) launch_interval_level_3d(p, std::max(blocks, 1), s);
-        ++launches;
-        if (timing) CU(cudaEventRecord(get_event(c, ev++), s));
-    }
-    {
-        VoxelParams q{};
-        q.tile = ts[L - 1];
-        if (!env_int("FIDGET_B200_NO_ZSORT", 0)) {
-            const uint32_t n_layers = (roots_z * T0) / ts[L - 1];
-            CU(c->zsort.ensure(size_t(n_layers + 1) * 4 + level_cap[L] * 4));
-            uint32_t* hist = c->zsort.as<uint32_t>();
-            uint32_t* order = hist + n_layers + 1;
-            launch_leaf_zsort(c->jobs[L].as<TileJob>(), &c->counters.as<Counters>()->n_jobs[L], uint32_t(level_cap[L]),
-                              z_begin, ts[L - 1], n_layers, hist, order, s);
-            launches += 3;
-            q.order = order;
-        }
-        q.width = cfg->width; q.height = cfg->height;
-        memcpy(q.mat.m, cfg->mat, sizeof q.mat.m);
-        q.jobs = c->jobs[L].as<TileJob>();
-        q.cap_jobs = uint32_t(level_cap[L]);
-        q.heightmap = c->heightmap.as<unsigned long long>();
-        q.ctr = c->counters.as<Counters>();
-        q.list = L; q.cursor = L;
-        q.stats = want_stats ? c->stats.as<Stats>() : nullptr;
-        q.vb = vb;
-        q.cancel = cc.ref;
-        launch_voxels_3d(q, c->sm_count * env_int("FIDGET_B200_VOXEL_BLOCKS_PER_SM", 12), s);
-        ++launches;
-    }
-    if (exact_census) {
-        // the counts collected so far describe what the device evaluated; replace them by the reference's census,
-        // judged against the final heightmap (k_census_3d)
-        Stats* ds = c->stats.as<Stats>();
-        CU(cudaMemsetAsync(ds, 0, offsetof(Stats, grads), s));                        // evaluated .. simplified, pixels
-        CensusParams cp{};
-        cp.recs = c->census.as<CensusRec>();
-        cp.n_recs = &c->counters.as<Counters>()->n_census;
-        cp.cap = uint32_t(cap_census);
-        for (int l = 0; l < L; ++l) cp.tile[l] = ts[l];
-        cp.last_level = L - 1;
-        cp.heightmap = c->heightmap.as<unsigned long long>();
-        cp.width = cfg->width;
-        cp.stats = ds;
-        cp.cancel = cc.ref;
-        launch_census_3d(cp, c->sm_count * 8, s);
-        ++launches;
-    }
-    if (timing) CU(cudaEventRecord(get_event(c, ev++), s));
-    {
-        NormalParams q{};
-        q.width = cfg->width; q.height = cfg->height; q.depth = cfg->depth;
-        q.y0 = band_y0; q.y1 = band_y1;
-        q.root_list = d_roots; q.n_root_list = n_list; q.roots_x = roots_x; q.root_tile = T0;
-        q.clamp = (cfg->flags & FC_FLAG_NO_CLAMP) ? 0 : 1;
-        memcpy(q.mat.m, cfg->mat, sizeof q.mat.m);
-        q.jobs = c->jobs[L].as<TileJob>();
-        q.heightmap = c->heightmap.as<unsigned long long>();
-        q.out = dimg;
-        q.stats = want_stats ? c->stats.as<Stats>() : nullptr;
-        q.vb = vb;
-        q.cancel = cc.ref;
-        launch_normals_3d(q, s);
-        ++launches;
-    }
-    if (timing) CU(cudaEventRecord(get_event(c, ev++), s));
-    CU(cudaGetLastError());
+    if (int32_t erc = enqueue_tiles_3d(c, tape, cfg, g, vb, dimg, band_y0, band_y1, want_stats, timing, cc, s, ev, launches))
+        return erc;
     const bool early_return = async && out_dev && !want_stats;
     if (cc.flag && !early_return) {   // a cancelled render copies nothing to the host
         if (int32_t wrc = wait_call(c, s, cc)) {
@@ -884,32 +988,246 @@ int32_t fc_render3d(fc_ctx* c, const fc_tape* tape, const fc_render3d_cfg* cfg, 
         Counters hc;
         CU(cudaMemcpy(&h, c->stats.p, sizeof h, cudaMemcpyDeviceToHost));
         CU(cudaMemcpy(&hc, c->counters.p, sizeof hc, cudaMemcpyDeviceToHost));
-        for (int l = 0; l < FC_MAX_TILE_LEVELS; ++l) {
-            stats->evaluated[l] = h.evaluated[l];
-            stats->filled_inside[l] = h.filled_inside[l];
-            stats->filled_outside[l] = h.filled_outside[l];
-            stats->ambiguous[l] = h.ambiguous[l];
-            stats->simplified[l] = h.simplified[l];
-        }
-        stats->pixels = h.pixels;
+        copy_census(h, stats);
         stats->grads = h.grads;
         stats->arena_bytes_used = hc.arena_top * sizeof(uint2);
         stats->kernel_launches = launches;
-        if (timing) {
-            float ms = 0;
-            for (int l = 0; l < L; ++l) {
-                cudaEventElapsedTime(&ms, c->events[l], c->events[l + 1]);
-                stats->stage_ms[l] = ms;
-            }
-            cudaEventElapsedTime(&ms, c->events[L], c->events[L + 1]);
-            stats->stage_ms[9] = ms;
-            cudaEventElapsedTime(&ms, c->events[L + 1], c->events[L + 2]);
-            stats->stage_ms[10] = ms;
-            cudaEventElapsedTime(&ms, c->events[0], c->events[L + 2]);
-            stats->stage_ms[15] = ms;
-        }
+        if (timing) add_stage_ms_3d(c, 0, L, stats->stage_ms);
     }
     return rc;
+}
+
+int32_t fc_render3d_frames(fc_ctx* c, const fc_tape* tape, const fc_render3d_cfg* cfg, const fc_frame3d* frames,
+                           uint32_t n_frames, fc_geometry_pixel* out, fc_render_stats* stats) {
+    if (!c || !tape || !cfg || !out || (n_frames && !frames)) return fail(FC_ERR_INVALID, "null argument");
+    if (int32_t vrc = check_3d(tape, cfg)) return vrc;
+    if (cfg->z_begin || cfg->z_end) return fail(FC_ERR_UNSUPPORTED, "Z slabs are not supported by frame batches");
+    if (cfg->root_row_begin || cfg->root_row_end) return fail(FC_ERR_UNSUPPORTED, "root row bands are not supported by frame batches");
+    if (cfg->root_stride > 1) return fail(FC_ERR_UNSUPPORTED, "the tile interleave is not supported by frame batches");
+    // every frame's ShapeVars binding, before anything is allocated or launched (z is unused in 3D)
+    std::vector<Frame2D> table(n_frames);
+    for (uint32_t k = 0; k < n_frames; ++k) {
+        if (frames[k].n_var_values > FC_MAX_VARS) return fail(FC_ERR_INVALID, "n_var_values above FC_MAX_VARS");
+        memcpy(table[k].mat.m, frames[k].mat, sizeof table[k].mat.m);
+        table[k].z = 0.0f;
+        if (int32_t brc = bind_vars(tape, frames[k].var_values, frames[k].n_var_values, table[k].vb)) return brc;
+    }
+    CallCancel cc;
+    if (int32_t crc = begin_call(c, cc)) return crc;
+    if (stats) memset(stats, 0, sizeof *stats);
+    if (n_frames == 0) return FC_OK;
+    std::lock_guard<std::mutex> guard(c->mu);
+    CU(cudaSetDevice(c->device));
+    Tiles3D g;
+    if (int32_t rc = prepare_3d(c, tape, cfg, g)) return rc;
+    const int L = int(g.ts.size());
+    const uint32_t T0 = g.ts[0];
+    const uint32_t W = cfg->width, H = cfg->height;
+    const uint32_t roots_y = (H + T0 - 1) / T0, frame_rows = roots_y * T0;   // root rows and grid rows per frame
+    g.roots_z = (cfg->depth + T0 - 1) / T0;
+    const uint64_t frame_roots = uint64_t(g.roots_x) * roots_y * g.roots_z;
+    if (frame_roots > 0xfffffff0ull) return fail(FC_ERR_UNSUPPORTED, "volume too large");
+    if (g.exact_census) {
+        if (!stats) return fail(FC_ERR_INVALID, "FC_FLAG_EXACT_CENSUS needs a stats struct");
+        if (W % T0 || H % T0)
+            return fail(FC_ERR_UNSUPPORTED, "the exact census needs a whole-volume render of an image whose sides are multiples of the root tile");
+    }
+    if (frame_rows % 16) g.use_occl = false;   // (root tiles below 16 never write the occlusion map)
+    g.frame_rows = frame_rows;
+    const bool timing = (cfg->flags & FC_FLAG_TIMING) != 0;
+    const bool async = (cfg->flags & FC_FLAG_ASYNC) != 0;
+    const bool want_stats = stats != nullptr;
+    const bool host_out = !is_device_ptr(out);
+    const size_t img_px = size_t(W) * H;
+    const size_t occl_frame = g.use_occl ? size_t(frame_rows / 16) * g.occl_w : 0;   // occlusion blocks per frame
+    cudaStream_t s = c->stream;
+
+    // ---- passes.  Lists and census of a pass of n frames are those of one grid of n stacked frames (capped as in
+    // fc_render3d); its heightmap rows, occlusion blocks and (host out) two staged images per frame are its own. ----
+    auto grid_of = [&](uint32_t n) {
+        Tiles3D gp = g;
+        gp.roots_y = roots_y * n;
+        gp.n_roots = frame_roots * n;
+        size_lists_3d(gp);
+        return gp;
+    };
+    auto pass_bytes = [&](uint32_t n) {
+        const Tiles3D gp = grid_of(n);
+        uint64_t b = uint64_t(n) * (size_t(frame_rows) * W * 8 + occl_frame * 4 + (host_out ? 2 * img_px * 16 : 0));
+        for (int l = 1; l <= L; ++l) b += gp.level_cap[l] * sizeof(TileJob);
+        return b + gp.level_cap[L] * 4 + gp.cap_census * sizeof(CensusRec);
+    };
+    // the most frames a pass may hold: FC_FRAMES_PASS_BYTES (at least one frame), 32-bit root ids, and (exact census)
+    // 16-bit census rows
+    uint32_t n_max = 1;
+    while (n_max < n_frames && pass_bytes(n_max + 1) <= FC_FRAMES_PASS_BYTES && frame_roots * (n_max + 1) <= 0xfffffff0ull &&
+           (!g.exact_census || uint64_t(frame_rows) * (n_max + 1) <= 65536))
+        ++n_max;
+    const int forced = env_int("FIDGET_B200_FRAMES_PER_PASS", 0);   // (diagnostic: at most the limits above)
+    if (forced > 0) n_max = std::min<uint32_t>(n_max, uint32_t(forced));
+    {
+        Tiles3D gm = grid_of(n_max);
+        if (int32_t erc = ensure_scratch_3d(c, gm, size_t(W) * frame_rows * n_max, occl_frame * n_max)) return erc;
+        if (!env_int("FIDGET_B200_NO_ZSORT", 0)) CU(c->zsort.ensure(size_t(zsort_layers(gm) + 1) * 4 + gm.level_cap[L] * 4));
+    }
+    CU(c->frame_table.ensure(size_t(n_frames) * sizeof(Frame2D)));
+    if (!c->pass_pin) CU(cudaHostAlloc(reinterpret_cast<void**>(&c->pass_pin), 2 * sizeof(PassStatus), cudaHostAllocDefault));
+    fc_geometry_pixel* stage[2] = {nullptr, nullptr};
+    if (host_out) {
+        CU(c->image.ensure(2 * img_px * 16 * n_max));
+        stage[0] = c->image.as<fc_geometry_pixel>();
+        stage[1] = stage[0] + img_px * n_max;
+    }
+    if (int32_t src = ensure_copy_stream(c)) return src;
+    CU(cudaMemcpyAsync(c->frame_table.p, table.data(), table.size() * sizeof(Frame2D), cudaMemcpyHostToDevice, s));
+    const uint64_t arena_clauses = std::min<uint64_t>(c->arena.cap, c->arena_bytes) / sizeof(uint2);
+
+    // Overflow policy: a pass fails (FC_ERR_ARENA, list overflow) only where one of its frames alone would.  The first
+    // pass holds one frame; later ones are sized from the largest per-frame use seen so far (arena clauses, jobs per
+    // level, census records) with headroom 1.5; a pass that still overflows is run again as two halves (the kernels
+    // report overflow, they do not fault), and only a one-frame pass returns the error.  Only capped lists can
+    // overflow: a job list whose cap is the worst case of the pass (every tile of the level queued) never does, so the
+    // headroom applies to the arena, to the job lists clamped by FIDGET_B200_MAX_TILES_M and to a clamped census.
+    double use_arena = 0, use_census = 0, use_jobs[MAX_LEVELS + 1] = {};
+    bool measured = forced > 0;
+    auto fits = [&](uint32_t n) {
+        const Tiles3D gp = grid_of(n);
+        const double h = 1.5 * n;
+        if (use_arena * h > double(arena_clauses)) return false;
+        uint64_t census_worst = gp.n_roots;
+        for (int l = 1; l <= L; ++l) {
+            const uint64_t r = g.ts[0] / g.ts[l - 1];
+            const bool clamped = gp.level_cap[l] < gp.n_roots * r * r * r;
+            if (clamped && use_jobs[l] * h > double(gp.level_cap[l])) return false;
+            if (l < L) { const uint64_t q = g.ts[l - 1] / g.ts[l]; census_worst += gp.level_cap[l] * q * q * q; }
+        }
+        const bool census_clamped = g.exact_census && gp.cap_census < census_worst;
+        return !census_clamped || use_census * h <= double(gp.cap_census);
+    };
+    struct Range { uint32_t f0, n; };
+    struct InFlight { Range r; int b; size_t ev0; };
+    std::vector<Range> redo;   // halves of overflowed passes (a stack: the first half runs next)
+    uint32_t next = 0;         // first frame no pass has taken yet
+    auto take = [&]() -> Range {
+        if (!redo.empty()) { const Range r = redo.back(); redo.pop_back(); return r; }
+        uint32_t n = std::min(n_max, n_frames - next);
+        if (!measured) n = 1;
+        else if (forced <= 0) while (n > 1 && !fits(n)) --n;
+        const Range r{next, n};
+        next += n;
+        return r;
+    };
+
+    Stats total{};
+    uint64_t arena_used = 0;
+    float stage_ms[16] = {};
+    size_t ev = 0;
+    uint32_t launches = 0;
+    bool copy_pending[2] = {false, false};
+    const VarBind vb0 = table[0].vb;   // (unused by the kernels: every frame comes from the table)
+    auto enqueue = [&](const Range& r, int b) -> int32_t {
+        Tiles3D gp = grid_of(r.n);
+        gp.frames = c->frame_table.as<Frame2D>() + r.f0;
+        if (host_out && copy_pending[b]) CU(cudaStreamWaitEvent(s, c->ev_copied[b], 0));   // staging buffer b is free again
+        CU(cudaMemsetAsync(c->counters.p, 0, sizeof(Counters), s));                         // (error bits are per pass)
+        CU(cudaMemsetAsync(c->heightmap.p, 0, size_t(r.n) * frame_rows * W * 8, s));
+        if (g.use_occl) CU(cudaMemsetAsync(c->occl.p, 0, occl_frame * r.n * 4, s));
+        if (want_stats) CU(cudaMemsetAsync(c->stats.p, 0, sizeof(Stats), s));
+        void* dimg = host_out ? static_cast<void*>(stage[b]) : static_cast<void*>(out + size_t(r.f0) * img_px);
+        if (int32_t erc = enqueue_tiles_3d(c, tape, cfg, gp, vb0, dimg, 0, r.n * H, want_stats, timing, cc, s, ev, launches))
+            return erc;
+        // the pass's counters and stats, into pinned slot b for the host to read while the next pass runs (the slot is
+        // read before buffer b takes another pass)
+        PassStatus* hs = c->pass_pin + b;
+        CU(cudaMemcpyAsync(&hs->ctr, c->counters.p, sizeof(Counters), cudaMemcpyDeviceToHost, s));
+        if (want_stats) CU(cudaMemcpyAsync(&hs->st, c->stats.p, sizeof(Stats), cudaMemcpyDeviceToHost, s));
+        CU(cudaEventRecord(c->ev_pass[b], s));
+        return FC_OK;
+    };
+    // Waits for a pass (watching the flag, as wait_call does) and reads its status.  Overflowed: its halves are queued
+    // again (one frame: the error).  Else its stats are added and, with a host `out`, its images copied back on the
+    // copy stream, which the host issues after the next pass is enqueued: a copy into pageable memory blocks the host.
+    auto settle = [&](const InFlight& f) -> int32_t {
+        if (int32_t wrc = wait_pass(c, f.b, cc, true)) return wrc;
+        const PassStatus& ps = c->pass_pin[f.b];
+        const double n = double(f.r.n);
+        use_arena = std::max(use_arena, double(ps.ctr.arena_top) / n);
+        use_census = std::max(use_census, double(ps.ctr.n_census) / n);
+        for (int l = 1; l <= L; ++l) use_jobs[l] = std::max(use_jobs[l], double(ps.ctr.n_jobs[l]) / n);
+        measured = true;
+        if (ps.ctr.error) {
+            if (f.r.n == 1 || (ps.ctr.error & ~3u)) return device_error(ps.ctr.error);
+            const uint32_t h = f.r.n / 2;
+            redo.push_back(Range{f.r.f0 + h, f.r.n - h});
+            redo.push_back(Range{f.r.f0, h});
+            return FC_OK;
+        }
+        if (want_stats) {
+            for (int l = 0; l < MAX_LEVELS; ++l) {
+                total.evaluated[l] += ps.st.evaluated[l];
+                total.filled_inside[l] += ps.st.filled_inside[l];
+                total.filled_outside[l] += ps.st.filled_outside[l];
+                total.ambiguous[l] += ps.st.ambiguous[l];
+                total.simplified[l] += ps.st.simplified[l];
+            }
+            total.pixels += ps.st.pixels;
+            total.grads += ps.st.grads;
+            arena_used = std::max<uint64_t>(arena_used, ps.ctr.arena_top * sizeof(uint2));
+            if (timing) add_stage_ms_3d(c, f.ev0, L, stage_ms);
+        }
+        if (host_out) {
+            copy_pending[f.b] = true;
+            return copy_pass_back(c, f.b, out + size_t(f.r.f0) * img_px, stage[f.b], size_t(f.r.n) * img_px * 16);
+        }
+        return FC_OK;
+    };
+    auto abandon = [&](int32_t rc) { return abandon_frames(c, s, stats, rc); };
+
+    const bool early_return = async && !host_out && !want_stats;
+    bool have_prev = false, stopped = false;
+    InFlight prev{};
+    int buf = 0;
+    for (;;) {
+        const bool more = next < n_frames || !redo.empty();
+        if (more && have_prev && cc.flag && __atomic_load_n(cc.flag, __ATOMIC_ACQUIRE)) stopped = true;   // enqueue no further pass
+        if (more && !stopped) {
+            if (have_prev && !measured) {   // the first pass is read before the second is sized
+                if (int32_t rc = settle(prev)) return abandon(rc);
+                have_prev = false;
+                continue;
+            }
+            const Range r = take();
+            const InFlight cur{r, buf, ev};
+            if (int32_t rc = enqueue(r, buf)) return abandon(rc);
+            if (have_prev)
+                if (int32_t rc = settle(prev)) return abandon(rc);
+            prev = cur;
+            have_prev = true;
+            buf ^= 1;
+            continue;
+        }
+        if (!have_prev) break;
+        if (early_return && !stopped) {   // FC_FLAG_ASYNC: the last pass is left running (its errors: fc_ctx_synchronize)
+            c->async_call = cc;
+            return FC_OK;
+        }
+        if (int32_t rc = settle(prev)) return abandon(rc);
+        have_prev = false;
+    }
+    if (cc.flag) {
+        if (int32_t wrc = wait_call(c, c->copy_stream, cc)) return abandon(wrc);
+    } else {
+        CU(cudaStreamSynchronize(c->copy_stream));
+    }
+    if (stopped) return abandon(fail(FC_ERR_CANCELLED, "cancelled"));   // the flag stopped the passes
+    if (stats) {
+        copy_census(total, stats);
+        stats->grads = total.grads;
+        stats->arena_bytes_used = arena_used;
+        stats->kernel_launches = launches;
+        memcpy(stats->stage_ms, stage_ms, sizeof stage_ms);
+    }
+    return FC_OK;
 }
 
 int32_t fc_merge_slabs(fc_ctx* c, const fc_geometry_pixel* const* slabs, uint32_t n_slabs, uint32_t width,

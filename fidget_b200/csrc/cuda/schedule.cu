@@ -349,8 +349,8 @@ int coop_blocks(fc_ctx* c, const fc_tape* tape, uint64_t n_roots, LevelParams& p
     for (int k = 1; k <= cap; ++k) if (rounds(k) < rounds(per_sm)) per_sm = k;
     // widest CTA for which the runtime really keeps per_sm of them resident (register granularity
     // makes 7 x 224 threads x 40 registers NOT fit although 7 * 224 * 40 < 64 K)
-    const bool frames = dim == 2 && p.frames;   // a 2D frame batch launches its own instantiation
-    auto& mm = c->coop_memo[dim == 3 ? 2 : int(frames)];
+    const bool frames = p.frames != nullptr;   // a frame batch launches its own instantiation
+    auto& mm = c->coop_memo[(dim == 3 ? 2 : 0) + int(frames)];
     if (mm.threads == 0 || mm.smem != smem || mm.per_sm != per_sm) {
         int t = COOP_THREADS;
         while (t > 64 && coop_occupancy(dim, frames, t, smem) < per_sm) t -= 32;

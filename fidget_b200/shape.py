@@ -566,10 +566,7 @@ def render2d_frames(shape: CudaShape, cfg: RenderConfig2D, z=None, var_values=No
     return (out, st.as_dict()) if stats else out
 
 
-def render3d(shape: CudaShape, cfg: RenderConfig3D, out=None, stats: bool = False, asynchronous: bool = False):
-    """voxel::render -> numpy structured array [h,w] of GEOMETRY_PIXEL (or fills ``out``); None when ``cfg.cancel``
-    cancelled it."""
-    lib = shape._lib
+def _render3d_cfg(cfg: RenderConfig3D, asynchronous: bool) -> _lib.FcRender3dCfg:
     c = _lib.FcRender3dCfg()
     c.width, c.height, c.depth = cfg.width, cfg.height, cfg.depth
     c.mat[:] = np.ascontiguousarray(cfg.matrix(), dtype=np.float32).reshape(16).tolist()
@@ -585,11 +582,85 @@ def render3d(shape: CudaShape, cfg: RenderConfig3D, out=None, stats: bool = Fals
     c.n_var_values = len(cfg.var_values)
     for i, v in enumerate(cfg.var_values):
         c.var_values[i] = float(v)
+    return c
+
+
+def render3d(shape: CudaShape, cfg: RenderConfig3D, out=None, stats: bool = False, asynchronous: bool = False):
+    """voxel::render -> numpy structured array [h,w] of GEOMETRY_PIXEL (or fills ``out``); None when ``cfg.cancel``
+    cancelled it."""
+    lib = shape._lib
+    c = _render3d_cfg(cfg, asynchronous)
     if out is None:
         out = np.zeros((cfg.height, cfg.width), dtype=GEOMETRY_PIXEL)
     st = _lib.FcRenderStats() if stats else None
     rc = shape.cuda._cancellable(cfg.cancel, lambda: lib.fc_render3d(shape.cuda._h, shape._h, C.byref(c), _ptr(out),
                                                                      C.byref(st) if stats else None), asynchronous)
+    if rc == _lib.FC_ERR_CANCELLED:
+        return None
+    _ck(rc)
+    return (out, st.as_dict()) if stats else out
+
+
+def frame_table_3d(cfg: RenderConfig3D, var_values=None, world_to_model=None, mats=None):
+    """The ``fc_frame3d`` table of ``render3d_frames``: frame k's matrix and ShapeVars, each exactly what ``render3d``
+    puts into ``fc_render3d_cfg`` for the config ``cfg`` with that frame's values: ``voxel_mat(w, h, d,
+    world_to_model[k])``, or ``mats[k]``, and ``var_values[k]``.  Every argument given is per frame (leading dimension
+    n: ``var_values`` [n, k], ``world_to_model`` [n, 4, 4], ``mats`` [n, 4, 4]); the others come from ``cfg``.
+    Lengths that disagree raise ValueError; with no per-frame argument at all there is one frame.  ``mats`` and
+    ``world_to_model`` are exclusive."""
+    if mats is not None and world_to_model is not None:
+        raise ValueError("give mats or world_to_model, not both")
+    per = {}
+    if var_values is not None:
+        vv = np.asarray(var_values, dtype=np.float32)
+        if vv.ndim != 2 or vv.shape[1] > _lib.FC_MAX_VARS:
+            raise ValueError(f"var_values must be [n, k] with k <= {_lib.FC_MAX_VARS}")
+        per["var_values"] = vv
+    for name, m in (("world_to_model", world_to_model), ("mats", mats)):
+        if m is not None:
+            m = np.asarray(m, dtype=np.float32)
+            if m.ndim != 3 or m.shape[1:] != (4, 4):
+                raise ValueError(f"{name} must be [n, 4, 4]")
+            per[name] = m
+    lengths = {k: len(v) for k, v in per.items()}
+    if len(set(lengths.values())) > 1:
+        raise ValueError(f"per-frame arguments disagree in length: {lengths}")
+    n = next(iter(lengths.values())) if lengths else 1
+    table = (_lib.FcFrame3d * n)()
+    base = None if ("mats" in per or "world_to_model" in per) else \
+        np.ascontiguousarray(cfg.matrix(), dtype=np.float32).reshape(16).tolist()
+    for k in range(n):
+        f = table[k]
+        if "mats" in per:
+            f.mat[:] = per["mats"][k].reshape(16).tolist()
+        elif "world_to_model" in per:
+            f.mat[:] = voxel_mat(cfg.width, cfg.height, cfg.depth, per["world_to_model"][k]).reshape(16).tolist()
+        else:
+            f.mat[:] = base
+        values = per["var_values"][k] if "var_values" in per else cfg.var_values
+        f.n_var_values = len(values)
+        for i, v in enumerate(values):
+            f.var_values[i] = float(v)
+    return table
+
+
+def render3d_frames(shape: CudaShape, cfg: RenderConfig3D, var_values=None, world_to_model=None, mats=None, out=None,
+                    stats: bool = False, asynchronous: bool = False):
+    """Many 3D frames of ``shape`` in one call (``fc_render3d_frames``): frame k is bit for bit ``render3d`` of
+    ``cfg`` with frame k's ``var_values`` / ``world_to_model`` / ``mats`` (see ``frame_table_3d``).  Returns a numpy
+    structured array [n, h, w] of GEOMETRY_PIXEL, or fills ``out`` (a numpy array or CUDA tensor of that many bytes,
+    contiguous).  None when ``cfg.cancel`` cancelled it."""
+    lib = shape._lib
+    table = frame_table_3d(cfg, var_values=var_values, world_to_model=world_to_model, mats=mats)
+    n = len(table)
+    c = _render3d_cfg(cfg, asynchronous)
+    if out is None:
+        out = np.zeros((n, cfg.height, cfg.width), dtype=GEOMETRY_PIXEL)
+    else:
+        _check_out(out, n * cfg.height * cfg.width * GEOMETRY_PIXEL.itemsize)
+    st = _lib.FcRenderStats() if stats else None
+    rc = shape.cuda._cancellable(cfg.cancel, lambda: lib.fc_render3d_frames(
+        shape.cuda._h, shape._h, C.byref(c), table, n, _ptr(out), C.byref(st) if stats else None), asynchronous)
     if rc == _lib.FC_ERR_CANCELLED:
         return None
     _ck(rc)

@@ -64,8 +64,8 @@ int32_t fc_ctx_set_arena_bytes(fc_ctx* ctx, uint64_t bytes);
 /* Cancellation (CancelToken, fidget-core/src/render/config.rs:59-80).  `flag` points to a caller-owned byte with the
  * layout of Rust's AtomicBool (CancelToken::into_raw() as *const u8): nonzero = cancelled.  The library reads it with
  * an acquire load, from any thread; NULL detaches it.  Context-wide, like fc_ctx_set_stream, and consulted only by
- * fc_render2d, fc_render2d_frames, fc_render3d, fc_octree_sample, fc_mesh_build, and fc_ctx_synchronize after the most recent
- * FC_FLAG_ASYNC call of those.  With a flag attached:
+ * fc_render2d, fc_render2d_frames, fc_render3d, fc_render3d_frames, fc_octree_sample, fc_mesh_build, and fc_ctx_synchronize
+ * after the most recent FC_FLAG_ASYNC call of those.  With a flag attached:
  *  - set on entry: the call returns FC_ERR_CANCELLED before it allocates or launches anything;
  *  - set while the call runs: the kernels stop claiming work and the call returns FC_ERR_CANCELLED ("cancelled" in
  *    fc_last_error); `out` is unspecified (a host `out` receives no copy), stats / info are zeroed, and the context
@@ -280,6 +280,34 @@ int32_t fc_render2d_frames(fc_ctx* ctx, const fc_tape* tape, const fc_render2d_c
  * GeometryPixel; host or device. */
 int32_t fc_render3d(fc_ctx* ctx, const fc_tape* tape, const fc_render3d_cfg* cfg, fc_geometry_pixel* out,
                     fc_render_stats* stats /* may be NULL */);
+
+/* Many 3D frames of one tape in one call: turntables, thumbnail views, camera paths, ShapeVars animations.  Frame k is
+ * bit-identical to fc_render3d called with `cfg` plus frame k's mat and var_values (depth and all three normal floats;
+ * same device arithmetic, libm operations included).  The frames of a pass share each launch of the tile pipeline.
+ *  - cfg supplies what the frames share: width, height, depth, tile_sizes, flags (FC_FLAG_FULL_LADDER,
+ *    FC_FLAG_NO_CLAMP, FC_FLAG_EXACT_CENSUS, FC_FLAG_TIMING, FC_FLAG_ASYNC); its mat and var_values are ignored.
+ *  - out (host or device) receives n_frames images of width*height fc_geometry_pixel back to back.
+ *  - stats: the per-level census, pixels and grads summed over all frames (the sum of the per-frame fc_render3d
+ *    stats, FC_FLAG_EXACT_CENSUS included), arena_bytes_used the largest of any pass, stage_ms summed over passes,
+ *    kernel_launches counting every pass run.
+ *  - passes: at most as many frames as fit FC_FRAMES_PASS_BYTES of device memory (heightmaps, occlusion maps, job
+ *    lists, and two staged images per frame with a host out).  FC_ERR_ARENA or a work-list overflow comes back only
+ *    where one frame alone overflows: the first pass renders one frame, later passes are sized from the largest
+ *    per-frame arena and list use seen so far, and a pass that still overflows is rendered again in halves.
+ *  - n_frames == 0 launches nothing and returns FC_OK.  FC_ERR_UNSUPPORTED for a spilled tape (as fc_render3d), Z slabs
+ *    (z_begin / z_end), root row bands and the tile interleave (root_stride > 1); FC_ERR_INVALID for a frame without a
+ *    value for a bound variable, a multi-output tape, and frames == NULL with n_frames > 0.
+ *  - The cancel flag behaves as in fc_render3d.  FC_FLAG_ASYNC (device out, no stats) returns once the last pass is
+ *    enqueued; every earlier pass has been waited on, because its overflow status decides whether it runs again.  An
+ *    overflow of the last pass is then reported by fc_ctx_synchronize, as fc_render3d's is. */
+typedef struct fc_frame3d {
+    float mat[16];                  /* row-major 4x4, as fc_render3d_cfg.mat (voxel::RenderConfig::mat) */
+    uint32_t n_var_values;          /* ShapeVars of this frame, as in fc_render3d_cfg */
+    float var_values[FC_MAX_VARS];
+} fc_frame3d;
+int32_t fc_render3d_frames(fc_ctx* ctx, const fc_tape* tape, const fc_render3d_cfg* cfg,
+                           const fc_frame3d* frames /* host */, uint32_t n_frames, fc_geometry_pixel* out,
+                           fc_render_stats* stats /* may be NULL */);
 /* Per-pixel merge of `n_slabs` slab images (each width*height, device
  * pointers, Z-ordered) into `out`, applying the final depth clamp of
  * voxel.rs:535-546.  Used after the all-gather in multi-GPU renders. */

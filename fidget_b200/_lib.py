@@ -129,6 +129,10 @@ FC_OUT_F32, FC_OUT_MASK_U8, FC_OUT_BITMAP_1BIT, FC_OUT_RGBA8 = 0, 1, 2, 3
 FC_ERR_CANCELLED = -6
 FC_FRAMES_PASS_BYTES = 512 << 20
 FC_MAX_VARS = 16
+FC_SCENE_MAX_SHAPES = 1024
+FC_SCENE_MAX_DEPTH = 262142
+FC_SCENE_MAX_ROOT_TILE = 1022
+FC_SCENE_MAX_LEAF_JOBS = 67108863
 
 # name -> (restype, argtypes); mirrors include/fidget_cuda.h one to one
 _vp, _u32, _i32, _u64, _u8 = C.c_void_p, C.c_uint32, C.c_int32, C.c_uint64, C.c_uint8
@@ -162,6 +166,7 @@ CUDA_API = {
     "fc_render2d_frames": (_i32, [_vp, _vp, _P(FcRender2dCfg), _P(FcFrame2d), _u32, _vp, _P(FcRenderStats)]),
     "fc_render3d": (_i32, [_vp, _vp, _P(FcRender3dCfg), _vp, _P(FcRenderStats)]),
     "fc_render3d_frames": (_i32, [_vp, _vp, _P(FcRender3dCfg), _P(FcFrame3d), _u32, _vp, _P(FcRenderStats)]),
+    "fc_render3d_scene": (_i32, [_vp, _P(_vp), _P(FcFrame3d), _u32, _P(FcRender3dCfg), _vp, _vp, _P(FcRenderStats)]),
     "fc_merge_slabs": (_i32, [_vp, _P(_vp), _u32, _u32, _u32, _u32, _vp]),
     "fc_tiles_per_rank": (_u32, [_u32, _u32, _u32, _u32]),
     "fc_tiles_pack": (_i32, [_vp, _vp, _u32, _u32, _u32, _u32, _u32, _u32, _vp]),

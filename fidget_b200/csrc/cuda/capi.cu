@@ -145,6 +145,9 @@ void fc_ctx_destroy(fc_ctx* c) {
     c->solve_res.release();
     c->frame_table.release();
     c->frame_tops.release();
+    c->scene_pl.release();
+    c->scene_backup.release();
+    c->scene_index.release();
     if (c->pass_pin) cudaFreeHost(c->pass_pin);
     if (c->copy_stream) {
         cudaStreamSynchronize(c->copy_stream);

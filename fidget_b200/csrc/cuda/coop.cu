@@ -38,7 +38,7 @@ __device__ __forceinline__ Rec load_rec(const CoopRec* recs, uint32_t i) {
     return Rec(__ldg(reinterpret_cast<const uint4*>(recs) + i));
 }
 
-template <int DIM, bool FRAMES = false>
+template <int DIM, bool FRAMES = false, bool SCENE = false>
 __global__ void __launch_bounds__(COOP_THREADS)
 k_interval_root_coop(const __grid_constant__ LevelParams p) {
     extern __shared__ __align__(16) unsigned char smem_raw[];
@@ -60,7 +60,7 @@ k_interval_root_coop(const __grid_constant__ LevelParams p) {
     const CoopRec* __restrict__ recs = p.sched.recs;
     const CoopFwd* __restrict__ fwd = p.sched.fwd;
     const uint32_t* __restrict__ ws = p.sched.wave_start;
-    const uint32_t n_roots = root_count(p, DIM == 3);
+    const uint32_t n_roots = SCENE ? scene_root_count(p) : root_count(p, DIM == 3);
     const uint2* __restrict__ tape = p.root_tape.ptr;
 
     for (;;) {
@@ -76,10 +76,11 @@ k_interval_root_coop(const __grid_constant__ LevelParams p) {
         __syncthreads();
         const uint32_t tile = s_tile;
         if (tile >= n_roots) break;
-        uint32_t cx, cy, cz;
-        root_corner(p, tile, T, cx, cy, cz);
+        uint32_t cx, cy, cz, pl = 0;
+        if (SCENE) pl = scene_root(p, tile, T, cx, cy, cz);
+        else root_corner(p, tile, T, cx, cy, cz);
         if (DIM != 3) cz = 0u;
-        const FrameView fv = frame_of<FRAMES>(p, cy);   // frame batch
+        const FrameView fv = view_of<FRAMES, SCENE>(p, cy, pl);   // frame batch, scene
         const VarBind& vb = *fv.vb;
         itv vx, vy, vz;
         xform_iv(*fv.mat, iv(float(cx), float(cx) + float(T)),
@@ -257,8 +258,9 @@ k_interval_root_coop(const __grid_constant__ LevelParams p) {
         const bool fill_in = !p.pixel_perfect && r.y < 0.0f;
         const bool fill_out = !p.pixel_perfect && !fill_in && r.x > 0.0f;
         const bool amb = !fill_in && !fill_out;
-        if (DIM == 3 && fill_in) {   // voxel.rs:310-317
-            const unsigned long long key = (unsigned long long)(cz + T + 1u) << 32;
+        if (DIM == 3 && fill_in) {   // voxel.rs:310-317 (scene: the fill's rank, kernels.cuh)
+            const unsigned long long key = SCENE ? scene_rank(cz + T + 1u, pl, p.clamp_at, p.depth)
+                                                 : (unsigned long long)(cz + T + 1u) << 32;
             for (uint32_t q = tid; q < T * T; q += NT) {   // (frame batch: rows below the frame are its padding)
                 const uint32_t x = cx + q % T, y = cy + q / T;
                 if (x < p.width && y - fv.y0 < p.height) atomicMax(&p.heightmap[size_t(y) * p.width + x], key);
@@ -266,7 +268,10 @@ k_interval_root_coop(const __grid_constant__ LevelParams p) {
             if (p.occl && T % 16u == 0u)
                 for (uint32_t q = tid; q < (T / 16u) * (T / 16u); q += NT) {
                     const uint32_t bx = cx / 16u + q % (T / 16u), by = cy / 16u + q / (T / 16u);
-                    if (bx < p.occl_w && by - fv.y0 / 16u < p.occl_h) atomicMax(p.occl + size_t(by) * p.occl_w + bx, cz + T + 1u);
+                    if (bx < p.occl_w && by - fv.y0 / 16u < p.occl_h) {
+                        if (SCENE) atomicMax(reinterpret_cast<unsigned long long*>(p.occl) + size_t(by) * p.occl_w + bx, key);
+                        else atomicMax(p.occl + size_t(by) * p.occl_w + bx, cz + T + 1u);
+                    }
                 }
         }
         if (tid == 0) {
@@ -482,7 +487,7 @@ k_interval_root_coop(const __grid_constant__ LevelParams p) {
                 o.x = cx;
                 o.y = cy;
                 o.z = cz;
-                o.pad = p.epoch;
+                o.pad = SCENE ? pl : p.epoch;
                 o.tape = child;
                 p.jobs_out[slot] = o;
                 atomicAdd(&p.ctr->outstanding, 1u);
@@ -492,45 +497,49 @@ k_interval_root_coop(const __grid_constant__ LevelParams p) {
     }
 }
 
-template <int DIM, bool FRAMES>
+template <int DIM, bool FRAMES, bool SCENE = false>
 static cudaError_t launch_coop(const LevelParams& p, int blocks, int threads, cudaStream_t s) {
     size_t smem = coop_smem_bytes(p.root_tape.n_ops, p.root_tape.n_choices, p.sched.n_slots);
     static size_t configured = 0;   // (per instantiation)
     if (smem > configured) {
-        cudaError_t e = cudaFuncSetAttribute(k_interval_root_coop<DIM, FRAMES>, cudaFuncAttributeMaxDynamicSharedMemorySize, int(smem));
+        cudaError_t e = cudaFuncSetAttribute(k_interval_root_coop<DIM, FRAMES, SCENE>, cudaFuncAttributeMaxDynamicSharedMemorySize, int(smem));
         if (e != cudaSuccess) return e;
         // many small CTAs per SM: ask for the largest shared-memory carve-out
-        cudaFuncSetAttribute(k_interval_root_coop<DIM, FRAMES>, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared);
+        cudaFuncSetAttribute(k_interval_root_coop<DIM, FRAMES, SCENE>, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared);
         configured = smem;
     }
-    k_interval_root_coop<DIM, FRAMES><<<blocks, threads, smem, s>>>(p);
+    k_interval_root_coop<DIM, FRAMES, SCENE><<<blocks, threads, smem, s>>>(p);
     return cudaGetLastError();
 }
-// the instantiation a launch takes: DIM, and whether it renders a frame batch (its register count differs)
-static void (*coop_kernel(int dim, bool frames))(LevelParams) {
-    if (dim == 3) return frames ? k_interval_root_coop<3, true> : k_interval_root_coop<3, false>;
-    return frames ? k_interval_root_coop<2, true> : k_interval_root_coop<2, false>;
+// the instantiation a launch takes: DIM, and whether it renders a frame batch or a 3D scene (register counts differ)
+static void (*coop_kernel(int dim, int variant))(LevelParams) {
+    if (dim == 3)
+        return variant == 2 ? k_interval_root_coop<3, false, true>
+             : variant == 1 ? k_interval_root_coop<3, true> : k_interval_root_coop<3, false>;
+    return variant ? k_interval_root_coop<2, true> : k_interval_root_coop<2, false>;
 }
-int coop_occupancy(int dim, bool frames, int threads, size_t smem) {
+int coop_occupancy(int dim, int variant, int threads, size_t smem) {
     int n = 0;
-    cudaOccupancyMaxActiveBlocksPerMultiprocessor(&n, coop_kernel(dim, frames), threads, smem);
+    cudaOccupancyMaxActiveBlocksPerMultiprocessor(&n, coop_kernel(dim, variant), threads, smem);
     return n;
 }
-int coop_regs_per_thread(int dim, bool frames) {
-    static int regs[4] = {0, 0, 0, 0};
-    int& r = regs[(dim == 3 ? 2 : 0) + int(frames)];
+int coop_regs_per_thread(int dim, int variant) {
+    static int regs[6] = {0, 0, 0, 0, 0, 0};
+    int& r = regs[(dim == 3 ? 3 : 0) + variant];
     if (!r) {
         cudaFuncAttributes a{};
-        cudaError_t e = cudaFuncGetAttributes(&a, coop_kernel(dim, frames));
+        cudaError_t e = cudaFuncGetAttributes(&a, coop_kernel(dim, variant));
         r = e == cudaSuccess ? a.numRegs : 64;
     }
     return r;
 }
-// (a frame batch, p.frames != null, takes the instantiation that reads its frames from the table)
+// (a frame batch, p.frames != null, takes the instantiation that reads its frames from the table; a scene, p.scene,
+// the one that reads its placements)
 cudaError_t launch_interval_root_coop_2d(const LevelParams& p, int blocks, int threads, cudaStream_t s) {
     return p.frames ? launch_coop<2, true>(p, blocks, threads, s) : launch_coop<2, false>(p, blocks, threads, s);
 }
 cudaError_t launch_interval_root_coop_3d(const LevelParams& p, int blocks, int threads, cudaStream_t s) {
+    if (p.scene) return launch_coop<3, false, true>(p, blocks, threads, s);
     return p.frames ? launch_coop<3, true>(p, blocks, threads, s) : launch_coop<3, false>(p, blocks, threads, s);
 }
 

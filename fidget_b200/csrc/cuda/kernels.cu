@@ -31,7 +31,7 @@ namespace fdev {
 // painted later by k_fill_2d).  DIM = 3: voxel::render tiles; an
 // interval-proven-inside tile raises the heightmap to its top + 1
 // (voxel.rs:310-317), heightmap entries are (depth << 32 | leaf job id + 1).
-template <int DIM, bool FUSED_PATH = false, bool FRAMES = false>
+template <int DIM, bool FUSED_PATH = false, bool FRAMES = false, bool SCENE = false>
 __global__ void __launch_bounds__(WARPS_PER_BLOCK * 32)
 k_interval_level(const __grid_constant__ LevelParams p) {
     __shared__ uint32_t live_s[WARPS_PER_BLOCK][8][32];
@@ -41,7 +41,7 @@ k_interval_level(const __grid_constant__ LevelParams p) {
     uint32_t* cs = p.choice_scratch + size_t(gw) * p.choice_words * 32u + lane;
     itv slots[REG_SLOTS];
 
-    const uint32_t n_roots = root_count(p, DIM == 3);
+    const uint32_t n_roots = SCENE ? scene_root_count(p) : root_count(p, DIM == 3);
     const uint32_t n_jobs = p.root_mode ? (n_roots + 31u) / 32u : min(p.ctr->n_jobs[p.level], p.cap_in);
 
     for (;;) {
@@ -53,7 +53,7 @@ k_interval_level(const __grid_constant__ LevelParams p) {
         j = __shfl_sync(FULL, j, 0);
         if (j >= n_jobs) break;
 
-        level_job<DIM, FUSED_PATH, FRAMES>(p, j, n_roots, slots, cs, live_s[wib], lane, p.epoch);
+        level_job<DIM, FUSED_PATH, FRAMES, SCENE>(p, j, n_roots, slots, cs, live_s[wib], lane, p.epoch);
     }
 }
 
@@ -66,7 +66,8 @@ void launch_interval_level_2d(const LevelParams& p, int blocks, cudaStream_t s) 
     else k_interval_level<2><<<blocks, WARPS_PER_BLOCK * 32, 0, s>>>(p);
 }
 void launch_interval_level_3d(const LevelParams& p, int blocks, cudaStream_t s) {
-    if (p.frames) k_interval_level<3, false, true><<<blocks, WARPS_PER_BLOCK * 32, 0, s>>>(p);   // a frame batch
+    if (p.scene) k_interval_level<3, false, false, true><<<blocks, WARPS_PER_BLOCK * 32, 0, s>>>(p);   // a scene
+    else if (p.frames) k_interval_level<3, false, true><<<blocks, WARPS_PER_BLOCK * 32, 0, s>>>(p);   // a frame batch
     else k_interval_level<3><<<blocks, WARPS_PER_BLOCK * 32, 0, s>>>(p);
 }
 
@@ -75,7 +76,8 @@ void launch_interval_level_3d(const LevelParams& p, int blocks, cudaStream_t s) 
 // and walks Z front to back (k descending), two points per tape pass; the
 // warp stops as soon as every column has hit the surface (voxel.rs:359-447).  FRAMES: a frame batch (the tile's
 // frame supplies matrix and vars; its screen rows are relative to the frame, its heightmap rows are grid rows).
-template <bool FRAMES>
+// SCENE: the tile's placement supplies them, and keys are scene ranks | id (kernels.cuh, scene_rank).
+template <bool FRAMES, bool SCENE = false>
 __global__ void __launch_bounds__(128) k_voxels_3d(const __grid_constant__ VoxelParams p) {
     const int lane = threadIdx.x & 31;
     float4 slots[REG_SLOTS];
@@ -96,7 +98,8 @@ __global__ void __launch_bounds__(128) k_voxels_3d(const __grid_constant__ Voxel
         const TapeRef tr = job->tape;
         const uint2* tape = tr.ptr;
         const unsigned long long id = (unsigned long long)(j + 1u);
-        const FrameView fv = frame_of<FRAMES>(p, cy);   // (uniform over the warp: one tile, one frame)
+        const uint32_t pl = SCENE ? job->pad : 0u;
+        const FrameView fv = view_of<FRAMES, SCENE>(p, cy, pl);   // (uniform over the warp: one tile, one frame)
         const Mat4& M = *fv.mat;
         for (uint32_t base = 0; base < ncol; base += 64u) {
             const uint32_t c0 = base + lane, c1 = c0 + 32u;
@@ -106,10 +109,18 @@ __global__ void __launch_bounds__(128) k_voxels_3d(const __grid_constant__ Voxel
             const uint32_t gx0 = cx + i0, gy0 = cy + j0, gx1 = cx + i1, gy1 = cy + j1;
             const uint32_t sy0 = gy0 - fv.y0, sy1 = gy1 - fv.y0;   // rows inside the frame
             const bool in0 = v0 && gx0 < p.width && sy0 < p.height, in1 = v1 && gx1 < p.width && sy1 < p.height;
-            // columns already at or above this tile's top are skipped (voxel.rs:376-381)
+            // columns already at or above this tile's top are skipped (voxel.rs:376-381); in a scene, columns whose
+            // rank is at least that of this placement's top voxel (a tie with a higher placement is not a skip)
             const uint32_t zmax = cz + T;
-            bool done0 = !in0 || uint32_t(p.heightmap[size_t(gy0) * p.width + gx0] >> 32) >= zmax;
-            bool done1 = !in1 || uint32_t(p.heightmap[size_t(gy1) * p.width + gx1] >> 32) >= zmax;
+            bool done0, done1;
+            if (SCENE) {
+                const unsigned long long top = scene_rank(zmax, pl, p.clamp_at, p.depth);
+                done0 = !in0 || (p.heightmap[size_t(gy0) * p.width + gx0] & ~SK_ID_MASK) >= top;
+                done1 = !in1 || (p.heightmap[size_t(gy1) * p.width + gx1] & ~SK_ID_MASK) >= top;
+            } else {
+                done0 = !in0 || uint32_t(p.heightmap[size_t(gy0) * p.width + gx0] >> 32) >= zmax;
+                done1 = !in1 || uint32_t(p.heightmap[size_t(gy1) * p.width + gx1] >> 32) >= zmax;
+            }
             // two Z levels per tape pass: (column 0, column 1) x (k, k - 1)
             for (int k = int(T) - 1; k >= 0; k -= 2) {
                 if (__all_sync(FULL, done0 && done1)) break;
@@ -123,8 +134,12 @@ __global__ void __launch_bounds__(128) k_voxels_3d(const __grid_constant__ Voxel
                 const float4 r = run_f32x4(tape, tr.n_ops, slots, [&](uint32_t i) {
                     return pick_input(*fv.vb, i, X, Y, Z, [](float f) { return make_float4(f, f, f, f); });
                 });
-                const unsigned long long key_hi = ((unsigned long long)(cz + uint32_t(k) + 1u) << 32) | id;
-                const unsigned long long key_lo = ((unsigned long long)(cz + uint32_t(k2) + 1u) << 32) | id;
+                const unsigned long long key_hi =
+                    (SCENE ? scene_rank(cz + uint32_t(k) + 1u, pl, p.clamp_at, p.depth)
+                           : (unsigned long long)(cz + uint32_t(k) + 1u) << 32) | id;
+                const unsigned long long key_lo =
+                    (SCENE ? scene_rank(cz + uint32_t(k2) + 1u, pl, p.clamp_at, p.depth)
+                           : (unsigned long long)(cz + uint32_t(k2) + 1u) << 32) | id;
                 const bool two = k > 0;
                 if (!done0) {
                     shaded += two ? 2 : 1;
@@ -145,7 +160,8 @@ __global__ void __launch_bounds__(128) k_voxels_3d(const __grid_constant__ Voxel
     }
 }
 void launch_voxels_3d(const VoxelParams& p, int blocks, cudaStream_t s) {
-    if (p.frames) k_voxels_3d<true><<<blocks, 128, 0, s>>>(p);
+    if (p.scene) k_voxels_3d<false, true><<<blocks, 128, 0, s>>>(p);
+    else if (p.frames) k_voxels_3d<true><<<blocks, 128, 0, s>>>(p);
     else k_voxels_3d<false><<<blocks, 128, 0, s>>>(p);
 }
 
@@ -234,14 +250,16 @@ void launch_census_3d(const CensusParams& p, int blocks, cudaStream_t s) { k_cen
 // at the surface voxel (x, y, depth - 1) with the tape of the
 // leaf tile that found it (voxel.rs:449-481); lanes of a warp that share a
 // leaf tile run its tape together.  FRAMES: a frame batch, whose output row y is row y % height of frame
-// y / height (a patch may straddle two frames: each lane takes its own frame's matrix and vars).
-template <bool FRAMES>
+// y / height (a patch may straddle two frames: each lane takes its own frame's matrix and vars).  SCENE: the key's
+// placement supplies them (kernels.cuh, scene_rank; NormalParams says which pixels a pass writes).
+template <bool FRAMES, bool SCENE = false>
 __global__ void __launch_bounds__(128) k_normals_3d(const __grid_constant__ NormalParams p) {
     grd slots[REG_SLOTS];
     const int lane = threadIdx.x & 31;
     // 8x4 pixel patch per warp
     const uint32_t warp = (blockIdx.x * blockDim.x + threadIdx.x) >> 5;
     if (cancel_poll(p.cancel, CS_NORMALS_3D, warp)) return;   // one patch per warp: the claim is the launch itself
+    if (SCENE && *p.error) return;                            // an overflowed pass is rendered again
     uint32_t x, y;
     if (p.root_list) {   // patches of the listed root tiles only
         const uint32_t ppt = (p.root_tile / 8u) * (p.root_tile / 4u), ppr = p.root_tile / 8u;
@@ -267,9 +285,23 @@ __global__ void __launch_bounds__(128) k_normals_3d(const __grid_constant__ Norm
         vb = &p.frames[f].vb;
     }
     const unsigned long long key = inb ? p.heightmap[size_t(hy) * p.width + x] : 0ull;
-    const uint32_t depth = uint32_t(key >> 32), id = uint32_t(key);
+    uint32_t depth = uint32_t(key >> 32), id = uint32_t(key);
+    bool write = inb;
+    uint32_t pl = 0;
+    if (SCENE) {   // decode the scene key: placement, raw depth (clamp zone: threshold + excess), leaf id
+        const uint32_t sub = uint32_t(key >> SK_ID_BITS) & ((1u << SK_SUB_BITS) - 1u);
+        const uint32_t prio = uint32_t(key >> (SK_ID_BITS + SK_SUB_BITS)) & (SK_MAX_SHAPES - 1u);
+        const uint32_t dc = uint32_t(key >> (SK_ID_BITS + SK_SUB_BITS + SK_PRIO_BITS));
+        id = uint32_t(key & SK_ID_MASK);
+        pl = key ? SK_MAX_SHAPES - 1u - prio : 0u;
+        depth = (p.clamp && dc == p.depth) ? p.depth - 1u + sub : dc;
+        write = inb && (key == 0ull || (pl >= p.pl0 && pl < p.pl1));   // an earlier pass's winner keeps its pixel
+        M = &p.frames[pl].mat;
+        vb = &p.frames[pl].vb;
+        if (p.clamp && p.depth <= 1u) pl = 0;   // (every image is clamped everywhere: the first one is kept)
+    }
     grd g = gr(0.0f, 0.0f, 0.0f, 0.0f);
-    bool pending = inb && id != 0u;
+    bool pending = write && id != 0u;
     unsigned long long n = 0;
     for (;;) {
         const uint32_t m = __ballot_sync(FULL, pending);
@@ -286,7 +318,7 @@ __global__ void __launch_bounds__(128) k_normals_3d(const __grid_constant__ Norm
         });
         if (mine) { g = r; pending = false; ++n; }
     }
-    if (inb) {
+    if (write) {
         float4 o;
         if (p.clamp && depth >= p.depth - 1u) {   // voxel.rs:535-546
             o = make_float4(0.0f, 0.0f, 1.0f, __uint_as_float(p.depth));
@@ -294,6 +326,7 @@ __global__ void __launch_bounds__(128) k_normals_3d(const __grid_constant__ Norm
             o = make_float4(g.y, g.z, g.w, __uint_as_float(depth));
         }
         reinterpret_cast<float4*>(p.out)[size_t(y) * p.width + x] = o;
+        if (SCENE && p.index) p.index[size_t(y) * p.width + x] = uint16_t(pl);
     }
     if (p.stats) {
         for (int o = 16; o > 0; o >>= 1) n += __shfl_xor_sync(FULL, n, o);
@@ -304,7 +337,8 @@ void launch_normals_3d(const NormalParams& p, cudaStream_t s) {
     const uint64_t warps = p.root_list ? uint64_t(p.n_root_list) * (p.root_tile / 8u) * (p.root_tile / 4u)
                                        : uint64_t((p.width + 7u) / 8u) * ((p.y1 - p.y0 + 3u) / 4u);
     if (!warps) return;
-    if (p.frames) k_normals_3d<true><<<unsigned((warps + 3) / 4), 128, 0, s>>>(p);
+    if (p.scene) k_normals_3d<false, true><<<unsigned((warps + 3) / 4), 128, 0, s>>>(p);
+    else if (p.frames) k_normals_3d<true><<<unsigned((warps + 3) / 4), 128, 0, s>>>(p);
     else k_normals_3d<false><<<unsigned((warps + 3) / 4), 128, 0, s>>>(p);
 }
 

@@ -153,6 +153,26 @@ struct Frame2D {
     VarBind vb;
 };
 
+// Scene renders (fc_render3d_scene): K placements (a tape and its Frame2D) share one heightmap and one occlusion map.
+// Placement k's jobs carry k in TileJob::pad.  A heightmap key orders what the merged image keeps: the greater clamped
+// depth, then the lower placement, then, inside one placement, what fc_render3d orders by (raw depth, then a leaf id
+// over a fill).  Packed high to low: clamped depth (SK_DEPTH_BITS), priority 1023 - k (SK_PRIO_BITS), raw depth above
+// the clamp threshold D - 1 (SK_SUB_BITS: 0 outside the clamp zone), leaf job id + 1 (SK_ID_BITS, 0 for a fill).  The
+// key without its id is the placement's rank of a depth: what a skipped tile is compared against.  The occlusion map of
+// a scene holds 64-bit ranks.  The host checks the limits the field widths imply (FC_SCENE_* in fidget_cuda.h).
+constexpr uint32_t SK_ID_BITS = 26, SK_SUB_BITS = 10, SK_PRIO_BITS = 10, SK_DEPTH_BITS = 18;
+constexpr uint32_t SK_MAX_SHAPES = 1u << SK_PRIO_BITS;
+constexpr unsigned long long SK_ID_MASK = (1ull << SK_ID_BITS) - 1ull;
+#ifdef __CUDACC__
+// rank of raw depth `raw` for placement `pl`; clamp_at = D - 1 when the final clamp applies (depths >= D - 1 compare
+// as D), 0xffffffff without it
+__device__ __forceinline__ unsigned long long scene_rank(uint32_t raw, uint32_t pl, uint32_t clamp_at, uint32_t depth) {
+    const bool zone = raw >= clamp_at;
+    const unsigned long long dc = zone ? depth : raw, sub = zone ? raw - clamp_at : 0u;
+    return ((((dc << SK_PRIO_BITS) | (SK_MAX_SHAPES - 1u - pl)) << SK_SUB_BITS) | sub) << SK_ID_BITS;
+}
+#endif
+
 struct LevelParams {
     CoopSched sched;
     int level;                 // index into tile sizes
@@ -209,6 +229,13 @@ struct LevelParams {
     // frame; 3D: occl_h counts the block rows of one frame, and frame k's blocks start at row k * frame_rows / 16
     const Frame2D* frames;
     uint32_t frame_rows;
+    // scene (fc_render3d_scene): `frames` is the placement table; level 0 evaluates the root tiles of the n_scene_pl
+    // placements listed in scene_pl (those of root_tape), roots_x * roots_y * roots_z per placement; the heightmap
+    // keys and the occlusion map hold scene ranks (clamp_at: see scene_rank)
+    uint32_t scene;
+    const uint32_t* scene_pl;
+    uint32_t n_scene_pl;
+    uint32_t clamp_at;
 };
 
 #ifdef __CUDACC__
@@ -225,6 +252,16 @@ __device__ __forceinline__ void root_corner(const LevelParams& p, uint32_t idx, 
     cx = p.root_x0 + (xy % p.roots_x) * T;
     cy = p.root_y0 + (xy / p.roots_x) * T;
     cz = p.root_z0 + zl * T;
+}
+// scene: the root tiles of every listed placement, placement-major; corner and placement of root `idx`
+__device__ __forceinline__ uint32_t scene_root_count(const LevelParams& p) {
+    return p.n_scene_pl * p.roots_x * p.roots_y * p.roots_z;
+}
+__device__ __forceinline__ uint32_t scene_root(const LevelParams& p, uint32_t idx, uint32_t T, uint32_t& cx, uint32_t& cy,
+                                               uint32_t& cz) {
+    const uint32_t per = p.roots_x * p.roots_y * p.roots_z;
+    root_corner(p, idx % per, T, cx, cy, cz);
+    return __ldg(p.scene_pl + idx / per);
 }
 #endif
 
@@ -267,6 +304,13 @@ __device__ __forceinline__ FrameView frame_of(const P& p, uint32_t y) {
     const Frame2D* fr = p.frames + f;
     return FrameView{&fr->mat, fr->z, &fr->vb, f * p.frame_rows, f * p.height};
 }
+// SCENE (another compile-time switch): the placement `pl` of the tile supplies matrix and vars; all placements share
+// the screen grid, so coordinates are not offset
+template <bool FRAMES, bool SCENE, class P>
+__device__ __forceinline__ FrameView view_of(const P& p, uint32_t y, uint32_t pl) {
+    if (SCENE) return FrameView{&p.frames[pl].mat, 0.0f, &p.frames[pl].vb, 0u, 0u};
+    return frame_of<FRAMES>(p, y);
+}
 #endif
 
 struct FillParams {
@@ -292,6 +336,7 @@ struct VoxelParams {
     CancelRef cancel;
     const Frame2D* frames;      // 3D frame batch, as in LevelParams (job y is a grid row; the heightmap has its rows)
     uint32_t frame_rows;
+    uint32_t scene, depth, clamp_at;   // scene: `frames` is the placement table, keys are scene ranks | id
 };
 struct NormalParams {
     uint32_t width, height, depth;
@@ -311,6 +356,12 @@ struct NormalParams {
     // heightmap row k * frame_rows + y), each frame with its matrix and vars from the table
     const Frame2D* frames;
     uint32_t frame_rows;
+    // scene: `frames` is the placement table.  Only pixels whose key belongs to placements pl0 .. pl1 - 1 (this pass's:
+    // their leaf ids index this pass's leaf list) or is empty are written, with the placement into `index` (or null),
+    // and nothing at all when the pass overflowed (`error` != 0: it is rendered again)
+    uint32_t scene, pl0, pl1;
+    uint16_t* index;
+    const uint32_t* error;
 };
 
 // One leaf of the Manifold-Dual-Contouring octree (LeafHermiteData, fidget-mesh/src/octree.rs:864-900)
@@ -367,9 +418,9 @@ void launch_tiles_copy(const void* src, void* dst, uint32_t width, uint32_t heig
                        uint32_t roots_x, uint32_t roots_y, const uint32_t* slots, uint32_t n_ranks, uint32_t per_rank, int rank,
                        cudaStream_t s);
 void launch_interval_level_2d(const LevelParams& p, int blocks, cudaStream_t s);
-// occupancy of the level-0 kernel instantiation a launch takes (frames: a 2D frame batch)
-int coop_regs_per_thread(int dim, bool frames);
-int coop_occupancy(int dim, bool frames, int threads, size_t smem);
+// occupancy of the level-0 kernel instantiation a launch takes (variant 0: one frame, 1: a frame batch, 2: a 3D scene)
+int coop_regs_per_thread(int dim, int variant);
+int coop_occupancy(int dim, int variant, int threads, size_t smem);
 size_t coop_smem_bytes(uint32_t n_ops, uint32_t n_choices, uint32_t n_slots);
 cudaError_t launch_interval_root_coop_2d(const LevelParams& p, int blocks, int threads, cudaStream_t s);
 cudaError_t launch_interval_root_coop_3d(const LevelParams& p, int blocks, int threads, cudaStream_t s);

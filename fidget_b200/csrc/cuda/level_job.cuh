@@ -42,13 +42,13 @@ __device__ __forceinline__ void store_fill(FillRec* dst, const FillRec& fr) {
     *reinterpret_cast<uint4*>(dst) = make_uint4(fr.x, fr.y, fr.value, fr.ready);
 }
 
-template <int DIM, bool FUSED, bool FRAMES = false>
+template <int DIM, bool FUSED, bool FRAMES = false, bool SCENE = false>
 __device__ __forceinline__ void level_job(const LevelParams& p, uint32_t j, uint32_t n_roots, itv* slots, uint32_t* cs,
                                           uint32_t (*live)[32], int lane, uint32_t epoch) {
     const uint32_t T = p.tile;
     bool cull_open = false, cull_check = false;
     TapeRef tr;
-    uint32_t px = 0, py = 0, pz = 0, nchild;
+    uint32_t px = 0, py = 0, pz = 0, nchild, ppl = 0;   // (SCENE: ppl = the parent's placement)
     if (p.root_mode) {
         tr = p.root_tape;
         nchild = min(32u, n_roots - j * 32u);
@@ -60,6 +60,7 @@ __device__ __forceinline__ void level_job(const LevelParams& p, uint32_t j, uint
         py = jb.y;
         pz = jb.z;
         tr = jb.tape;
+        if (SCENE) ppl = jb.pad;
         nchild = p.n_axis * p.n_axis * (DIM == 3 ? p.n_axis : 1u);
         if (DIM == 3 && p.mode != 1u && p.cull) {
             // Every pixel under this parent already holds depth >= its top + 1 (tiles in front, proven inside by coarser
@@ -68,9 +69,15 @@ __device__ __forceinline__ void level_job(const LevelParams& p, uint32_t j, uint
             // front, which arrive last here.  One small read of the occlusion map per lane, not the heightmap itself.
             const uint32_t nb = (T * p.n_axis) / 16u, need = pz + T * p.n_axis + 1u;   // blocks per side of the parent
             const uint32_t fb0 = frame_of<FRAMES>(p, py).y0 / 16u;                      // (frame batch: its first block row)
+            // (scene: every block must hold at least the rank of this placement's fill at top + 1: a greater depth, or
+            //  that depth from this placement or a lower one -- a tie with a higher placement must still be evaluated)
+            const unsigned long long need_rank = SCENE ? scene_rank(need, ppl, p.clamp_at, p.depth) : 0ull;
             for (uint32_t q = lane; q < nb * nb; q += 32u) {
                 const uint32_t bx = px / 16u + q % nb, by = py / 16u + q / nb;
-                if (bx < p.occl_w && by - fb0 < p.occl_h) cull_open |= __ldcg(p.occl + size_t(by) * p.occl_w + bx) < need;
+                if (bx < p.occl_w && by - fb0 < p.occl_h) {
+                    if constexpr (SCENE) cull_open |= __ldcg(reinterpret_cast<const unsigned long long*>(p.occl) + size_t(by) * p.occl_w + bx) < need_rank;
+                    else cull_open |= __ldcg(p.occl + size_t(by) * p.occl_w + bx) < need;
+                }
             }
             cull_check = true;
         }
@@ -80,9 +87,10 @@ __device__ __forceinline__ void level_job(const LevelParams& p, uint32_t j, uint
     for (uint32_t chunk = 0; chunk * 32u < nchild; ++chunk) {
         const uint32_t c = chunk * 32u + lane;
         const bool valid = c < nchild;
-        uint32_t cx, cy, cz = 0;
+        uint32_t cx, cy, cz = 0, pl = ppl;
         if (p.root_mode) {
-            root_corner(p, j * 32u + (valid ? c : 0u), T, cx, cy, cz);
+            if (SCENE) pl = scene_root(p, j * 32u + (valid ? c : 0u), T, cx, cy, cz);
+            else root_corner(p, j * 32u + (valid ? c : 0u), T, cx, cy, cz);
         } else {
             uint32_t cc = valid ? c : 0u;
             cx = px + (cc % p.n_axis) * T;
@@ -91,7 +99,7 @@ __device__ __forceinline__ void level_job(const LevelParams& p, uint32_t j, uint
         }
         // Region in screen coordinates -> model space (pixel.rs:325-342, voxel.rs:291-306); in a frame batch a
         // tile's coordinates are relative to its frame (per lane at level 0, whose 32 roots may span frames)
-        const FrameView fv = frame_of<FRAMES>(p, cy);
+        const FrameView fv = view_of<FRAMES, SCENE>(p, cy, pl);
         const Mat4& M = *fv.mat;
         const VarBind& vb = *fv.vb;
         itv X = iv(float(cx), float(cx) + float(T));
@@ -137,7 +145,9 @@ __device__ __forceinline__ void level_job(const LevelParams& p, uint32_t j, uint
                 m &= m - 1;
                 const uint32_t fx = __shfl_sync(FULL, cx, src), fy = __shfl_sync(FULL, cy, src),
                                fz = __shfl_sync(FULL, cz, src);
-                const unsigned long long key = (unsigned long long)(fz + T + 1u) << 32;
+                // (scene: the fill's rank, which carries its placement)
+                const unsigned long long key = SCENE ? scene_rank(fz + T + 1u, __shfl_sync(FULL, pl, src), p.clamp_at, p.depth)
+                                                     : (unsigned long long)(fz + T + 1u) << 32;
                 // (frame batch: rows past the bottom of the tile's frame are its padding, not the next frame's image)
                 const uint32_t fy0 = frame_of<FRAMES>(p, fy).y0;
                 for (uint32_t q = lane; q < T * T; q += 32u) {
@@ -147,7 +157,10 @@ __device__ __forceinline__ void level_job(const LevelParams& p, uint32_t j, uint
                 if (p.occl && T % 16u == 0u)   // the whole blocks this tile covers now hold its depth (the same value the heightmap gets)
                     for (uint32_t q = lane; q < (T / 16u) * (T / 16u); q += 32u) {
                         const uint32_t bx = fx / 16u + q % (T / 16u), by = fy / 16u + q / (T / 16u);
-                        if (bx < p.occl_w && by - fy0 / 16u < p.occl_h) atomicMax(p.occl + size_t(by) * p.occl_w + bx, fz + T + 1u);
+                        if (bx < p.occl_w && by - fy0 / 16u < p.occl_h) {
+                            if (SCENE) atomicMax(reinterpret_cast<unsigned long long*>(p.occl) + size_t(by) * p.occl_w + bx, key);
+                            else atomicMax(p.occl + size_t(by) * p.occl_w + bx, fz + T + 1u);
+                        }
                     }
             }
             if (p.stats) {
@@ -268,7 +281,7 @@ __device__ __forceinline__ void level_job(const LevelParams& p, uint32_t j, uint
                     o.pad = 0;
                     o.tape = child;
                     if (FUSED) publish_job(p.jobs_out + slot, o, epoch);   // fields, fence, then the ready mark
-                    else { o.pad = epoch; p.jobs_out[slot] = o; }
+                    else { o.pad = SCENE ? pl : epoch; p.jobs_out[slot] = o; }
                 } else {
                     atomicOr(&p.ctr->error, 2u);
                     atomicSub(&p.ctr->outstanding, 1u);   // never claimable: do not wait for it

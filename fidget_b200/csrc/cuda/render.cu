@@ -1,5 +1,5 @@
 // The fused tile renderers: fc_render2d (pixel::render), fc_render3d (voxel::render), their frame batches
-// (fc_render2d_frames, fc_render3d_frames), fc_merge_slabs.
+// (fc_render2d_frames, fc_render3d_frames), 3D scenes of several shapes (fc_render3d_scene), fc_merge_slabs.
 #include <cstddef>
 
 #include "capi_internal.h"
@@ -399,6 +399,13 @@ struct Tiles3D {
     uint32_t occl_w = 0, occl_h = 0;    // occlusion blocks per row, block rows of one frame
     const Frame2D* frames = nullptr;
     uint32_t frame_rows = 0xffffffffu;
+    // scene (fc_render3d_scene): `frames` is the placement table; a pass renders placements pl0 .. pl1 - 1, listed at
+    // d_pl grouped by tape (level 0 runs once per group, with the group's tape); clamp_at as in scene_rank
+    struct Group { const fc_tape* tape; uint32_t first, n; };
+    bool scene = false;
+    std::vector<Group> groups;
+    const uint32_t* d_pl = nullptr;
+    uint32_t pl0 = 0, pl1 = 0, clamp_at = 0xffffffffu;
 };
 
 static int32_t check_3d(const fc_tape* tape, const fc_render3d_cfg* cfg) {
@@ -479,11 +486,13 @@ static int32_t ensure_scratch_3d(fc_ctx* c, const Tiles3D& g, size_t hm_pixels, 
 static uint32_t zsort_layers(const Tiles3D& g) { return (g.roots_z * g.ts[0]) / g.ts.back(); }
 
 // The tile pipeline of fc_render3d (voxel::render), enqueued on `s`: the interval levels, the front-to-back sort of
-// the leaf tiles, the leaf voxels, the exact census and the normals of output rows y0 .. y1 into `dimg`.  The caller
+// the leaf tiles, the leaf voxels, the exact census and the normals of output rows y0 .. y1 into `dimg` (a scene pass:
+// level 0 once per group of g, and the placement of every pixel it finishes into `index`, if not null).  The caller
 // has sized the scratch and zeroed the counters, the heightmap rows, the occlusion map and the stats.
 static int32_t enqueue_tiles_3d(fc_ctx* c, const fc_tape* tape, const fc_render3d_cfg* cfg, const Tiles3D& g,
                                 const VarBind& vb, void* dimg, uint32_t y0, uint32_t y1, bool want_stats, bool timing,
-                                const CallCancel& cc, cudaStream_t s, size_t& ev, uint32_t& launches) {
+                                const CallCancel& cc, cudaStream_t s, size_t& ev, uint32_t& launches,
+                                uint16_t* index = nullptr) {
     const std::vector<uint32_t>& ts = g.ts;
     const int L = int(ts.size());
     const uint32_t T0 = ts[0];
@@ -526,22 +535,45 @@ static int32_t enqueue_tiles_3d(fc_ctx* c, const fc_tape* tape, const fc_render3
         p.cancel = cc.ref;
         p.frames = g.frames;
         p.frame_rows = g.frame_rows;
-        int blocks = (l == L - 1 && l > 0) ? g.grid_blocks_last : g.grid_blocks;
-        if (l == 0) {
-            uint64_t warps = (g.n_roots + 31) / 32;
-            blocks = int(std::min<uint64_t>((warps + WARPS_PER_BLOCK - 1) / WARPS_PER_BLOCK, uint64_t(g.grid_blocks)));
-        }
-        bool coop = false;
-        if (l == 0) {
-            int ct = COOP_THREADS;
-            int cb = coop_blocks(c, tape, g.n_roots, p, 3, ct);
-            if (cb > 0) {
-                CU(launch_interval_root_coop_3d(p, cb, ct, s));
-                coop = true;
+        p.scene = g.scene ? 1u : 0u;
+        p.clamp_at = g.clamp_at;
+        auto launch = [&](const fc_tape* t, uint64_t n_roots) -> int32_t {
+            int blocks = (l == L - 1 && l > 0) ? g.grid_blocks_last : g.grid_blocks;
+            if (l == 0) {
+                uint64_t warps = (n_roots + 31) / 32;
+                blocks = int(std::min<uint64_t>((warps + WARPS_PER_BLOCK - 1) / WARPS_PER_BLOCK, uint64_t(g.grid_blocks)));
             }
+            bool coop = false;
+            if (l == 0) {
+                int ct = COOP_THREADS;
+                int cb = coop_blocks(c, t, n_roots, p, 3, ct);
+                if (cb > 0) {
+                    CU(launch_interval_root_coop_3d(p, cb, ct, s));
+                    coop = true;
+                }
+            }
+            if (!coop) launch_interval_level_3d(p, std::max(blocks, 1), s);
+            ++launches;
+            return FC_OK;
+        };
+        if (l == 0 && g.scene) {
+            // level 0 of a scene: one launch per distinct tape over the root tiles of its placements, each with that
+            // tape's schedule; their children go to one shared level-1 list (the claim cursor restarts per launch)
+            const uint64_t per = uint64_t(g.roots_x) * g.roots_y * g.roots_z;
+            for (size_t k = 0; k < g.groups.size(); ++k) {
+                const Tiles3D::Group& gr = g.groups[k];
+                p.root_tape.ptr = gr.tape->dev;
+                p.root_tape.n_ops = gr.tape->info.n_ops;
+                p.root_tape.ref_len = gr.tape->info.ref_len;
+                p.root_tape.n_choices = gr.tape->info.choice_count;
+                p.scene_pl = g.d_pl + gr.first;
+                p.n_scene_pl = gr.n;
+                if (k) CU(cudaMemsetAsync(&c->counters.as<Counters>()->cursor[0], 0, sizeof(uint32_t), s));
+                if (int32_t lrc = launch(gr.tape, per * gr.n)) return lrc;
+            }
+        } else if (int32_t lrc = launch(tape, g.n_roots)) {
+            return lrc;
         }
-        if (!coop) launch_interval_level_3d(p, std::max(blocks, 1), s);
-        ++launches;
         if (timing) CU(cudaEventRecord(get_event(c, ev++), s));
     }
     {
@@ -569,6 +601,9 @@ static int32_t enqueue_tiles_3d(fc_ctx* c, const fc_tape* tape, const fc_render3
         q.cancel = cc.ref;
         q.frames = g.frames;
         q.frame_rows = g.frame_rows;
+        q.scene = g.scene ? 1u : 0u;
+        q.depth = cfg->depth;
+        q.clamp_at = g.clamp_at;
         launch_voxels_3d(q, c->sm_count * env_int("FIDGET_B200_VOXEL_BLOCKS_PER_SM", 12), s);
         ++launches;
     }
@@ -607,6 +642,11 @@ static int32_t enqueue_tiles_3d(fc_ctx* c, const fc_tape* tape, const fc_render3
         q.cancel = cc.ref;
         q.frames = g.frames;
         q.frame_rows = g.frame_rows;
+        q.scene = g.scene ? 1u : 0u;
+        q.pl0 = g.pl0;
+        q.pl1 = g.pl1;
+        q.index = index;
+        q.error = &c->counters.as<Counters>()->error;
         launch_normals_3d(q, s);
         ++launches;
     }
@@ -1220,6 +1260,238 @@ int32_t fc_render3d_frames(fc_ctx* c, const fc_tape* tape, const fc_render3d_cfg
         CU(cudaStreamSynchronize(c->copy_stream));
     }
     if (stopped) return abandon(fail(FC_ERR_CANCELLED, "cancelled"));   // the flag stopped the passes
+    if (stats) {
+        copy_census(total, stats);
+        stats->grads = total.grads;
+        stats->arena_bytes_used = arena_used;
+        stats->kernel_launches = launches;
+        memcpy(stats->stage_ms, stage_ms, sizeof stage_ms);
+    }
+    return FC_OK;
+}
+
+// A scene: every placement's tiles go through one tile pipeline over one shared heightmap and occlusion map, whose keys
+// order what the fold of the per-shape images keeps (kernels.cuh, scene_rank).  Placements run in passes: a pass lists
+// its placements grouped by tape for level 0, then shares every later launch; its normals finish the pixels it won.
+int32_t fc_render3d_scene(fc_ctx* c, const fc_tape* const* tapes, const fc_frame3d* placements, uint32_t n_shapes,
+                          const fc_render3d_cfg* cfg, fc_geometry_pixel* out, uint16_t* index, fc_render_stats* stats) {
+    static_assert(FC_SCENE_MAX_SHAPES == SK_MAX_SHAPES, "FC_SCENE_MAX_SHAPES is the key's placement field");
+    static_assert(FC_SCENE_MAX_DEPTH + 2 == (1u << SK_DEPTH_BITS), "FC_SCENE_MAX_DEPTH + 1 is the key's largest depth");
+    static_assert(FC_SCENE_MAX_ROOT_TILE + 1 == (1u << SK_SUB_BITS) - 1, "depths reach a root tile + 1 above the clamp threshold");
+    static_assert(FC_SCENE_MAX_LEAF_JOBS == SK_ID_MASK, "leaf id + 1 is the key's id field");
+    if (!c || !cfg || !out || (n_shapes && (!tapes || !placements))) return fail(FC_ERR_INVALID, "null argument");
+    if (n_shapes > FC_SCENE_MAX_SHAPES) return fail(FC_ERR_UNSUPPORTED, "more than FC_SCENE_MAX_SHAPES shapes");
+    if (cfg->flags & FC_FLAG_EXACT_CENSUS) return fail(FC_ERR_UNSUPPORTED, "the exact census is not supported by scenes");
+    if (cfg->z_begin || cfg->z_end) return fail(FC_ERR_UNSUPPORTED, "Z slabs are not supported by scenes");
+    if (cfg->root_row_begin || cfg->root_row_end) return fail(FC_ERR_UNSUPPORTED, "root row bands are not supported by scenes");
+    if (cfg->root_stride > 1) return fail(FC_ERR_UNSUPPORTED, "the tile interleave is not supported by scenes");
+    // every placement's tape and ShapeVars binding, and the key's limits, before anything is allocated or launched
+    std::vector<Frame2D> table(n_shapes);
+    for (uint32_t k = 0; k < n_shapes; ++k) {
+        if (!tapes[k]) return fail(FC_ERR_INVALID, "null tape in the scene");
+        if (int32_t vrc = check_3d(tapes[k], cfg)) return vrc;
+        if (placements[k].n_var_values > FC_MAX_VARS) return fail(FC_ERR_INVALID, "n_var_values above FC_MAX_VARS");
+        memcpy(table[k].mat.m, placements[k].mat, sizeof table[k].mat.m);
+        table[k].z = 0.0f;
+        if (int32_t brc = bind_vars(tapes[k], placements[k].var_values, placements[k].n_var_values, table[k].vb)) return brc;
+    }
+    Tiles3D g;
+    const bool clamp = !(cfg->flags & FC_FLAG_NO_CLAMP);
+    if (n_shapes) {
+        if (int32_t rc = prepare_3d(c, tapes[0], cfg, g)) return rc;
+        const uint32_t T0 = g.ts[0];
+        if (uint64_t((cfg->depth + T0 - 1) / T0) * T0 > FC_SCENE_MAX_DEPTH)
+            return fail(FC_ERR_UNSUPPORTED, "scene depth (rounded up to whole root tiles) above FC_SCENE_MAX_DEPTH");
+        if (clamp && T0 > FC_SCENE_MAX_ROOT_TILE)
+            return fail(FC_ERR_UNSUPPORTED, "scene root tile edge above FC_SCENE_MAX_ROOT_TILE");
+    }
+    CallCancel cc;
+    if (int32_t crc = begin_call(c, cc)) return crc;
+    if (stats) memset(stats, 0, sizeof *stats);
+    if (n_shapes == 0) return FC_OK;
+    std::lock_guard<std::mutex> guard(c->mu);
+    CU(cudaSetDevice(c->device));
+    const int L = int(g.ts.size());
+    const uint32_t T0 = g.ts[0];
+    const uint32_t W = cfg->width, H = cfg->height;
+    g.roots_y = (H + T0 - 1) / T0;
+    g.roots_z = (cfg->depth + T0 - 1) / T0;
+    const uint64_t vol_roots = uint64_t(g.roots_x) * g.roots_y * g.roots_z;
+    if (vol_roots > 0xfffffff0ull) return fail(FC_ERR_UNSUPPORTED, "volume too large");
+    for (uint32_t k = 0; k < n_shapes; ++k)   // choice scratch for the largest choice_count
+        g.choice_words = std::max(g.choice_words, (tapes[k]->info.choice_count + 15) / 16 + 1);
+    g.scene = true;
+    g.clamp_at = clamp ? cfg->depth - 1u : 0xffffffffu;
+    const bool timing = (cfg->flags & FC_FLAG_TIMING) != 0;
+    const bool async = (cfg->flags & FC_FLAG_ASYNC) != 0;
+    const bool want_stats = stats != nullptr;
+    const bool host_out = !is_device_ptr(out), host_index = index && !is_device_ptr(index);
+    const size_t npix = size_t(W) * H, occl_blocks = size_t(g.occl_w) * g.occl_h;   // (scene occlusion blocks: 8 bytes)
+    cudaStream_t s = c->stream;
+
+    // Lists of a pass of n placements are those of one grid of n volumes (capped as in fc_render3d; the leaf list also
+    // at FC_SCENE_MAX_LEAF_JOBS, whose ids fill the key's id field); heightmap and occlusion map are the call's.
+    auto grid_of = [&](uint32_t n) {
+        Tiles3D gp = g;
+        gp.n_roots = vol_roots * n;
+        size_lists_3d(gp);
+        gp.level_cap[L] = std::min<uint64_t>(gp.level_cap[L], FC_SCENE_MAX_LEAF_JOBS);
+        return gp;
+    };
+    auto pass_bytes = [&](uint32_t n) {
+        const Tiles3D gp = grid_of(n);
+        uint64_t b = gp.level_cap[L] * 4;
+        for (int l = 1; l <= L; ++l) b += gp.level_cap[l] * sizeof(TileJob);
+        return b;
+    };
+    uint32_t n_max = 1;
+    while (n_max < n_shapes && pass_bytes(n_max + 1) <= FC_FRAMES_PASS_BYTES && vol_roots * (n_max + 1) <= 0xfffffff0ull)
+        ++n_max;
+    const int forced = env_int("FIDGET_B200_FRAMES_PER_PASS", 0);   // (diagnostic: at most the limits above)
+    if (forced > 0) n_max = std::min<uint32_t>(n_max, uint32_t(forced));
+    {
+        Tiles3D gm = grid_of(n_max);
+        if (int32_t erc = ensure_scratch_3d(c, gm, npix, occl_blocks * 2)) return erc;
+        if (!env_int("FIDGET_B200_NO_ZSORT", 0)) CU(c->zsort.ensure(size_t(zsort_layers(gm) + 1) * 4 + gm.level_cap[L] * 4));
+    }
+    CU(c->frame_table.ensure(size_t(n_shapes) * sizeof(Frame2D)));
+    CU(c->scene_pl.ensure(size_t(n_shapes) * 4));
+    if (n_shapes > 1) CU(c->scene_backup.ensure(npix * 8 + (g.use_occl ? occl_blocks * 8 : 0)));
+    if (!c->pass_pin) CU(cudaHostAlloc(reinterpret_cast<void**>(&c->pass_pin), 2 * sizeof(PassStatus), cudaHostAllocDefault));
+    void* dimg = out;
+    if (host_out) {
+        CU(c->image.ensure(npix * 16));
+        dimg = c->image.p;
+    }
+    uint16_t* dindex = index;
+    if (host_index) {
+        CU(c->scene_index.ensure(npix * 2));
+        dindex = c->scene_index.as<uint16_t>();
+    }
+    g.frames = c->frame_table.as<Frame2D>();
+    CU(cudaMemcpyAsync(c->frame_table.p, table.data(), table.size() * sizeof(Frame2D), cudaMemcpyHostToDevice, s));
+    CU(cudaMemsetAsync(c->heightmap.p, 0, npix * 8, s));
+    if (g.use_occl) CU(cudaMemsetAsync(c->occl.p, 0, occl_blocks * 8, s));
+    const uint64_t arena_clauses = std::min<uint64_t>(c->arena.cap, c->arena_bytes) / sizeof(uint2);
+
+    // Overflow policy, as fc_render3d_frames's per frame: the first pass holds one placement, later ones are sized from
+    // the largest per-placement use so far with headroom 1.5.  Passes build on each other's heightmap, so each is waited
+    // for before the next; one of several placements keeps a copy of the heightmap and occlusion map from before it,
+    // and if it overflows anyway (the kernels report it, they do not fault; its normals write nothing) the copy is
+    // restored and its halves run instead.  Only a one-placement pass returns the error.
+    double use_arena = 0, use_jobs[MAX_LEVELS + 1] = {};
+    bool measured = forced > 0;
+    auto fits = [&](uint32_t n) {
+        const Tiles3D gp = grid_of(n);
+        const double h = 1.5 * n;
+        if (use_arena * h > double(arena_clauses)) return false;
+        for (int l = 1; l <= L; ++l) {
+            const uint64_t r = g.ts[0] / g.ts[l - 1];
+            const bool clamped = gp.level_cap[l] < gp.n_roots * r * r * r;
+            if (clamped && use_jobs[l] * h > double(gp.level_cap[l])) return false;
+        }
+        return true;
+    };
+    struct Range { uint32_t f0, n; };
+    std::vector<Range> redo;   // halves of overflowed passes (a stack: the first half runs next)
+    uint32_t next = 0;
+    auto take = [&]() -> Range {
+        if (!redo.empty()) { const Range r = redo.back(); redo.pop_back(); return r; }
+        uint32_t n = std::min(n_max, n_shapes - next);
+        if (!measured) n = 1;
+        else if (forced <= 0) while (n > 1 && !fits(n)) --n;
+        const Range r{next, n};
+        next += n;
+        return r;
+    };
+    auto abandon = [&](int32_t rc) { return abandon_frames(c, s, stats, rc); };
+    const size_t backup_occl = npix * 8;   // (byte offset of the occlusion map's copy)
+    auto snapshot = [&](bool restore) -> int32_t {
+        char* b = c->scene_backup.as<char>();
+        CU(cudaMemcpyAsync(restore ? c->heightmap.p : b, restore ? b : c->heightmap.p, npix * 8, cudaMemcpyDeviceToDevice, s));
+        if (g.use_occl)
+            CU(cudaMemcpyAsync(restore ? c->occl.p : b + backup_occl, restore ? b + backup_occl : c->occl.p, occl_blocks * 8,
+                               cudaMemcpyDeviceToDevice, s));
+        return FC_OK;
+    };
+
+    Stats total{};
+    uint64_t arena_used = 0;
+    float stage_ms[16] = {};
+    size_t ev = 0;
+    uint32_t launches = 0;
+    std::vector<uint32_t> pl_host;
+    const bool early_return = async && !host_out && !host_index && !want_stats;
+    for (bool first = true; next < n_shapes || !redo.empty(); first = false) {
+        if (!first && cc.flag && __atomic_load_n(cc.flag, __ATOMIC_ACQUIRE))
+            return abandon(fail(FC_ERR_CANCELLED, "cancelled"));   // the flag stops the passes
+        const Range r = take();
+        // level-0 groups: the pass's placements by tape, in order of first appearance
+        Tiles3D gp = grid_of(r.n);
+        gp.pl0 = r.f0;
+        gp.pl1 = r.f0 + r.n;
+        pl_host.clear();
+        for (uint32_t k = r.f0; k < r.f0 + r.n; ++k) {
+            bool seen = false;
+            for (const Tiles3D::Group& gr : gp.groups) seen |= gr.tape == tapes[k];
+            if (seen) continue;
+            const uint32_t first_pl = uint32_t(pl_host.size());
+            for (uint32_t q = k; q < r.f0 + r.n; ++q)
+                if (tapes[q] == tapes[k]) pl_host.push_back(q);
+            gp.groups.push_back(Tiles3D::Group{tapes[k], first_pl, uint32_t(pl_host.size()) - first_pl});
+        }
+        gp.d_pl = c->scene_pl.as<uint32_t>();
+        CU(cudaMemcpyAsync(c->scene_pl.p, pl_host.data(), pl_host.size() * 4, cudaMemcpyHostToDevice, s));
+        if (r.n > 1) {
+            if (int32_t brc = snapshot(false)) return abandon(brc);
+        }
+        CU(cudaMemsetAsync(c->counters.p, 0, sizeof(Counters), s));
+        if (want_stats) CU(cudaMemsetAsync(c->stats.p, 0, sizeof(Stats), s));
+        const size_t ev0 = ev;
+        if (int32_t erc = enqueue_tiles_3d(c, tapes[r.f0], cfg, gp, table[r.f0].vb, dimg, 0, H, want_stats, timing, cc, s, ev,
+                                           launches, dindex))
+            return abandon(erc);
+        PassStatus* hs = c->pass_pin;
+        CU(cudaMemcpyAsync(&hs->ctr, c->counters.p, sizeof(Counters), cudaMemcpyDeviceToHost, s));
+        if (want_stats) CU(cudaMemcpyAsync(&hs->st, c->stats.p, sizeof(Stats), cudaMemcpyDeviceToHost, s));
+        if (early_return && next >= n_shapes && redo.empty()) {   // FC_FLAG_ASYNC: the last pass is left running
+            c->async_call = cc;
+            return FC_OK;
+        }
+        if (cc.flag) {
+            if (int32_t wrc = wait_call(c, s, cc)) return abandon(wrc);
+        } else {
+            CU(cudaStreamSynchronize(s));
+        }
+        const double n = double(r.n);
+        use_arena = std::max(use_arena, double(hs->ctr.arena_top) / n);
+        for (int l = 1; l <= L; ++l) use_jobs[l] = std::max(use_jobs[l], double(hs->ctr.n_jobs[l]) / n);
+        measured = true;
+        if (hs->ctr.error) {
+            if (r.n == 1 || (hs->ctr.error & ~3u)) return abandon(device_error(hs->ctr.error));
+            if (int32_t brc = snapshot(true)) return abandon(brc);
+            const uint32_t h = r.n / 2;
+            redo.push_back(Range{r.f0 + h, r.n - h});
+            redo.push_back(Range{r.f0, h});
+            continue;
+        }
+        if (want_stats) {
+            for (int l = 0; l < MAX_LEVELS; ++l) {
+                total.evaluated[l] += hs->st.evaluated[l];
+                total.filled_inside[l] += hs->st.filled_inside[l];
+                total.filled_outside[l] += hs->st.filled_outside[l];
+                total.ambiguous[l] += hs->st.ambiguous[l];
+                total.simplified[l] += hs->st.simplified[l];
+            }
+            total.pixels += hs->st.pixels;
+            total.grads += hs->st.grads;
+            arena_used = std::max<uint64_t>(arena_used, hs->ctr.arena_top * sizeof(uint2));
+            if (timing) add_stage_ms_3d(c, ev0, L, stage_ms);
+        }
+    }
+    if (host_out) CU(cudaMemcpyAsync(out, dimg, npix * 16, cudaMemcpyDeviceToHost, s));
+    if (host_index) CU(cudaMemcpyAsync(index, dindex, npix * 2, cudaMemcpyDeviceToHost, s));
+    CU(cudaStreamSynchronize(s));
     if (stats) {
         copy_census(total, stats);
         stats->grads = total.grads;

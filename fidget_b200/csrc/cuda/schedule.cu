@@ -349,18 +349,19 @@ int coop_blocks(fc_ctx* c, const fc_tape* tape, uint64_t n_roots, LevelParams& p
     for (int k = 1; k <= cap; ++k) if (rounds(k) < rounds(per_sm)) per_sm = k;
     // widest CTA for which the runtime really keeps per_sm of them resident (register granularity
     // makes 7 x 224 threads x 40 registers NOT fit although 7 * 224 * 40 < 64 K)
-    const bool frames = p.frames != nullptr;   // a frame batch launches its own instantiation
-    auto& mm = c->coop_memo[(dim == 3 ? 2 : 0) + int(frames)];
+    // a frame batch and a 3D scene launch their own instantiations
+    const int variant = p.scene ? 2 : p.frames != nullptr ? 1 : 0;
+    auto& mm = c->coop_memo[(dim == 3 ? 2 : 0) + variant];
     if (mm.threads == 0 || mm.smem != smem || mm.per_sm != per_sm) {
         int t = COOP_THREADS;
-        while (t > 64 && coop_occupancy(dim, frames, t, smem) < per_sm) t -= 32;
+        while (t > 64 && coop_occupancy(dim, variant, t, smem) < per_sm) t -= 32;
         mm = {smem, per_sm, t};
     }
     threads = mm.threads;
     threads = env_int("FIDGET_B200_COOP_THREADS", threads);
     if (env_int("FIDGET_B200_COOP_DEBUG", 0))
         fprintf(stderr, "coop: %u clauses, %u slots, %zu B smem, %d CTAs/SM x %d threads (%d regs), %llu roots, occupancy %d CTAs/SM\n",
-                tape->info.n_ops, sc->n_slots, smem, per_sm, threads, coop_regs_per_thread(dim, frames), (unsigned long long)n_roots,
-                coop_occupancy(dim, frames, threads, smem));
+                tape->info.n_ops, sc->n_slots, smem, per_sm, threads, coop_regs_per_thread(dim, variant), (unsigned long long)n_roots,
+                coop_occupancy(dim, variant, threads, smem));
     return int(std::max<uint64_t>(1, std::min<uint64_t>(n_roots, uint64_t(c->sm_count) * per_sm)));
 }

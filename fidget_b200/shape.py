@@ -667,6 +667,66 @@ def render3d_frames(shape: CudaShape, cfg: RenderConfig3D, var_values=None, worl
     return (out, st.as_dict()) if stats else out
 
 
+def scene_table(cfg: RenderConfig3D, n: int, var_values=None, world_to_model=None, mats=None):
+    """The ``fc_frame3d`` placement table of ``render3d_scene`` for ``n`` shapes: entry k is what ``frame_table_3d``
+    gives for placement k's values (``world_to_model`` [n, 4, 4], ``mats`` [n, 4, 4], ``var_values`` [n, k]).  What is
+    not given per placement comes from ``cfg``, for all n; lengths other than n raise ValueError."""
+    per = {name: v for name, v in (("var_values", var_values), ("world_to_model", world_to_model), ("mats", mats))
+           if v is not None}
+    for name, v in per.items():
+        if len(v) != n:
+            raise ValueError(f"{name} has {len(v)} entries for {n} shapes")
+    if not per:   # every placement is cfg's own view and vars
+        one = frame_table_3d(cfg)[0]
+        table = (_lib.FcFrame3d * n)()
+        for k in range(n):
+            C.memmove(C.byref(table[k]), C.byref(one), C.sizeof(one))
+        return table
+    return frame_table_3d(cfg, **per)
+
+
+def render3d_scene(shapes, cfg: RenderConfig3D, var_values=None, world_to_model=None, mats=None, out=None,
+                   index_out=None, stats: bool = False, asynchronous: bool = False):
+    """Several shapes rendered into one image (``fc_render3d_scene``): a viewer's draw list, or fidget-wgpu's merge
+    of voxel images.  Shape k is ``shapes[k]`` placed by entry k of ``scene_table`` (per-placement ``var_values`` /
+    ``world_to_model`` / ``mats``, leading dimension ``len(shapes)``; the rest from ``cfg``).  Each pixel is that of
+    the per-shape ``render3d`` image with the greatest depth (after the final clamp), the lowest k on equal depth, bit
+    for bit; ``index`` holds that k (0 where every image is empty).  Returns ``(image, index)`` -- GEOMETRY_PIXEL
+    [h, w] and uint16 [h, w], or the given ``out`` / ``index_out`` (numpy arrays or CUDA tensors of that many bytes,
+    contiguous) -- plus the stats with ``stats=True``; None when ``cfg.cancel`` cancelled it.  Without ``index_out`` the
+    index lands next to ``out``: a numpy uint16 array for a host ``out``, an int16 CUDA tensor (the same bits) on
+    ``out``'s device for a CUDA ``out``, so that ``asynchronous=True`` stays asynchronous.  All shapes must live on one
+    CudaContext."""
+    shapes = list(shapes)
+    n = len(shapes)
+    if n == 0:
+        raise ValueError("a scene needs at least one shape")
+    lib, cuda = shapes[0]._lib, shapes[0].cuda
+    if any(sh.cuda is not cuda for sh in shapes):
+        raise ValueError("the shapes of a scene must belong to one CudaContext")
+    table = scene_table(cfg, n, var_values=var_values, world_to_model=world_to_model, mats=mats)
+    c = _render3d_cfg(cfg, asynchronous)
+    if out is None:
+        out = np.zeros((cfg.height, cfg.width), dtype=GEOMETRY_PIXEL)
+    else:
+        _check_out(out, cfg.height * cfg.width * GEOMETRY_PIXEL.itemsize)
+    if index_out is None and getattr(out, "is_cuda", False):
+        import torch
+        index_out = torch.zeros((cfg.height, cfg.width), dtype=torch.int16, device=out.device)
+    elif index_out is None:
+        index_out = np.zeros((cfg.height, cfg.width), dtype=np.uint16)
+    else:
+        _check_out(index_out, cfg.height * cfg.width * 2)
+    handles = (C.c_void_p * n)(*[sh._h for sh in shapes])
+    st = _lib.FcRenderStats() if stats else None
+    rc = cuda._cancellable(cfg.cancel, lambda: lib.fc_render3d_scene(
+        cuda._h, handles, table, n, C.byref(c), _ptr(out), _ptr(index_out), C.byref(st) if stats else None), asynchronous)
+    if rc == _lib.FC_ERR_CANCELLED:
+        return None
+    _ck(rc)
+    return (out, index_out, st.as_dict()) if stats else (out, index_out)
+
+
 OCTREE_LEAF = np.dtype([("ix", np.uint16), ("iy", np.uint16), ("iz", np.uint16), ("mask", np.uint8),
                         ("n_edges", np.uint8), ("present", np.uint16), ("pad", np.uint16),
                         ("pos", np.float32, (12, 3)), ("grad", np.float32, (12, 4))])

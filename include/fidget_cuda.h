@@ -64,8 +64,8 @@ int32_t fc_ctx_set_arena_bytes(fc_ctx* ctx, uint64_t bytes);
 /* Cancellation (CancelToken, fidget-core/src/render/config.rs:59-80).  `flag` points to a caller-owned byte with the
  * layout of Rust's AtomicBool (CancelToken::into_raw() as *const u8): nonzero = cancelled.  The library reads it with
  * an acquire load, from any thread; NULL detaches it.  Context-wide, like fc_ctx_set_stream, and consulted only by
- * fc_render2d, fc_render2d_frames, fc_render3d, fc_render3d_frames, fc_octree_sample, fc_mesh_build, and fc_ctx_synchronize
- * after the most recent FC_FLAG_ASYNC call of those.  With a flag attached:
+ * fc_render2d, fc_render2d_frames, fc_render3d, fc_render3d_frames, fc_render3d_scene, fc_octree_sample, fc_mesh_build, and
+ * fc_ctx_synchronize after the most recent FC_FLAG_ASYNC call of those.  With a flag attached:
  *  - set on entry: the call returns FC_ERR_CANCELLED before it allocates or launches anything;
  *  - set while the call runs: the kernels stop claiming work and the call returns FC_ERR_CANCELLED ("cancelled" in
  *    fc_last_error); `out` is unspecified (a host `out` receives no copy), stats / info are zeroed, and the context
@@ -308,6 +308,39 @@ typedef struct fc_frame3d {
 int32_t fc_render3d_frames(fc_ctx* ctx, const fc_tape* tape, const fc_render3d_cfg* cfg,
                            const fc_frame3d* frames /* host */, uint32_t n_frames, fc_geometry_pixel* out,
                            fc_render_stats* stats /* may be NULL */);
+/* Several shapes rendered into one image: a viewer's draw list (every draw(shape) of a script rendered and composited),
+ * or the merge of several voxel images that fidget-wgpu's effects pipeline starts with (merge.wgsl).  Shape k is
+ * tapes[k] placed by placements[k] (its mat and var_values, as in fc_render3d_frames; the same tape may appear any number
+ * of times).  Let img_k be fc_render3d(tapes[k], cfg with placements[k]'s mat and var_values), final clamp included
+ * unless FC_FLAG_NO_CLAMP.  Then, bit for bit (depth and all three normal floats):
+ *    out = img_0, then for k = 1 .. n_shapes - 1: out = (out.depth >= img_k.depth) ? out : img_k
+ * per pixel -- the greatest (clamped) depth wins, and on equal depth the lowest k; index (may be NULL) receives the k
+ * kept, 0 where every image is empty (depth 0).  All shapes share one heightmap and one occlusion map, so a tile proven
+ * full for a front shape culls the tiles of the shapes behind it.
+ *  - cfg supplies width, height, depth, tile_sizes and the flags FC_FLAG_NO_CLAMP, FC_FLAG_FULL_LADDER, FC_FLAG_TIMING
+ *    and FC_FLAG_ASYNC; its mat and var_values are ignored.  out and index are host or device memory.
+ *  - stats: the per-level census of the tiles evaluated across the scene (tiles culled behind other shapes are not
+ *    counted), pixels, grads (normals evaluated), arena_bytes_used the largest of any pass, kernel_launches and stage_ms
+ *    over all passes.  Every field but pixels is the same for two identical calls.
+ *  - passes: placements go in passes that share the heightmap; FC_ERR_ARENA or a work-list overflow comes back only
+ *    where one placement alone overflows (the first pass renders one placement, later ones are sized from the largest
+ *    per-placement use so far, and a pass that overflows anyway is restored and rendered again in halves).
+ *  - n_shapes == 0 launches nothing and returns FC_OK.  FC_ERR_UNSUPPORTED for a spilled tape, FC_FLAG_EXACT_CENSUS,
+ *    Z slabs, root row bands, the tile interleave, n_shapes > FC_SCENE_MAX_SHAPES, a volume depth rounded up to whole
+ *    root tiles above FC_SCENE_MAX_DEPTH, and (with the clamp) a root tile edge above FC_SCENE_MAX_ROOT_TILE.
+ *    FC_ERR_INVALID for a multi-output tape, a placement without a value for a bound variable, a NULL entry of tapes,
+ *    and tapes or placements NULL with n_shapes > 0.  All of these before anything is allocated or launched.
+ *  - The cancel flag and FC_FLAG_ASYNC (device out and index, no stats) behave as in fc_render3d_frames.
+ * Limits of the heightmap key (clamped depth, shape, depth above the clamp threshold, leaf tile): the shapes, the depth
+ * and the root tile edge below; a pass holds at most FC_SCENE_MAX_LEAF_JOBS leaf tiles (more is a list overflow). */
+#define FC_SCENE_MAX_SHAPES 1024
+#define FC_SCENE_MAX_DEPTH 262142        /* depth rounded up to whole root tiles */
+#define FC_SCENE_MAX_ROOT_TILE 1022      /* with the clamp: the root tile edge */
+#define FC_SCENE_MAX_LEAF_JOBS 67108863  /* leaf tiles of one pass */
+int32_t fc_render3d_scene(fc_ctx* ctx, const fc_tape* const* tapes /* host, n_shapes */,
+                          const fc_frame3d* placements /* host, n_shapes */, uint32_t n_shapes,
+                          const fc_render3d_cfg* cfg, fc_geometry_pixel* out, uint16_t* index /* may be NULL */,
+                          fc_render_stats* stats /* may be NULL */);
 /* Per-pixel merge of `n_slabs` slab images (each width*height, device
  * pointers, Z-ordered) into `out`, applying the final depth clamp of
  * voxel.rs:535-546.  Used after the all-gather in multi-GPU renders. */

@@ -21,7 +21,7 @@
 
 namespace fdev {
 
-constexpr int TMA_THREADS = 256;
+constexpr int TMA_THREADS = int(SLICE_TMA_TILE);   // one float4 per thread and variable
 constexpr int TMA_STAGES = 3;
 
 __device__ __forceinline__ uint32_t smem_u32(const void* p) { return uint32_t(__cvta_generic_to_shared(p)); }
@@ -207,32 +207,33 @@ __global__ void __launch_bounds__(TMA_THREADS) k_slice_tma(const __grid_constant
     }
 }
 
-// Returns false when the fast path does not apply (the caller then uses the per-thread kernel)
-bool launch_slice_tma(const SliceTmaParams& p, bool grad, int sm_count, cudaStream_t s) {
-    if (p.n_vars > 4 || p.n_outputs == 0 || p.n_outputs > 2 || p.n_regs > 40 || p.n_ops == 0 || p.n_ops > 2048) return false;
-    for (uint32_t k = 0; k < p.n_vars; ++k) if (reinterpret_cast<uintptr_t>(p.vars[k]) & 15u) return false;
-    for (uint32_t o = 0; o < p.n_outputs; ++o) if (reinterpret_cast<uintptr_t>(p.outs[o]) & 15u) return false;
-    if (reinterpret_cast<uintptr_t>(p.tape) & 15u) return false;
+// Returns the number of CTAs launched, or 0 when the fast path does not apply (the caller then uses the per-thread
+// kernel)
+unsigned launch_slice_tma(const SliceTmaParams& p, bool grad, int sm_count, cudaStream_t s) {
+    if (p.n_vars > 4 || p.n_outputs == 0 || p.n_outputs > 2 || p.n_regs > 40 || p.n_ops == 0 || p.n_ops > 2048) return 0;
+    for (uint32_t k = 0; k < p.n_vars; ++k) if (reinterpret_cast<uintptr_t>(p.vars[k]) & 15u) return 0;
+    for (uint32_t o = 0; o < p.n_outputs; ++o) if (reinterpret_cast<uintptr_t>(p.outs[o]) & 15u) return 0;
+    if (reinterpret_cast<uintptr_t>(p.tape) & 15u) return 0;
     const size_t smem = slice_tma_smem(p.n_ops, p.n_vars, p.n_regs);
-    if (smem > 220 * 1024) return false;
+    if (smem > 220 * 1024) return 0;
     auto kern = grad ? k_slice_tma<true> : k_slice_tma<false>;
     static size_t configured[2] = {0, 0};
     if (smem > configured[grad]) {
         if (cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, int(smem)) != cudaSuccess) {
             cudaGetLastError();
-            return false;
+            return 0;
         }
         configured[grad] = smem;
     }
     int per_sm = 0;
     if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kern, TMA_THREADS, smem) != cudaSuccess || per_sm < 1) {
         cudaGetLastError();
-        return false;
+        return 0;
     }
     const uint64_t tiles = p.n / (uint64_t(TMA_THREADS) * (grad ? 1 : 4)) + 1;
     const unsigned grid = unsigned(std::min<uint64_t>(tiles, uint64_t(sm_count) * per_sm));
     kern<<<grid, TMA_THREADS, smem, s>>>(p);
-    return true;
+    return grid;
 }
 
 }  // namespace fdev

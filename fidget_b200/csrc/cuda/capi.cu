@@ -96,7 +96,10 @@ int32_t fc_ctx_create(int32_t device, fc_ctx** out) {
     c->device = device;
     cudaDeviceProp prop;
     CU(cudaGetDeviceProperties(&prop, device));
-    c->sm_count = prop.multiProcessorCount;
+    // FIDGET_B200_SM_COUNT=<n> sizes every SM-scaled grid of this context as if the device had n SMs (clamped to
+    // 1 .. the real count): the launch shapes of a MIG slice or a smaller part, on the whole device.  Never more than
+    // the real count, because the fused 2D tail needs all of its CTAs resident.
+    c->sm_count = std::max(1, std::min(env_int("FIDGET_B200_SM_COUNT", prop.multiProcessorCount), prop.multiProcessorCount));
     if (prop.major != 9 || prop.minor != 0) {   // sm_90a code loads on compute capability 9.0 and nothing else
         delete c;
         return fail(FC_ERR_NO_DEVICE, "libfidget_cuda is built for sm_90a (H100) only; found sm_" +
@@ -568,7 +571,7 @@ static int32_t bulk_eval(fc_eval* e, const fc_tape* t, const void* const* vars, 
     p.n = n;
     p.vars = e->ptrs.as<const void*>();
     p.outs = reinterpret_cast<void* const*>(e->ptrs.as<void*>() + nv);
-    bool fast = false;
+    unsigned tma_ctas = 0;
     if (!t->info.mem_count && n >= 4096 && nv <= 4 && no <= 2 && !env_int("FIDGET_B200_NO_TMA", 0)) {
         SliceTmaParams q{};
         q.tape = t->dev;
@@ -579,9 +582,17 @@ static int32_t bulk_eval(fc_eval* e, const fc_tape* t, const void* const* vars, 
         q.n = n;
         for (uint32_t i = 0; i < nv; ++i) q.vars[i] = static_cast<const float4*>(dptr[i]);
         for (uint32_t o = 0; o < no; ++o) q.outs[o] = static_cast<float4*>(const_cast<void*>(dptr[nv + o]));
-        fast = launch_slice_tma(q, grad, c->sm_count, c->stream);
+        tma_ctas = launch_slice_tma(q, grad, c->sm_count, c->stream);
     }
-    if (!fast) { if (grad) launch_grad_slice(p, c->stream); else launch_float_slice(p, c->stream); }
+    if (!tma_ctas) { if (grad) launch_grad_slice(p, c->stream); else launch_float_slice(p, c->stream); }
+    if (env_int("FIDGET_B200_SLICE_DEBUG", 0)) {   // which kernel ran, and how many tiles each TMA CTA had to cycle
+        const uint64_t tile = uint64_t(SLICE_TMA_TILE) * (grad ? 1 : 4);
+        if (tma_ctas)
+            fprintf(stderr, "slice: TMA kernel, %llu points, %llu full tiles, %u CTAs, %d SMs\n", (unsigned long long)n,
+                    (unsigned long long)(n / tile), tma_ctas, c->sm_count);
+        else
+            fprintf(stderr, "slice: per-thread kernel, %llu points\n", (unsigned long long)n);
+    }
     CU(cudaGetLastError());
     for (auto& cb : copy_back)
         if (n) CU(cudaMemcpyAsync(cb.first, cb.second, n * elem, cudaMemcpyDeviceToHost, c->stream));

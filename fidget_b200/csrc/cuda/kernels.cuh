@@ -463,7 +463,8 @@ struct SliceTmaParams {
     const float4* vars[4];
     float4* outs[2];
 };
-bool launch_slice_tma(const SliceTmaParams& p, bool grad, int sm_count, cudaStream_t s);
+constexpr uint32_t SLICE_TMA_TILE = 256;   // float4 per variable in a tile of k_slice_tma: 1024 points f32, 256 gradients
+unsigned launch_slice_tma(const SliceTmaParams& p, bool grad, int sm_count, cudaStream_t s);
 void launch_grad_slice(const BulkParams& p, cudaStream_t s);
 
 struct TracingParams {

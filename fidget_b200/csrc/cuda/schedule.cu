@@ -360,8 +360,8 @@ int coop_blocks(fc_ctx* c, const fc_tape* tape, uint64_t n_roots, LevelParams& p
     threads = mm.threads;
     threads = env_int("FIDGET_B200_COOP_THREADS", threads);
     if (env_int("FIDGET_B200_COOP_DEBUG", 0))
-        fprintf(stderr, "coop: %u clauses, %u slots, %zu B smem, %d CTAs/SM x %d threads (%d regs), %llu roots, occupancy %d CTAs/SM\n",
+        fprintf(stderr, "coop: %u clauses, %u slots, %zu B smem, %d CTAs/SM x %d threads (%d regs), %llu roots, occupancy %d CTAs/SM, %d SMs\n",
                 tape->info.n_ops, sc->n_slots, smem, per_sm, threads, coop_regs_per_thread(dim, variant), (unsigned long long)n_roots,
-                coop_occupancy(dim, variant, threads, smem));
+                coop_occupancy(dim, variant, threads, smem), c->sm_count);
     return int(std::max<uint64_t>(1, std::min<uint64_t>(n_roots, uint64_t(c->sm_count) * per_sm)));
 }

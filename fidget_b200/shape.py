@@ -199,13 +199,18 @@ class CudaShape:
         _ck(self._lib.fc_tape_serialize(self._h, buf, n.value, C.byref(n)))
         return bytes(buf)
 
-    def __del__(self):
+    def close(self):
+        """Releases the tape and its evaluator now (a second call does nothing).  Both belong to the CudaContext, so
+        they must go before ``CudaContext.close``; the shape cannot be used afterwards."""
         if getattr(self, "_eval", None):
             self._lib.fc_eval_destroy(self._eval)
             self._eval = None
         if getattr(self, "_h", None):
             self._lib.fc_tape_release(self._h)
             self._h = None
+
+    def __del__(self):
+        self.close()
 
     # Function::size / choice_count / vars
     def size(self): return self.info.ref_len

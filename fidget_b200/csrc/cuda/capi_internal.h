@@ -133,10 +133,12 @@ struct fc_ctx {
     uint32_t mesh_n_cells = 0;
     DevBuf fx_in, fx_out, fx_tmp, fx_tables;  // effects: staged host images, intermediate maps, SSAO tables
     DevBuf solve_meta, solve_vals, solve_res; // fc_solve_batch: tape table + slot maps, staged host values / results
-    // fc_render2d_frames: the frame table, each pass's arena high-water mark, and the copy stream that returns a pass's
-    // images to a host `out` while the next pass runs (ev_pass: pass k's images are complete; ev_copied: copied back)
+    // the batches (fc_render2d_frames, fc_render3d_frames, fc_render3d_scene): the frame or placement table, and the copy
+    // stream that returns a frame batch's pass to a host `out` while the next pass runs (ev_pass: the pass in staging
+    // buffer b is complete; ev_copied: copied back).  fc_render2d_frames: each pass's arena high-water mark.
     DevBuf frame_table, frame_tops;
-    // fc_render3d_frames: each in-flight pass's counters and stats (two pinned host slots, one per staging buffer)
+    // the 3D batches: each in-flight pass's counters and stats (two pinned host slots, one per staging buffer; a scene
+    // waits for every pass and uses the first)
     struct PassStatus* pass_pin = nullptr;
     cudaStream_t copy_stream = nullptr;
     cudaEvent_t ev_pass[2] = {}, ev_copied[2] = {};
@@ -171,7 +173,8 @@ struct fc_ctx {
     CallCancel async_call;                    // the last FC_FLAG_ASYNC call that returned before its work was done
 };
 
-// What the host reads of a finished pass of fc_render3d_frames: its counters (error bits, list and arena use) and stats
+// What the host reads of a finished pass of fc_render3d_frames or fc_render3d_scene: its counters (error bits, list and
+// arena use) and stats
 struct PassStatus {
     Counters ctr;
     Stats st;

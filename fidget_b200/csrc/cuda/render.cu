@@ -1,6 +1,7 @@
 // The fused tile renderers: fc_render2d (pixel::render), fc_render3d (voxel::render), their frame batches
 // (fc_render2d_frames, fc_render3d_frames), 3D scenes of several shapes (fc_render3d_scene), fc_merge_slabs.
 #include <cstddef>
+#include <functional>
 
 #include "capi_internal.h"
 
@@ -291,7 +292,10 @@ static void add_stage_ms_2d(fc_ctx* c, size_t first, int L, bool fused, const St
     }
 }
 
-static void copy_census(const Stats& h, fc_render_stats* stats) {
+// A call's fc_render_stats: the census and pixels of `h`, its grads (the 3D renders only), the arena high-water mark
+// in clauses and the launch count; stage_ms starts at zero for the caller to add to
+static void write_stats(fc_render_stats* stats, const Stats& h, bool grads, unsigned long long arena_top, uint32_t launches) {
+    memset(stats, 0, sizeof *stats);
     for (int l = 0; l < FC_MAX_TILE_LEVELS; ++l) {
         stats->evaluated[l] = h.evaluated[l];
         stats->filled_inside[l] = h.filled_inside[l];
@@ -300,6 +304,19 @@ static void copy_census(const Stats& h, fc_render_stats* stats) {
         stats->simplified[l] = h.simplified[l];
     }
     stats->pixels = h.pixels;
+    if (grads) stats->grads = h.grads;
+    stats->arena_bytes_used = arena_top * sizeof(uint2);
+    stats->kernel_launches = launches;
+}
+
+// Frame `f` of a batch (fc_frame2d, fc_frame3d or a scene placement) as the kernels read it: its matrix, Z and
+// ShapeVars binding for `tape`
+template <class F>
+static int32_t bind_frame(const fc_tape* tape, const F& f, float z, Frame2D& out) {
+    if (f.n_var_values > FC_MAX_VARS) return fail(FC_ERR_INVALID, "n_var_values above FC_MAX_VARS");
+    memcpy(out.mat.m, f.mat, sizeof out.mat.m);
+    out.z = z;
+    return bind_vars(tape, f.var_values, f.n_var_values, out.vb);
 }
 
 // Validation and tile grid shared by fc_render2d and fc_render2d_frames
@@ -470,7 +487,9 @@ static void size_lists_3d(Tiles3D& g) {
         g.cap_census = std::min<uint64_t>(g.cap_census, 64ull << 20);
     }
 }
-// scratch of a pipeline over g's lists, with heightmap pixels and occlusion blocks for hm_pixels / occl_blocks
+static uint32_t zsort_layers(const Tiles3D& g) { return (g.roots_z * g.ts[0]) / g.ts.back(); }
+// scratch of a pipeline over g's lists (the z-sort's too), with heightmap pixels and occlusion blocks for hm_pixels /
+// occl_blocks.  A batch sizes it for its largest pass before it enqueues any, so no pass reallocates a buffer.
 static int32_t ensure_scratch_3d(fc_ctx* c, const Tiles3D& g, size_t hm_pixels, size_t occl_blocks) {
     const int L = int(g.ts.size());
     CU(c->choice_scratch.ensure(size_t(g.grid_blocks_last) * WARPS_PER_BLOCK * g.choice_words * 32 * 4));
@@ -481,9 +500,9 @@ static int32_t ensure_scratch_3d(fc_ctx* c, const Tiles3D& g, size_t hm_pixels, 
     CU(c->heightmap.ensure(hm_pixels * 8));
     if (g.exact_census) CU(c->census.ensure(g.cap_census * sizeof(CensusRec)));
     if (g.use_occl) CU(c->occl.ensure(occl_blocks * 4));
+    if (!env_int("FIDGET_B200_NO_ZSORT", 0)) CU(c->zsort.ensure(size_t(zsort_layers(g) + 1) * 4 + g.level_cap[L] * 4));
     return FC_OK;
 }
-static uint32_t zsort_layers(const Tiles3D& g) { return (g.roots_z * g.ts[0]) / g.ts.back(); }
 
 // The tile pipeline of fc_render3d (voxel::render), enqueued on `s`: the interval levels, the front-to-back sort of
 // the leaf tiles, the leaf voxels, the exact census and the normals of output rows y0 .. y1 into `dimg` (a scene pass:
@@ -581,7 +600,6 @@ static int32_t enqueue_tiles_3d(fc_ctx* c, const fc_tape* tape, const fc_render3
         q.tile = ts[L - 1];
         if (!env_int("FIDGET_B200_NO_ZSORT", 0)) {
             const uint32_t n_layers = zsort_layers(g);
-            CU(c->zsort.ensure(size_t(n_layers + 1) * 4 + g.level_cap[L] * 4));
             uint32_t* hist = c->zsort.as<uint32_t>();
             uint32_t* order = hist + n_layers + 1;
             launch_leaf_zsort(c->jobs[L].as<TileJob>(), &c->counters.as<Counters>()->n_jobs[L], uint32_t(g.level_cap[L]),
@@ -669,6 +687,116 @@ static void add_stage_ms_3d(fc_ctx* c, size_t first, int L, float* stage_ms) {
     stage_ms[10] += ms;
     cudaEventElapsedTime(&ms, e[0], e[L + 2]);
     stage_ms[15] += ms;
+}
+
+// ---- passes of the 3D batches (fc_render3d_frames: frames; fc_render3d_scene: placements) ----
+// Overflow policy: a pass fails (FC_ERR_ARENA, list overflow) only where one of its items alone would.  The first pass
+// holds one item; later ones are sized from the largest per-item use seen so far (arena clauses, jobs per level, census
+// records) with headroom 1.5; a pass that still overflows is run again as two halves (the kernels report overflow, they
+// do not fault), and only a one-item pass returns the error.  Only capped lists can overflow: a job list whose cap is
+// the worst case of the pass (every tile of the level queued) never does, so the headroom applies to the arena, to the
+// job lists clamped by FIDGET_B200_MAX_TILES_M and to a clamped census.  The caller runs the passes: take() the next
+// one, observe() its counters once it is done, until more() is false.
+namespace {
+struct PassPlan {
+    struct Range { uint32_t f0, n; };
+    const fc_ctx* c;
+    std::function<Tiles3D(uint32_t)> grid_of;   // the tile grid of a pass of n items, lists and census capped
+    uint32_t n_items, n_max = 1, next = 0;      // next: the first item no pass has taken yet
+    int L = 0, forced = 0;
+    double use_arena = 0, use_census = 0, use_jobs[MAX_LEVELS + 1] = {};
+    bool measured = false;
+    std::vector<Range> redo;                    // halves of overflowed passes (a stack: the first half runs next)
+
+    // n_max: the most items a pass may hold: FC_FRAMES_PASS_BYTES (at least one item) for its lists, census, z-sort
+    // order and item_bytes per item, 32-bit root ids and the caller's own limit n_cap
+    PassPlan(const fc_ctx* ctx, std::function<Tiles3D(uint32_t)> grid, uint32_t n, uint64_t item_bytes, uint32_t n_cap)
+        : c(ctx), grid_of(std::move(grid)), n_items(n) {
+        L = int(grid_of(1).ts.size());
+        auto allowed = [&](uint32_t k) {
+            const Tiles3D gp = grid_of(k);
+            uint64_t b = uint64_t(k) * item_bytes + gp.level_cap[L] * 4 + gp.cap_census * sizeof(CensusRec);
+            for (int l = 1; l <= L; ++l) b += gp.level_cap[l] * sizeof(TileJob);
+            return b <= FC_FRAMES_PASS_BYTES && gp.n_roots <= 0xfffffff0ull;
+        };
+        while (n_max < std::min(n_items, n_cap) && allowed(n_max + 1)) ++n_max;
+        // (diagnostic: passes of this size, at most the limits above, neither measured first nor shrunk to fit)
+        forced = env_int("FIDGET_B200_FRAMES_PER_PASS", 0);
+        if (forced > 0) n_max = std::min<uint32_t>(n_max, uint32_t(forced));
+        measured = forced > 0;
+    }
+    bool more() const { return next < n_items || !redo.empty(); }
+    bool fits(uint32_t n) const {
+        const Tiles3D gp = grid_of(n);
+        const double h = 1.5 * n;
+        if (use_arena * h > double(std::min<uint64_t>(c->arena.cap, c->arena_bytes) / sizeof(uint2))) return false;
+        uint64_t census_worst = gp.n_roots;
+        for (int l = 1; l <= L; ++l) {
+            const uint64_t r = gp.ts[0] / gp.ts[l - 1];
+            const bool clamped = gp.level_cap[l] < gp.n_roots * r * r * r;
+            if (clamped && use_jobs[l] * h > double(gp.level_cap[l])) return false;
+            if (l < L) { const uint64_t q = gp.ts[l - 1] / gp.ts[l]; census_worst += gp.level_cap[l] * q * q * q; }
+        }
+        const bool census_clamped = gp.exact_census && gp.cap_census < census_worst;
+        return !census_clamped || use_census * h <= double(gp.cap_census);
+    }
+    Range take() {
+        if (!redo.empty()) { const Range r = redo.back(); redo.pop_back(); return r; }
+        uint32_t n = std::min(n_max, n_items - next);
+        if (!measured) n = 1;
+        else if (forced <= 0) while (n > 1 && !fits(n)) --n;
+        const Range r{next, n};
+        next += n;
+        return r;
+    }
+    // Records the use of the finished pass r from its counters.  Its error if it fails; else `split` says that it
+    // overflowed and its halves are queued in its place.
+    int32_t observe(const Counters& ctr, const Range& r, bool& split) {
+        const double n = double(r.n);
+        use_arena = std::max(use_arena, double(ctr.arena_top) / n);
+        use_census = std::max(use_census, double(ctr.n_census) / n);
+        for (int l = 1; l <= L; ++l) use_jobs[l] = std::max(use_jobs[l], double(ctr.n_jobs[l]) / n);
+        measured = true;
+        split = false;
+        if (!ctr.error) return FC_OK;
+        if (r.n == 1 || (ctr.error & ~3u)) return device_error(ctr.error);
+        const uint32_t h = r.n / 2;
+        redo.push_back(Range{r.f0 + h, r.n - h});
+        redo.push_back(Range{r.f0, h});
+        split = true;
+        return FC_OK;
+    }
+};
+
+// The stats of a 3D batch, summed over the passes that stand: census, pixels, grads, the largest arena use and
+// (FC_FLAG_TIMING) the stage times
+struct PassStats {
+    Stats total{};
+    unsigned long long arena_top = 0;
+    float stage_ms[16] = {};
+    void add(fc_ctx* c, const PassStatus& ps, bool timing, size_t ev0, int L) {
+        for (int l = 0; l < MAX_LEVELS; ++l) {
+            total.evaluated[l] += ps.st.evaluated[l];
+            total.filled_inside[l] += ps.st.filled_inside[l];
+            total.filled_outside[l] += ps.st.filled_outside[l];
+            total.ambiguous[l] += ps.st.ambiguous[l];
+            total.simplified[l] += ps.st.simplified[l];
+        }
+        total.pixels += ps.st.pixels;
+        total.grads += ps.st.grads;
+        arena_top = std::max<unsigned long long>(arena_top, ps.ctr.arena_top);
+        if (timing) add_stage_ms_3d(c, ev0, L, stage_ms);
+    }
+    void write(fc_render_stats* stats, uint32_t launches) const {
+        write_stats(stats, total, true, arena_top, launches);
+        memcpy(stats->stage_ms, stage_ms, sizeof stage_ms);
+    }
+};
+}  // namespace
+// the two pinned slots (one per staging buffer) that a 3D batch reads its passes' status from
+static int32_t ensure_pass_pin(fc_ctx* c) {
+    if (!c->pass_pin) CU(cudaHostAlloc(reinterpret_cast<void**>(&c->pass_pin), 2 * sizeof(PassStatus), cudaHostAllocDefault));
+    return FC_OK;
 }
 
 extern "C" {
@@ -776,9 +904,7 @@ int32_t fc_render2d(fc_ctx* c, const fc_tape* tape, const fc_render2d_cfg* cfg, 
         Counters hc;
         CU(cudaMemcpy(&h, c->stats.p, sizeof h, cudaMemcpyDeviceToHost));
         CU(cudaMemcpy(&hc, c->counters.p, sizeof hc, cudaMemcpyDeviceToHost));
-        copy_census(h, stats);
-        stats->arena_bytes_used = hc.arena_top * sizeof(uint2);
-        stats->kernel_launches = launches;
+        write_stats(stats, h, false, hc.arena_top, launches);
         if (timing) add_stage_ms_2d(c, 0, L, fused, h, stats->stage_ms);
     }
     return rc;
@@ -795,12 +921,8 @@ int32_t fc_render2d_frames(fc_ctx* c, const fc_tape* tape, const fc_render2d_cfg
     if (fmt > FC_OUT_RGBA8) return fail(FC_ERR_INVALID, "unknown out_format");
     // every frame's ShapeVars binding, before anything is allocated or launched
     std::vector<Frame2D> table(n_frames);
-    for (uint32_t k = 0; k < n_frames; ++k) {
-        if (frames[k].n_var_values > FC_MAX_VARS) return fail(FC_ERR_INVALID, "n_var_values above FC_MAX_VARS");
-        memcpy(table[k].mat.m, frames[k].mat, sizeof table[k].mat.m);
-        table[k].z = frames[k].z;
-        if (int32_t brc = bind_vars(tape, frames[k].var_values, frames[k].n_var_values, table[k].vb)) return brc;
-    }
+    for (uint32_t k = 0; k < n_frames; ++k)
+        if (int32_t brc = bind_frame(tape, frames[k], frames[k].z, table[k])) return brc;
     CallCancel cc;
     if (int32_t crc = begin_call(c, cc)) return crc;
     if (stats) memset(stats, 0, sizeof *stats);
@@ -927,9 +1049,7 @@ int32_t fc_render2d_frames(fc_ctx* c, const fc_tape* tape, const fc_render2d_cfg
         std::vector<unsigned long long> tops(n_passes);
         CU(cudaMemcpy(&h, c->stats.p, sizeof h, cudaMemcpyDeviceToHost));
         CU(cudaMemcpy(tops.data(), c->frame_tops.p, tops.size() * sizeof(unsigned long long), cudaMemcpyDeviceToHost));
-        copy_census(h, stats);
-        stats->arena_bytes_used = *std::max_element(tops.begin(), tops.end()) * sizeof(uint2);
-        stats->kernel_launches = launches;
+        write_stats(stats, h, false, *std::max_element(tops.begin(), tops.end()), launches);
         if (timing)
             for (uint32_t k = 0; k < n_passes; ++k) add_stage_ms_2d(c, size_t(k) * (L + 3), L, false, h, stats->stage_ms);
     }
@@ -1028,10 +1148,7 @@ int32_t fc_render3d(fc_ctx* c, const fc_tape* tape, const fc_render3d_cfg* cfg, 
         Counters hc;
         CU(cudaMemcpy(&h, c->stats.p, sizeof h, cudaMemcpyDeviceToHost));
         CU(cudaMemcpy(&hc, c->counters.p, sizeof hc, cudaMemcpyDeviceToHost));
-        copy_census(h, stats);
-        stats->grads = h.grads;
-        stats->arena_bytes_used = hc.arena_top * sizeof(uint2);
-        stats->kernel_launches = launches;
+        write_stats(stats, h, true, hc.arena_top, launches);
         if (timing) add_stage_ms_3d(c, 0, L, stats->stage_ms);
     }
     return rc;
@@ -1046,12 +1163,8 @@ int32_t fc_render3d_frames(fc_ctx* c, const fc_tape* tape, const fc_render3d_cfg
     if (cfg->root_stride > 1) return fail(FC_ERR_UNSUPPORTED, "the tile interleave is not supported by frame batches");
     // every frame's ShapeVars binding, before anything is allocated or launched (z is unused in 3D)
     std::vector<Frame2D> table(n_frames);
-    for (uint32_t k = 0; k < n_frames; ++k) {
-        if (frames[k].n_var_values > FC_MAX_VARS) return fail(FC_ERR_INVALID, "n_var_values above FC_MAX_VARS");
-        memcpy(table[k].mat.m, frames[k].mat, sizeof table[k].mat.m);
-        table[k].z = 0.0f;
-        if (int32_t brc = bind_vars(tape, frames[k].var_values, frames[k].n_var_values, table[k].vb)) return brc;
-    }
+    for (uint32_t k = 0; k < n_frames; ++k)
+        if (int32_t brc = bind_frame(tape, frames[k], 0.0f, table[k])) return brc;
     CallCancel cc;
     if (int32_t crc = begin_call(c, cc)) return crc;
     if (stats) memset(stats, 0, sizeof *stats);
@@ -1091,27 +1204,13 @@ int32_t fc_render3d_frames(fc_ctx* c, const fc_tape* tape, const fc_render3d_cfg
         size_lists_3d(gp);
         return gp;
     };
-    auto pass_bytes = [&](uint32_t n) {
-        const Tiles3D gp = grid_of(n);
-        uint64_t b = uint64_t(n) * (size_t(frame_rows) * W * 8 + occl_frame * 4 + (host_out ? 2 * img_px * 16 : 0));
-        for (int l = 1; l <= L; ++l) b += gp.level_cap[l] * sizeof(TileJob);
-        return b + gp.level_cap[L] * 4 + gp.cap_census * sizeof(CensusRec);
-    };
-    // the most frames a pass may hold: FC_FRAMES_PASS_BYTES (at least one frame), 32-bit root ids, and (exact census)
-    // 16-bit census rows
-    uint32_t n_max = 1;
-    while (n_max < n_frames && pass_bytes(n_max + 1) <= FC_FRAMES_PASS_BYTES && frame_roots * (n_max + 1) <= 0xfffffff0ull &&
-           (!g.exact_census || uint64_t(frame_rows) * (n_max + 1) <= 65536))
-        ++n_max;
-    const int forced = env_int("FIDGET_B200_FRAMES_PER_PASS", 0);   // (diagnostic: at most the limits above)
-    if (forced > 0) n_max = std::min<uint32_t>(n_max, uint32_t(forced));
-    {
-        Tiles3D gm = grid_of(n_max);
-        if (int32_t erc = ensure_scratch_3d(c, gm, size_t(W) * frame_rows * n_max, occl_frame * n_max)) return erc;
-        if (!env_int("FIDGET_B200_NO_ZSORT", 0)) CU(c->zsort.ensure(size_t(zsort_layers(gm) + 1) * 4 + gm.level_cap[L] * 4));
-    }
+    // (exact census: a pass keeps its census rows within 16 bits)
+    PassPlan plan(c, grid_of, n_frames, size_t(frame_rows) * W * 8 + occl_frame * 4 + (host_out ? 2 * img_px * 16 : 0),
+                  g.exact_census ? 65536 / frame_rows : 0xffffffffu);
+    const uint32_t n_max = plan.n_max;
+    if (int32_t erc = ensure_scratch_3d(c, grid_of(n_max), size_t(W) * frame_rows * n_max, occl_frame * n_max)) return erc;
     CU(c->frame_table.ensure(size_t(n_frames) * sizeof(Frame2D)));
-    if (!c->pass_pin) CU(cudaHostAlloc(reinterpret_cast<void**>(&c->pass_pin), 2 * sizeof(PassStatus), cudaHostAllocDefault));
+    if (int32_t prc = ensure_pass_pin(c)) return prc;
     fc_geometry_pixel* stage[2] = {nullptr, nullptr};
     if (host_out) {
         CU(c->image.ensure(2 * img_px * 16 * n_max));
@@ -1120,47 +1219,10 @@ int32_t fc_render3d_frames(fc_ctx* c, const fc_tape* tape, const fc_render3d_cfg
     }
     if (int32_t src = ensure_copy_stream(c)) return src;
     CU(cudaMemcpyAsync(c->frame_table.p, table.data(), table.size() * sizeof(Frame2D), cudaMemcpyHostToDevice, s));
-    const uint64_t arena_clauses = std::min<uint64_t>(c->arena.cap, c->arena_bytes) / sizeof(uint2);
 
-    // Overflow policy: a pass fails (FC_ERR_ARENA, list overflow) only where one of its frames alone would.  The first
-    // pass holds one frame; later ones are sized from the largest per-frame use seen so far (arena clauses, jobs per
-    // level, census records) with headroom 1.5; a pass that still overflows is run again as two halves (the kernels
-    // report overflow, they do not fault), and only a one-frame pass returns the error.  Only capped lists can
-    // overflow: a job list whose cap is the worst case of the pass (every tile of the level queued) never does, so the
-    // headroom applies to the arena, to the job lists clamped by FIDGET_B200_MAX_TILES_M and to a clamped census.
-    double use_arena = 0, use_census = 0, use_jobs[MAX_LEVELS + 1] = {};
-    bool measured = forced > 0;
-    auto fits = [&](uint32_t n) {
-        const Tiles3D gp = grid_of(n);
-        const double h = 1.5 * n;
-        if (use_arena * h > double(arena_clauses)) return false;
-        uint64_t census_worst = gp.n_roots;
-        for (int l = 1; l <= L; ++l) {
-            const uint64_t r = g.ts[0] / g.ts[l - 1];
-            const bool clamped = gp.level_cap[l] < gp.n_roots * r * r * r;
-            if (clamped && use_jobs[l] * h > double(gp.level_cap[l])) return false;
-            if (l < L) { const uint64_t q = g.ts[l - 1] / g.ts[l]; census_worst += gp.level_cap[l] * q * q * q; }
-        }
-        const bool census_clamped = g.exact_census && gp.cap_census < census_worst;
-        return !census_clamped || use_census * h <= double(gp.cap_census);
-    };
-    struct Range { uint32_t f0, n; };
+    using Range = PassPlan::Range;
     struct InFlight { Range r; int b; size_t ev0; };
-    std::vector<Range> redo;   // halves of overflowed passes (a stack: the first half runs next)
-    uint32_t next = 0;         // first frame no pass has taken yet
-    auto take = [&]() -> Range {
-        if (!redo.empty()) { const Range r = redo.back(); redo.pop_back(); return r; }
-        uint32_t n = std::min(n_max, n_frames - next);
-        if (!measured) n = 1;
-        else if (forced <= 0) while (n > 1 && !fits(n)) --n;
-        const Range r{next, n};
-        next += n;
-        return r;
-    };
-
-    Stats total{};
-    uint64_t arena_used = 0;
-    float stage_ms[16] = {};
+    PassStats sum;
     size_t ev = 0;
     uint32_t launches = 0;
     bool copy_pending[2] = {false, false};
@@ -1190,31 +1252,10 @@ int32_t fc_render3d_frames(fc_ctx* c, const fc_tape* tape, const fc_render3d_cfg
     auto settle = [&](const InFlight& f) -> int32_t {
         if (int32_t wrc = wait_pass(c, f.b, cc, true)) return wrc;
         const PassStatus& ps = c->pass_pin[f.b];
-        const double n = double(f.r.n);
-        use_arena = std::max(use_arena, double(ps.ctr.arena_top) / n);
-        use_census = std::max(use_census, double(ps.ctr.n_census) / n);
-        for (int l = 1; l <= L; ++l) use_jobs[l] = std::max(use_jobs[l], double(ps.ctr.n_jobs[l]) / n);
-        measured = true;
-        if (ps.ctr.error) {
-            if (f.r.n == 1 || (ps.ctr.error & ~3u)) return device_error(ps.ctr.error);
-            const uint32_t h = f.r.n / 2;
-            redo.push_back(Range{f.r.f0 + h, f.r.n - h});
-            redo.push_back(Range{f.r.f0, h});
-            return FC_OK;
-        }
-        if (want_stats) {
-            for (int l = 0; l < MAX_LEVELS; ++l) {
-                total.evaluated[l] += ps.st.evaluated[l];
-                total.filled_inside[l] += ps.st.filled_inside[l];
-                total.filled_outside[l] += ps.st.filled_outside[l];
-                total.ambiguous[l] += ps.st.ambiguous[l];
-                total.simplified[l] += ps.st.simplified[l];
-            }
-            total.pixels += ps.st.pixels;
-            total.grads += ps.st.grads;
-            arena_used = std::max<uint64_t>(arena_used, ps.ctr.arena_top * sizeof(uint2));
-            if (timing) add_stage_ms_3d(c, f.ev0, L, stage_ms);
-        }
+        bool split = false;
+        if (int32_t orc = plan.observe(ps.ctr, f.r, split)) return orc;
+        if (split) return FC_OK;
+        if (want_stats) sum.add(c, ps, timing, f.ev0, L);
         if (host_out) {
             copy_pending[f.b] = true;
             return copy_pass_back(c, f.b, out + size_t(f.r.f0) * img_px, stage[f.b], size_t(f.r.n) * img_px * 16);
@@ -1228,15 +1269,15 @@ int32_t fc_render3d_frames(fc_ctx* c, const fc_tape* tape, const fc_render3d_cfg
     InFlight prev{};
     int buf = 0;
     for (;;) {
-        const bool more = next < n_frames || !redo.empty();
+        const bool more = plan.more();
         if (more && have_prev && cc.flag && __atomic_load_n(cc.flag, __ATOMIC_ACQUIRE)) stopped = true;   // enqueue no further pass
         if (more && !stopped) {
-            if (have_prev && !measured) {   // the first pass is read before the second is sized
+            if (have_prev && !plan.measured) {   // the first pass is read before the second is sized
                 if (int32_t rc = settle(prev)) return abandon(rc);
                 have_prev = false;
                 continue;
             }
-            const Range r = take();
+            const Range r = plan.take();
             const InFlight cur{r, buf, ev};
             if (int32_t rc = enqueue(r, buf)) return abandon(rc);
             if (have_prev)
@@ -1260,13 +1301,7 @@ int32_t fc_render3d_frames(fc_ctx* c, const fc_tape* tape, const fc_render3d_cfg
         CU(cudaStreamSynchronize(c->copy_stream));
     }
     if (stopped) return abandon(fail(FC_ERR_CANCELLED, "cancelled"));   // the flag stopped the passes
-    if (stats) {
-        copy_census(total, stats);
-        stats->grads = total.grads;
-        stats->arena_bytes_used = arena_used;
-        stats->kernel_launches = launches;
-        memcpy(stats->stage_ms, stage_ms, sizeof stage_ms);
-    }
+    if (stats) sum.write(stats, launches);
     return FC_OK;
 }
 
@@ -1290,10 +1325,7 @@ int32_t fc_render3d_scene(fc_ctx* c, const fc_tape* const* tapes, const fc_frame
     for (uint32_t k = 0; k < n_shapes; ++k) {
         if (!tapes[k]) return fail(FC_ERR_INVALID, "null tape in the scene");
         if (int32_t vrc = check_3d(tapes[k], cfg)) return vrc;
-        if (placements[k].n_var_values > FC_MAX_VARS) return fail(FC_ERR_INVALID, "n_var_values above FC_MAX_VARS");
-        memcpy(table[k].mat.m, placements[k].mat, sizeof table[k].mat.m);
-        table[k].z = 0.0f;
-        if (int32_t brc = bind_vars(tapes[k], placements[k].var_values, placements[k].n_var_values, table[k].vb)) return brc;
+        if (int32_t brc = bind_frame(tapes[k], placements[k], 0.0f, table[k])) return brc;
     }
     Tiles3D g;
     const bool clamp = !(cfg->flags & FC_FLAG_NO_CLAMP);
@@ -1338,26 +1370,12 @@ int32_t fc_render3d_scene(fc_ctx* c, const fc_tape* const* tapes, const fc_frame
         gp.level_cap[L] = std::min<uint64_t>(gp.level_cap[L], FC_SCENE_MAX_LEAF_JOBS);
         return gp;
     };
-    auto pass_bytes = [&](uint32_t n) {
-        const Tiles3D gp = grid_of(n);
-        uint64_t b = gp.level_cap[L] * 4;
-        for (int l = 1; l <= L; ++l) b += gp.level_cap[l] * sizeof(TileJob);
-        return b;
-    };
-    uint32_t n_max = 1;
-    while (n_max < n_shapes && pass_bytes(n_max + 1) <= FC_FRAMES_PASS_BYTES && vol_roots * (n_max + 1) <= 0xfffffff0ull)
-        ++n_max;
-    const int forced = env_int("FIDGET_B200_FRAMES_PER_PASS", 0);   // (diagnostic: at most the limits above)
-    if (forced > 0) n_max = std::min<uint32_t>(n_max, uint32_t(forced));
-    {
-        Tiles3D gm = grid_of(n_max);
-        if (int32_t erc = ensure_scratch_3d(c, gm, npix, occl_blocks * 2)) return erc;
-        if (!env_int("FIDGET_B200_NO_ZSORT", 0)) CU(c->zsort.ensure(size_t(zsort_layers(gm) + 1) * 4 + gm.level_cap[L] * 4));
-    }
+    PassPlan plan(c, grid_of, n_shapes, 0, 0xffffffffu);
+    if (int32_t erc = ensure_scratch_3d(c, grid_of(plan.n_max), npix, occl_blocks * 2)) return erc;
     CU(c->frame_table.ensure(size_t(n_shapes) * sizeof(Frame2D)));
     CU(c->scene_pl.ensure(size_t(n_shapes) * 4));
     if (n_shapes > 1) CU(c->scene_backup.ensure(npix * 8 + (g.use_occl ? occl_blocks * 8 : 0)));
-    if (!c->pass_pin) CU(cudaHostAlloc(reinterpret_cast<void**>(&c->pass_pin), 2 * sizeof(PassStatus), cudaHostAllocDefault));
+    if (int32_t prc = ensure_pass_pin(c)) return prc;
     void* dimg = out;
     if (host_out) {
         CU(c->image.ensure(npix * 16));
@@ -1372,38 +1390,10 @@ int32_t fc_render3d_scene(fc_ctx* c, const fc_tape* const* tapes, const fc_frame
     CU(cudaMemcpyAsync(c->frame_table.p, table.data(), table.size() * sizeof(Frame2D), cudaMemcpyHostToDevice, s));
     CU(cudaMemsetAsync(c->heightmap.p, 0, npix * 8, s));
     if (g.use_occl) CU(cudaMemsetAsync(c->occl.p, 0, occl_blocks * 8, s));
-    const uint64_t arena_clauses = std::min<uint64_t>(c->arena.cap, c->arena_bytes) / sizeof(uint2);
 
-    // Overflow policy, as fc_render3d_frames's per frame: the first pass holds one placement, later ones are sized from
-    // the largest per-placement use so far with headroom 1.5.  Passes build on each other's heightmap, so each is waited
+    // Passes follow PassPlan's overflow policy per placement.  They build on each other's heightmap, so each is waited
     // for before the next; one of several placements keeps a copy of the heightmap and occlusion map from before it,
-    // and if it overflows anyway (the kernels report it, they do not fault; its normals write nothing) the copy is
-    // restored and its halves run instead.  Only a one-placement pass returns the error.
-    double use_arena = 0, use_jobs[MAX_LEVELS + 1] = {};
-    bool measured = forced > 0;
-    auto fits = [&](uint32_t n) {
-        const Tiles3D gp = grid_of(n);
-        const double h = 1.5 * n;
-        if (use_arena * h > double(arena_clauses)) return false;
-        for (int l = 1; l <= L; ++l) {
-            const uint64_t r = g.ts[0] / g.ts[l - 1];
-            const bool clamped = gp.level_cap[l] < gp.n_roots * r * r * r;
-            if (clamped && use_jobs[l] * h > double(gp.level_cap[l])) return false;
-        }
-        return true;
-    };
-    struct Range { uint32_t f0, n; };
-    std::vector<Range> redo;   // halves of overflowed passes (a stack: the first half runs next)
-    uint32_t next = 0;
-    auto take = [&]() -> Range {
-        if (!redo.empty()) { const Range r = redo.back(); redo.pop_back(); return r; }
-        uint32_t n = std::min(n_max, n_shapes - next);
-        if (!measured) n = 1;
-        else if (forced <= 0) while (n > 1 && !fits(n)) --n;
-        const Range r{next, n};
-        next += n;
-        return r;
-    };
+    // and if it overflows anyway (its normals write nothing) the copy is restored and its halves run instead.
     auto abandon = [&](int32_t rc) { return abandon_frames(c, s, stats, rc); };
     const size_t backup_occl = npix * 8;   // (byte offset of the occlusion map's copy)
     auto snapshot = [&](bool restore) -> int32_t {
@@ -1415,17 +1405,15 @@ int32_t fc_render3d_scene(fc_ctx* c, const fc_tape* const* tapes, const fc_frame
         return FC_OK;
     };
 
-    Stats total{};
-    uint64_t arena_used = 0;
-    float stage_ms[16] = {};
+    PassStats sum;
     size_t ev = 0;
     uint32_t launches = 0;
     std::vector<uint32_t> pl_host;
     const bool early_return = async && !host_out && !host_index && !want_stats;
-    for (bool first = true; next < n_shapes || !redo.empty(); first = false) {
+    for (bool first = true; plan.more(); first = false) {
         if (!first && cc.flag && __atomic_load_n(cc.flag, __ATOMIC_ACQUIRE))
             return abandon(fail(FC_ERR_CANCELLED, "cancelled"));   // the flag stops the passes
-        const Range r = take();
+        const PassPlan::Range r = plan.take();
         // level-0 groups: the pass's placements by tape, in order of first appearance
         Tiles3D gp = grid_of(r.n);
         gp.pl0 = r.f0;
@@ -1454,7 +1442,7 @@ int32_t fc_render3d_scene(fc_ctx* c, const fc_tape* const* tapes, const fc_frame
         PassStatus* hs = c->pass_pin;
         CU(cudaMemcpyAsync(&hs->ctr, c->counters.p, sizeof(Counters), cudaMemcpyDeviceToHost, s));
         if (want_stats) CU(cudaMemcpyAsync(&hs->st, c->stats.p, sizeof(Stats), cudaMemcpyDeviceToHost, s));
-        if (early_return && next >= n_shapes && redo.empty()) {   // FC_FLAG_ASYNC: the last pass is left running
+        if (early_return && !plan.more()) {   // FC_FLAG_ASYNC: the last pass is left running
             c->async_call = cc;
             return FC_OK;
         }
@@ -1463,42 +1451,18 @@ int32_t fc_render3d_scene(fc_ctx* c, const fc_tape* const* tapes, const fc_frame
         } else {
             CU(cudaStreamSynchronize(s));
         }
-        const double n = double(r.n);
-        use_arena = std::max(use_arena, double(hs->ctr.arena_top) / n);
-        for (int l = 1; l <= L; ++l) use_jobs[l] = std::max(use_jobs[l], double(hs->ctr.n_jobs[l]) / n);
-        measured = true;
-        if (hs->ctr.error) {
-            if (r.n == 1 || (hs->ctr.error & ~3u)) return abandon(device_error(hs->ctr.error));
+        bool split = false;
+        if (int32_t orc = plan.observe(hs->ctr, r, split)) return abandon(orc);
+        if (split) {
             if (int32_t brc = snapshot(true)) return abandon(brc);
-            const uint32_t h = r.n / 2;
-            redo.push_back(Range{r.f0 + h, r.n - h});
-            redo.push_back(Range{r.f0, h});
             continue;
         }
-        if (want_stats) {
-            for (int l = 0; l < MAX_LEVELS; ++l) {
-                total.evaluated[l] += hs->st.evaluated[l];
-                total.filled_inside[l] += hs->st.filled_inside[l];
-                total.filled_outside[l] += hs->st.filled_outside[l];
-                total.ambiguous[l] += hs->st.ambiguous[l];
-                total.simplified[l] += hs->st.simplified[l];
-            }
-            total.pixels += hs->st.pixels;
-            total.grads += hs->st.grads;
-            arena_used = std::max<uint64_t>(arena_used, hs->ctr.arena_top * sizeof(uint2));
-            if (timing) add_stage_ms_3d(c, ev0, L, stage_ms);
-        }
+        if (want_stats) sum.add(c, *hs, timing, ev0, L);
     }
     if (host_out) CU(cudaMemcpyAsync(out, dimg, npix * 16, cudaMemcpyDeviceToHost, s));
     if (host_index) CU(cudaMemcpyAsync(index, dindex, npix * 2, cudaMemcpyDeviceToHost, s));
     CU(cudaStreamSynchronize(s));
-    if (stats) {
-        copy_census(total, stats);
-        stats->grads = total.grads;
-        stats->arena_bytes_used = arena_used;
-        stats->kernel_launches = launches;
-        memcpy(stats->stage_ms, stage_ms, sizeof stage_ms);
-    }
+    if (stats) sum.write(stats, launches);
     return FC_OK;
 }
 

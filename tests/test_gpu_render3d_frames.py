@@ -56,9 +56,9 @@ def _single_cfg(cfg, f):
 
 
 def _singles(shape, cfg, table):
-    """render3d of every frame of `table` on its own: (images, summed stats)"""
+    """render3d of every frame of `table` on its own: (images, summed stats; "launches": those of one call)"""
     imgs, tot = [], {k: [0] * 8 for k in CENSUS}
-    tot.update(pixels=0, grads=0, arena=0)
+    tot.update(pixels=0, grads=0, arena=0, launches=0)
     for f in table:
         img, st = fb.render3d(shape, _single_cfg(cfg, f), stats=True)
         imgs.append(img)
@@ -67,6 +67,7 @@ def _singles(shape, cfg, table):
         tot["pixels"] += st["pixels"]
         tot["grads"] += st["grads"]
         tot["arena"] = max(tot["arena"], st["arena_bytes_used"])
+        tot["launches"] = max(tot["launches"], st["kernel_launches"])
     return np.stack(imgs), tot
 
 
@@ -209,7 +210,8 @@ def test_asynchronous_into_a_cuda_tensor(cuda):
 @pytest.mark.parametrize("forced", [0, 16])
 def test_small_arena_batch_equals_singles(cuda, monkeypatch, forced):
     """An arena of 1.5x the largest single frame's use: 16 frames do not fit one pass, and the batch still equals the
-    singles (sized from the first frame's use, or, with 16 frames forced into one pass, split in halves on overflow)"""
+    singles (sized from the first frame's use, or, with 16 frames forced into one pass, split in halves on overflow).
+    A pass makes the launches of one single call, overflowed passes included, so the launch count says how many ran."""
     cfg = fb.RenderConfig3D(512, 512, 512)
     views = _orbit(16)
     want, tot = _singles(_shape(cuda, "prospero.vm"), cfg, fb.frame_table_3d(cfg, world_to_model=views))
@@ -225,6 +227,8 @@ def test_small_arena_batch_equals_singles(cuda, monkeypatch, forced):
     for k in DETERMINISTIC:
         assert st[k] == tot[k], k
     assert st["arena_bytes_used"] <= arena
+    passes, rest = divmod(st["kernel_launches"], tot["launches"])
+    assert rest == 0 and passes >= (3 if forced else 2), (st["kernel_launches"], tot["launches"])
 
 
 def test_arena_too_small_for_one_frame(cuda):

@@ -236,7 +236,8 @@ def test_forced_passes_change_nothing(cuda, monkeypatch, per_pass):
 @pytest.mark.parametrize("forced", [0, 8])
 def test_small_arena_changes_nothing(cuda, monkeypatch, forced):
     """an arena of 1.5x the largest single shape's use: the eight placements do not fit one pass (with eight forced into
-    one, it overflows and is restored and split), and the image is still the fold"""
+    one, it overflows and is restored and split), and the image is still the fold.  A pass of one tape makes the launches
+    of one render3d call, overflowed passes included, so the launch count says how many ran."""
     cfg = fb.RenderConfig3D(512, 512, 512)
     views = queue()
     singles = _singles([_shape(cuda, "prospero.vm")] * 8, cfg, world_to_model=views)
@@ -252,6 +253,9 @@ def test_small_arena_changes_nothing(cuda, monkeypatch, forced):
     img, index, st = fb.render3d_scene([shape] * 8, cfg, world_to_model=views, stats=True)
     assert np.array_equal(_bits(img), _bits(want)) and np.array_equal(index, want_index)
     assert st["arena_bytes_used"] <= arena
+    one = singles[0][1]["kernel_launches"]
+    passes, rest = divmod(st["kernel_launches"], one)
+    assert rest == 0 and passes >= (3 if forced else 2), (st["kernel_launches"], one)
 
 
 def test_error_only_where_one_placement_overflows(cuda):

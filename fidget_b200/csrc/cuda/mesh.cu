@@ -20,6 +20,8 @@
 //
 // The 3x3 symmetric eigen-problem is solved with cyclic Jacobi rotations in f32 (the reference calls nalgebra's
 // SVD, a third-party algorithm not under /root/reference); positions agree to ~1e-5 of a cell, not bit for bit.
+#include <cstddef>
+
 #include "capi_internal.h"
 
 namespace fdev {
@@ -280,6 +282,16 @@ __global__ void k_mesh_assign(MeshScratch m) {
         const OctreeLeaf& L = m.leaves[leaf];
         m.out_verts[id] = make_float3(L.pos[k - 4u][0], L.pos[k - 4u][1], L.pos[k - 4u][2]);
     }
+}
+
+// Octree::build's last step (octree.rs:58-65): every vertex goes from the [-1,1]^3 cube the octree was built in back to
+// model space, through Matrix4::transform_point.  `pos` is the first of *count (at most cap) float triples `stride`
+// bytes apart: the vertex buffer, or the vertex field of the final-leaf list.
+__global__ void k_mesh_to_model(char* pos, size_t stride, const uint32_t* count, uint32_t cap, Mat4 M) {
+    const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= min(*count, cap)) return;
+    float* p = reinterpret_cast<float*>(pos + size_t(i) * stride);
+    xform_f32(M, p[0], p[1], p[2], p[0], p[1], p[2]);
 }
 
 // Mesh::write_stl (output.rs:7-38): 80-byte header, u32 count, 50 bytes per triangle
@@ -780,7 +792,8 @@ int32_t octree_sample_device(fc_ctx* c, const fc_tape* tape, const fc_octree_cfg
                              uint32_t* n_out, fc_octree_stats* stats, const CallCancel& cc);
 
 // fc_mesh_build with FC_FLAG_MESH_COLLAPSE, after the sampler (n > 0 surface leaves in c->mesh_leaves; c->mu held)
-static int32_t mesh_build_collapse(fc_ctx* c, uint32_t n, uint32_t depth, fc_mesh_info* info, const CallCancel& cc) {
+static int32_t mesh_build_collapse(fc_ctx* c, uint32_t n, uint32_t depth, const fdev::Mat4* to_model, fc_mesh_info* info,
+                                   const CallCancel& cc) {
     using namespace fdev;
     cudaStream_t s = c->stream;
     // nodes: the leaves plus at most min(n, 8^d) ancestors at every depth d < D
@@ -869,6 +882,12 @@ static int32_t mesh_build_collapse(fc_ctx* c, uint32_t n, uint32_t depth, fc_mes
     m.cap_tris = n_tris;
     k_tree_assign<<<unsigned((uint64_t(n_nodes) * 16 + 255) / 256), 256, 0, s>>>(m);
     k_tree_faces<1><<<(n_nodes * 12u + 127) / 128, 128, 0, s>>>(m);
+    if (to_model) {
+        k_mesh_to_model<<<unsigned((v_cap + 255) / 256), 256, 0, s>>>(reinterpret_cast<char*>(m.out_verts), sizeof(float3), m.counts,
+                                                                     m.cap_verts, *to_model);
+        k_mesh_to_model<<<(n_nodes + 255) / 256, 256, 0, s>>>(reinterpret_cast<char*>(m.out_cells) + offsetof(fc_mesh_cell, vertex),
+                                                             sizeof(fc_mesh_cell), m.counts + 5, n_nodes, *to_model);
+    }
     CU(cudaEventRecord(e1, s));
     CU(cudaGetLastError());
     if (int32_t wrc = wait_read(c, s, cc, cnt, m.counts, sizeof cnt)) return wrc;
@@ -923,7 +942,13 @@ int32_t fc_mesh_build(fc_ctx* c, const fc_tape* tape, const fc_octree_cfg* cfg, 
     info->sampler_ms = ost.total_ms;
     c->mesh_n_verts = c->mesh_n_tris = c->mesh_n_cells = 0;
     if (n == 0) return FC_OK;
-    if (cfg->flags & FC_FLAG_MESH_COLLAPSE) return cancelled(mesh_build_collapse(c, n, cfg->depth, info, cc));
+    // Octree::build maps the vertices through Settings::world_to_model unless that is the identity (octree.rs:58-65)
+    fdev::Mat4 view;
+    memcpy(view.m, cfg->world_to_model, sizeof view.m);
+    bool to_model = false;
+    for (int i = 0; i < 16 && cfg->has_transform; ++i) to_model |= view.m[i] != (i % 5 == 0 ? 1.0f : 0.0f);
+    if (cfg->flags & FC_FLAG_MESH_COLLAPSE)
+        return cancelled(mesh_build_collapse(c, n, cfg->depth, to_model ? &view : nullptr, info, cc));
     uint32_t hsize = 1024;
     while (hsize < 2u * n) hsize <<= 1;
     const size_t b_keys = size_t(hsize) * 8, b_vals = size_t(hsize) * 4, b_cv = size_t(n) * 4 * sizeof(float3), b_cn = size_t(n) * 4,
@@ -961,6 +986,9 @@ int32_t fc_mesh_build(fc_ctx* c, const fc_tape* tape, const fc_octree_cfg* cfg, 
     m.cap_tris = n_tris;
     k_mesh_assign<<<unsigned((uint64_t(n) * 16 + 255) / 256), 256, 0, s>>>(m);
     k_mesh_faces<1><<<(n * 3u + 127) / 128, 128, 0, s>>>(m);
+    if (to_model)
+        k_mesh_to_model<<<unsigned((v_cap + 255) / 256), 256, 0, s>>>(reinterpret_cast<char*>(m.out_verts), sizeof(float3), m.counts,
+                                                                     m.cap_verts, view);
     CU(cudaEventRecord(e1, s));
     CU(cudaGetLastError());
     if (int32_t wrc = wait_read(c, s, cc, cnt, m.counts, sizeof cnt)) return cancelled(wrc);

@@ -403,7 +403,12 @@ int32_t fc_octree_sample(fc_ctx* ctx, const fc_tape* tape, const fc_octree_cfg* 
  * cell are merged into one leaf as Octree::check_done / try_collapse do (octree.rs:252-440: manifold topology and a
  * merged QEF error below twice the children's), and the dual is walked over leaves of different depths, as
  * Octree::build(..).walk_dual() does: fewer triangles in flat regions.  Edges on the boundary of the [-1,1]^3 domain
- * get no triangles (open_edges). */
+ * get no triangles (open_edges).
+ * With fc_octree_cfg.has_transform the octree is built over the [-1,1]^3 world cube in the field seen through
+ * world_to_model, and, as the last step of Octree::build (octree.rs:58-65), every vertex is mapped back to model space
+ * through Matrix4::transform_point (f32, divided by the homogeneous term where that is not zero) unless the matrix is
+ * the identity: fc_mesh_read, fc_mesh_write_stl and fc_mesh_cell.vertex are in model space, the cell coordinates of
+ * fc_mesh_read_cells stay those of the world cube. */
 #define FC_FLAG_MESH_COLLAPSE 64u /* fc_mesh_build: cell collapse and the adaptive dual walk */
 typedef struct fc_mesh_info {
     uint64_t n_leaves, n_vertices, n_triangles, open_edges;

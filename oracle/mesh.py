@@ -9,6 +9,9 @@ numpy restatement of the meshing back half of fidget-mesh for leaves of equal de
   triangles       dc_edge for four leaves of equal depth (fidget-mesh/src/dc.rs:104-213)
   STL             Mesh::write_stl (fidget-mesh/src/output.rs:7-38)
 
+  model space     Octree::build's last step (fidget-mesh/src/octree.rs:58-65): the vertices of an octree sampled through
+                  ``world_to_model`` go back through that matrix (``to_model``)
+
 Cell collapse (octree.rs:252-440) is out of scope on both sides.  Only tests/ may import this module.
 """
 from __future__ import annotations
@@ -76,6 +79,22 @@ def qef_vertex(points, grads):
     return pos if not np.isnan(pos).any() else center
 
 
+def to_model(verts, world_to_model):
+    """Matrix4::transform_point on every row of ``verts`` [n,3], in float32 and nalgebra's order: ((m0 x + m1 y) + m2 z)
+    + m3 per row, divided by the homogeneous term where that is not zero.  Octree::build applies it to every octree
+    vertex unless the matrix is the identity (octree.rs:58-65); None stands for the identity here."""
+    v = np.asarray(verts, dtype=np.float32).reshape(-1, 3)
+    if world_to_model is None or np.array_equal(np.asarray(world_to_model, dtype=np.float32).reshape(4, 4),
+                                                np.eye(4, dtype=np.float32)):
+        return v
+    m = np.asarray(world_to_model, dtype=np.float32).reshape(4, 4)
+    x, y, z = v[:, 0], v[:, 1], v[:, 2]
+    with np.errstate(all="ignore"):
+        r = [((m[i, 0] * x + m[i, 1] * y) + m[i, 2] * z) + m[i, 3] for i in range(4)]
+        out = np.stack([np.where(r[3] != 0, r[i] / np.where(r[3] != 0, r[3], np.float32(1)), r[i]) for i in range(3)], axis=-1)
+    return out.astype(np.float32)
+
+
 def build(leaves):
     """leaves: the structured array of ``oracle.octree_sample``.  Returns (cell_vertices dict (leaf, group) -> pos,
     triangles as a list of three positions each, open edge count)."""
@@ -84,17 +103,18 @@ def build(leaves):
     return verts, tris, open_edges
 
 
-def build_indexed(leaves, vertex=qef_vertex):
+def build_indexed(leaves, vertex=qef_vertex, world_to_model=None):
     """build() indexed the way fc_mesh_build returns the mesh: one vertex per slot the triangles use (MeshBuilder's
     dedup), ``(vertices [n,3] float32, triangles [m,3] int64, open edge count, slots)``, where a slot is
     ('v', leaf, group) for a cell vertex or ('i', leaf, edge) for an intersection.  ``vertex(points, grads)``
-    places a cell vertex (qef_vertex by default); the triangles do not depend on it."""
+    places a cell vertex (qef_vertex by default); the triangles do not depend on it.  ``leaves`` sampled through
+    ``world_to_model``: the vertices are returned in model space (``to_model``)."""
     verts, tri_slots, open_edges = _walk(leaves, vertex)
     index = {}
     for t in tri_slots:
         for k in t:
             index.setdefault(k, len(index))
-    pos = np.array([_slot_pos(leaves, verts, k) for k in index], dtype=np.float32).reshape(-1, 3)
+    pos = to_model(np.array([_slot_pos(leaves, verts, k) for k in index], dtype=np.float32), world_to_model)
     tris = np.array([[index[k] for k in t] for t in tri_slots], dtype=np.int64).reshape(-1, 3)
     return pos, tris, open_edges, list(index)
 

@@ -472,8 +472,9 @@ Mat4 pixel_mat(uint32_t w, uint32_t h, const float wm[9]) {
 
 // nalgebra 0.35 Matrix4::transform_point (shape/mod.rs:906-915): linear part
 // accumulated left to right, plus translation, divided by the homogeneous
-// term when that is non-zero.  Summation order is PARITY-UNPINNED for
-// matrices with non-zero cross terms (SURVEY.md §8c).
+// term when that is non-zero.  For matrices with non-zero cross terms the
+// three transforms below are pinned against float64 (tests/test_views_oracle.py);
+// the summation order inside nalgebra itself stays unpinned (SURVEY.md §8c).
 void transform_f32(float x, float y, float z, const Mat4& m, float out[3]) {
     float n = ((m.m[3][0] * x + m.m[3][1] * y) + m.m[3][2] * z) + m.m[3][3];
     for (int i = 0; i < 3; ++i) {

@@ -413,11 +413,13 @@ class Octree:
         d, x, y, z = k
         return (d + 1, 2 * x + (c & 1), 2 * y + ((c >> 1) & 1), 2 * z + ((c >> 2) & 1))
 
-    def walk_dual(self):
-        """Octree::walk_dual: (vertices [n,3] float32, triangles [m,3] int64, open edge count)."""
+    def walk_dual(self, world_to_model=None):
+        """Octree::walk_dual: (vertices [n,3] float32, triangles [m,3] int64, open edge count).  For leaves sampled
+        through ``world_to_model`` the vertices come back in model space, as Octree::build leaves them (octree.rs:58-65);
+        ``cells`` keeps the world-cube positions the QEFs were solved in."""
         w = _Walk(self)
         w.cell((0, 0, 0, 0))
-        verts = np.array(w.verts, dtype=f32).reshape(-1, 3)
+        verts = om.to_model(np.array(w.verts, dtype=f32), world_to_model)
         return verts, np.array(w.tris, dtype=np.int64).reshape(-1, 3), self.open_edges()
 
     def open_edges(self):
@@ -573,9 +575,9 @@ class _Walk:
                 self.tris.append((vs[j], vs[(j + winding) % 4], iv))
 
 
-def build(orc, tape, depth, sign_at=None):
-    """Octree::build over ``orc.octree_sample(tape, depth)``."""
-    leaves, _ = orc.octree_sample(tape, depth)
+def build(orc, tape, depth, sign_at=None, world_to_model=None):
+    """Octree::build over ``orc.octree_sample(tape, depth, world_to_model)``; pass the matrix to ``walk_dual`` too."""
+    leaves, _ = orc.octree_sample(tape, depth, world_to_model)
     return Octree(leaves, depth, sign_at)
 
 

@@ -71,14 +71,15 @@ class Report:
                 f"{self.ambiguous} rank-ambiguous, {self.forced} forced")
 
 
-def compare_collapse(cuda, g, leaves, depth):
+def compare_collapse(cuda, g, leaves, depth, world_to_model=None):
     """fb.mesh(g, depth, collapse=True) against mco.Octree(leaves, depth).walk_dual(), exactly: final leaves, cell
     vertices, vertices, triangles, open_edges; then every final leaf's vertex against the float64 solve of the QEF
-    the oracle solved for that cell.  Returns (vertices, triangles, info, octree, Report)."""
-    verts, tris, info = fb.mesh(g, depth, collapse=True)
+    the oracle solved for that cell.  ``leaves`` sampled through ``world_to_model``: both meshes are in model space, the
+    float64 check stays in the world cube the QEFs live in.  Returns (vertices, triangles, info, octree, Report)."""
+    verts, tris, info = fb.mesh(g, depth, world_to_model=world_to_model, collapse=True)
     cells = fb.mesh_cells(cuda)
     octree = mco.Octree(leaves, depth)
-    o_verts, o_tris, o_open = octree.walk_dual()
+    o_verts, o_tris, o_open = octree.walk_dual(world_to_model)
     final = octree.final_leaves()
     assert leaf_set(cells) == [tuple(int(v) for v in c) for c in final], "final leaves differ"
     assert info["n_triangles"] == len(tris) and info["n_vertices"] == len(verts)
@@ -87,49 +88,55 @@ def compare_collapse(cuda, g, leaves, depth):
     rep = Report()
     for cell in cells:
         key = (int(cell["depth"]), int(cell["ix"]), int(cell["iy"]), int(cell["iz"]))
-        want = octree.cells[key]["verts"][0]
-        assert np.array_equal(cell["vertex"].view(np.uint32), np.asarray(want, dtype=f32).view(np.uint32)), \
+        world = octree.cells[key]["verts"][0]
+        want = om.to_model(world, world_to_model)[0]
+        assert np.array_equal(cell["vertex"].view(np.uint32), want.view(np.uint32)), \
             f"cell {key}: vertex {cell['vertex']} vs the oracle's {want}"
         q = octree.qefs[key]
-        rep.vertex(cell["vertex"], q[0] if isinstance(q, list) else q, octree.leaves.get(key), f"cell {key}")
+        rep.vertex(world, q[0] if isinstance(q, list) else q, octree.leaves.get(key), f"cell {key}")
     return verts, tris, info, octree, rep
 
 
 class _F32Vertex:
     """oracle/mesh.py's vertex callback with the device's float32 solve (mco.Qef, k_mesh_vertices' order); keeps
-    each call's QEF (None when a NaN gradient forced the vertex onto that intersection)"""
+    each call's QEF (None when a NaN gradient forced the vertex onto that intersection) and the vertex it returned"""
 
     def __init__(self):
         self.calls = []
+        self.pos = []
 
     def __call__(self, pts, grs):
         q = mco.Qef()
         for p, g in zip(pts, grs):
             if np.isnan(g).any():
                 self.calls.append(None)
-                return np.asarray(p, dtype=f32)
+                self.pos.append(np.asarray(p, dtype=f32))
+                return self.pos[-1]
             q.add_intersection(p, g)
         self.calls.append(q)
-        return q.solve()[0]
+        self.pos.append(q.solve()[0])
+        return self.pos[-1]
 
 
-def compare_uniform(g, leaves, depth):
+def compare_uniform(g, leaves, depth, world_to_model=None):
     """fb.mesh(g, depth) against oracle/mesh.py's walk over the same leaves, exactly, with the device's float32 vertex
-    solve; then every cell vertex the mesh uses against the float64 solve of its QEF.  Returns a Report."""
-    verts, tris, info = fb.mesh(g, depth)
+    solve; then every cell vertex the mesh uses against the float64 solve of its QEF.  ``leaves`` sampled through
+    ``world_to_model``: both meshes are in model space, the float64 check stays in the world cube the QEFs live in.
+    Returns a Report."""
+    verts, tris, info = fb.mesh(g, depth, world_to_model=world_to_model)
     solve = _F32Vertex()
-    o_verts, o_tris, o_open, slots = om.build_indexed(leaves, vertex=solve)
+    o_verts, o_tris, o_open, slots = om.build_indexed(leaves, vertex=solve, world_to_model=world_to_model)
     assert info["n_leaves"] == len(leaves)
     assert info["open_edges"] == o_open, (info["open_edges"], o_open)
     assert info["n_triangles"] == len(tris) and info["n_vertices"] == len(verts)
     assert_same_mesh(verts, tris, o_verts, o_tris)
-    qefs, k = {}, 0
+    solved, k = {}, 0
     for i, leaf in enumerate(leaves):
         for grp in range(om.corner_groups(int(leaf["mask"]))[1]):
-            qefs[(i, grp)] = solve.calls[k]
+            solved[(i, grp)] = (solve.pos[k], solve.calls[k])
             k += 1
     rep = Report()
-    for pos, (kind, i, j) in zip(o_verts, slots):
+    for kind, i, j in slots:
         if kind == "v":
-            rep.vertex(pos, qefs[(i, j)], leaves[i], f"leaf {i} group {j}")
+            rep.vertex(*solved[(i, j)], leaves[i], f"leaf {i} group {j}")
     return rep

@@ -211,8 +211,7 @@ static int32_t cancel_site_of(const std::string& name) {
     static const char* const names[] = {
         "k_interval_root_coop", "k_fill_2d", "k_pixels_2d", "k_tail_2d", "k_voxels_3d", "k_normals_3d", "k_census_3d",
         "k_octree_leaf", "k_octree_grads", "k_mesh_hash", "k_mesh_vertices", "k_mesh_faces0", "k_mesh_faces1",
-        "k_mesh_assign", "k_tree_leaves", "k_tree_parents", "k_tree_leaf_err", "k_tree_collapse", "k_tree_final",
-        "k_tree_faces0", "k_tree_faces1", "k_tree_assign"};
+        "k_mesh_assign", "k_tree_parents", "k_tree_collapse", "k_tree_final", "k_tree_faces0", "k_tree_faces1"};
     static_assert(sizeof(names) / sizeof(names[0]) == CS_WAIT - CS_ROOT_COOP, "one name per poll site");
     for (int i = 0; i < MAX_LEVELS; ++i)
         if (name == "k_interval_level" + std::to_string(i)) return CS_LEVEL0 + i;

@@ -22,8 +22,7 @@ enum CancelSite : int32_t {
     CS_ROOT_COOP = 16, CS_FILL_2D, CS_PIXELS_2D, CS_TAIL_2D, CS_VOXELS_3D, CS_NORMALS_3D, CS_CENSUS_3D,
     CS_OCTREE_LEAF, CS_OCTREE_GRADS,
     CS_MESH_HASH, CS_MESH_VERTICES, CS_MESH_FACES0, CS_MESH_FACES1, CS_MESH_ASSIGN,
-    CS_TREE_LEAVES, CS_TREE_PARENTS, CS_TREE_LEAF_ERR, CS_TREE_COLLAPSE, CS_TREE_FINAL, CS_TREE_FACES0, CS_TREE_FACES1,
-    CS_TREE_ASSIGN,
+    CS_TREE_PARENTS, CS_TREE_COLLAPSE, CS_TREE_FINAL, CS_TREE_FACES0, CS_TREE_FACES1,
     CS_WAIT,                                              // polls inside spin waits: not a claim, never a trigger site
     CS_COUNT
 };

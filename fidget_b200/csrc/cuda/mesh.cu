@@ -15,8 +15,13 @@
 //              collapsible / try_collapse (octree.rs:252-440) merge the eight children of a cell into one leaf when
 //              the topology stays manifold and the merged QEF error (LeafHermiteData::merge / solve,
 //              octree.rs:912-1033) is below twice the children's; one launch per depth, bottom-up, over a tree of
-//              the surface leaves' ancestors keyed by (depth, x, y, z); the dual is then walked over leaves of
-//              different depths (k_tree_faces: dc_cell / dc_face / dc_edge's result, one thread per leaf edge).
+//              the surface leaves' ancestors; the dual is then walked over leaves of different depths (k_tree_faces:
+//              dc_cell / dc_face / dc_edge's result, one thread per leaf edge).
+//
+// Both modes share one scratch layout (MeshScratch), one cell table keyed by (depth, x, y, z), the surface leaves'
+// vertices (k_mesh_vertices, which also gives the collapse its leaf errors), the vertex compaction (k_mesh_assign) and
+// the host steps after pass 0 of their face kernels (mesh_finish).  Only the face kernels differ: k_mesh_faces looks
+// up the three equal-depth neighbours directly, k_tree_faces finds the final leaves covering them.
 //
 // The 3x3 symmetric eigen-problem is solved with cyclic Jacobi rotations in f32 (the reference calls nalgebra's
 // SVD, a third-party algorithm not under /root/reference); positions agree to ~1e-5 of a cell, not bit for bit.
@@ -27,51 +32,69 @@
 namespace fdev {
 
 __host__ __device__ inline uint32_t next_axis(uint32_t a) { return a == 1u ? 2u : (a == 2u ? 4u : 1u); }   // X -> Y -> Z -> X
+__device__ __forceinline__ uint32_t axis_index(uint32_t a) { return a == 1u ? 0u : (a == 2u ? 1u : 2u); }
 
+// The tree of the collapse: node ids [0, n_leaves) are the sampler's surface leaves (depth D); the ids after them are
+// their ancestors, built level by level bottom-up, so every depth is one contiguous id range.  A cell that is not a node
+// is Empty or Full as a whole (it holds no surface leaf, and neighbouring cells share their corner samples); its sign is
+// the sign at its parent's centre, which every child of that parent shares and a node child knows from its corner mask.
+constexpr float QEF_ERR_EMPTY = -1.0f, QEF_ERR_INVALID = -2.0f;   // octree.rs:895-899
+enum : uint8_t { NODE_LEAF = 1, NODE_BRANCH = 2, NODE_FINAL = 4 };
+
+struct Qef { float ata[6], atb[3], btb, mp[4]; };   // QuadraticErrorSolver; ata = xx xy xz yy yz zz
+struct Hermite { float ipos[12][4], igrad[12][4]; Qef face[6], center; };   // LeafHermiteData (qef_err: node_err)
+
+// The uniform mesh has no nodes beyond the leaves (n_nodes == n_leaves) and leaves the tree's fields (node_*, herm,
+// out_cells) null.
 struct MeshScratch {
     const OctreeLeaf* leaves;
-    uint32_t n_leaves;
-    unsigned long long* hkeys;   // open-addressing table: packed cell coordinates -> leaf index
+    uint32_t n_leaves, depth, n_nodes;
+    unsigned long long* hkeys;   // open-addressing table: tree_key(depth, x, y, z) -> node id
     uint32_t* hvals;
     uint32_t hmask;
     float3* cell_verts;          // [n_leaves][4]
-    uint32_t* corner_vert;       // [n_leaves]: 2 bits per corner = vertex (group) of an inside corner
-    uint32_t* remap;             // [n_leaves][16]: slot (4 cell vertices, 12 edge vertices) -> output vertex, or ~0
-    uint32_t* counts;            // [0] vertices, [1] triangles, [2] triangle cursor, [3] edges without four leaves
+    uint32_t* corner_vert;       // [n_leaves]: 2 bits per corner = vertex (group) of an inside corner; group count << 16
+    unsigned long long* node_key;
+    uint32_t* node_mask;         // corner mask (leaves: CellMask; branches: the signs at their eight corners)
+    uint8_t* node_state;
+    float* node_err;             // LeafHermiteData::qef_err
+    float3* node_vert;           // vertex of a collapsed leaf
+    Hermite* herm;               // [node - n_leaves]
+    uint32_t* remap;             // [n_nodes][16]: slot (4 cell vertices, 12 edge vertices) -> output vertex, or ~0
+    uint32_t* counts;            // [0] vertices [1] triangles [2] triangle cursor [3] open edges [4] nodes [5] final leaves
     float3* out_verts;
     uint32_t cap_verts;
     uint3* out_tris;
     uint32_t cap_tris;
+    fc_mesh_cell* out_cells;
     CancelRef cancel;            // polled at block entry of every kernel (item = block index)
 };
 
-__device__ __forceinline__ unsigned long long cell_key(uint32_t x, uint32_t y, uint32_t z) {
-    return (unsigned long long)x | ((unsigned long long)y << 16) | ((unsigned long long)z << 32);
+__host__ __device__ __forceinline__ unsigned long long tree_key(uint32_t d, uint32_t x, uint32_t y, uint32_t z) {
+    return (unsigned long long)x | ((unsigned long long)y << 16) | ((unsigned long long)z << 32) | ((unsigned long long)d << 48);
 }
+__device__ __forceinline__ uint32_t key_x(unsigned long long k, int a) { return uint32_t(k >> (16 * a)) & 0xffffu; }
+__device__ __forceinline__ uint32_t key_depth(unsigned long long k) { return uint32_t(k >> 48); }
 __device__ __forceinline__ uint32_t hash_key(unsigned long long k) {
     k ^= k >> 33; k *= 0xff51afd7ed558ccdull; k ^= k >> 33; k *= 0xc4ceb9fe1a85ec53ull; k ^= k >> 33;
     return uint32_t(k);
 }
-__global__ void k_mesh_hash(MeshScratch m) {
-    if (cancel_poll(m.cancel, CS_MESH_HASH, blockIdx.x)) return;
-    const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
-    if (i >= m.n_leaves) return;
-    const OctreeLeaf& L = m.leaves[i];
-    const unsigned long long key = cell_key(L.ix, L.iy, L.iz);
-    uint32_t h = hash_key(key) & m.hmask;
-    for (;;) {
-        const unsigned long long old = atomicCAS(&m.hkeys[h], ~0ull, key);
-        if (old == ~0ull || old == key) { m.hvals[h] = i; return; }
-        h = (h + 1u) & m.hmask;
-    }
-}
-__device__ __forceinline__ uint32_t find_leaf(const MeshScratch& m, uint32_t x, uint32_t y, uint32_t z) {
-    const unsigned long long key = cell_key(x, y, z);
+__device__ __forceinline__ uint32_t hash_find(const MeshScratch& m, unsigned long long key) {
     uint32_t h = hash_key(key) & m.hmask;
     for (;;) {
         const unsigned long long k = m.hkeys[h];
         if (k == key) return m.hvals[h];
         if (k == ~0ull) return ~0u;
+        h = (h + 1u) & m.hmask;
+    }
+}
+// returns true when `key` was new; the caller owns hvals[slot] then
+__device__ __forceinline__ bool hash_insert(const MeshScratch& m, unsigned long long key, uint32_t& slot) {
+    uint32_t h = hash_key(key) & m.hmask;
+    for (;;) {
+        const unsigned long long old = atomicCAS(&m.hkeys[h], ~0ull, key);
+        if (old == ~0ull) { slot = h; return true; }
+        if (old == key) return false;
         h = (h + 1u) & m.hmask;
     }
 }
@@ -108,15 +131,70 @@ __device__ inline void jacobi3(float a[3][3], float w[3], float v[3][3]) {
     for (int i = 0; i < 3; ++i) w[i] = a[i][i];
 }
 
-// One thread per leaf: groups of inside corners, one QEF vertex per group
-__global__ void __launch_bounds__(128) k_mesh_vertices(MeshScratch m) {
-    if (cancel_poll(m.cancel, CS_MESH_VERTICES, blockIdx.x)) return;
-    const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
-    if (i >= m.n_leaves) return;
-    const OctreeLeaf& L = m.leaves[i];
-    const uint32_t mask = L.mask;
-    // connected groups of inside corners along cube edges (label = lowest corner of the group)
-    uint32_t label[8];
+__device__ inline void qef_zero(Qef& q) {
+    for (int k = 0; k < 6; ++k) q.ata[k] = 0.0f;
+    for (int k = 0; k < 3; ++k) q.atb[k] = 0.0f;
+    q.btb = 0.0f;
+    for (int k = 0; k < 4; ++k) q.mp[k] = 0.0f;
+}
+__device__ inline void qef_add(Qef& q, const Qef& r) {   // AddAssign (qef.rs:19-26)
+    for (int k = 0; k < 6; ++k) q.ata[k] += r.ata[k];
+    for (int k = 0; k < 3; ++k) q.atb[k] += r.atb[k];
+    q.btb += r.btb;
+    for (int k = 0; k < 4; ++k) q.mp[k] += r.mp[k];
+}
+__device__ inline void qef_add_intersection(Qef& q, const float p[3], const float g[4]) {   // qef.rs:48-59
+    q.mp[0] += p[0]; q.mp[1] += p[1]; q.mp[2] += p[2]; q.mp[3] += 1.0f;
+    const float nl = sqrtf(g[0] * g[0] + g[1] * g[1] + g[2] * g[2]);
+    const float n[3] = {g[0] / nl, g[1] / nl, g[2] / nl};
+    const float d = n[0] * p[0] + n[1] * p[1] + n[2] * p[2];
+    q.ata[0] += n[0] * n[0]; q.ata[1] += n[0] * n[1]; q.ata[2] += n[0] * n[2];
+    q.ata[3] += n[1] * n[1]; q.ata[4] += n[1] * n[2]; q.ata[5] += n[2] * n[2];
+    for (int r = 0; r < 3; ++r) q.atb[r] += n[r] * d;
+    q.btb += d * d;
+}
+// QuadraticErrorSolver::solve (qef.rs:67-118): the vertex, or the mass point when the solve gives NaN
+__device__ inline void qef_vertex(const Qef& q, float pos[3]) {
+    const float ata[3][3] = {{q.ata[0], q.ata[1], q.ata[2]}, {q.ata[1], q.ata[3], q.ata[4]}, {q.ata[2], q.ata[4], q.ata[5]}};
+    const float center[3] = {q.mp[0] / q.mp[3], q.mp[1] / q.mp[3], q.mp[2] / q.mp[3]};
+    float b[3];
+    for (int r = 0; r < 3; ++r) b[r] = q.atb[r] - (ata[r][0] * center[0] + ata[r][1] * center[1] + ata[r][2] * center[2]);
+    float w[3], V[3][3], a2[3][3];
+    for (int r = 0; r < 3; ++r) for (int c2 = 0; c2 < 3; ++c2) a2[r][c2] = ata[r][c2];
+    jacobi3(a2, w, V);
+    // singular values of a symmetric matrix = |eigenvalues|, sorted descending
+    int order[3] = {0, 1, 2};
+    for (int x = 0; x < 2; ++x) for (int y = x + 1; y < 3; ++y)
+        if (fabsf(w[order[y]]) > fabsf(w[order[x]])) { const int tmp = order[x]; order[x] = order[y]; order[y] = tmp; }
+    const float cutoff = fabsf(w[order[0]]) * 1e-3f;
+    int rank = 3;
+    for (int k = 0; k < 3; ++k) if (fabsf(w[order[k]]) < cutoff) { rank = k; break; }
+    const float eps = rank < 3 ? fabsf(w[order[rank]]) : 0.0f;
+    float sol[3] = {0, 0, 0};
+    for (int k = 0; k < 3; ++k) {
+        const int j = order[k];
+        if (!(fabsf(w[j]) > eps)) continue;   // svd.solve: singular values <= eps are dropped
+        const float coef = (V[0][j] * b[0] + V[1][j] * b[1] + V[2][j] * b[2]) / w[j];
+        sol[0] += coef * V[0][j]; sol[1] += coef * V[1][j]; sol[2] += coef * V[2][j];
+    }
+    for (int r = 0; r < 3; ++r) pos[r] = sol[r] + center[r];
+    if (!(pos[0] == pos[0] && pos[1] == pos[1] && pos[2] == pos[2])) for (int r = 0; r < 3; ++r) pos[r] = center[r];
+}
+// The error at the vertex qef_vertex placed: pos^T A^T A pos - 2 pos^T A^T b + b^T b, clamped to >= 1e-6 (qef.rs:111-115)
+__device__ inline float qef_error(const Qef& q, const float pos[3]) {
+    const float ata[3][3] = {{q.ata[0], q.ata[1], q.ata[2]}, {q.ata[1], q.ata[3], q.ata[4]}, {q.ata[2], q.ata[4], q.ata[5]}};
+    float row[3];
+    for (int c2 = 0; c2 < 3; ++c2) row[c2] = pos[0] * ata[0][c2] + pos[1] * ata[1][c2] + pos[2] * ata[2][c2];
+    const float quad = row[0] * pos[0] + row[1] * pos[1] + row[2] * pos[2];
+    const float lin = (2.0f * pos[0]) * q.atb[0] + (2.0f * pos[1]) * q.atb[1] + (2.0f * pos[2]) * q.atb[2];
+    const float err = (quad - lin) + q.btb;
+    return err > 1e-6f ? err : 1e-6f;   // f32::max: a NaN error becomes 1e-6
+}
+
+// Connected groups of a mask's inside corners along cube edges: returns their count and each inside corner's group,
+// numbered in the order of their lowest corners (0 for outside corners)
+__device__ inline uint32_t corner_groups(uint32_t mask, uint32_t group_of[8]) {
+    uint32_t label[8];   // lowest corner of the group
     for (uint32_t c = 0; c < 8; ++c) label[c] = c;
     for (int it = 0; it < 8; ++it) {
         bool changed = false;
@@ -133,76 +211,78 @@ __global__ void __launch_bounds__(128) k_mesh_vertices(MeshScratch m) {
         }
         if (!changed) break;
     }
-    uint32_t n_groups = 0, group_of[8], packed = 0;
+    uint32_t n_groups = 0;
     for (uint32_t c = 0; c < 8; ++c) {
         group_of[c] = 0;
         if (!((mask >> c) & 1u)) continue;
         if (label[c] == c) group_of[c] = n_groups++;
         else group_of[c] = group_of[label[c]];   // label[c] < c: already numbered
-        packed |= (group_of[c] & 3u) << (2u * c);
     }
+    return n_groups;
+}
+
+// Surface leaves enter the table at depth D and, when collapsing, the tree as its first nodes
+__global__ void k_mesh_hash(MeshScratch m) {
+    if (cancel_poll(m.cancel, CS_MESH_HASH, blockIdx.x)) return;
+    const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= m.n_leaves) return;
+    const OctreeLeaf& L = m.leaves[i];
+    const unsigned long long key = tree_key(m.depth, L.ix, L.iy, L.iz);
+    uint32_t slot;
+    if (hash_insert(m, key, slot)) m.hvals[slot] = i;
+    if (!m.node_key) return;
+    m.node_key[i] = key;
+    m.node_mask[i] = L.mask;
+    m.node_state[i] = NODE_LEAF;
+}
+
+// One thread per leaf: groups of inside corners, one QEF vertex per group.  LEAF_ERR (collapse): also the leaf's
+// LeafHermiteData::qef_err (OctreeBuilder::leaf, octree.rs:810-851): the last group's error wins; a NaN gradient marks
+// the group QEF_ERR_INVALID.  A template argument, not a branch: keeping the QEF live through the solve for its error
+// takes registers the uniform mesh need not pay for.
+template <bool LEAF_ERR>
+__global__ void __launch_bounds__(128) k_mesh_vertices(MeshScratch m) {
+    if (cancel_poll(m.cancel, CS_MESH_VERTICES, blockIdx.x)) return;
+    const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= m.n_leaves) return;
+    const OctreeLeaf& L = m.leaves[i];
+    const uint32_t mask = L.mask;
+    uint32_t group_of[8], packed = 0;
+    const uint32_t n_groups = corner_groups(mask, group_of);
+    for (uint32_t c = 0; c < 8; ++c)
+        if ((mask >> c) & 1u) packed |= (group_of[c] & 3u) << (2u * c);
     m.corner_vert[i] = packed | (n_groups << 16);
+    float err = QEF_ERR_EMPTY;
     for (uint32_t g = 0; g < n_groups && g < 4u; ++g) {
-        // QuadraticErrorSolver (qef.rs:44-61)
-        float ata[3][3] = {{0, 0, 0}, {0, 0, 0}, {0, 0, 0}}, atb[3] = {0, 0, 0}, mp[4] = {0, 0, 0, 0};
+        Qef q;
+        qef_zero(q);
         bool forced = false;
-        float3 force_pos = make_float3(0, 0, 0);
+        float pos[3];
         for (uint32_t s = 0; s < 8 && !forced; ++s) {
             if (!((mask >> s) & 1u) || group_of[s] != g) continue;
-            for (uint32_t t = 1; t < 8 && !forced; t <<= 1) {
-                const uint32_t e_end = s ^ t;
-                if ((mask >> e_end) & 1u) continue;   // not a transition
+            for (uint32_t t = 1; t < 8; t <<= 1) {
+                if ((mask >> (s ^ t)) & 1u) continue;   // not a transition
                 const uint32_t u = next_axis(t), v = next_axis(u);
-                const uint32_t ti = t == 1u ? 0u : (t == 2u ? 1u : 2u);
-                const uint32_t e = ti * 4u + ((s & u) ? 1u : 0u) + ((s & v) ? 2u : 0u);
-                const float px = L.pos[e][0], py = L.pos[e][1], pz = L.pos[e][2];
-                const float gx = L.grad[e][0], gy = L.grad[e][1], gz = L.grad[e][2], gw = L.grad[e][3];
-                if (gx != gx || gy != gy || gz != gz || gw != gw) {   // octree.rs:793-801
+                const uint32_t e = axis_index(t) * 4u + ((s & u) ? 1u : 0u) + ((s & v) ? 2u : 0u);
+                const float p[3] = {L.pos[e][0], L.pos[e][1], L.pos[e][2]};
+                const float gr[4] = {L.grad[e][0], L.grad[e][1], L.grad[e][2], L.grad[e][3]};
+                if (gr[0] != gr[0] || gr[1] != gr[1] || gr[2] != gr[2] || gr[3] != gr[3]) {   // octree.rs:793-801
                     forced = true;
-                    force_pos = make_float3(px, py, pz);
+                    for (int k = 0; k < 3; ++k) pos[k] = p[k];
                     break;
                 }
-                mp[0] += px; mp[1] += py; mp[2] += pz; mp[3] += 1.0f;
-                const float nl = sqrtf(gx * gx + gy * gy + gz * gz);
-                const float n[3] = {gx / nl, gy / nl, gz / nl};
-                const float d = n[0] * px + n[1] * py + n[2] * pz;
-                for (int r = 0; r < 3; ++r) {
-                    for (int c2 = 0; c2 < 3; ++c2) ata[r][c2] += n[r] * n[c2];
-                    atb[r] += n[r] * d;
-                }
+                qef_add_intersection(q, p, gr);
             }
         }
-        float3 pos;
         if (forced) {
-            pos = force_pos;
+            err = QEF_ERR_INVALID;
         } else {
-            // QuadraticErrorSolver::solve (qef.rs:67-168)
-            const float center[3] = {mp[0] / mp[3], mp[1] / mp[3], mp[2] / mp[3]};
-            float b[3];
-            for (int r = 0; r < 3; ++r) b[r] = atb[r] - (ata[r][0] * center[0] + ata[r][1] * center[1] + ata[r][2] * center[2]);
-            float w[3], V[3][3], a2[3][3];
-            for (int r = 0; r < 3; ++r) for (int c2 = 0; c2 < 3; ++c2) a2[r][c2] = ata[r][c2];
-            jacobi3(a2, w, V);
-            // singular values of a symmetric matrix = |eigenvalues|, sorted descending
-            int order[3] = {0, 1, 2};
-            for (int x = 0; x < 2; ++x) for (int y = x + 1; y < 3; ++y)
-                if (fabsf(w[order[y]]) > fabsf(w[order[x]])) { const int tmp = order[x]; order[x] = order[y]; order[y] = tmp; }
-            const float cutoff = fabsf(w[order[0]]) * 1e-3f;
-            int rank = 3;
-            for (int k = 0; k < 3; ++k) if (fabsf(w[order[k]]) < cutoff) { rank = k; break; }
-            const float eps = rank < 3 ? fabsf(w[order[rank]]) : 0.0f;
-            float sol[3] = {0, 0, 0};
-            for (int k = 0; k < 3; ++k) {
-                const int j = order[k];
-                if (!(fabsf(w[j]) > eps)) continue;   // svd.solve: singular values <= eps are dropped
-                const float coef = (V[0][j] * b[0] + V[1][j] * b[1] + V[2][j] * b[2]) / w[j];
-                sol[0] += coef * V[0][j]; sol[1] += coef * V[1][j]; sol[2] += coef * V[2][j];
-            }
-            pos = make_float3(sol[0] + center[0], sol[1] + center[1], sol[2] + center[2]);
-            if (!(pos.x == pos.x && pos.y == pos.y && pos.z == pos.z)) pos = make_float3(center[0], center[1], center[2]);
+            qef_vertex(q, pos);
+            if (LEAF_ERR) err = qef_error(q, pos);
         }
-        m.cell_verts[size_t(i) * 4 + g] = pos;
+        m.cell_verts[size_t(i) * 4 + g] = make_float3(pos[0], pos[1], pos[2]);
     }
+    if (LEAF_ERR) m.node_err[i] = err;
 }
 
 // The four leaves around the +T edge at corner 0 of leaf `c` (dc.rs:104-119), or false at the domain boundary
@@ -210,14 +290,14 @@ struct EdgeCells { uint32_t leaf[4]; };
 __device__ __forceinline__ bool edge_cells(const MeshScratch& m, uint32_t ci, uint32_t t, EdgeCells& ec) {
     const OctreeLeaf& C = m.leaves[ci];
     const uint32_t u = next_axis(t), v = next_axis(u);
-    const uint32_t x = C.ix, y = C.iy, z = C.iz;
+    const uint32_t x = C.ix, y = C.iy, z = C.iz, D = m.depth;
     const uint32_t du[3] = {(u & 1u) ? 1u : 0u, (u & 2u) ? 1u : 0u, (u & 4u) ? 1u : 0u};
     const uint32_t dv[3] = {(v & 1u) ? 1u : 0u, (v & 2u) ? 1u : 0u, (v & 4u) ? 1u : 0u};
     if ((du[0] + dv[0]) > x || (du[1] + dv[1]) > y || (du[2] + dv[2]) > z) return false;
-    ec.leaf[2] = ci;                                                                   // c = a + U + V
-    ec.leaf[0] = find_leaf(m, x - du[0] - dv[0], y - du[1] - dv[1], z - du[2] - dv[2]);  // a
-    ec.leaf[1] = find_leaf(m, x - dv[0], y - dv[1], z - dv[2]);                          // b = a + U
-    ec.leaf[3] = find_leaf(m, x - du[0], y - du[1], z - du[2]);                          // d = a + V
+    ec.leaf[2] = ci;                                                                              // c = a + U + V
+    ec.leaf[0] = hash_find(m, tree_key(D, x - du[0] - dv[0], y - du[1] - dv[1], z - du[2] - dv[2]));  // a
+    ec.leaf[1] = hash_find(m, tree_key(D, x - dv[0], y - dv[1], z - dv[2]));                          // b = a + U
+    ec.leaf[3] = hash_find(m, tree_key(D, x - du[0], y - du[1], z - du[2]));                          // d = a + V
     return ec.leaf[0] != ~0u && ec.leaf[1] != ~0u && ec.leaf[3] != ~0u;
 }
 
@@ -267,20 +347,24 @@ __global__ void __launch_bounds__(128) k_mesh_faces(MeshScratch m) {
         if (base + j < m.cap_tris) m.out_tris[base + j] = make_uint3(m.remap[slot[j]], m.remap[slot[(j + winding) & 3u]], iv);
 }
 
-// compaction of the used vertex slots
+// compaction of the used vertex slots (MeshBuilder::vertex: one output vertex per octree vertex)
 __global__ void k_mesh_assign(MeshScratch m) {
     if (cancel_poll(m.cancel, CS_MESH_ASSIGN, blockIdx.x)) return;
     const uint64_t s = uint64_t(blockIdx.x) * blockDim.x + threadIdx.x;
-    if (s >= uint64_t(m.n_leaves) * 16u) return;
+    if (s >= uint64_t(m.n_nodes) * 16u) return;
     if (m.remap[s] != 1u) { m.remap[s] = ~0u; return; }
     const uint32_t id = atomicAdd(&m.counts[0], 1u);
     m.remap[s] = id;
     if (id >= m.cap_verts) return;
-    const uint32_t leaf = uint32_t(s / 16u), k = uint32_t(s % 16u);
-    if (k < 4u) m.out_verts[id] = m.cell_verts[size_t(leaf) * 4 + k];
-    else {
-        const OctreeLeaf& L = m.leaves[leaf];
+    const uint32_t node = uint32_t(s / 16u), k = uint32_t(s % 16u);
+    if (k < 4u) {
+        m.out_verts[id] = node < m.n_leaves ? m.cell_verts[size_t(node) * 4 + k] : m.node_vert[node];
+    } else if (node < m.n_leaves) {
+        const OctreeLeaf& L = m.leaves[node];
         m.out_verts[id] = make_float3(L.pos[k - 4u][0], L.pos[k - 4u][1], L.pos[k - 4u][2]);
+    } else {
+        const Hermite& H = m.herm[node - m.n_leaves];
+        m.out_verts[id] = make_float3(H.ipos[k - 4u][0], H.ipos[k - 4u][1], H.ipos[k - 4u][2]);
     }
 }
 
@@ -318,185 +402,23 @@ __global__ void k_mesh_stl(const float3* verts, const uint3* tris, uint32_t n_tr
 }
 
 // ---- cell collapse and the adaptive dual walk (FC_FLAG_MESH_COLLAPSE) ---------------------------------------------
-// The tree: node ids [0, n_leaves) are the sampler's surface leaves (depth D); the ids after them are their ancestors,
-// built level by level bottom-up, so every depth is one contiguous id range.  A cell that is not a node is Empty or
-// Full as a whole (it holds no surface leaf, and neighbouring cells share their corner samples); its sign is the sign
-// at its parent's centre, which every child of that parent shares and a node child knows from its corner mask.
-constexpr float QEF_ERR_EMPTY = -1.0f, QEF_ERR_INVALID = -2.0f;   // octree.rs:895-899
-enum : uint8_t { NODE_LEAF = 1, NODE_BRANCH = 2, NODE_FINAL = 4 };
-
-struct Qef { float ata[6], atb[3], btb, mp[4]; };   // QuadraticErrorSolver; ata = xx xy xz yy yz zz
-struct Hermite { float ipos[12][4], igrad[12][4]; Qef face[6], center; };   // LeafHermiteData (qef_err: node_err)
-
-struct TreeScratch {
-    const OctreeLeaf* leaves;
-    uint32_t n_leaves, depth;
-    unsigned long long* hkeys;   // (depth, x, y, z) -> node id
-    uint32_t* hvals;
-    uint32_t hmask;
-    unsigned long long* node_key;
-    uint32_t* node_mask;         // corner mask (leaves: CellMask; branches: the signs at their eight corners)
-    uint8_t* node_state;
-    float* node_err;             // LeafHermiteData::qef_err
-    float3* node_vert;           // vertex of a collapsed leaf
-    Hermite* herm;               // [node - n_leaves]
-    const float3* cell_verts;    // k_mesh_vertices' output for the surface leaves
-    const uint32_t* corner_vert;
-    uint32_t n_nodes;
-    uint32_t* remap;             // [n_nodes][16] as MeshScratch::remap
-    uint32_t* counts;            // [0] vertices [1] triangles [2] triangle cursor [3] open edges [4] nodes [5] final leaves
-    float3* out_verts;
-    uint32_t cap_verts;
-    uint3* out_tris;
-    uint32_t cap_tris;
-    fc_mesh_cell* out_cells;
-    CancelRef cancel;            // as MeshScratch::cancel
-};
-
-__host__ __device__ __forceinline__ unsigned long long tree_key(uint32_t d, uint32_t x, uint32_t y, uint32_t z) {
-    return (unsigned long long)x | ((unsigned long long)y << 16) | ((unsigned long long)z << 32) | ((unsigned long long)d << 48);
-}
-__device__ __forceinline__ uint32_t key_x(unsigned long long k, int a) { return uint32_t(k >> (16 * a)) & 0xffffu; }
-__device__ __forceinline__ uint32_t key_depth(unsigned long long k) { return uint32_t(k >> 48); }
-__device__ __forceinline__ uint32_t tree_find(const TreeScratch& m, unsigned long long key) {
-    uint32_t h = hash_key(key) & m.hmask;
-    for (;;) {
-        const unsigned long long k = m.hkeys[h];
-        if (k == key) return m.hvals[h];
-        if (k == ~0ull) return ~0u;
-        h = (h + 1u) & m.hmask;
-    }
-}
-// returns true when `key` was new; the caller owns hvals[slot] then
-__device__ __forceinline__ bool tree_insert(const TreeScratch& m, unsigned long long key, uint32_t& slot) {
-    uint32_t h = hash_key(key) & m.hmask;
-    for (;;) {
-        const unsigned long long old = atomicCAS(&m.hkeys[h], ~0ull, key);
-        if (old == ~0ull) { slot = h; return true; }
-        if (old == key) return false;
-        h = (h + 1u) & m.hmask;
-    }
-}
-
-__device__ inline void qef_zero(Qef& q) {
-    for (int k = 0; k < 6; ++k) q.ata[k] = 0.0f;
-    for (int k = 0; k < 3; ++k) q.atb[k] = 0.0f;
-    q.btb = 0.0f;
-    for (int k = 0; k < 4; ++k) q.mp[k] = 0.0f;
-}
-__device__ inline void qef_add(Qef& q, const Qef& r) {   // AddAssign (qef.rs:19-26)
-    for (int k = 0; k < 6; ++k) q.ata[k] += r.ata[k];
-    for (int k = 0; k < 3; ++k) q.atb[k] += r.atb[k];
-    q.btb += r.btb;
-    for (int k = 0; k < 4; ++k) q.mp[k] += r.mp[k];
-}
-__device__ inline void qef_add_intersection(Qef& q, const float p[3], const float g[4]) {   // qef.rs:48-59
-    q.mp[0] += p[0]; q.mp[1] += p[1]; q.mp[2] += p[2]; q.mp[3] += 1.0f;
-    const float nl = sqrtf(g[0] * g[0] + g[1] * g[1] + g[2] * g[2]);
-    const float n[3] = {g[0] / nl, g[1] / nl, g[2] / nl};
-    const float d = n[0] * p[0] + n[1] * p[1] + n[2] * p[2];
-    q.ata[0] += n[0] * n[0]; q.ata[1] += n[0] * n[1]; q.ata[2] += n[0] * n[2];
-    q.ata[3] += n[1] * n[1]; q.ata[4] += n[1] * n[2]; q.ata[5] += n[2] * n[2];
-    for (int r = 0; r < 3; ++r) q.atb[r] += n[r] * d;
-    q.btb += d * d;
-}
-// QuadraticErrorSolver::solve (qef.rs:67-118): the vertex as k_mesh_vertices places it, and the clamped error
-__device__ inline float qef_solve(const Qef& q, float pos[3]) {
-    const float ata[3][3] = {{q.ata[0], q.ata[1], q.ata[2]}, {q.ata[1], q.ata[3], q.ata[4]}, {q.ata[2], q.ata[4], q.ata[5]}};
-    const float center[3] = {q.mp[0] / q.mp[3], q.mp[1] / q.mp[3], q.mp[2] / q.mp[3]};
-    float b[3];
-    for (int r = 0; r < 3; ++r) b[r] = q.atb[r] - (ata[r][0] * center[0] + ata[r][1] * center[1] + ata[r][2] * center[2]);
-    float w[3], V[3][3], a2[3][3];
-    for (int r = 0; r < 3; ++r) for (int c2 = 0; c2 < 3; ++c2) a2[r][c2] = ata[r][c2];
-    jacobi3(a2, w, V);
-    int order[3] = {0, 1, 2};
-    for (int x = 0; x < 2; ++x) for (int y = x + 1; y < 3; ++y)
-        if (fabsf(w[order[y]]) > fabsf(w[order[x]])) { const int tmp = order[x]; order[x] = order[y]; order[y] = tmp; }
-    const float cutoff = fabsf(w[order[0]]) * 1e-3f;
-    int rank = 3;
-    for (int k = 0; k < 3; ++k) if (fabsf(w[order[k]]) < cutoff) { rank = k; break; }
-    const float eps = rank < 3 ? fabsf(w[order[rank]]) : 0.0f;
-    float sol[3] = {0, 0, 0};
-    for (int k = 0; k < 3; ++k) {
-        const int j = order[k];
-        if (!(fabsf(w[j]) > eps)) continue;
-        const float coef = (V[0][j] * b[0] + V[1][j] * b[1] + V[2][j] * b[2]) / w[j];
-        sol[0] += coef * V[0][j]; sol[1] += coef * V[1][j]; sol[2] += coef * V[2][j];
-    }
-    for (int r = 0; r < 3; ++r) pos[r] = sol[r] + center[r];
-    if (!(pos[0] == pos[0] && pos[1] == pos[1] && pos[2] == pos[2])) for (int r = 0; r < 3; ++r) pos[r] = center[r];
-    // pos^T A^T A pos - 2 pos^T A^T b + b^T b, clamped to >= 1e-6 (qef.rs:111-115)
-    float row[3];
-    for (int c2 = 0; c2 < 3; ++c2) row[c2] = pos[0] * ata[0][c2] + pos[1] * ata[1][c2] + pos[2] * ata[2][c2];
-    const float quad = row[0] * pos[0] + row[1] * pos[1] + row[2] * pos[2];
-    const float lin = (2.0f * pos[0]) * q.atb[0] + (2.0f * pos[1]) * q.atb[1] + (2.0f * pos[2]) * q.atb[2];
-    const float err = (quad - lin) + q.btb;
-    return err > 1e-6f ? err : 1e-6f;   // f32::max: a NaN error becomes 1e-6
-}
-
-// Surface leaves enter the tree at depth D
-__global__ void k_tree_leaves(TreeScratch m) {
-    if (cancel_poll(m.cancel, CS_TREE_LEAVES, blockIdx.x)) return;
-    const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
-    if (i >= m.n_leaves) return;
-    const OctreeLeaf& L = m.leaves[i];
-    const unsigned long long key = tree_key(m.depth, L.ix, L.iy, L.iz);
-    uint32_t slot;
-    if (tree_insert(m, key, slot)) m.hvals[slot] = i;
-    m.node_key[i] = key;
-    m.node_mask[i] = L.mask;
-    m.node_state[i] = NODE_LEAF;
-}
 // The parents of the nodes [lo, hi) (one depth), appended as new nodes
-__global__ void k_tree_parents(TreeScratch m, uint32_t lo, uint32_t hi) {
+__global__ void k_tree_parents(MeshScratch m, uint32_t lo, uint32_t hi) {
     if (cancel_poll(m.cancel, CS_TREE_PARENTS, blockIdx.x)) return;
     const uint32_t i = lo + blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= hi) return;
     const unsigned long long k = m.node_key[i];
     const unsigned long long pk = tree_key(key_depth(k) - 1u, key_x(k, 0) >> 1, key_x(k, 1) >> 1, key_x(k, 2) >> 1);
     uint32_t slot;
-    if (!tree_insert(m, pk, slot)) return;
+    if (!hash_insert(m, pk, slot)) return;
     const uint32_t id = atomicAdd(&m.counts[4], 1u);
     m.hvals[slot] = id;
     m.node_key[id] = pk;
 }
 
-// LeafHermiteData::qef_err of every surface leaf (OctreeBuilder::leaf, octree.rs:810-851): one QEF per vertex group,
-// the last group's error wins; a NaN gradient marks the group QEF_ERR_INVALID
-__global__ void __launch_bounds__(128) k_tree_leaf_err(TreeScratch m) {
-    if (cancel_poll(m.cancel, CS_TREE_LEAF_ERR, blockIdx.x)) return;
-    const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
-    if (i >= m.n_leaves) return;
-    const OctreeLeaf& L = m.leaves[i];
-    const uint32_t mask = L.mask, cv = m.corner_vert[i], n_groups = cv >> 16;
-    float err = QEF_ERR_EMPTY;
-    for (uint32_t g = 0; g < n_groups && g < 4u; ++g) {
-        Qef q;
-        qef_zero(q);
-        bool invalid = false;
-        for (uint32_t s = 0; s < 8 && !invalid; ++s) {
-            if (!((mask >> s) & 1u) || ((cv >> (2u * s)) & 3u) != g) continue;
-            for (uint32_t t = 1; t < 8; t <<= 1) {
-                if ((mask >> (s ^ t)) & 1u) continue;
-                const uint32_t u = next_axis(t), v = next_axis(u);
-                const uint32_t ti = t == 1u ? 0u : (t == 2u ? 1u : 2u);
-                const uint32_t e = ti * 4u + ((s & u) ? 1u : 0u) + ((s & v) ? 2u : 0u);
-                const float p[3] = {L.pos[e][0], L.pos[e][1], L.pos[e][2]};
-                const float gr[4] = {L.grad[e][0], L.grad[e][1], L.grad[e][2], L.grad[e][3]};
-                if (gr[0] != gr[0] || gr[1] != gr[1] || gr[2] != gr[2] || gr[3] != gr[3]) { invalid = true; break; }
-                qef_add_intersection(q, p, gr);
-            }
-        }
-        if (invalid) { err = QEF_ERR_INVALID; continue; }
-        float pos[3];
-        err = qef_solve(q, pos);
-    }
-    m.node_err[i] = err;
-}
-
 // Hermite data of one child, as LeafHermiteData::merge reads it: a surface leaf's intersections, a collapsed leaf's
 // merged record, or the default record of an Empty / Full cell (no intersections, zero QEFs)
-__device__ __forceinline__ bool child_inter(const TreeScratch& m, uint32_t ch, uint32_t e, float p[3], float g[4]) {
+__device__ __forceinline__ bool child_inter(const MeshScratch& m, uint32_t ch, uint32_t e, float p[3], float g[4]) {
     if (ch == ~0u) return false;
     if (ch < m.n_leaves) {
         const OctreeLeaf& L = m.leaves[ch];
@@ -511,18 +433,17 @@ __device__ __forceinline__ bool child_inter(const TreeScratch& m, uint32_t ch, u
     for (int k = 0; k < 4; ++k) g[k] = H.igrad[e][k];
     return true;
 }
-__device__ __forceinline__ void add_child_inter(const TreeScratch& m, uint32_t ch, uint32_t e, Qef& q) {   // From<LeafIntersection>
+__device__ __forceinline__ void add_child_inter(const MeshScratch& m, uint32_t ch, uint32_t e, Qef& q) {   // From<LeafIntersection>
     float p[3], g[4];
     if (child_inter(m, ch, e, p, g)) qef_add_intersection(q, p, g);
 }
-__device__ __forceinline__ void add_child_face(const TreeScratch& m, uint32_t ch, uint32_t f, Qef& q) {
+__device__ __forceinline__ void add_child_face(const MeshScratch& m, uint32_t ch, uint32_t f, Qef& q) {
     if (ch != ~0u && ch >= m.n_leaves) qef_add(q, m.herm[ch - m.n_leaves].face[f]);
 }
-__device__ __forceinline__ uint32_t axis_index(uint32_t a) { return a == 1u ? 0u : (a == 2u ? 1u : 2u); }
 
 // One thread per node of one depth: Octree::check_done / collapsible / try_collapse (octree.rs:252-440) with
 // LeafHermiteData::merge / solve (octree.rs:917-1033)
-__global__ void __launch_bounds__(128) k_tree_collapse(TreeScratch m, uint32_t lo, uint32_t hi) {
+__global__ void __launch_bounds__(128) k_tree_collapse(MeshScratch m, uint32_t lo, uint32_t hi) {
     if (cancel_poll(m.cancel, CS_TREE_COLLAPSE, blockIdx.x)) return;
     const uint32_t id = lo + blockIdx.x * blockDim.x + threadIdx.x;
     if (id >= hi) return;
@@ -530,7 +451,7 @@ __global__ void __launch_bounds__(128) k_tree_collapse(TreeScratch m, uint32_t l
     const uint32_t d = key_depth(key), x = key_x(key, 0), y = key_x(key, 1), z = key_x(key, 2);
     uint32_t ch[8];
     for (uint32_t c = 0; c < 8; ++c)
-        ch[c] = tree_find(m, tree_key(d + 1u, 2u * x + (c & 1u), 2u * y + ((c >> 1) & 1u), 2u * z + ((c >> 2) & 1u)));
+        ch[c] = hash_find(m, tree_key(d + 1u, 2u * x + (c & 1u), 2u * y + ((c >> 1) & 1u), 2u * z + ((c >> 2) & 1u)));
     uint32_t centre = 0;   // sign at this cell's centre: corner 7 ^ c of child c
     for (uint32_t c = 0; c < 8; ++c)
         if (ch[c] != ~0u) { centre = (m.node_mask[ch[c]] >> (7u ^ c)) & 1u; break; }
@@ -570,17 +491,8 @@ __global__ void __launch_bounds__(128) k_tree_collapse(TreeScratch m, uint32_t l
         if (!agree) return;
     }
     if (cmask == 0u || cmask == 0xffu) return;
-    {   // one vertex group (the collapsed cell is manifold)
-        uint32_t label[8];
-        for (uint32_t c = 0; c < 8; ++c) label[c] = c;
-        for (int it = 0; it < 8; ++it)
-            for (uint32_t c = 0; c < 8; ++c)
-                for (uint32_t ax = 1; ax < 8; ax <<= 1) {
-                    const uint32_t g = c ^ ax;
-                    if (((cmask >> c) & 1u) && ((cmask >> g) & 1u)) { const uint32_t lo2 = min(label[c], label[g]); label[c] = label[g] = lo2; }
-                }
-        for (uint32_t c = 0; c < 8; ++c) if (((cmask >> c) & 1u) && label[c] != label[__ffs(cmask) - 1]) return;
-    }
+    uint32_t group_of[8];
+    if (corner_groups(cmask, group_of) != 1u) return;   // the collapsed cell must be manifold: one vertex group
     // merge: any invalid child QEF stops the collapse
     float child_err = INFINITY;
     for (uint32_t c = 0; c < 8; ++c) {
@@ -639,7 +551,8 @@ __global__ void __launch_bounds__(128) k_tree_collapse(TreeScratch m, uint32_t l
         }
     for (int f = 0; f < 6; ++f) qef_add(q, out.face[f]);
     float pos[3];
-    const float err = qef_solve(q, pos);
+    qef_vertex(q, pos);
+    const float err = qef_error(q, pos);
     // CellBounds::contains: closed intervals of the cell's bounds
     const float size = 2.0f / float(1u << d), lo3[3] = {-1.0f + float(x) * size, -1.0f + float(y) * size, -1.0f + float(z) * size};
     bool inside = true;
@@ -651,14 +564,14 @@ __global__ void __launch_bounds__(128) k_tree_collapse(TreeScratch m, uint32_t l
 }
 
 // Final leaves: leaves whose parent stayed a branch (or the root); listed for fc_mesh_read_cells
-__global__ void k_tree_final(TreeScratch m) {
+__global__ void k_tree_final(MeshScratch m) {
     if (cancel_poll(m.cancel, CS_TREE_FINAL, blockIdx.x)) return;
     const uint32_t id = blockIdx.x * blockDim.x + threadIdx.x;
     if (id >= m.n_nodes || !(m.node_state[id] & NODE_LEAF)) return;
     const unsigned long long k = m.node_key[id];
     const uint32_t d = key_depth(k);
     if (d > 0) {
-        const uint32_t p = tree_find(m, tree_key(d - 1u, key_x(k, 0) >> 1, key_x(k, 1) >> 1, key_x(k, 2) >> 1));
+        const uint32_t p = hash_find(m, tree_key(d - 1u, key_x(k, 0) >> 1, key_x(k, 1) >> 1, key_x(k, 2) >> 1));
         if (!(m.node_state[p] & NODE_BRANCH)) return;
     }
     m.node_state[id] = NODE_LEAF | NODE_FINAL;
@@ -674,9 +587,9 @@ __global__ void k_tree_final(TreeScratch m) {
 
 // The final leaf covering cell (d, p) of the domain: 0 = found (id, depth), 1 = smaller leaves own this spot (a branch
 // at depth d), 2 = an Empty / Full cell
-__device__ inline int tree_cover(const TreeScratch& m, uint32_t d, const uint32_t p[3], uint32_t& id, uint32_t& depth) {
+__device__ inline int tree_cover(const MeshScratch& m, uint32_t d, const uint32_t p[3], uint32_t& id, uint32_t& depth) {
     for (uint32_t k = 0; k <= d; ++k) {
-        const uint32_t dk = d - k, n = tree_find(m, tree_key(dk, p[0] >> k, p[1] >> k, p[2] >> k));
+        const uint32_t dk = d - k, n = hash_find(m, tree_key(dk, p[0] >> k, p[1] >> k, p[2] >> k));
         if (n == ~0u) continue;
         const uint8_t st = m.node_state[n];
         if (st & NODE_FINAL) { id = n; depth = dk; return 0; }
@@ -690,7 +603,7 @@ __device__ inline int tree_cover(const TreeScratch& m, uint32_t d, const uint32_
 // as Iterator::max_by_key picks), with the vertex of every shallower leaf being its single one, the intersection
 // vertex from the emitting leaf, and no triangle between two corners that are the same cell.
 template <int PASS>
-__global__ void __launch_bounds__(128) k_tree_faces(TreeScratch m) {
+__global__ void __launch_bounds__(128) k_tree_faces(MeshScratch m) {
     if (cancel_poll(m.cancel, PASS == 0 ? CS_TREE_FACES0 : CS_TREE_FACES1, blockIdx.x)) return;
     const uint32_t gid = blockIdx.x * blockDim.x + threadIdx.x;
     if (gid >= m.n_nodes * 12u) return;
@@ -764,85 +677,94 @@ __global__ void __launch_bounds__(128) k_tree_faces(TreeScratch m) {
         }
 }
 
-// compaction of the used vertex slots (MeshBuilder::vertex: one output vertex per octree vertex)
-__global__ void k_tree_assign(TreeScratch m) {
-    if (cancel_poll(m.cancel, CS_TREE_ASSIGN, blockIdx.x)) return;
-    const uint64_t s = uint64_t(blockIdx.x) * blockDim.x + threadIdx.x;
-    if (s >= uint64_t(m.n_nodes) * 16u) return;
-    if (m.remap[s] != 1u) { m.remap[s] = ~0u; return; }
-    const uint32_t id = atomicAdd(&m.counts[0], 1u);
-    m.remap[s] = id;
-    if (id >= m.cap_verts) return;
-    const uint32_t node = uint32_t(s / 16u), k = uint32_t(s % 16u);
-    if (k < 4u) {
-        m.out_verts[id] = node < m.n_leaves ? m.cell_verts[size_t(node) * 4 + k] : m.node_vert[node];
-    } else if (node < m.n_leaves) {
-        const OctreeLeaf& L = m.leaves[node];
-        m.out_verts[id] = make_float3(L.pos[k - 4u][0], L.pos[k - 4u][1], L.pos[k - 4u][2]);
-    } else {
-        const Hermite& H = m.herm[node - m.n_leaves];
-        m.out_verts[id] = make_float3(H.ipos[k - 4u][0], H.ipos[k - 4u][1], H.ipos[k - 4u][2]);
-    }
-}
-
 }  // namespace fdev
 
 // fc_octree_sample's device half (octree_capi.cu)
 int32_t octree_sample_device(fc_ctx* c, const fc_tape* tape, const fc_octree_cfg* cfg, OctreeLeaf* dout, uint64_t cap,
                              uint32_t* n_out, fc_octree_stats* stats, const CallCancel& cc);
 
-// fc_mesh_build with FC_FLAG_MESH_COLLAPSE, after the sampler (n > 0 surface leaves in c->mesh_leaves; c->mu held)
-static int32_t mesh_build_collapse(fc_ctx* c, uint32_t n, uint32_t depth, const fdev::Mat4* to_model, fc_mesh_info* info,
-                                   const CallCancel& cc) {
+// Consecutive 256-byte-aligned arrays of one device buffer: take() points each at its place
+struct Carve {
+    char* base;
+    size_t used = 0;
+    template <class T> void take(T*& p, size_t bytes) {
+        p = base ? reinterpret_cast<T*>(base + used) : nullptr;
+        used += (bytes + 255) & ~size_t(255);
+    }
+};
+// Grows `buf` to the arrays lay_out(Carve&) takes, then points them into it
+template <class F> static cudaError_t carve(DevBuf& buf, F lay_out) {
+    Carve size{nullptr};
+    lay_out(size);
+    if (cudaError_t e = buf.ensure(size.used)) return e;
+    Carve at{buf.as<char>()};
+    lay_out(at);
+    return cudaSuccess;
+}
+
+// The uniform mesh up to pass 0 of its face kernel (m: the surface leaves)
+static int32_t mesh_enqueue_uniform(fc_ctx* c, fdev::MeshScratch& m) {
     using namespace fdev;
     cudaStream_t s = c->stream;
+    const uint32_t n = m.n_leaves;
+    uint32_t hsize = 1024;
+    while (hsize < 2u * n) hsize <<= 1;
+    const size_t b_keys = size_t(hsize) * 8, b_remap = size_t(n) * 16 * 4;
+    CU(carve(c->mesh_scratch, [&](Carve& cv) {
+        cv.take(m.hkeys, b_keys);
+        cv.take(m.hvals, size_t(hsize) * 4);
+        cv.take(m.cell_verts, size_t(n) * 4 * sizeof(float3));
+        cv.take(m.corner_vert, size_t(n) * 4);
+        cv.take(m.remap, b_remap);
+        cv.take(m.counts, 64);
+    }));
+    m.hmask = hsize - 1;
+    CU(cudaEventRecord(get_event(c, 0), s));
+    CU(cudaMemsetAsync(m.hkeys, 0xff, b_keys, s));
+    CU(cudaMemsetAsync(m.remap, 0, b_remap, s));
+    CU(cudaMemsetAsync(m.counts, 0, 64, s));
+    const unsigned bl = (n + 127) / 128;
+    k_mesh_hash<<<bl, 128, 0, s>>>(m);
+    k_mesh_vertices<false><<<bl, 128, 0, s>>>(m);
+    k_mesh_faces<0><<<(n * 3u + 127) / 128, 128, 0, s>>>(m);
+    return FC_OK;
+}
+
+// The collapsing mesh up to pass 0 of its face kernel: the tree of the surface leaves' ancestors, the collapse one depth
+// at a time bottom-up, and the final leaves
+static int32_t mesh_enqueue_collapse(fc_ctx* c, fdev::MeshScratch& m, const CallCancel& cc) {
+    using namespace fdev;
+    cudaStream_t s = c->stream;
+    const uint32_t n = m.n_leaves, depth = m.depth;
     // nodes: the leaves plus at most min(n, 8^d) ancestors at every depth d < D
     uint64_t cap_nodes = n;
     for (uint32_t d = 0; d < depth; ++d) cap_nodes += std::min<uint64_t>(n, 1ull << (3 * d));
     if (cap_nodes * 16 >= (1ull << 32)) return fail(FC_ERR_INVALID, "mesh too large for cell collapse");
     uint64_t hsize = 1024;
     while (hsize < 2 * cap_nodes) hsize <<= 1;
-    auto al = [](size_t x) { return (x + 255) & ~size_t(255); };
-    const size_t b_keys = hsize * 8, b_vals = hsize * 4, b_nkey = cap_nodes * 8, b_nmask = cap_nodes * 4, b_nstate = cap_nodes,
-                 b_nerr = cap_nodes * 4, b_nvert = cap_nodes * sizeof(float3), b_cv = size_t(n) * 4 * sizeof(float3), b_cn = size_t(n) * 4;
-    CU(c->mesh_tree.ensure(al(b_keys) + al(b_vals) + al(b_nkey) + al(b_nmask) + al(b_nstate) + al(b_nerr) + al(b_nvert) + al(b_cv) +
-                           al(b_cn) + 256));
-    TreeScratch m{};
-    char* q = c->mesh_tree.as<char>();
-    m.hkeys = reinterpret_cast<unsigned long long*>(q); q += al(b_keys);
-    m.hvals = reinterpret_cast<uint32_t*>(q); q += al(b_vals);
-    m.node_key = reinterpret_cast<unsigned long long*>(q); q += al(b_nkey);
-    m.node_mask = reinterpret_cast<uint32_t*>(q); q += al(b_nmask);
-    m.node_state = reinterpret_cast<uint8_t*>(q); q += al(b_nstate);
-    m.node_err = reinterpret_cast<float*>(q); q += al(b_nerr);
-    m.node_vert = reinterpret_cast<float3*>(q); q += al(b_nvert);
-    float3* cell_verts = reinterpret_cast<float3*>(q); q += al(b_cv);
-    uint32_t* corner_vert = reinterpret_cast<uint32_t*>(q); q += al(b_cn);
-    m.counts = reinterpret_cast<uint32_t*>(q);
-    m.leaves = c->mesh_leaves.as<OctreeLeaf>();
-    m.n_leaves = n;
-    m.depth = depth;
+    const size_t b_keys = hsize * 8, b_nstate = cap_nodes;
+    CU(carve(c->mesh_tree, [&](Carve& cv) {
+        cv.take(m.hkeys, b_keys);
+        cv.take(m.hvals, hsize * 4);
+        cv.take(m.node_key, cap_nodes * 8);
+        cv.take(m.node_mask, cap_nodes * 4);
+        cv.take(m.node_state, b_nstate);
+        cv.take(m.node_err, cap_nodes * 4);
+        cv.take(m.node_vert, cap_nodes * sizeof(float3));
+        cv.take(m.cell_verts, size_t(n) * 4 * sizeof(float3));
+        cv.take(m.corner_vert, size_t(n) * 4);
+        cv.take(m.counts, 64);
+    }));
     m.hmask = uint32_t(hsize - 1);
-    m.cell_verts = cell_verts;
-    m.corner_vert = corner_vert;
-    m.cancel = cc.ref;
-    MeshScratch ms{};   // k_mesh_vertices: the surface leaves' vertices, exactly as the uniform mesh places them
-    ms.leaves = m.leaves;
-    ms.n_leaves = n;
-    ms.cell_verts = cell_verts;
-    ms.corner_vert = corner_vert;
-    ms.cancel = cc.ref;
-
-    cudaEvent_t e0 = get_event(c, 0), e1 = get_event(c, 1);
-    CU(cudaEventRecord(e0, s));
+    CU(cudaEventRecord(get_event(c, 0), s));
     CU(cudaMemsetAsync(m.hkeys, 0xff, b_keys, s));
     CU(cudaMemsetAsync(m.node_state, 0, b_nstate, s));
     CU(cudaMemsetAsync(m.counts, 0, 64, s));
     const uint32_t first_branch = n;
     CU(cudaMemcpyAsync(m.counts + 4, &first_branch, 4, cudaMemcpyHostToDevice, s));
     const unsigned bl = (n + 127) / 128;
-    k_mesh_vertices<<<bl, 128, 0, s>>>(ms);
-    k_tree_leaves<<<bl, 128, 0, s>>>(m);
+    k_mesh_hash<<<bl, 128, 0, s>>>(m);
+    k_mesh_vertices<true><<<bl, 128, 0, s>>>(m);
     // ancestors, one depth at a time: range[d] = ids of depth d
     uint32_t range_lo[FC_MAX_OCTREE_DEPTH + 1], range_hi[FC_MAX_OCTREE_DEPTH + 1];
     range_lo[depth] = 0;
@@ -857,37 +779,52 @@ static int32_t mesh_build_collapse(fc_ctx* c, uint32_t n, uint32_t depth, const 
     }
     const uint32_t n_nodes = range_hi[0];
     m.n_nodes = n_nodes;
-    const size_t b_herm = std::max<size_t>(n_nodes - n, 1) * sizeof(Hermite), b_remap = size_t(n_nodes) * 16 * 4;
-    CU(c->mesh_herm.ensure(al(b_herm) + al(b_remap)));
-    m.herm = c->mesh_herm.as<Hermite>();
-    m.remap = reinterpret_cast<uint32_t*>(c->mesh_herm.as<char>() + al(b_herm));
+    const size_t b_remap = size_t(n_nodes) * 16 * 4;
+    CU(carve(c->mesh_herm, [&](Carve& cv) {
+        cv.take(m.herm, std::max<size_t>(n_nodes - n, 1) * sizeof(Hermite));
+        cv.take(m.remap, b_remap);
+    }));
     CU(c->mesh_cells.ensure(size_t(n_nodes) * sizeof(fc_mesh_cell)));
     m.out_cells = c->mesh_cells.as<fc_mesh_cell>();
     CU(cudaMemsetAsync(m.remap, 0, b_remap, s));
-    k_tree_leaf_err<<<bl, 128, 0, s>>>(m);
     for (int d = int(depth) - 1; d >= 0; --d)
         k_tree_collapse<<<(range_hi[d] - range_lo[d] + 127) / 128, 128, 0, s>>>(m, range_lo[d], range_hi[d]);
     k_tree_final<<<(n_nodes + 127) / 128, 128, 0, s>>>(m);
     k_tree_faces<0><<<(n_nodes * 12u + 127) / 128, 128, 0, s>>>(m);
+    return FC_OK;
+}
+
+// Both modes after pass 0 of their face kernel: size the outputs by the triangle count, compact the used vertex slots,
+// emit the triangles, map to model space and publish the counts
+static int32_t mesh_finish(fc_ctx* c, fdev::MeshScratch& m, bool collapse, const fdev::Mat4* to_model, fc_mesh_info* info,
+                           const CallCancel& cc) {
+    using namespace fdev;
+    cudaStream_t s = c->stream;
     CU(cudaGetLastError());
     uint32_t cnt[6];
     if (int32_t wrc = wait_read(c, s, cc, cnt, m.counts, sizeof cnt)) return wrc;
     const uint32_t n_tris = cnt[1];
-    const uint64_t v_cap = std::min<uint64_t>(uint64_t(n_nodes) * 16, uint64_t(n_tris) * 5 + 16);
+    // every used slot becomes a vertex: count them on the device, sized by the worst case (5 slots per triangle fan,
+    // which keeps all 4 triangles in the uniform mesh and may keep only one in the adaptive walk)
+    const uint64_t fan_slots = collapse ? uint64_t(n_tris) * 5 : uint64_t(n_tris) * 5 / 4;
+    const uint64_t v_cap = std::min<uint64_t>(uint64_t(m.n_nodes) * 16, fan_slots + 16);
     CU(c->mesh_verts.ensure(std::max<uint64_t>(v_cap, 1) * sizeof(float3)));
     CU(c->mesh_tris.ensure(std::max<uint64_t>(n_tris, 1) * sizeof(uint3)));
     m.out_verts = c->mesh_verts.as<float3>();
     m.cap_verts = uint32_t(v_cap);
     m.out_tris = c->mesh_tris.as<uint3>();
     m.cap_tris = n_tris;
-    k_tree_assign<<<unsigned((uint64_t(n_nodes) * 16 + 255) / 256), 256, 0, s>>>(m);
-    k_tree_faces<1><<<(n_nodes * 12u + 127) / 128, 128, 0, s>>>(m);
+    k_mesh_assign<<<unsigned((uint64_t(m.n_nodes) * 16 + 255) / 256), 256, 0, s>>>(m);
+    if (collapse) k_tree_faces<1><<<(m.n_nodes * 12u + 127) / 128, 128, 0, s>>>(m);
+    else k_mesh_faces<1><<<(m.n_nodes * 3u + 127) / 128, 128, 0, s>>>(m);
     if (to_model) {
         k_mesh_to_model<<<unsigned((v_cap + 255) / 256), 256, 0, s>>>(reinterpret_cast<char*>(m.out_verts), sizeof(float3), m.counts,
                                                                      m.cap_verts, *to_model);
-        k_mesh_to_model<<<(n_nodes + 255) / 256, 256, 0, s>>>(reinterpret_cast<char*>(m.out_cells) + offsetof(fc_mesh_cell, vertex),
-                                                             sizeof(fc_mesh_cell), m.counts + 5, n_nodes, *to_model);
+        if (collapse)
+            k_mesh_to_model<<<(m.n_nodes + 255) / 256, 256, 0, s>>>(reinterpret_cast<char*>(m.out_cells) + offsetof(fc_mesh_cell, vertex),
+                                                                   sizeof(fc_mesh_cell), m.counts + 5, m.n_nodes, *to_model);
     }
+    cudaEvent_t e1 = get_event(c, 1);
     CU(cudaEventRecord(e1, s));
     CU(cudaGetLastError());
     if (int32_t wrc = wait_read(c, s, cc, cnt, m.counts, sizeof cnt)) return wrc;
@@ -898,7 +835,7 @@ static int32_t mesh_build_collapse(fc_ctx* c, uint32_t n, uint32_t depth, const 
     info->n_vertices = cnt[0];
     info->n_triangles = n_tris;
     info->open_edges = cnt[3];
-    cudaEventElapsedTime(&info->mesh_ms, e0, e1);
+    cudaEventElapsedTime(&info->mesh_ms, get_event(c, 0), e1);
     return FC_OK;
 }
 
@@ -930,14 +867,6 @@ int32_t fc_mesh_build(fc_ctx* c, const fc_tape* tape, const fc_octree_cfg* cfg, 
         return rc;
     }
     std::unique_lock<std::mutex> guard(c->mu);
-    auto cancelled = [&](int32_t rc) {
-        guard.unlock();
-        return rc == FC_ERR_CANCELLED ? no_mesh(rc) : rc;
-    };
-    cudaStream_t s = c->stream;
-    MeshScratch m{};
-    m.leaves = c->mesh_leaves.as<OctreeLeaf>();
-    m.n_leaves = n;
     info->n_leaves = n;
     info->sampler_ms = ost.total_ms;
     c->mesh_n_verts = c->mesh_n_tris = c->mesh_n_cells = 0;
@@ -947,59 +876,16 @@ int32_t fc_mesh_build(fc_ctx* c, const fc_tape* tape, const fc_octree_cfg* cfg, 
     memcpy(view.m, cfg->world_to_model, sizeof view.m);
     bool to_model = false;
     for (int i = 0; i < 16 && cfg->has_transform; ++i) to_model |= view.m[i] != (i % 5 == 0 ? 1.0f : 0.0f);
-    if (cfg->flags & FC_FLAG_MESH_COLLAPSE)
-        return cancelled(mesh_build_collapse(c, n, cfg->depth, to_model ? &view : nullptr, info, cc));
-    uint32_t hsize = 1024;
-    while (hsize < 2u * n) hsize <<= 1;
-    const size_t b_keys = size_t(hsize) * 8, b_vals = size_t(hsize) * 4, b_cv = size_t(n) * 4 * sizeof(float3), b_cn = size_t(n) * 4,
-                 b_remap = size_t(n) * 16 * 4;
-    auto al = [](size_t x) { return (x + 255) & ~size_t(255); };
-    CU(c->mesh_scratch.ensure(al(b_keys) + al(b_vals) + al(b_cv) + al(b_cn) + al(b_remap) + 256));
-    char* q = c->mesh_scratch.as<char>();
-    m.hkeys = reinterpret_cast<unsigned long long*>(q); q += al(b_keys);
-    m.hvals = reinterpret_cast<uint32_t*>(q); q += al(b_vals);
-    m.cell_verts = reinterpret_cast<float3*>(q); q += al(b_cv);
-    m.corner_vert = reinterpret_cast<uint32_t*>(q); q += al(b_cn);
-    m.remap = reinterpret_cast<uint32_t*>(q); q += al(b_remap);
-    m.counts = reinterpret_cast<uint32_t*>(q);
-    m.hmask = hsize - 1;
+    fdev::MeshScratch m{};
+    m.leaves = c->mesh_leaves.as<OctreeLeaf>();
+    m.n_leaves = m.n_nodes = n;
+    m.depth = cfg->depth;
     m.cancel = cc.ref;
-    cudaEvent_t e0 = get_event(c, 0), e1 = get_event(c, 1);
-    CU(cudaEventRecord(e0, s));
-    CU(cudaMemsetAsync(m.hkeys, 0xff, b_keys, s));
-    CU(cudaMemsetAsync(m.remap, 0, b_remap, s));
-    CU(cudaMemsetAsync(m.counts, 0, 64, s));
-    const unsigned bl = (n + 127) / 128;
-    k_mesh_hash<<<bl, 128, 0, s>>>(m);
-    k_mesh_vertices<<<bl, 128, 0, s>>>(m);
-    k_mesh_faces<0><<<(n * 3u + 127) / 128, 128, 0, s>>>(m);
-    uint32_t cnt[4];
-    if (int32_t wrc = wait_read(c, s, cc, cnt, m.counts, sizeof cnt)) return cancelled(wrc);
-    const uint32_t n_tris = cnt[1];
-    // every used slot becomes a vertex: count them on the device, sized by the worst case (5 slots per triangle fan)
-    const uint64_t v_cap = std::min<uint64_t>(uint64_t(n) * 16, uint64_t(n_tris) * 5 / 4 + 16);
-    CU(c->mesh_verts.ensure(std::max<uint64_t>(v_cap, 1) * sizeof(float3)));
-    CU(c->mesh_tris.ensure(std::max<uint64_t>(n_tris, 1) * sizeof(uint3)));
-    m.out_verts = c->mesh_verts.as<float3>();
-    m.cap_verts = uint32_t(v_cap);
-    m.out_tris = c->mesh_tris.as<uint3>();
-    m.cap_tris = n_tris;
-    k_mesh_assign<<<unsigned((uint64_t(n) * 16 + 255) / 256), 256, 0, s>>>(m);
-    k_mesh_faces<1><<<(n * 3u + 127) / 128, 128, 0, s>>>(m);
-    if (to_model)
-        k_mesh_to_model<<<unsigned((v_cap + 255) / 256), 256, 0, s>>>(reinterpret_cast<char*>(m.out_verts), sizeof(float3), m.counts,
-                                                                     m.cap_verts, view);
-    CU(cudaEventRecord(e1, s));
-    CU(cudaGetLastError());
-    if (int32_t wrc = wait_read(c, s, cc, cnt, m.counts, sizeof cnt)) return cancelled(wrc);
-    if (cnt[0] > v_cap) return fail(FC_ERR_CUDA, "mesh vertex buffer overflow");
-    c->mesh_n_verts = cnt[0];
-    c->mesh_n_tris = n_tris;
-    info->n_vertices = cnt[0];
-    info->n_triangles = n_tris;
-    info->open_edges = cnt[3];
-    cudaEventElapsedTime(&info->mesh_ms, e0, e1);
-    return FC_OK;
+    const bool collapse = cfg->flags & FC_FLAG_MESH_COLLAPSE;
+    int32_t rc = collapse ? mesh_enqueue_collapse(c, m, cc) : mesh_enqueue_uniform(c, m);
+    if (rc == FC_OK) rc = mesh_finish(c, m, collapse, to_model ? &view : nullptr, info, cc);
+    guard.unlock();
+    return rc == FC_ERR_CANCELLED ? no_mesh(rc) : rc;
 }
 
 int32_t fc_mesh_read(fc_ctx* c, float* vertices, uint32_t* triangles) {

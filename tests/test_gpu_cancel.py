@@ -234,8 +234,8 @@ SITES = [
     ("k_octree_leaf", "octree", 100, {}),
     ("k_octree_grads", "octree", 100, {}),
 ] + [(k, "mesh", 10, {}) for k in ("k_mesh_hash", "k_mesh_vertices", "k_mesh_faces0", "k_mesh_faces1", "k_mesh_assign")] + \
-    [(k, "mesh_c", 10, {}) for k in ("k_mesh_vertices", "k_tree_leaves", "k_tree_parents", "k_tree_leaf_err", "k_tree_collapse",
-                                     "k_tree_final", "k_tree_faces0", "k_tree_faces1", "k_tree_assign")]
+    [(k, "mesh_c", 10, {}) for k in ("k_mesh_hash", "k_mesh_vertices", "k_tree_parents", "k_tree_collapse", "k_tree_final",
+                                     "k_tree_faces0", "k_tree_faces1", "k_mesh_assign")]
 
 
 @pytest.mark.parametrize("at", ["first", "mid"])

@@ -1,4 +1,4 @@
-"""The mesher's float32 QEF solve (mesh_collapse_oracle.Qef.solve, which the device's qef_solve / k_mesh_vertices
+"""The mesher's float32 QEF solve (mesh_collapse_oracle.Qef.solve, which the device's qef_vertex / qef_error
 match bit for bit) held against QuadraticErrorSolver::solve restated in float64 (tests/qef_f64.py).  CPU only: this is
 what vouches for the device's vertex solve on a machine without a GPU.
 

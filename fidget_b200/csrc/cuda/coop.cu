@@ -490,7 +490,7 @@ k_interval_root_coop(const __grid_constant__ LevelParams p) {
                 o.pad = SCENE ? pl : p.epoch;
                 o.tape = child;
                 p.jobs_out[slot] = o;
-                atomicAdd(&p.ctr->outstanding, 1u);
+                if (p.fused_tail) atomicAdd(&p.ctr->outstanding, 1u);
             } else atomicOr(&p.ctr->error, 2u);
         }
         __syncthreads();

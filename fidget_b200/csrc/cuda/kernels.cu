@@ -31,7 +31,11 @@ namespace fdev {
 // painted later by k_fill_2d).  DIM = 3: voxel::render tiles; an
 // interval-proven-inside tile raises the heightmap to its top + 1
 // (voxel.rs:310-317), heightmap entries are (depth << 32 | leaf job id + 1).
-template <int DIM, bool FUSED_PATH = false, bool FRAMES = false, bool SCENE = false>
+// ONE_EACH (2D, chosen by the launcher): the list cannot be longer than the grid.  It is final when the launch starts,
+// so warp w takes job w and no claim crosses the GPU (prospero 4096^2, level 1: 763 jobs, where four claims out of
+// five found nothing).  Consecutive jobs go to consecutive CTAs, so that the list spreads over every SM.  Longer lists
+// keep the shared cursor, which balances them: with a fixed stride the warps that draw two long jobs finish last.
+template <int DIM, bool FUSED_PATH = false, bool FRAMES = false, bool SCENE = false, bool ONE_EACH = false>
 __global__ void __launch_bounds__(WARPS_PER_BLOCK * 32)
 k_interval_level(const __grid_constant__ LevelParams p) {
     __shared__ uint32_t live_s[WARPS_PER_BLOCK][8][32];
@@ -44,16 +48,22 @@ k_interval_level(const __grid_constant__ LevelParams p) {
     const uint32_t n_roots = SCENE ? scene_root_count(p) : root_count(p, DIM == 3);
     const uint32_t n_jobs = p.root_mode ? (n_roots + 31u) / 32u : min(p.ctr->n_jobs[p.level], p.cap_in);
 
-    for (;;) {
-        uint32_t j = 0;
-        if (lane == 0) {
-            j = atomicAdd(&p.ctr->cursor[p.level], 1u);
-            if (j < n_jobs && cancel_poll(p.cancel, CS_LEVEL0 + p.level, j)) j = ~0u;   // cancelled: claim nothing more
-        }
-        j = __shfl_sync(FULL, j, 0);
-        if (j >= n_jobs) break;
-
+    if constexpr (ONE_EACH) {
+        const uint32_t j = wib * gridDim.x + blockIdx.x;
+        if (j >= n_jobs || __any_sync(FULL, lane == 0 && cancel_poll(p.cancel, CS_LEVEL0 + p.level, j))) return;
         level_job<DIM, FUSED_PATH, FRAMES, SCENE>(p, j, n_roots, slots, cs, live_s[wib], lane, p.epoch);
+    } else {
+        for (;;) {
+            uint32_t j = 0;
+            if (lane == 0) {
+                j = atomicAdd(&p.ctr->cursor[p.level], 1u);
+                if (j < n_jobs && cancel_poll(p.cancel, CS_LEVEL0 + p.level, j)) j = ~0u;   // cancelled: claim nothing more
+            }
+            j = __shfl_sync(FULL, j, 0);
+            if (j >= n_jobs) break;
+
+            level_job<DIM, FUSED_PATH, FRAMES, SCENE>(p, j, n_roots, slots, cs, live_s[wib], lane, p.epoch);
+        }
     }
 }
 
@@ -63,6 +73,8 @@ void launch_interval_level_2d(const LevelParams& p, int blocks, cudaStream_t s) 
     static const bool fused_path = getenv("FIDGET_B200_LEVEL_FUSED_PATH") && atoi(getenv("FIDGET_B200_LEVEL_FUSED_PATH"));
     if (p.frames) k_interval_level<2, false, true><<<blocks, WARPS_PER_BLOCK * 32, 0, s>>>(p);   // a frame batch
     else if (fused_path && !p.root_mode) k_interval_level<2, true><<<blocks, WARPS_PER_BLOCK * 32, 0, s>>>(p);
+    else if (!p.root_mode && p.cap_in <= uint32_t(blocks) * WARPS_PER_BLOCK)
+        k_interval_level<2, false, false, false, true><<<blocks, WARPS_PER_BLOCK * 32, 0, s>>>(p);
     else k_interval_level<2><<<blocks, WARPS_PER_BLOCK * 32, 0, s>>>(p);
 }
 void launch_interval_level_3d(const LevelParams& p, int blocks, cudaStream_t s) {

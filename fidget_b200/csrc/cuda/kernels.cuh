@@ -78,17 +78,19 @@ struct Stats {
     unsigned long long culled[MAX_LEVELS];
 };
 
-// Device-side counters of one render call
+// Device-side counters of one render call.  The words that every warp of a launch bumps (the next level's list
+// length, the fill count, the arena top, a shared cursor) sit in different 128-byte lines, so that their atomics queue
+// at different L2 slices instead of one; the host resets and reads the struct as a whole.
 struct Counters {
-    uint32_t n_jobs[MAX_LEVELS + 1];   // n_jobs[l] = tiles queued FOR level l (parents whose children are evaluated at l)
-    uint32_t n_fills[MAX_LEVELS];      // 2D fill records produced by level l
-    uint32_t cursor[MAX_LEVELS + 2];   // dynamic work cursors (one per kernel)
-    uint32_t error;                    // bit 0: arena exhausted, bit 1: list overflow, bit 2: fused kernel watchdog
+    alignas(128) uint32_t n_jobs[MAX_LEVELS + 1];   // n_jobs[l] = tiles queued FOR level l (parents whose children are evaluated at l)
+    alignas(128) uint32_t n_fills[MAX_LEVELS];      // 2D fill records produced by level l
+    alignas(128) uint32_t cursor[MAX_LEVELS + 2];   // dynamic work cursors (one per kernel)
+    alignas(128) uint32_t error;       // bit 0: arena exhausted, bit 1: list overflow, bit 2: fused kernel watchdog
     uint32_t outstanding;              // fused 2D kernel: interval / pixel jobs queued or running
     uint32_t fill_cursor[MAX_LEVELS];  // fused 2D kernel: fill records painted so far, per level
     uint32_t n_census;                 // exact 3D census: records appended
     uint32_t pad;
-    unsigned long long arena_top;      // bump pointer (clauses)
+    alignas(128) unsigned long long arena_top;      // bump pointer (clauses)
 };
 
 // Cooperative level-0 schedule (built on the host at fc_tape_create): the root
@@ -235,6 +237,7 @@ struct LevelParams {
     const uint32_t* scene_pl;
     uint32_t n_scene_pl;
     uint32_t clamp_at;
+    uint32_t fused_tail;           // the fused 2D tail consumes this level's jobs: count them in Counters::outstanding
 };
 
 #ifdef __CUDACC__

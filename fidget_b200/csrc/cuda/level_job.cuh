@@ -266,8 +266,10 @@ __device__ __forceinline__ void level_job(const LevelParams& p, uint32_t j, uint
         if (mamb) {
             uint32_t base = 0;
             if (lane == 0) {
-                atomicAdd(&p.ctr->outstanding, uint32_t(__popc(mamb)));   // before the jobs become claimable
-                if (FUSED) __threadfence();
+                if (FUSED || p.fused_tail) {   // (only the fused kernel reads `outstanding`; it may consume a root launch's jobs)
+                    atomicAdd(&p.ctr->outstanding, uint32_t(__popc(mamb)));   // before the jobs become claimable
+                    if (FUSED) __threadfence();
+                }
                 base = atomicAdd(&p.ctr->n_jobs[p.level + 1], uint32_t(__popc(mamb)));
             }
             base = __shfl_sync(FULL, base, 0);
@@ -284,7 +286,7 @@ __device__ __forceinline__ void level_job(const LevelParams& p, uint32_t j, uint
                     else { o.pad = SCENE ? pl : epoch; p.jobs_out[slot] = o; }
                 } else {
                     atomicOr(&p.ctr->error, 2u);
-                    atomicSub(&p.ctr->outstanding, 1u);   // never claimable: do not wait for it
+                    if (FUSED || p.fused_tail) atomicSub(&p.ctr->outstanding, 1u);   // never claimable: do not wait for it
                 }
             }
         }

@@ -153,17 +153,16 @@ static int32_t enqueue_tiles_2d(fc_ctx* c, const fc_tape* tape, const fc_render2
         p.cancel = cc.ref;
         p.frames = g.frames;
         p.frame_rows = g.frame_rows;
+        p.fused_tail = fused;
         if (fused) {
             tail.fill_tile[l] = ts[l];
             tail.fills[l] = c->fills[l].as<FillRec>();
             tail.fill_cap[l] = uint32_t(g.level_tiles[l + 1]);
             if (l) { tail.lv[l - 1] = p; continue; }
         }
-        int blocks = g.grid_blocks;
-        if (l == 0) {
-            uint64_t warps = (g.n_roots + 31) / 32;
-            blocks = int(std::min<uint64_t>((warps + WARPS_PER_BLOCK - 1) / WARPS_PER_BLOCK, uint64_t(g.grid_blocks)));
-        }
+        // no more warps than the list can hold jobs (one warp per job; level 0: per 32 root tiles)
+        const uint64_t warps = l ? g.level_tiles[l] : (g.n_roots + 31) / 32;
+        const int blocks = int(std::min<uint64_t>((warps + WARPS_PER_BLOCK - 1) / WARPS_PER_BLOCK, uint64_t(g.grid_blocks)));
         bool coop = false;
         if (l == 0) {
             int ct = COOP_THREADS;
@@ -331,7 +330,10 @@ static int32_t prepare_2d(fc_ctx* c, const fc_tape* tape, const fc_render2d_cfg*
     if (int32_t rc = pick_tile_sizes(cfg->tile_sizes, cfg->n_tile_sizes, DFLT, 3, std::max(cfg->width, cfg->height), g.ts))
         return rc;
     g.roots_x = (cfg->width + g.ts[0] - 1) / g.ts[0];
-    const int bps = env_int("FIDGET_B200_BLOCKS_PER_SM", 6);
+    // 8 CTAs per SM: a list longer than the grid (prospero 4096^2, level 2: 5520 jobs) ends sooner the more warps share
+    // it (0.066 ms at 8, 0.071 at 6, 0.079 at 4 on H100), and a short list no longer pays for the grid's idle warps
+    // (enqueue_tiles_2d caps a level's grid by its list's capacity)
+    const int bps = env_int("FIDGET_B200_BLOCKS_PER_SM", 8);
     g.grid_blocks = c->sm_count * bps;
     g.choice_words = (tape->info.choice_count + 15) / 16 + 1;
     return FC_OK;

@@ -133,6 +133,7 @@ FC_SCENE_MAX_SHAPES = 1024
 FC_SCENE_MAX_DEPTH = 262142
 FC_SCENE_MAX_ROOT_TILE = 1022
 FC_SCENE_MAX_LEAF_JOBS = 67108863
+FC_SCENE2D_NONE = 0xFFFF
 
 # name -> (restype, argtypes); mirrors include/fidget_cuda.h one to one
 _vp, _u32, _i32, _u64, _u8 = C.c_void_p, C.c_uint32, C.c_int32, C.c_uint64, C.c_uint8
@@ -167,6 +168,7 @@ CUDA_API = {
     "fc_render3d": (_i32, [_vp, _vp, _P(FcRender3dCfg), _vp, _P(FcRenderStats)]),
     "fc_render3d_frames": (_i32, [_vp, _vp, _P(FcRender3dCfg), _P(FcFrame3d), _u32, _vp, _P(FcRenderStats)]),
     "fc_render3d_scene": (_i32, [_vp, _P(_vp), _P(FcFrame3d), _u32, _P(FcRender3dCfg), _vp, _vp, _P(FcRenderStats)]),
+    "fc_render2d_scene": (_i32, [_vp, _P(_vp), _P(FcFrame2d), _u32, _P(FcRender2dCfg), _vp, _vp, _vp, _P(FcRenderStats)]),
     "fc_merge_slabs": (_i32, [_vp, _P(_vp), _u32, _u32, _u32, _u32, _vp]),
     "fc_tiles_per_rank": (_u32, [_u32, _u32, _u32, _u32]),
     "fc_tiles_pack": (_i32, [_vp, _vp, _u32, _u32, _u32, _u32, _u32, _u32, _vp]),

@@ -151,6 +151,9 @@ void fc_ctx_destroy(fc_ctx* c) {
     c->scene_pl.release();
     c->scene_backup.release();
     c->scene_index.release();
+    c->scene_cover.release();
+    c->scene_key.release();
+    c->scene_colors.release();
     if (c->pass_pin) cudaFreeHost(c->pass_pin);
     if (c->copy_stream) {
         cudaStreamSynchronize(c->copy_stream);
@@ -217,6 +220,8 @@ static int32_t cancel_site_of(const std::string& name) {
         if (name == "k_interval_level" + std::to_string(i)) return CS_LEVEL0 + i;
     for (int i = 0; i < CS_WAIT - CS_ROOT_COOP; ++i)
         if (name == names[i]) return CS_ROOT_COOP + i;
+    static_assert(CS_SCENE2D_RESOLVE + 1 == CS_COUNT, "one name per poll site");
+    if (name == "k_scene2d_resolve") return CS_SCENE2D_RESOLVE;
     return -1;
 }
 

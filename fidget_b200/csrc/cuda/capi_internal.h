@@ -145,6 +145,8 @@ struct fc_ctx {
     // fc_render3d_scene: each pass's placements grouped by tape, the heightmap and occlusion map as they were before a
     // pass of several placements (restored when it overflows), and the staged index image of a host `index`
     DevBuf scene_pl, scene_backup, scene_index;
+    // fc_render2d_scene: the cover maps (read, write), the pixel key map and the colour table (kernels.cuh, Scene2D)
+    DevBuf scene_cover, scene_key, scene_colors;
     // tile interleave: device list of this rank's XY root tiles (cached on its key), and the
     // tile -> gathered-slot table of fc_tiles_unpack
     DevBuf root_list, tile_slots;
@@ -158,8 +160,9 @@ struct fc_ctx {
     void* stage = nullptr;
     size_t stage_cap = 0;
     cudaEvent_t stage_ev = nullptr;
-    // level-0 launch shape (occupancy query cached) per instantiation: 2D, 2D frame batch, 3D, 3D frame batch, 3D scene
-    struct { size_t smem; int per_sm, threads; } coop_memo[5] = {};
+    // level-0 launch shape (occupancy query cached) per instantiation: 2D, 2D frame batch, 2D scene, 3D, 3D frame batch,
+    // 3D scene
+    struct { size_t smem; int per_sm, threads; } coop_memo[6] = {};
     std::shared_ptr<struct Sched> sched_cache[4];
     unsigned sched_next = 0;
     // cancellation (fc_ctx_set_cancel): the caller's flag; the device word kernels poll, written from pinned memory on

@@ -80,6 +80,15 @@ k_interval_root_coop(const __grid_constant__ LevelParams p) {
         if (SCENE) pl = scene_root(p, tile, T, cx, cy, cz);
         else root_corner(p, tile, T, cx, cy, cz);
         if (DIM != 3) cz = 0u;
+        if constexpr (DIM == 2 && SCENE) {   // a root tile under higher shapes' proven interiors is not evaluated
+            bool open = false;
+            const uint32_t nb = T / p.cull;
+            for (uint32_t q = tid; q < nb * nb; q += NT) {
+                const uint32_t bx = cx / p.cull + q % nb, by = cy / p.cull + q / nb;
+                open |= bx >= p.occl_w || by >= p.occl_h || p.occl[size_t(by) * p.occl_w + bx] <= pl + 1u;
+            }
+            if (!__syncthreads_or(open)) continue;   // (every thread has read s_tile)
+        }
         const FrameView fv = view_of<FRAMES, SCENE>(p, cy, pl);   // frame batch, scene
         const VarBind& vb = *fv.vb;
         itv vx, vy, vz;
@@ -274,8 +283,12 @@ k_interval_root_coop(const __grid_constant__ LevelParams p) {
                     }
                 }
         }
+        if constexpr (DIM == 2 && SCENE) {   // 2D scene: the write cover map instead of a fill record
+            if (fill_in)
+                scene2d_cover(p.occl + size_t(p.occl_w) * p.occl_h, p.occl_w, p.occl_h, p.cull, cx, cy, T, pl, tid, NT);
+        }
         if (tid == 0) {
-            if (DIM == 2 && !amb) {
+            if (DIM == 2 && !SCENE && !amb) {
                 uint32_t slot = atomicAdd(&p.ctr->n_fills[0], 1u);
                 if (slot < p.cap_fills) {
                     FillRec fr;
@@ -516,7 +529,8 @@ static void (*coop_kernel(int dim, int variant))(LevelParams) {
     if (dim == 3)
         return variant == 2 ? k_interval_root_coop<3, false, true>
              : variant == 1 ? k_interval_root_coop<3, true> : k_interval_root_coop<3, false>;
-    return variant ? k_interval_root_coop<2, true> : k_interval_root_coop<2, false>;
+    return variant == 2 ? k_interval_root_coop<2, false, true>
+         : variant == 1 ? k_interval_root_coop<2, true> : k_interval_root_coop<2, false>;
 }
 int coop_occupancy(int dim, int variant, int threads, size_t smem) {
     int n = 0;
@@ -536,6 +550,7 @@ int coop_regs_per_thread(int dim, int variant) {
 // (a frame batch, p.frames != null, takes the instantiation that reads its frames from the table; a scene, p.scene,
 // the one that reads its placements)
 cudaError_t launch_interval_root_coop_2d(const LevelParams& p, int blocks, int threads, cudaStream_t s) {
+    if (p.scene) return launch_coop<2, false, true>(p, blocks, threads, s);
     return p.frames ? launch_coop<2, true>(p, blocks, threads, s) : launch_coop<2, false>(p, blocks, threads, s);
 }
 cudaError_t launch_interval_root_coop_3d(const LevelParams& p, int blocks, int threads, cudaStream_t s) {

@@ -71,7 +71,8 @@ void launch_interval_level_2d(const LevelParams& p, int blocks, cudaStream_t s) 
     // (diagnostic: FIDGET_B200_LEVEL_FUSED_PATH=1 runs the per-level launch with the code path of the fused tail --
     //  plain tape loads, published jobs, line-aligned arena slots -- to tell code-path cost from scheduling cost)
     static const bool fused_path = getenv("FIDGET_B200_LEVEL_FUSED_PATH") && atoi(getenv("FIDGET_B200_LEVEL_FUSED_PATH"));
-    if (p.frames) k_interval_level<2, false, true><<<blocks, WARPS_PER_BLOCK * 32, 0, s>>>(p);   // a frame batch
+    if (p.scene) k_interval_level<2, false, false, true><<<blocks, WARPS_PER_BLOCK * 32, 0, s>>>(p);   // a scene
+    else if (p.frames) k_interval_level<2, false, true><<<blocks, WARPS_PER_BLOCK * 32, 0, s>>>(p);   // a frame batch
     else if (fused_path && !p.root_mode) k_interval_level<2, true><<<blocks, WARPS_PER_BLOCK * 32, 0, s>>>(p);
     else if (!p.root_mode && p.cap_in <= uint32_t(blocks) * WARPS_PER_BLOCK)
         k_interval_level<2, false, false, false, true><<<blocks, WARPS_PER_BLOCK * 32, 0, s>>>(p);
@@ -405,9 +406,11 @@ void launch_tiles_copy(const void* src, void* dst, uint32_t width, uint32_t heig
 }
 
 // ---------------------------------------------------------------------------
-// K2: leaf pixels (2D); FRAMES: a frame batch (kernels.cuh, Frame2D)
-template <bool FRAMES>
-__global__ void __launch_bounds__(128) k_pixels_2d(const __grid_constant__ PixelParams p) {
+// K2: leaf pixels (2D); FRAMES: a frame batch (kernels.cuh, Frame2D).  SCENE: a 2D scene (kernels.cuh, Scene2D): the
+// tile's placement supplies matrix, Z and vars, a tile under higher shapes' proven interiors is skipped, and a pixel
+// found inside raises its key to placement + 1 instead of being written
+template <bool FRAMES, bool SCENE = false, class P = PixelParams>
+__global__ void __launch_bounds__(128) k_pixels_2d(const __grid_constant__ P p) {
     const int lane = threadIdx.x & 31;
     float2 slots[REG_SLOTS];
     const uint32_t n_jobs = min(p.ctr->n_jobs[p.list], 0xffffffffu);
@@ -424,7 +427,11 @@ __global__ void __launch_bounds__(128) k_pixels_2d(const __grid_constant__ Pixel
         const TileJob* job = p.jobs + j;
         const TapeRef tr = job->tape;
         const uint2* tape = tr.ptr;
-        const FrameView fv = frame_of<FRAMES>(p, job->y);   // (uniform over the warp: one tile, one frame)
+        const uint32_t pl = SCENE ? job->pad : 0u;
+        if constexpr (SCENE) {   // (the leaf tile is one block)
+            if (scene2d_hidden(p.cover, p.blocks_x, p.blocks_y, T, job->x, job->y, T, pl)) continue;
+        }
+        const FrameView fv = view_of<FRAMES, SCENE>(p, job->y, pl);   // (uniform over the warp: one tile, one frame)
         const uint32_t cx = job->x, cy = job->y - fv.y0;
         float* const out = p.out + size_t(fv.out_row0) * p.width;
         for (uint32_t base = 0; base < npix; base += 64u) {
@@ -443,8 +450,13 @@ __global__ void __launch_bounds__(128) k_pixels_2d(const __grid_constant__ Pixel
             if (r.x != r.x) r.x = nanf_();
             if (r.y != r.y) r.y = nanf_();
             uint32_t gx0 = cx + i0, gy0 = cy + j0, gx1 = cx + i1, gy1 = cy + j1;
-            if (v0 && gx0 < p.width && gy0 < p.height) out[size_t(gy0) * p.width + gx0] = r.x;
-            if (v1 && gx1 < p.width && gy1 < p.height) out[size_t(gy1) * p.width + gx1] = r.y;
+            if constexpr (SCENE) {   // RawDistancePixel::inside of a distance (a canonical NaN is outside)
+                if (v0 && gx0 < p.width && gy0 < p.height && r.x < 0.0f) atomicMax(&p.key[size_t(gy0) * p.width + gx0], pl + 1u);
+                if (v1 && gx1 < p.width && gy1 < p.height && r.y < 0.0f) atomicMax(&p.key[size_t(gy1) * p.width + gx1], pl + 1u);
+            } else {
+                if (v0 && gx0 < p.width && gy0 < p.height) out[size_t(gy0) * p.width + gx0] = r.x;
+                if (v1 && gx1 < p.width && gy1 < p.height) out[size_t(gy1) * p.width + gx1] = r.y;
+            }
             shaded += (v0 ? 1 : 0) + (v1 ? 1 : 0);
         }
     }
@@ -457,6 +469,38 @@ __global__ void __launch_bounds__(128) k_pixels_2d(const __grid_constant__ Pixel
 void launch_pixels_2d(const PixelParams& p, int blocks, cudaStream_t s) {
     if (p.frames) k_pixels_2d<true><<<blocks, 128, 0, s>>>(p);
     else k_pixels_2d<false><<<blocks, 128, 0, s>>>(p);
+}
+void launch_pixels_2d_scene(const ScenePixelParams& p, int blocks, cudaStream_t s) {
+    k_pixels_2d<false, true, ScenePixelParams><<<blocks, 128, 0, s>>>(p);
+}
+
+// The image of a 2D scene (kernels.cuh, Scene2D): one warp per 32 consecutive pixels of a row, whose ballot is the
+// 1-bit packing, as in k_to_mask
+__global__ void __launch_bounds__(256) k_scene2d_resolve(const __grid_constant__ Scene2DResolveParams p) {
+    const uint32_t words = (p.width + 31u) / 32u, lane = threadIdx.x & 31u;
+    const uint64_t warp = (uint64_t(blockIdx.x) * blockDim.x + threadIdx.x) >> 5;
+    if (warp >= uint64_t(words) * p.height) return;
+    if (cancel_poll(p.cancel, CS_SCENE2D_RESOLVE, uint32_t(warp))) return;   // (uniform over the warp)
+    const uint32_t y = uint32_t(warp / words), x = uint32_t(warp % words) * 32u + lane;
+    const size_t i = size_t(y) * p.width + x;
+    const uint32_t top = x < p.width ? max(p.cover[size_t(y / p.leaf) * p.blocks_x + x / p.leaf], p.key[i]) : 0u;
+    if (x < p.width && p.index) p.index[i] = top ? uint16_t(top - 1u) : uint16_t(0xFFFFu);
+    if (!p.out) return;
+    if (p.fmt == 2u) {
+        const uint32_t m = __ballot_sync(0xffffffffu, top != 0u), stride = (p.width + 7u) / 8u;
+        if (lane < 4u && x - lane + lane * 8u < p.width) p.out[size_t(y) * stride + (x - lane) / 8u + lane] = uint8_t(m >> (8u * lane));
+    } else if (x < p.width) {
+        if (p.fmt == 1u) {
+            p.out[i] = top ? 255 : 0;
+        } else {
+            const uint8_t* c = p.colors + 3u * (top - 1u);
+            reinterpret_cast<uint32_t*>(p.out)[i] = top ? (uint32_t(c[0]) | uint32_t(c[1]) << 8 | uint32_t(c[2]) << 16 | 0xFF000000u) : 0u;
+        }
+    }
+}
+void launch_scene2d_resolve(const Scene2DResolveParams& p, cudaStream_t s) {
+    const uint64_t warps = uint64_t((p.width + 31u) / 32u) * p.height;
+    if (warps) k_scene2d_resolve<<<unsigned((warps * 32 + 255) / 256), 256, 0, s>>>(p);
 }
 
 // ---------------------------------------------------------------------------

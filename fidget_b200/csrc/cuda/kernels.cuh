@@ -24,6 +24,7 @@ enum CancelSite : int32_t {
     CS_MESH_HASH, CS_MESH_VERTICES, CS_MESH_FACES0, CS_MESH_FACES1, CS_MESH_ASSIGN,
     CS_TREE_PARENTS, CS_TREE_COLLAPSE, CS_TREE_FINAL, CS_TREE_FACES0, CS_TREE_FACES1,
     CS_WAIT,                                              // polls inside spin waits: not a claim, never a trigger site
+    CS_SCENE2D_RESOLVE,                                   // (after CS_WAIT: the ids the kernels above compare stay put)
     CS_COUNT
 };
 struct CancelRef {
@@ -219,6 +220,8 @@ struct LevelParams {
     // 3D occlusion map: per 16 x 16 block of pixels, a lower bound of the depth EVERY pixel of the block already has
     // (raised by interval-proven-inside tiles that cover whole blocks).  A parent whose blocks all reach its top + 1
     // cannot show anything: its children are skipped (cull != 0: this level's parents are made of whole blocks).
+    // 2D scene (fc_render2d_scene): occl holds the two cover maps of kernels.cuh (Scene2D), the read map then the write
+    // map, occl_w x occl_h leaf blocks each, and cull is the leaf tile edge (the block edge)
     uint32_t* occl;
     uint32_t occl_w, occl_h;        // blocks per row, block rows (tiles may overhang a ragged image: blocks outside are skipped)
     uint32_t cull;
@@ -310,10 +313,62 @@ __device__ __forceinline__ FrameView frame_of(const P& p, uint32_t y) {
 // the screen grid, so coordinates are not offset
 template <bool FRAMES, bool SCENE, class P>
 __device__ __forceinline__ FrameView view_of(const P& p, uint32_t y, uint32_t pl) {
-    if (SCENE) return FrameView{&p.frames[pl].mat, 0.0f, &p.frames[pl].vb, 0u, 0u};
+    if (SCENE) return FrameView{&p.frames[pl].mat, p.frames[pl].z, &p.frames[pl].vb, 0u, 0u};
     return frame_of<FRAMES>(p, y);
 }
 #endif
+
+// 2D scenes (fc_render2d_scene).  Placement k's jobs carry k in TileJob::pad, as a 3D scene's do.  Two maps replace the
+// per-shape images:
+//  - the cover map, one word per leaf block (leaf tile edge, aligned to the grid): max(k + 1) over the tiles of shape k
+//    proven inside by interval arithmetic that cover the block.  Every tile is a union of whole blocks (each tile size
+//    divides the one before it), so an inside fill is recorded exactly; outside fills record nothing.
+//  - the key map, one word per pixel: max(k + 1) over the shapes whose leaf pixel evaluation found the pixel inside.
+// The topmost shape inside pixel p is max(cover[block(p)], key[p]) - 1.  Both maps only take maxima of proven facts, so
+// the result does not depend on the order of the work.  A tile of shape j whose every block already holds cover > j + 1
+// cannot change that maximum and is not evaluated (culled).  Cull decisions read a copy of the cover map that only
+// changes between launches (the read map; launches write the write map, which is copied over the read map after each
+// launch), so which tiles are evaluated, and the census, do not depend on the launch grid or the timing of the work.
+struct ScenePixelParams : PixelParams {
+    const uint32_t* cover;     // the read cover map
+    uint32_t* key;             // width * height words
+    uint32_t blocks_x, blocks_y;
+};
+#ifdef __CUDACC__
+// true when every leaf block of the T x T tile at (x, y) holds cover > pl + 1 (blocks outside the map count as open)
+__device__ __forceinline__ bool scene2d_hidden(const uint32_t* cover, uint32_t blocks_x, uint32_t blocks_y, uint32_t leaf,
+                                               uint32_t x, uint32_t y, uint32_t T, uint32_t pl) {
+    const uint32_t nb = T / leaf, bx0 = x / leaf, by0 = y / leaf;
+    for (uint32_t q = 0; q < nb * nb; ++q) {
+        const uint32_t bx = bx0 + q % nb, by = by0 + q / nb;
+        if (bx >= blocks_x || by >= blocks_y || cover[size_t(by) * blocks_x + bx] <= pl + 1u) return false;
+    }
+    return true;
+}
+// an interval-proven-inside T x T tile of placement pl at (x, y): its blocks of the write cover map, lanes lane0,
+// lane0 + stride, ...
+__device__ __forceinline__ void scene2d_cover(uint32_t* cover_out, uint32_t blocks_x, uint32_t blocks_y, uint32_t leaf,
+                                              uint32_t x, uint32_t y, uint32_t T, uint32_t pl, uint32_t lane0,
+                                              uint32_t stride) {
+    const uint32_t nb = T / leaf;
+    for (uint32_t q = lane0; q < nb * nb; q += stride) {
+        const uint32_t bx = x / leaf + q % nb, by = y / leaf + q / nb;
+        if (bx < blocks_x && by < blocks_y) atomicMax(cover_out + size_t(by) * blocks_x + bx, pl + 1u);
+    }
+}
+#endif
+// The image of a 2D scene from its maps: index (or null) and `out` (or null) in `fmt` (FC_OUT_MASK_U8 = 1,
+// FC_OUT_BITMAP_1BIT = 2, FC_OUT_RGBA8 = 3 with colors[3 * k .. 3 * k + 2] the RGB of shape k)
+struct Scene2DResolveParams {
+    const uint32_t* cover;     // the final cover map
+    const uint32_t* key;
+    uint32_t width, height, leaf, blocks_x;
+    uint32_t fmt;
+    const uint8_t* colors;
+    uint8_t* out;
+    uint16_t* index;
+    CancelRef cancel;
+};
 
 struct FillParams {
     uint32_t tile, width, height;
@@ -420,13 +475,15 @@ void launch_tiles_copy(const void* src, void* dst, uint32_t width, uint32_t heig
                        uint32_t roots_x, uint32_t roots_y, const uint32_t* slots, uint32_t n_ranks, uint32_t per_rank, int rank,
                        cudaStream_t s);
 void launch_interval_level_2d(const LevelParams& p, int blocks, cudaStream_t s);
-// occupancy of the level-0 kernel instantiation a launch takes (variant 0: one frame, 1: a frame batch, 2: a 3D scene)
+// occupancy of the level-0 kernel instantiation a launch takes (variant 0: one frame, 1: a frame batch, 2: a scene)
 int coop_regs_per_thread(int dim, int variant);
 int coop_occupancy(int dim, int variant, int threads, size_t smem);
 size_t coop_smem_bytes(uint32_t n_ops, uint32_t n_choices, uint32_t n_slots);
 cudaError_t launch_interval_root_coop_2d(const LevelParams& p, int blocks, int threads, cudaStream_t s);
 cudaError_t launch_interval_root_coop_3d(const LevelParams& p, int blocks, int threads, cudaStream_t s);
 void launch_pixels_2d(const PixelParams& p, int blocks, cudaStream_t s);
+void launch_pixels_2d_scene(const ScenePixelParams& p, int blocks, cudaStream_t s);
+void launch_scene2d_resolve(const Scene2DResolveParams& p, cudaStream_t s);
 // Fused 2D tail (tail2d.cu): every level after the root level, the leaf pixels and the fills in ONE
 // persistent launch that drains a dependency-ordered queue
 constexpr int TAIL_MAX_LEVELS = 4;

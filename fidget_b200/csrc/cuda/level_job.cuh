@@ -86,7 +86,7 @@ __device__ __forceinline__ void level_job(const LevelParams& p, uint32_t j, uint
 
     for (uint32_t chunk = 0; chunk * 32u < nchild; ++chunk) {
         const uint32_t c = chunk * 32u + lane;
-        const bool valid = c < nchild;
+        bool valid = c < nchild;
         uint32_t cx, cy, cz = 0, pl = ppl;
         if (p.root_mode) {
             if (SCENE) pl = scene_root(p, j * 32u + (valid ? c : 0u), T, cx, cy, cz);
@@ -96,6 +96,10 @@ __device__ __forceinline__ void level_job(const LevelParams& p, uint32_t j, uint
             cx = px + (cc % p.n_axis) * T;
             cy = py + ((cc / p.n_axis) % p.n_axis) * T;
             if (DIM == 3) cz = pz + (cc / (p.n_axis * p.n_axis)) * T;
+        }
+        if constexpr (DIM == 2 && SCENE) {   // a tile under higher shapes' proven interiors is not evaluated (Scene2D)
+            valid = valid && !scene2d_hidden(p.occl, p.occl_w, p.occl_h, p.cull, cx, cy, T, pl);
+            if (!__any_sync(FULL, valid)) continue;
         }
         // Region in screen coordinates -> model space (pixel.rs:325-342, voxel.rs:291-306); in a frame batch a
         // tile's coordinates are relative to its frame (per lane at level 0, whose 32 roots may span frames)
@@ -174,22 +178,34 @@ __device__ __forceinline__ void level_job(const LevelParams& p, uint32_t j, uint
                 }
             }
         } else {
-            uint32_t m = __ballot_sync(FULL, fill_in || fill_out);
-            if (m) {
-                uint32_t base = 0;
-                if (lane == 0) base = atomicAdd(&p.ctr->n_fills[p.level], uint32_t(__popc(m)));
-                base = __shfl_sync(FULL, base, 0);
-                if (fill_in || fill_out) {
-                    uint32_t slot = base + __popc(m & lanemask_lt());
-                    if (slot < p.cap_fills) {
-                        FillRec fr;
-                        fr.x = cx;
-                        fr.y = cy;
-                        fr.value = 0x7FC00000u | (uint32_t(p.level & 0xff) << 1) | (fill_in ? 1u : 0u) | (0xF6u << 9);
-                        fr.ready = epoch;
-                        store_fill(p.fills + slot, fr);   // one 16-byte store: the ready mark travels with the record
-                    } else {
-                        atomicOr(&p.ctr->error, 2u);
+            if constexpr (SCENE) {
+                // 2D scene: an inside tile raises its blocks of the write cover map; nothing is painted
+                uint32_t m = __ballot_sync(FULL, fill_in);
+                uint32_t* const cover_out = p.occl + size_t(p.occl_w) * p.occl_h;
+                while (m) {
+                    const int src = __ffs(m) - 1;
+                    m &= m - 1;
+                    scene2d_cover(cover_out, p.occl_w, p.occl_h, p.cull, __shfl_sync(FULL, cx, src),
+                                  __shfl_sync(FULL, cy, src), T, __shfl_sync(FULL, pl, src), lane, 32u);
+                }
+            } else {
+                uint32_t m = __ballot_sync(FULL, fill_in || fill_out);
+                if (m) {
+                    uint32_t base = 0;
+                    if (lane == 0) base = atomicAdd(&p.ctr->n_fills[p.level], uint32_t(__popc(m)));
+                    base = __shfl_sync(FULL, base, 0);
+                    if (fill_in || fill_out) {
+                        uint32_t slot = base + __popc(m & lanemask_lt());
+                        if (slot < p.cap_fills) {
+                            FillRec fr;
+                            fr.x = cx;
+                            fr.y = cy;
+                            fr.value = 0x7FC00000u | (uint32_t(p.level & 0xff) << 1) | (fill_in ? 1u : 0u) | (0xF6u << 9);
+                            fr.ready = epoch;
+                            store_fill(p.fills + slot, fr);   // one 16-byte store: the ready mark travels with the record
+                        } else {
+                            atomicOr(&p.ctr->error, 2u);
+                        }
                     }
                 }
             }

@@ -1,5 +1,6 @@
 // The fused tile renderers: fc_render2d (pixel::render), fc_render3d (voxel::render), their frame batches
-// (fc_render2d_frames, fc_render3d_frames), 3D scenes of several shapes (fc_render3d_scene), fc_merge_slabs.
+// (fc_render2d_frames, fc_render3d_frames), scenes of several shapes (fc_render2d_scene, fc_render3d_scene),
+// fc_merge_slabs.
 #include <cstddef>
 #include <functional>
 
@@ -87,6 +88,24 @@ static int32_t size_lists_2d(const std::vector<uint32_t>& ts, uint64_t n_roots, 
     return FC_OK;
 }
 
+// The placements of a scene pass grouped by tape for level 0, which runs once per distinct tape with that tape's
+// schedule: each group's placements are appended to `pl` (first: the group's offset there), groups in order of first
+// appearance along `order`
+struct SceneGroup { const fc_tape* tape; uint32_t first, n; };
+static void group_by_tape(const fc_tape* const* tapes, const std::vector<uint32_t>& order, std::vector<uint32_t>& pl,
+                          std::vector<SceneGroup>& groups) {
+    for (size_t i = 0; i < order.size(); ++i) {
+        const fc_tape* t = tapes[order[i]];
+        bool seen = false;
+        for (const SceneGroup& gr : groups) seen |= gr.tape == t;
+        if (seen) continue;
+        const uint32_t first = uint32_t(pl.size());
+        for (size_t q = i; q < order.size(); ++q)
+            if (tapes[order[q]] == t) pl.push_back(order[q]);
+        groups.push_back(SceneGroup{t, first, uint32_t(pl.size()) - first});
+    }
+}
+
 // The tile pipeline of fc_render2d (pixel::render), enqueued on `s`: the interval levels, the fills of every level
 // (on the auxiliary stream, joined back into `s`) and the leaf pixels, into the distance image `dimg`.  The grid is
 // roots_x x roots_y root tiles from root row row0 (or the listed ones, d_roots); with a frame table it stacks the
@@ -103,6 +122,15 @@ struct Tiles2D {
     int grid_blocks = 0;
     const Frame2D* frames = nullptr;
     uint32_t frame_rows = 0xffffffffu;
+    // scene (fc_render2d_scene): `frames` is the placement table and roots_x x roots_y the grid of one placement.  Level
+    // 0 runs once per group (placements listed at d_pl), every later launch is shared.  No image: inside tiles go to the
+    // cover maps (read map, then write map, blocks_x x blocks_y each), inside leaf pixels to the key map (Scene2D)
+    bool scene = false;
+    std::vector<SceneGroup> groups;
+    const uint32_t* d_pl = nullptr;
+    uint32_t* cover = nullptr;
+    uint32_t* key = nullptr;
+    uint32_t blocks_x = 0, blocks_y = 0;
 };
 static int32_t enqueue_tiles_2d(fc_ctx* c, const fc_tape* tape, const fc_render2d_cfg* cfg, const Tiles2D& g,
                                 const VarBind& vb, float* dimg, bool want_stats, bool timing, const CallCancel& cc,
@@ -154,28 +182,58 @@ static int32_t enqueue_tiles_2d(fc_ctx* c, const fc_tape* tape, const fc_render2
         p.frames = g.frames;
         p.frame_rows = g.frame_rows;
         p.fused_tail = fused;
+        if (g.scene) {
+            p.scene = 1;
+            p.occl = g.cover;
+            p.occl_w = g.blocks_x;
+            p.occl_h = g.blocks_y;
+            p.cull = ts[L - 1];
+        }
         if (fused) {
             tail.fill_tile[l] = ts[l];
             tail.fills[l] = c->fills[l].as<FillRec>();
             tail.fill_cap[l] = uint32_t(g.level_tiles[l + 1]);
             if (l) { tail.lv[l - 1] = p; continue; }
         }
-        // no more warps than the list can hold jobs (one warp per job; level 0: per 32 root tiles)
-        const uint64_t warps = l ? g.level_tiles[l] : (g.n_roots + 31) / 32;
-        const int blocks = int(std::min<uint64_t>((warps + WARPS_PER_BLOCK - 1) / WARPS_PER_BLOCK, uint64_t(g.grid_blocks)));
-        bool coop = false;
-        if (l == 0) {
-            int ct = COOP_THREADS;
-            int cb = coop_blocks(c, tape, g.n_roots, p, 2, ct);
-            if (cb > 0) {
-                CU(launch_interval_root_coop_2d(p, cb, ct, s));
-                coop = true;
+        auto launch = [&](const fc_tape* t, uint64_t n_roots) -> int32_t {
+            // no more warps than the list can hold jobs (one warp per job; level 0: per 32 root tiles)
+            const uint64_t warps = l ? g.level_tiles[l] : (n_roots + 31) / 32;
+            const int blocks = int(std::min<uint64_t>((warps + WARPS_PER_BLOCK - 1) / WARPS_PER_BLOCK, uint64_t(g.grid_blocks)));
+            bool coop = false;
+            if (l == 0) {
+                int ct = COOP_THREADS;
+                int cb = coop_blocks(c, t, n_roots, p, 2, ct);
+                if (cb > 0) {
+                    CU(launch_interval_root_coop_2d(p, cb, ct, s));
+                    coop = true;
+                }
             }
+            if (!coop) launch_interval_level_2d(p, std::max(blocks, 1), s);
+            ++launches;
+            // a scene's later launches cull against what this one proved inside: its write map becomes the read map
+            if (g.scene)
+                CU(cudaMemcpyAsync(g.cover, g.cover + size_t(g.blocks_x) * g.blocks_y, size_t(g.blocks_x) * g.blocks_y * 4,
+                                   cudaMemcpyDeviceToDevice, s));
+            return FC_OK;
+        };
+        if (l == 0 && g.scene) {
+            // level 0 of a scene: one launch per distinct tape over the root tiles of its placements, as in a 3D scene
+            for (size_t k = 0; k < g.groups.size(); ++k) {
+                const SceneGroup& gr = g.groups[k];
+                p.root_tape.ptr = gr.tape->dev;
+                p.root_tape.n_ops = gr.tape->info.n_ops;
+                p.root_tape.ref_len = gr.tape->info.ref_len;
+                p.root_tape.n_choices = gr.tape->info.choice_count;
+                p.scene_pl = g.d_pl + gr.first;
+                p.n_scene_pl = gr.n;
+                if (k) CU(cudaMemsetAsync(&c->counters.as<Counters>()->cursor[0], 0, sizeof(uint32_t), s));
+                if (int32_t lrc = launch(gr.tape, uint64_t(g.roots_x) * g.roots_y * gr.n)) return lrc;
+            }
+        } else if (int32_t lrc = launch(tape, g.n_roots)) {
+            return lrc;
         }
-        if (!coop) launch_interval_level_2d(p, std::max(blocks, 1), s);
-        ++launches;
         if (timing) CU(cudaEventRecord(get_event(c, ev++), s));
-        if (!fused) {
+        if (!fused && !g.scene) {
             // the tiles this level proved inside/outside are painted on a second stream while the
             // next (latency-bound) levels run: fills and leaf pixels never touch the same pixel
             FillParams f{};
@@ -241,12 +299,20 @@ static int32_t enqueue_tiles_2d(fc_ctx* c, const fc_tape* tape, const fc_render2
                 CU(cudaEventRecord(c->ev_join, c->aux_stream));
                 CU(cudaStreamWaitEvent(s, c->ev_join, 0));
             }
+        } else if (g.scene) {
+            ScenePixelParams sq;
+            static_cast<PixelParams&>(sq) = q;
+            sq.cover = g.cover;
+            sq.key = g.key;
+            sq.blocks_x = g.blocks_x;
+            sq.blocks_y = g.blocks_y;
+            launch_pixels_2d_scene(sq, c->sm_count * env_int("FIDGET_B200_PIXEL_BLOCKS_PER_SM", 8), s);
         } else {
             launch_pixels_2d(q, c->sm_count * env_int("FIDGET_B200_PIXEL_BLOCKS_PER_SM", 8), s);
         }
         ++launches;
     }
-    if (!serial_fill && !fused) {
+    if (!serial_fill && !fused && !g.scene) {
         CU(cudaEventRecord(c->ev_join, c->aux_stream));
         CU(cudaStreamWaitEvent(s, c->ev_join, 0));
     }
@@ -347,7 +413,7 @@ static int32_t ensure_scratch_2d(fc_ctx* c, const Tiles2D& g) {
     CU(c->stats.ensure(sizeof(Stats)));
     for (int l = 1; l <= L; ++l) {
         CU(c->jobs[l].ensure(g.level_tiles[l] * sizeof(TileJob)));
-        CU(c->fills[l - 1].ensure(g.level_tiles[l] * sizeof(FillRec)));
+        if (!g.scene) CU(c->fills[l - 1].ensure(g.level_tiles[l] * sizeof(FillRec)));   // (a scene writes no fills)
     }
     return FC_OK;
 }
@@ -420,9 +486,8 @@ struct Tiles3D {
     uint32_t frame_rows = 0xffffffffu;
     // scene (fc_render3d_scene): `frames` is the placement table; a pass renders placements pl0 .. pl1 - 1, listed at
     // d_pl grouped by tape (level 0 runs once per group, with the group's tape); clamp_at as in scene_rank
-    struct Group { const fc_tape* tape; uint32_t first, n; };
     bool scene = false;
-    std::vector<Group> groups;
+    std::vector<SceneGroup> groups;
     const uint32_t* d_pl = nullptr;
     uint32_t pl0 = 0, pl1 = 0, clamp_at = 0xffffffffu;
 };
@@ -582,7 +647,7 @@ static int32_t enqueue_tiles_3d(fc_ctx* c, const fc_tape* tape, const fc_render3
             // tape's schedule; their children go to one shared level-1 list (the claim cursor restarts per launch)
             const uint64_t per = uint64_t(g.roots_x) * g.roots_y * g.roots_z;
             for (size_t k = 0; k < g.groups.size(); ++k) {
-                const Tiles3D::Group& gr = g.groups[k];
+                const SceneGroup& gr = g.groups[k];
                 p.root_tape.ptr = gr.tape->dev;
                 p.root_tape.n_ops = gr.tape->info.n_ops;
                 p.root_tape.ref_len = gr.tape->info.ref_len;
@@ -1058,6 +1123,181 @@ int32_t fc_render2d_frames(fc_ctx* c, const fc_tape* tape, const fc_render2d_cfg
     return rc;
 }
 
+// A 2D scene (kernels.cuh, Scene2D): every placement's tiles go through the tile pipeline of fc_render2d_frames, which
+// records inside tiles in the cover map and inside leaf pixels in the key map instead of painting images.  Passes run
+// from the top of the draw list down, so that the shapes of a pass are culled against every shape above them; one
+// resolve launch then writes the index and the image.
+int32_t fc_render2d_scene(fc_ctx* c, const fc_tape* const* tapes, const fc_frame2d* placements, uint32_t n_shapes,
+                          const fc_render2d_cfg* cfg, const uint8_t* colors, void* out, uint16_t* index,
+                          fc_render_stats* stats) {
+    static_assert(FC_OUT_MASK_U8 == 1 && FC_OUT_BITMAP_1BIT == 2 && FC_OUT_RGBA8 == 3, "Scene2DResolveParams::fmt");
+    static_assert(FC_SCENE_MAX_SHAPES < FC_SCENE2D_NONE, "a shape's index is never FC_SCENE2D_NONE");
+    if (!c || !cfg || (!out && !index) || (n_shapes && (!tapes || !placements))) return fail(FC_ERR_INVALID, "null argument");
+    if (n_shapes > FC_SCENE_MAX_SHAPES) return fail(FC_ERR_UNSUPPORTED, "more than FC_SCENE_MAX_SHAPES shapes");
+    if (cfg->flags & FC_FLAG_FUSED_TAIL) return fail(FC_ERR_UNSUPPORTED, "FC_FLAG_FUSED_TAIL is not supported by scenes");
+    if (cfg->root_row_begin || cfg->root_row_end) return fail(FC_ERR_UNSUPPORTED, "root row bands are not supported by scenes");
+    if (cfg->root_stride > 1) return fail(FC_ERR_UNSUPPORTED, "the tile interleave is not supported by scenes");
+    const uint32_t fmt = cfg->out_format;
+    if (fmt > FC_OUT_RGBA8) return fail(FC_ERR_INVALID, "unknown out_format");
+    if (fmt == FC_OUT_F32) return fail(FC_ERR_UNSUPPORTED, "a 2D scene keeps no distances: FC_OUT_F32 is not supported");
+    // every placement's tape and ShapeVars binding, before anything is allocated or launched
+    std::vector<Frame2D> table(n_shapes);
+    for (uint32_t k = 0; k < n_shapes; ++k) {
+        if (!tapes[k]) return fail(FC_ERR_INVALID, "null tape in the scene");
+        if (int32_t vrc = check_2d(tapes[k], cfg)) return vrc;
+        if (int32_t brc = bind_frame(tapes[k], placements[k], placements[k].z, table[k])) return brc;
+    }
+    Tiles2D g;
+    if (n_shapes)
+        if (int32_t rc = prepare_2d(c, tapes[0], cfg, g)) return rc;
+    CallCancel cc;
+    if (int32_t crc = begin_call(c, cc)) return crc;
+    if (stats) memset(stats, 0, sizeof *stats);
+    if (n_shapes == 0) return FC_OK;
+    std::lock_guard<std::mutex> guard(c->mu);
+    CU(cudaSetDevice(c->device));
+    const int L = int(g.ts.size());
+    const uint32_t T0 = g.ts[0], leaf = g.ts[L - 1];
+    const uint32_t W = cfg->width, H = cfg->height;
+    g.roots_y = (H + T0 - 1) / T0;
+    for (uint32_t k = 0; k < n_shapes; ++k)   // choice scratch for the largest choice_count
+        g.choice_words = std::max(g.choice_words, (tapes[k]->info.choice_count + 15) / 16 + 1);
+    g.scene = true;
+    g.blocks_x = (W + leaf - 1) / leaf;
+    g.blocks_y = (H + leaf - 1) / leaf;
+    const bool timing = (cfg->flags & FC_FLAG_TIMING) != 0;
+    const bool async = (cfg->flags & FC_FLAG_ASYNC) != 0;
+    const bool want_stats = stats != nullptr;
+    const bool host_out = out && !is_device_ptr(out), host_index = index && !is_device_ptr(index);
+    const size_t npix = size_t(W) * H, n_blocks = size_t(g.blocks_x) * g.blocks_y, img_fmt = format_bytes(fmt, W, H);
+    cudaStream_t s = c->stream;
+
+    // ---- shapes per pass: their worst-case job lists within FC_FRAMES_PASS_BYTES (the maps are the call's) ----
+    const uint64_t shape_roots = uint64_t(g.roots_x) * g.roots_y;
+    std::vector<uint64_t> shape_tiles;
+    if (int32_t src = size_lists_2d(g.ts, shape_roots, shape_tiles)) return src;
+    uint64_t per_shape = 0;
+    for (int l = 1; l <= L; ++l) per_shape += shape_tiles[l] * sizeof(TileJob);
+    uint32_t per_pass = uint32_t(std::min<uint64_t>(n_shapes, std::max<uint64_t>(1, FC_FRAMES_PASS_BYTES / per_shape)));
+    if (const int forced = env_int("FIDGET_B200_FRAMES_PER_PASS", 0); forced > 0) per_pass = std::min<uint32_t>(n_shapes, forced);
+    const uint32_t n_passes = (n_shapes + per_pass - 1) / per_pass;
+    auto pass_range = [&](uint32_t k, uint32_t& lo, uint32_t& hi) {   // pass k: shapes [lo, hi), the top pass first
+        hi = n_shapes - k * per_pass;
+        lo = hi - std::min(hi, per_pass);
+    };
+    // each pass's level-0 groups, the top shapes' tapes first
+    std::vector<uint32_t> pl_host;
+    std::vector<std::vector<SceneGroup>> groups(n_passes);
+    for (uint32_t k = 0; k < n_passes; ++k) {
+        uint32_t lo, hi;
+        pass_range(k, lo, hi);
+        std::vector<uint32_t> order;
+        for (uint32_t q = hi; q > lo; --q) order.push_back(q - 1);
+        group_by_tape(tapes, order, pl_host, groups[k]);
+    }
+
+    g.n_roots = shape_roots * per_pass;
+    if (int32_t src = size_lists_2d(g.ts, g.n_roots, g.level_tiles)) return src;
+    if (int32_t erc = ensure_scratch_2d(c, g)) return erc;
+    CU(c->frame_table.ensure(size_t(n_shapes) * sizeof(Frame2D)));
+    CU(c->frame_tops.ensure(size_t(n_passes) * sizeof(unsigned long long)));
+    CU(c->scene_pl.ensure(size_t(n_shapes) * 4));
+    CU(c->scene_cover.ensure(2 * n_blocks * 4));
+    CU(c->scene_key.ensure(npix * 4));
+    CU(c->scene_colors.ensure(size_t(n_shapes) * 3));
+    uint8_t* dout = static_cast<uint8_t*>(out);
+    if (host_out) {
+        CU(c->fx_out.ensure(img_fmt));
+        dout = c->fx_out.as<uint8_t>();
+    }
+    uint16_t* dindex = index;
+    if (host_index) {
+        CU(c->scene_index.ensure(npix * 2));
+        dindex = c->scene_index.as<uint16_t>();
+    }
+    const std::vector<uint8_t> white(colors ? 0 : size_t(n_shapes) * 3, 255);   // draw(): every shape white
+    CU(cudaMemcpyAsync(c->frame_table.p, table.data(), table.size() * sizeof(Frame2D), cudaMemcpyHostToDevice, s));
+    CU(cudaMemcpyAsync(c->scene_pl.p, pl_host.data(), pl_host.size() * 4, cudaMemcpyHostToDevice, s));
+    if (out && fmt == FC_OUT_RGBA8)
+        CU(cudaMemcpyAsync(c->scene_colors.p, colors ? colors : white.data(), size_t(n_shapes) * 3, cudaMemcpyHostToDevice, s));
+    CU(cudaMemsetAsync(c->counters.p, 0, sizeof(Counters), s));
+    if (want_stats) CU(cudaMemsetAsync(c->stats.p, 0, sizeof(Stats), s));
+    CU(cudaMemsetAsync(c->scene_cover.p, 0, 2 * n_blocks * 4, s));
+    CU(cudaMemsetAsync(c->scene_key.p, 0, npix * 4, s));
+    g.frames = c->frame_table.as<Frame2D>();
+    g.d_pl = c->scene_pl.as<uint32_t>();
+    g.cover = c->scene_cover.as<uint32_t>();
+    g.key = c->scene_key.as<uint32_t>();
+
+    size_t ev = 0;
+    uint32_t launches = 0, passes_run = 0;
+    for (uint32_t k = 0; k < n_passes; ++k) {
+        if (k && cc.flag && __atomic_load_n(cc.flag, __ATOMIC_ACQUIRE)) break;   // cancelled: enqueue no further pass
+        uint32_t lo, hi;
+        pass_range(k, lo, hi);
+        Tiles2D gp = g;
+        gp.n_roots = shape_roots * (hi - lo);
+        gp.groups = groups[k];
+        if (k) {   // a new pass: fresh lists, cursors and arena; error bits accumulate over the call
+            CU(cudaMemsetAsync(c->counters.p, 0, offsetof(Counters, error), s));
+            CU(cudaMemsetAsync(&c->counters.as<Counters>()->arena_top, 0, sizeof(unsigned long long), s));
+        }
+        bool fused = false;
+        if (int32_t erc = enqueue_tiles_2d(c, tapes[hi - 1], cfg, gp, table[hi - 1].vb, nullptr, want_stats, timing, cc, s,
+                                           ev, launches, fused))
+            return abandon_frames(c, s, stats, erc);
+        if (want_stats)
+            CU(cudaMemcpyAsync(c->frame_tops.as<unsigned long long>() + k, &c->counters.as<Counters>()->arena_top,
+                               sizeof(unsigned long long), cudaMemcpyDeviceToDevice, s));
+        ++passes_run;
+    }
+    if (passes_run == n_passes) {
+        Scene2DResolveParams rp{};
+        rp.cover = g.cover + n_blocks;
+        rp.key = g.key;
+        rp.width = W;
+        rp.height = H;
+        rp.leaf = leaf;
+        rp.blocks_x = g.blocks_x;
+        rp.fmt = fmt;
+        rp.colors = c->scene_colors.as<uint8_t>();
+        rp.out = out ? dout : nullptr;
+        rp.index = dindex;
+        rp.cancel = cc.ref;
+        launch_scene2d_resolve(rp, s);
+        ++launches;
+        CU(cudaGetLastError());
+    }
+    if (async && !host_out && !host_index && !want_stats) {
+        c->async_call = cc;
+        return FC_OK;
+    }
+    if (cc.flag) {   // a cancelled call copies nothing to the host
+        if (int32_t wrc = wait_call(c, s, cc)) {
+            if (stats) memset(stats, 0, sizeof *stats);
+            return wrc;
+        }
+        if (passes_run < n_passes) {   // the flag stopped the passes, but was cleared before the wait saw it
+            if (stats) memset(stats, 0, sizeof *stats);
+            return fail(FC_ERR_CANCELLED, "cancelled");
+        }
+    }
+    if (host_out) CU(cudaMemcpyAsync(out, dout, img_fmt, cudaMemcpyDeviceToHost, s));
+    if (host_index) CU(cudaMemcpyAsync(index, dindex, npix * 2, cudaMemcpyDeviceToHost, s));
+    CU(cudaStreamSynchronize(s));
+    int32_t rc = check_device_errors(c);
+    if (stats) {
+        Stats h;
+        std::vector<unsigned long long> tops(n_passes);
+        CU(cudaMemcpy(&h, c->stats.p, sizeof h, cudaMemcpyDeviceToHost));
+        CU(cudaMemcpy(tops.data(), c->frame_tops.p, tops.size() * sizeof(unsigned long long), cudaMemcpyDeviceToHost));
+        write_stats(stats, h, false, *std::max_element(tops.begin(), tops.end()), launches);
+        if (timing)
+            for (uint32_t k = 0; k < n_passes; ++k) add_stage_ms_2d(c, size_t(k) * (L + 3), L, false, h, stats->stage_ms);
+    }
+    return rc;
+}
+
 int32_t fc_render3d(fc_ctx* c, const fc_tape* tape, const fc_render3d_cfg* cfg, fc_geometry_pixel* out,
                     fc_render_stats* stats) {
     if (!c || !tape || !cfg || !out) return fail(FC_ERR_INVALID, "null argument");
@@ -1421,15 +1661,9 @@ int32_t fc_render3d_scene(fc_ctx* c, const fc_tape* const* tapes, const fc_frame
         gp.pl0 = r.f0;
         gp.pl1 = r.f0 + r.n;
         pl_host.clear();
-        for (uint32_t k = r.f0; k < r.f0 + r.n; ++k) {
-            bool seen = false;
-            for (const Tiles3D::Group& gr : gp.groups) seen |= gr.tape == tapes[k];
-            if (seen) continue;
-            const uint32_t first_pl = uint32_t(pl_host.size());
-            for (uint32_t q = k; q < r.f0 + r.n; ++q)
-                if (tapes[q] == tapes[k]) pl_host.push_back(q);
-            gp.groups.push_back(Tiles3D::Group{tapes[k], first_pl, uint32_t(pl_host.size()) - first_pl});
-        }
+        std::vector<uint32_t> order(r.n);
+        for (uint32_t k = 0; k < r.n; ++k) order[k] = r.f0 + k;
+        group_by_tape(tapes, order, pl_host, gp.groups);
         gp.d_pl = c->scene_pl.as<uint32_t>();
         CU(cudaMemcpyAsync(c->scene_pl.p, pl_host.data(), pl_host.size() * 4, cudaMemcpyHostToDevice, s));
         if (r.n > 1) {

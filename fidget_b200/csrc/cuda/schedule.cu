@@ -349,9 +349,9 @@ int coop_blocks(fc_ctx* c, const fc_tape* tape, uint64_t n_roots, LevelParams& p
     for (int k = 1; k <= cap; ++k) if (rounds(k) < rounds(per_sm)) per_sm = k;
     // widest CTA for which the runtime really keeps per_sm of them resident (register granularity
     // makes 7 x 224 threads x 40 registers NOT fit although 7 * 224 * 40 < 64 K)
-    // a frame batch and a 3D scene launch their own instantiations
+    // a frame batch and a scene launch their own instantiations
     const int variant = p.scene ? 2 : p.frames != nullptr ? 1 : 0;
-    auto& mm = c->coop_memo[(dim == 3 ? 2 : 0) + variant];
+    auto& mm = c->coop_memo[(dim == 3 ? 3 : 0) + variant];
     if (mm.threads == 0 || mm.smem != smem || mm.per_sm != per_sm) {
         int t = COOP_THREADS;
         while (t > 64 && coop_occupancy(dim, variant, t, smem) < per_sm) t -= 32;

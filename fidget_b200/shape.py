@@ -201,7 +201,14 @@ class CudaShape:
 
     def close(self):
         """Releases the tape and its evaluator now (a second call does nothing).  Both belong to the CudaContext, so
-        they must go before ``CudaContext.close``; the shape cannot be used afterwards."""
+        they must go before ``CudaContext.close``; the shape cannot be used afterwards.  A shape whose context is already
+        closed -- the collector frees a reference cycle holding both in any order -- only drops its handles: releasing
+        them would read the destroyed context."""
+        cuda = getattr(self, "cuda", None)
+        if cuda is not None and getattr(cuda, "_h", None) is None:
+            self._eval = None
+            self._h = None
+            return
         if getattr(self, "_eval", None):
             self._lib.fc_eval_destroy(self._eval)
             self._eval = None
@@ -732,7 +739,85 @@ def render3d_scene(shapes, cfg: RenderConfig3D, var_values=None, world_to_model=
     return (out, index_out, st.as_dict()) if stats else (out, index_out)
 
 
-OCTREE_LEAF = np.dtype([("ix", np.uint16), ("iy", np.uint16), ("iz", np.uint16), ("mask", np.uint8),
+def scene_table_2d(cfg: RenderConfig2D, n: int, z=None, var_values=None, world_to_model=None, mats=None):
+    """The ``fc_frame2d`` placement table of ``render2d_scene`` for ``n`` shapes: entry k is what ``frame_table`` gives
+    for placement k's values (``z`` [n], ``var_values`` [n, k], ``world_to_model`` [n, 3, 3], ``mats`` [n, 4, 4]).  What
+    is not given per placement comes from ``cfg``, for all n; lengths other than n raise ValueError."""
+    per = {name: v for name, v in (("z", z), ("var_values", var_values), ("world_to_model", world_to_model),
+                                   ("mats", mats)) if v is not None}
+    for name, v in per.items():
+        if len(v) != n:
+            raise ValueError(f"{name} has {len(v)} entries for {n} shapes")
+    if not per:   # every placement is cfg's own view, Z and vars
+        one = frame_table(cfg)[0]
+        table = (_lib.FcFrame2d * n)()
+        for k in range(n):
+            C.memmove(C.byref(table[k]), C.byref(one), C.sizeof(one))
+        return table
+    return frame_table(cfg, **per)
+
+
+def scene_colors(colors, n: int) -> np.ndarray:
+    """The [n, 3] uint8 colour table of ``render2d_scene``.  uint8 input is taken as is; other numbers are converted
+    per channel as the viewer's ``draw_rgb`` does: below 0 -> 0, above 1 -> 255, otherwise ``a * 255`` truncated (in
+    f64), NaN -> 0."""
+    a = np.asarray(colors)
+    if a.shape != (n, 3):
+        raise ValueError(f"colors must be [{n}, 3], got {list(a.shape)}")
+    if a.dtype == np.uint8:
+        return np.ascontiguousarray(a)
+    a = a.astype(np.float64)
+    with np.errstate(invalid="ignore"):
+        out = np.where(a < 0.0, 0.0, np.where(a > 1.0, 255.0, np.trunc(a * 255.0)))
+    return np.nan_to_num(out, nan=0.0).astype(np.uint8)
+
+
+def render2d_scene(shapes, cfg: RenderConfig2D, colors=None, z=None, var_values=None, world_to_model=None, mats=None,
+                   out=None, index_out=None, stats: bool = False, asynchronous: bool = False):
+    """A 2D draw list in one call (``fc_render2d_scene``): the viewer's 2D mode, each shape painted opaque over the
+    ones before it.  Shape k is ``shapes[k]`` placed by entry k of ``scene_table_2d`` (per-placement ``z`` /
+    ``var_values`` / ``world_to_model`` / ``mats``, leading dimension ``len(shapes)``; the rest from ``cfg``).
+    ``index`` holds, per pixel, the last k whose ``render2d`` is inside there (``FC_SCENE2D_NONE`` where none is), bit
+    for bit; the image is ``cfg.out_format`` of that: "rgba8" the colour of shape k (``colors``, see ``scene_colors``;
+    None: white) with alpha 255 and zeros elsewhere, "mask_u8" / "bitmap_1bit" the union of the shapes.  "f32" is
+    refused.  Returns ``(image, index)`` -- or the given ``out`` / ``index_out`` (numpy arrays or CUDA tensors of that
+    many bytes, contiguous) -- plus the stats with ``stats=True``; None when ``cfg.cancel`` cancelled it.  Without
+    ``index_out`` the index lands next to ``out``: a numpy uint16 array for a host ``out``, an int16 CUDA tensor (the
+    same bits) on ``out``'s device for a CUDA ``out``.  All shapes must live on one CudaContext."""
+    shapes = list(shapes)
+    n = len(shapes)
+    if n == 0:
+        raise ValueError("a scene needs at least one shape")
+    lib, cuda = shapes[0]._lib, shapes[0].cuda
+    if any(sh.cuda is not cuda for sh in shapes):
+        raise ValueError("the shapes of a scene must belong to one CudaContext")
+    table = scene_table_2d(cfg, n, z=z, var_values=var_values, world_to_model=world_to_model, mats=mats)
+    col = scene_colors(colors, n) if colors is not None else None
+    c = _render2d_cfg(cfg, asynchronous)
+    dims, dtype = _image_shape_2d(cfg)
+    if out is None:
+        out = np.zeros(dims, dtype=dtype)
+    else:
+        _check_out(out, int(np.prod(dims)) * np.dtype(dtype).itemsize)
+    if index_out is None and getattr(out, "is_cuda", False):
+        import torch
+        index_out = torch.zeros((cfg.height, cfg.width), dtype=torch.int16, device=out.device)
+    elif index_out is None:
+        index_out = np.zeros((cfg.height, cfg.width), dtype=np.uint16)
+    else:
+        _check_out(index_out, cfg.height * cfg.width * 2)
+    handles = (C.c_void_p * n)(*[sh._h for sh in shapes])
+    st = _lib.FcRenderStats() if stats else None
+    rc = cuda._cancellable(cfg.cancel, lambda: lib.fc_render2d_scene(
+        cuda._h, handles, table, n, C.byref(c), None if col is None else col.ctypes.data, _ptr(out), _ptr(index_out),
+        C.byref(st) if stats else None), asynchronous)
+    if rc == _lib.FC_ERR_CANCELLED:
+        return None
+    _ck(rc)
+    return (out, index_out, st.as_dict()) if stats else (out, index_out)
+
+
+OCTREE_LEAF =np.dtype([("ix", np.uint16), ("iy", np.uint16), ("iz", np.uint16), ("mask", np.uint8),
                         ("n_edges", np.uint8), ("present", np.uint16), ("pad", np.uint16),
                         ("pos", np.float32, (12, 3)), ("grad", np.float32, (12, 4))])
 

@@ -64,7 +64,8 @@ int32_t fc_ctx_set_arena_bytes(fc_ctx* ctx, uint64_t bytes);
 /* Cancellation (CancelToken, fidget-core/src/render/config.rs:59-80).  `flag` points to a caller-owned byte with the
  * layout of Rust's AtomicBool (CancelToken::into_raw() as *const u8): nonzero = cancelled.  The library reads it with
  * an acquire load, from any thread; NULL detaches it.  Context-wide, like fc_ctx_set_stream, and consulted only by
- * fc_render2d, fc_render2d_frames, fc_render3d, fc_render3d_frames, fc_render3d_scene, fc_octree_sample, fc_mesh_build, and
+ * fc_render2d, fc_render2d_frames, fc_render2d_scene, fc_render3d, fc_render3d_frames, fc_render3d_scene, fc_octree_sample,
+ * fc_mesh_build, and
  * fc_ctx_synchronize after the most recent FC_FLAG_ASYNC call of those.  With a flag attached:
  *  - set on entry: the call returns FC_ERR_CANCELLED before it allocates or launches anything;
  *  - set while the call runs: the kernels stop claiming work and the call returns FC_ERR_CANCELLED ("cancelled" in
@@ -340,6 +341,40 @@ int32_t fc_render3d_frames(fc_ctx* ctx, const fc_tape* tape, const fc_render3d_c
 int32_t fc_render3d_scene(fc_ctx* ctx, const fc_tape* const* tapes /* host, n_shapes */,
                           const fc_frame3d* placements /* host, n_shapes */, uint32_t n_shapes,
                           const fc_render3d_cfg* cfg, fc_geometry_pixel* out, uint16_t* index /* may be NULL */,
+                          fc_render_stats* stats /* may be NULL */);
+/* A 2D draw list in one call: the reference viewer's 2D mode, where each draw(shape) / draw_rgb(shape, r, g, b) of a
+ * script is rendered and painted over the layers before it, opaque (BlendComponent::OVER).  Shape k is tapes[k] placed
+ * by placements[k] (its mat, z and var_values, as fc_render2d_frames reads a frame; the same tape may appear any number
+ * of times).  Let in_k(p) be RawDistancePixel::inside of pixel p in fc_render2d(tapes[k], cfg with placements[k]'s mat,
+ * z and var_values).  Then, bit for bit:
+ *  - index (may be NULL) receives the largest k with in_k(p), or FC_SCENE2D_NONE where no shape is inside: later shapes
+ *    are on top, as the viewer paints them.
+ *  - out (may be NULL) receives the image in cfg->out_format: FC_OUT_RGBA8 [r_k, g_k, b_k, 255] for k = index[p] and
+ *    [0, 0, 0, 0] where no shape is inside, with colors[3k .. 3k + 2] (host, n_shapes * 3 bytes; NULL: white for every
+ *    shape, the colour of draw()); FC_OUT_MASK_U8 and FC_OUT_BITMAP_1BIT: the union of the shapes' inside sets, in
+ *    fc_render2d's layouts.  FC_OUT_F32 is FC_ERR_UNSUPPORTED: no per-shape distance is kept.
+ *  - cfg supplies what the shapes share: width, height, pixel_perfect, tile_sizes, out_format and the flags
+ *    FC_FLAG_TIMING and FC_FLAG_ASYNC; its mat, z and var_values are ignored.  out and index are host or device memory.
+ *  - The shapes share one cover map (per leaf tile block: the topmost shape with an interval-proven-inside tile over
+ *    it) and one key map (per pixel: the topmost shape whose leaf evaluation found it inside).  A tile whose every block
+ *    is covered by a higher shape is not evaluated.  With pixel_perfect no tile is proven inside, so nothing is culled.
+ *  - stats: the per-level census of the tiles evaluated (culled tiles are not counted) and the leaf pixels evaluated,
+ *    arena_bytes_used the largest of any pass, stage_ms and kernel_launches summed over passes.  Every field is the same
+ *    for two identical calls and at any launch grid: a cull decision only reads what earlier launches proved.
+ *  - passes: as many shapes as their worst-case job lists fit FC_FRAMES_PASS_BYTES, from the top of the draw list down,
+ *    so that lower shapes are culled against everything above them.  The tape arena is reset per pass; FC_ERR_ARENA if
+ *    a pass exhausts it.
+ *  - n_shapes == 0 launches nothing and returns FC_OK.  Refused before anything is allocated or launched, with out and
+ *    index untouched: every tape fc_render2d refuses (with its code); FC_ERR_INVALID for a placement without a value
+ *    for a bound variable, a NULL entry of tapes, tapes or placements NULL with n_shapes > 0, and out and index both
+ *    NULL; FC_ERR_UNSUPPORTED for n_shapes > FC_SCENE_MAX_SHAPES, FC_FLAG_FUSED_TAIL, root row bands, the tile
+ *    interleave and FC_OUT_F32.
+ *  - The cancel flag and FC_FLAG_ASYNC (device out and index, no stats) behave as in fc_render2d_frames. */
+#define FC_SCENE2D_NONE 0xFFFFu
+int32_t fc_render2d_scene(fc_ctx* ctx, const fc_tape* const* tapes /* host, n_shapes */,
+                          const fc_frame2d* placements /* host, n_shapes */, uint32_t n_shapes,
+                          const fc_render2d_cfg* cfg, const uint8_t* colors /* host, n_shapes * 3 RGB, or NULL */,
+                          void* out /* may be NULL */, uint16_t* index /* may be NULL */,
                           fc_render_stats* stats /* may be NULL */);
 /* Per-pixel merge of `n_slabs` slab images (each width*height, device
  * pointers, Z-ordered) into `out`, applying the final depth clamp of

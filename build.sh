@@ -11,7 +11,10 @@ FLAGS="-gencode arch=compute_90a,code=sm_90a -lineinfo -O3 -std=c++17 \
 if [ "$1" = "-v" ]; then FLAGS="$FLAGS -Xptxas -v"; fi
 # EXTRA="-DSOME_SWITCH" OUT=fidget_b200/libfidget_cuda_variant.so ./build.sh builds a variant for FIDGET_B200_LIB
 FLAGS="$FLAGS $EXTRA"
-$NVCC $FLAGS -o $OUT $SRC/cuda/kernels.cu $SRC/cuda/coop.cu $SRC/cuda/bulk.cu $SRC/cuda/tail2d.cu $SRC/cuda/octree.cu $SRC/cuda/effects.cu $SRC/cuda/capi.cu $SRC/cuda/schedule.cu $SRC/cuda/render.cu $SRC/cuda/octree_capi.cu $SRC/cuda/mesh.cu $SRC/cuda/effects_capi.cu $SRC/cuda/solve.cu $SRC/cuda/solve_capi.cu $SRC/host/tape.cc $SRC/host/host_capi.cc
+# dev_ops.cuh as a string for the tape compiler (compile.cu): NVRTC compiles the same device arithmetic at run time
+mkdir -p build
+{ echo 'extern const char k_dev_ops_source[] = R"FC_DEV_OPS('; cat $SRC/cuda/dev_ops.cuh; echo ')FC_DEV_OPS";'; } > build/dev_ops_src.cc
+$NVCC $FLAGS -o $OUT build/dev_ops_src.cc $SRC/cuda/compile.cu $SRC/cuda/kernels.cu $SRC/cuda/coop.cu $SRC/cuda/bulk.cu $SRC/cuda/tail2d.cu $SRC/cuda/octree.cu $SRC/cuda/effects.cu $SRC/cuda/capi.cu $SRC/cuda/schedule.cu $SRC/cuda/render.cu $SRC/cuda/octree_capi.cu $SRC/cuda/mesh.cu $SRC/cuda/effects_capi.cu $SRC/cuda/solve.cu $SRC/cuda/solve_capi.cu $SRC/host/tape.cc $SRC/host/host_capi.cc -ldl
 make -s -C oracle liboracle.so
 # the solver's CPU oracle (oracle/solve.cc) on top of liboracle's point and gradient VM
 CXX=$([ -x /usr/bin/g++ ] && echo /usr/bin/g++ || echo g++)

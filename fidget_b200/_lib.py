@@ -16,9 +16,27 @@ class BackendMissing(RuntimeError):
     pass
 
 
+def _default_nvrtc():
+    """The library opens NVRTC at its first tape compile (fc_tape_compile); point it at the copy that ships with torch
+    (the nvidia-cuda-nvrtc wheel) unless FIDGET_B200_NVRTC already names one."""
+    if os.environ.get("FIDGET_B200_NVRTC"):
+        return
+    import importlib.util
+    try:
+        spec = importlib.util.find_spec("nvidia.cuda_nvrtc")
+    except (ImportError, ValueError):
+        return
+    for base in (spec.submodule_search_locations or []) if spec else []:
+        lib = os.path.join(base, "lib")
+        if os.path.isdir(lib):
+            os.environ["FIDGET_B200_NVRTC"] = lib
+            return
+
+
 def load() -> C.CDLL:
     global _LIB
     if _LIB is None:
+        _default_nvrtc()
         if not os.path.exists(LIB_PATH):
             raise BackendMissing(
                 f"{LIB_PATH} not found: build it with ./build.sh (nvcc, sm_90a). "
@@ -111,6 +129,17 @@ class FcSolveResult(C.Structure):
     _fields_ = [("status", C.c_uint32), ("iterations", C.c_uint32), ("err", C.c_float), ("pad", C.c_uint32)]
 
 
+class FcCompiledInfo(C.Structure):
+    _fields_ = [("kinds", C.c_uint32), ("nvrtc_version", C.c_uint32), ("regs", C.c_uint32 * 3),
+                ("local_bytes", C.c_uint32 * 3), ("compile_ms", C.c_float * 3), ("cubin_bytes", C.c_uint64)]
+
+    def as_dict(self):
+        return {"kinds": int(self.kinds), "nvrtc_version": int(self.nvrtc_version), "regs": list(self.regs),
+                "local_bytes": list(self.local_bytes), "compile_ms": list(self.compile_ms),
+                "cubin_bytes": int(self.cubin_bytes)}
+
+
+FC_COMPILE_FLOAT, FC_COMPILE_GRAD, FC_COMPILE_INTERVAL = 1, 2, 4
 FC_SOLVE_MAX_FREE, FC_SOLVE_MAX_CONSTRAINTS, FC_SOLVE_MAX_PARAMS = 64, 256, 1024
 FC_SOLVE_ZERO_RESIDUAL = 0
 FC_SOLVE_UNCHANGED = 1
@@ -163,6 +192,14 @@ CUDA_API = {
     "fc_float_slice_eval": (_i32, [_vp, _vp, _P(_vp), _P(_vp), _u64]),
     "fc_grad_slice_eval": (_i32, [_vp, _vp, _P(_vp), _P(_vp), _u64]),
     "fc_simplify": (_i32, [_vp, _vp, _vp, C.c_size_t, _P(_vp)]),
+    "fc_tape_compile": (_i32, [_vp, _vp, _u32, _P(_vp)]),
+    "fc_compiled_get_info": (_i32, [_vp, _P(FcCompiledInfo)]),
+    "fc_compiled_release": (_i32, [_vp]),
+    "fc_compiled_float_slice_eval": (_i32, [_vp, _vp, _P(_vp), _P(_vp), _u64]),
+    "fc_compiled_grad_slice_eval": (_i32, [_vp, _vp, _P(_vp), _P(_vp), _u64]),
+    "fc_compiled_interval_eval_batch": (_i32, [_vp, _vp, _vp, _u64, _vp, _vp, _vp]),
+    "fc_compile_check": (_i32, [_P(_u32), C.c_size_t, _u8, _u32, _u32, _u32, _u32, C.c_char_p, C.c_size_t,
+                                _P(C.c_size_t), _P(FcCompiledInfo)]),
     "fc_render2d": (_i32, [_vp, _vp, _P(FcRender2dCfg), _vp, _P(FcRenderStats)]),
     "fc_render2d_frames": (_i32, [_vp, _vp, _P(FcRender2dCfg), _P(FcFrame2d), _u32, _vp, _P(FcRenderStats)]),
     "fc_render3d": (_i32, [_vp, _vp, _P(FcRender3dCfg), _vp, _P(FcRenderStats)]),

@@ -1,6 +1,7 @@
 // C ABI of libfidget_cuda (include/fidget_cuda.h): contexts, tapes, the trait-level evaluators and
 // fc_simplify.  The renderers live in render.cu, the octree sampler in octree_capi.cu, the effects in
 // effects_capi.cu, the level-0 schedule in schedule.cu.
+#include <functional>
 #include <thread>
 
 #include "capi_internal.h"
@@ -479,8 +480,12 @@ void fc_eval_destroy(fc_eval* e) {
     delete e;
 }
 
-static int32_t tracing_eval(fc_eval* e, const fc_tape* t, const float* vars, uint64_t n, float* out, uint8_t* choices,
-                            uint8_t* simplify, bool interval) {
+}  // extern "C"
+
+// Staging shared by the tracing batch calls (interpreted and compiled): host buffers go through the evaluator's
+// device buffers, results come back, and the call ends with a synchronise; `launch` enqueues the kernel
+int32_t tracing_eval(fc_eval* e, const fc_tape* t, const float* vars, uint64_t n, float* out, uint8_t* choices,
+                     uint8_t* simplify, bool interval, const std::function<int32_t(TracingParams&)>& launch) {
     if (!e || !t || (!vars && t->info.n_vars) || !out) return fail(FC_ERR_INVALID, "null argument");
     fc_ctx* c = e->ctx;
     CU(cudaSetDevice(c->device));
@@ -510,7 +515,7 @@ static int32_t tracing_eval(fc_eval* e, const fc_tape* t, const float* vars, uin
     if (simplify) {
         if (dsi) p.simplify = simplify; else { CU(e->simplify.ensure(n)); p.simplify = e->simplify.as<uint8_t>(); }
     }
-    if (interval) launch_interval_batch(p, c->stream); else launch_point_batch(p, c->stream);
+    if (int32_t rc = launch(p)) return rc;
     CU(cudaGetLastError());
     if (!dout && out_bytes) CU(cudaMemcpyAsync(out, p.out, out_bytes, cudaMemcpyDeviceToHost, c->stream));
     if (choices && ch_bytes && !dch) CU(cudaMemcpyAsync(choices, p.choices, ch_bytes, cudaMemcpyDeviceToHost, c->stream));
@@ -519,19 +524,62 @@ static int32_t tracing_eval(fc_eval* e, const fc_tape* t, const float* vars, uin
     return FC_OK;
 }
 
+static int32_t interpret_interval(fc_eval* e, TracingParams& p) {
+    launch_interval_batch(p, e->ctx->stream);
+    return FC_OK;
+}
+
+extern "C" {
+
 int32_t fc_interval_eval(fc_eval* e, const fc_tape* t, const float* vars, float* out, uint8_t* choices, uint8_t* simplify) {
-    return tracing_eval(e, t, vars, 1, out, choices, simplify, true);
+    return tracing_eval(e, t, vars, 1, out, choices, simplify, true, [&](TracingParams& p) { return interpret_interval(e, p); });
 }
 int32_t fc_point_eval(fc_eval* e, const fc_tape* t, const float* vars, float* out, uint8_t* choices, uint8_t* simplify) {
-    return tracing_eval(e, t, vars, 1, out, choices, simplify, false);
+    return tracing_eval(e, t, vars, 1, out, choices, simplify, false, [&](TracingParams& p) {
+        launch_point_batch(p, e->ctx->stream);
+        return FC_OK;
+    });
 }
 int32_t fc_interval_eval_batch(fc_eval* e, const fc_tape* t, const float* vars, uint64_t n, float* out, uint8_t* choices,
                                uint8_t* simplify) {
-    return tracing_eval(e, t, vars, n, out, choices, simplify, true);
+    return tracing_eval(e, t, vars, n, out, choices, simplify, true, [&](TracingParams& p) { return interpret_interval(e, p); });
 }
 
-static int32_t bulk_eval(fc_eval* e, const fc_tape* t, const void* const* vars, void* const* outs, uint64_t n,
-                         size_t elem, bool grad) {
+}  // extern "C"
+
+// The interpreters' launch: the TMA-fed kernel when the tape and the buffers fit it, else the per-thread kernel
+static int32_t interpret_slice(fc_eval* e, const fc_tape* t, BulkParams& p, const std::vector<const void*>& dptr, bool grad) {
+    fc_ctx* c = e->ctx;
+    const uint32_t nv = p.n_vars, no = p.n_outputs;
+    const uint64_t n = p.n;
+    unsigned tma_ctas = 0;
+    if (!t->info.mem_count && n >= 4096 && nv <= 4 && no <= 2 && !env_int("FIDGET_B200_NO_TMA", 0)) {
+        SliceTmaParams q{};
+        q.tape = t->dev;
+        q.n_ops = t->info.n_ops;
+        q.n_vars = nv;
+        q.n_outputs = no;
+        q.n_regs = t->info.reg_count;
+        q.n = n;
+        for (uint32_t i = 0; i < nv; ++i) q.vars[i] = static_cast<const float4*>(dptr[i]);
+        for (uint32_t o = 0; o < no; ++o) q.outs[o] = static_cast<float4*>(const_cast<void*>(dptr[nv + o]));
+        tma_ctas = launch_slice_tma(q, grad, c->sm_count, c->stream);
+    }
+    if (!tma_ctas) { if (grad) launch_grad_slice(p, c->stream); else launch_float_slice(p, c->stream); }
+    if (env_int("FIDGET_B200_SLICE_DEBUG", 0)) {   // which kernel ran, and how many tiles each TMA CTA had to cycle
+        const uint64_t tile = uint64_t(SLICE_TMA_TILE) * (grad ? 1 : 4);
+        if (tma_ctas)
+            fprintf(stderr, "slice: TMA kernel, %llu points, %llu full tiles, %u CTAs, %d SMs\n", (unsigned long long)n,
+                    (unsigned long long)(n / tile), tma_ctas, c->sm_count);
+        else
+            fprintf(stderr, "slice: per-thread kernel, %llu points\n", (unsigned long long)n);
+    }
+    return FC_OK;
+}
+
+// Staging shared by the slice calls (interpreted and compiled), as tracing_eval's
+int32_t bulk_eval(fc_eval* e, const fc_tape* t, const void* const* vars, void* const* outs, uint64_t n, size_t elem,
+                  const std::function<int32_t(BulkParams&, const std::vector<const void*>&)>& launch) {
     if (!e || !t || (!vars && t->info.n_vars) || !outs) return fail(FC_ERR_INVALID, "null argument");
     fc_ctx* c = e->ctx;
     CU(cudaSetDevice(c->device));
@@ -575,28 +623,7 @@ static int32_t bulk_eval(fc_eval* e, const fc_tape* t, const void* const* vars, 
     p.n = n;
     p.vars = e->ptrs.as<const void*>();
     p.outs = reinterpret_cast<void* const*>(e->ptrs.as<void*>() + nv);
-    unsigned tma_ctas = 0;
-    if (!t->info.mem_count && n >= 4096 && nv <= 4 && no <= 2 && !env_int("FIDGET_B200_NO_TMA", 0)) {
-        SliceTmaParams q{};
-        q.tape = t->dev;
-        q.n_ops = t->info.n_ops;
-        q.n_vars = nv;
-        q.n_outputs = no;
-        q.n_regs = t->info.reg_count;
-        q.n = n;
-        for (uint32_t i = 0; i < nv; ++i) q.vars[i] = static_cast<const float4*>(dptr[i]);
-        for (uint32_t o = 0; o < no; ++o) q.outs[o] = static_cast<float4*>(const_cast<void*>(dptr[nv + o]));
-        tma_ctas = launch_slice_tma(q, grad, c->sm_count, c->stream);
-    }
-    if (!tma_ctas) { if (grad) launch_grad_slice(p, c->stream); else launch_float_slice(p, c->stream); }
-    if (env_int("FIDGET_B200_SLICE_DEBUG", 0)) {   // which kernel ran, and how many tiles each TMA CTA had to cycle
-        const uint64_t tile = uint64_t(SLICE_TMA_TILE) * (grad ? 1 : 4);
-        if (tma_ctas)
-            fprintf(stderr, "slice: TMA kernel, %llu points, %llu full tiles, %u CTAs, %d SMs\n", (unsigned long long)n,
-                    (unsigned long long)(n / tile), tma_ctas, c->sm_count);
-        else
-            fprintf(stderr, "slice: per-thread kernel, %llu points\n", (unsigned long long)n);
-    }
+    if (int32_t rc = launch(p, dptr)) return rc;
     CU(cudaGetLastError());
     for (auto& cb : copy_back)
         if (n) CU(cudaMemcpyAsync(cb.first, cb.second, n * elem, cudaMemcpyDeviceToHost, c->stream));
@@ -604,11 +631,15 @@ static int32_t bulk_eval(fc_eval* e, const fc_tape* t, const void* const* vars, 
     return FC_OK;
 }
 
+extern "C" {
+
 int32_t fc_float_slice_eval(fc_eval* e, const fc_tape* t, const float* const* vars, float* const* out, uint64_t n) {
-    return bulk_eval(e, t, reinterpret_cast<const void* const*>(vars), reinterpret_cast<void* const*>(out), n, 4, false);
+    return bulk_eval(e, t, reinterpret_cast<const void* const*>(vars), reinterpret_cast<void* const*>(out), n, 4,
+                     [&](BulkParams& p, const std::vector<const void*>& dptr) { return interpret_slice(e, t, p, dptr, false); });
 }
 int32_t fc_grad_slice_eval(fc_eval* e, const fc_tape* t, const fc_grad* const* vars, fc_grad* const* out, uint64_t n) {
-    return bulk_eval(e, t, reinterpret_cast<const void* const*>(vars), reinterpret_cast<void* const*>(out), n, 16, true);
+    return bulk_eval(e, t, reinterpret_cast<const void* const*>(vars), reinterpret_cast<void* const*>(out), n, 16,
+                     [&](BulkParams& p, const std::vector<const void*>& dptr) { return interpret_slice(e, t, p, dptr, true); });
 }
 
 int32_t fc_simplify(fc_eval* e, const fc_tape* parent, const uint8_t* choices, size_t n_choices, fc_tape** child) {

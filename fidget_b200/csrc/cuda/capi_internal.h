@@ -8,6 +8,7 @@
 #include <cstdio>
 #include <cstdlib>
 #include <cstring>
+#include <functional>
 #include <mutex>
 #include <string>
 #include <vector>
@@ -234,6 +235,12 @@ int32_t wait_call(fc_ctx* c, cudaStream_t s, const CallCancel& cc);
 // The readback of device counters that ends a wait: a copy to pageable memory would block the host until the stream
 // drains, so with a flag attached the (cancellable) wait comes first
 int32_t wait_read(fc_ctx* c, cudaStream_t s, const CallCancel& cc, void* dst, const void* src, size_t bytes);
+// The batch evaluators' staging of host / device inputs and outputs around one kernel launch (`launch`), shared by the
+// interpreted calls and the compiled ones (compile.cu); both end with a synchronise of the context's stream
+int32_t tracing_eval(fc_eval* e, const fc_tape* t, const float* vars, uint64_t n, float* out, uint8_t* choices,
+                     uint8_t* simplify, bool interval, const std::function<int32_t(TracingParams&)>& launch);
+int32_t bulk_eval(fc_eval* e, const fc_tape* t, const void* const* vars, void* const* outs, uint64_t n, size_t elem,
+                  const std::function<int32_t(BulkParams&, const std::vector<const void*>&)>& launch);
 int32_t transcode(const uint32_t* words, size_t n_words, uint8_t reg_count, uint32_t mem_count, uint32_t n_vars,
                   uint32_t n_outputs, std::vector<uint2>& out, uint32_t& n_choices);
 // render.cu

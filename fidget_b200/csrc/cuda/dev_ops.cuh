@@ -11,8 +11,14 @@
 // Build flags that matter: -fmad=false (the reference never fuses a*b+c),
 // -prec-div=true -prec-sqrt=true -ftz=false.
 #pragma once
+#ifdef __CUDACC_RTC__   // compiled tapes (compile.cu): NVRTC has no host headers
+typedef unsigned char uint8_t;
+typedef unsigned int uint32_t;
+typedef unsigned long uint64_t;
+#else
 #include <cuda_runtime.h>
 #include <stdint.h>
+#endif
 
 namespace fdev {
 

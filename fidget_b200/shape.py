@@ -240,6 +240,11 @@ class CudaShape:
         _ck(self._lib.fc_tape_read(self._h, w.ctypes.data_as(C.POINTER(C.c_uint32)), n.value, C.byref(n)))
         return w
 
+    def compile(self, kinds=("float", "grad", "interval")) -> "CompiledShape":
+        """Compiles the tape to sm_90a kernels for the given evaluator kinds with NVRTC (``fc_tape_compile``): host
+        time up front, then the same results as this shape's evaluators from kernels that keep values in registers."""
+        return CompiledShape(self, kinds)
+
     # ---- tracing evaluators ------------------------------------------------
     def interval_eval(self, vars_lo_hi):
         """-> (out [n_out,2], choices uint8[choice_count], simplify flag)"""
@@ -260,12 +265,15 @@ class CudaShape:
 
     def interval_eval_batch(self, boxes, want_choices=False):
         """boxes: [n, n_vars, 2] -> out [n, n_out, 2] (+ choices [n, choice_count], simplify [n])"""
+        return self._interval_batch(self._lib.fc_interval_eval_batch, self._h, boxes, want_choices)
+
+    def _interval_batch(self, fn, h, boxes, want_choices):
         v = np.ascontiguousarray(boxes, dtype=np.float32).reshape(-1, max(self.n_vars, 1), 2)
         n = v.shape[0]
         out = np.zeros((n, self.info.n_outputs, 2), dtype=np.float32)
         ch = np.zeros((n, max(self.choice_count, 1)), dtype=np.uint8) if want_choices else None
         s = np.zeros(n, dtype=np.uint8)
-        _ck(self._lib.fc_interval_eval_batch(self._ev(), self._h, _ptr(v), n, _ptr(out), _ptr(ch), _ptr(s)))
+        _ck(fn(self._ev(), h, _ptr(v), n, _ptr(out), _ptr(ch), _ptr(s)))
         if want_choices:
             return out, ch[:, :self.choice_count], s.astype(bool)
         return out
@@ -273,6 +281,9 @@ class CudaShape:
     # ---- bulk evaluators ---------------------------------------------------
     def float_slice_eval(self, vars_, out=None):
         """vars_: n_vars arrays (numpy or torch, host or device) of n floats"""
+        return self._float_slice(self._lib.fc_float_slice_eval, self._h, vars_, out)
+
+    def _float_slice(self, fn, h, vars_, out):
         n = int(vars_[0].shape[0]) if len(vars_) else 0
         host = not (len(vars_) and hasattr(vars_[0], "data_ptr"))
         if host:
@@ -288,11 +299,14 @@ class CudaShape:
             outs = out if isinstance(out, (list, tuple)) else [out]
         va = (C.c_void_p * max(len(vars_), 1))(*[_ptr(v) for v in vars_])
         oa = (C.c_void_p * len(outs))(*[_ptr(o) for o in outs])
-        _ck(self._lib.fc_float_slice_eval(self._ev(), self._h, va, oa, n))
+        _ck(fn(self._ev(), h, va, oa, n))
         return outs[0] if self.info.n_outputs == 1 else outs
 
     def grad_slice_eval(self, vars_, out=None):
         """vars_: n_vars arrays [n,4] = {v,dx,dy,dz}"""
+        return self._grad_slice(self._lib.fc_grad_slice_eval, self._h, vars_, out)
+
+    def _grad_slice(self, fn, h, vars_, out):
         n = int(vars_[0].shape[0]) if len(vars_) else 0
         host = not (len(vars_) and hasattr(vars_[0], "data_ptr"))
         if host:
@@ -308,7 +322,7 @@ class CudaShape:
             outs = out if isinstance(out, (list, tuple)) else [out]
         va = (C.c_void_p * max(len(vars_), 1))(*[_ptr(v) for v in vars_])
         oa = (C.c_void_p * len(outs))(*[_ptr(o) for o in outs])
-        _ck(self._lib.fc_grad_slice_eval(self._ev(), self._h, va, oa, n))
+        _ck(fn(self._ev(), h, va, oa, n))
         return outs[0] if self.info.n_outputs == 1 else outs
 
     def simplify(self, choices) -> "CudaShape":
@@ -332,6 +346,77 @@ class CudaShape:
                 raise ValueError(f"input slot {s} is not an axis, and a shape loaded from a blob does not know which "
                                  "Var it is; build the shape from its TapeData to solve with it")
         return keys
+
+
+_COMPILE_KINDS = {"float": _lib.FC_COMPILE_FLOAT, "grad": _lib.FC_COMPILE_GRAD, "interval": _lib.FC_COMPILE_INTERVAL}
+
+
+def _compile_mask(kinds) -> int:
+    if isinstance(kinds, str):
+        kinds = (kinds,)
+    mask = 0
+    for k in kinds:
+        if k not in _COMPILE_KINDS:
+            raise ValueError(f"unknown kind {k!r}: expected some of {sorted(_COMPILE_KINDS)}")
+        mask |= _COMPILE_KINDS[k]
+    return mask
+
+
+class CompiledShape:
+    """``JitShape``'s counterpart: a CudaShape's tape compiled to sm_90a kernels for some of the bulk evaluators
+    (``fc_tape_compile``).  Same signatures, return types and bits as the CudaShape's evaluators; ``info`` has the
+    registers, local memory and compile time per kind."""
+
+    def __init__(self, shape: CudaShape, kinds=("float", "grad", "interval")):
+        self.shape = shape
+        self._lib = shape._lib
+        h = C.c_void_p()
+        _ck(self._lib.fc_tape_compile(shape.cuda._h, shape._h, _compile_mask(kinds), C.byref(h)))
+        self._h = h
+        info = _lib.FcCompiledInfo()
+        _ck(self._lib.fc_compiled_get_info(h, C.byref(info)))
+        self.info = info.as_dict()
+
+    def float_slice_eval(self, vars_, out=None):
+        return self.shape._float_slice(self._lib.fc_compiled_float_slice_eval, self._h, vars_, out)
+
+    def grad_slice_eval(self, vars_, out=None):
+        return self.shape._grad_slice(self._lib.fc_compiled_grad_slice_eval, self._h, vars_, out)
+
+    def interval_eval_batch(self, boxes, want_choices=False):
+        return self.shape._interval_batch(self._lib.fc_compiled_interval_eval_batch, self._h, boxes, want_choices)
+
+    def close(self):
+        """Releases the compiled kernels now (a second call does nothing); like ``CudaShape.close``, a handle whose
+        context is already closed is only dropped."""
+        cuda = getattr(getattr(self, "shape", None), "cuda", None)
+        if cuda is not None and getattr(cuda, "_h", None) is None:
+            self._h = None
+            return
+        if getattr(self, "_h", None):
+            self._lib.fc_compiled_release(self._h)
+            self._h = None
+
+    def __del__(self):
+        self.close()
+
+
+def compile_check(tape: TapeData, kinds=("float", "grad", "interval")):
+    """Host-only (no GPU): generate and compile ``tape`` for ``kinds`` with NVRTC (``fc_compile_check``).
+    -> (info dict, generated source)"""
+    lib = _lib.load()
+    bc = tape.bytecode()
+    info = _lib.FcCompiledInfo()
+    n = C.c_size_t()
+    words = bc.words.ctypes.data_as(C.POINTER(C.c_uint32))
+    args = (words, len(bc.words), bc.reg_count, bc.mem_count, tape.n_vars, tape.output_count, _compile_mask(kinds))
+    cap = 65536 + 256 * len(bc.words)   # above what the generator writes for any tape: one compile, not two
+    buf = C.create_string_buffer(cap)
+    _ck(lib.fc_compile_check(*args, buf, cap, C.byref(n), C.byref(info)))
+    if n.value >= cap:
+        buf = C.create_string_buffer(n.value + 1)
+        _ck(lib.fc_compile_check(*args, buf, n.value + 1, C.byref(n), C.byref(info)))
+    return info.as_dict(), buf.value.decode()
 
 
 # ---------------------------------------------------------------------------

@@ -145,6 +145,53 @@ typedef struct fc_grad { float v, dx, dy, dz; } fc_grad; /* types/grad.rs:2-13, 
 /* VmGradSliceEval::eval (vm/mod.rs:1097-1396) */
 int32_t fc_grad_slice_eval(fc_eval* e, const fc_tape* tape, const fc_grad* const* vars,
                            fc_grad* const* out, uint64_t n);
+/* ---- compiled tapes (JitFunction / JitShape, fidget-jit) ----------------------------------------------------
+ * fc_tape_compile turns one tape into straight-line sm_90a kernels for the bulk evaluators, compiled at run time
+ * with NVRTC: every VM register and memory slot is a local variable, so values stay in registers instead of the
+ * interpreters' per-thread register file.  Compiling takes host time (seconds for a tape of thousands of clauses), so
+ * it is explicit and per kind; the compiled calls pay off over many points.
+ *  - Results: for every tape fc_tape_create accepts (multi-output tapes and tapes with memory slots included), each
+ *    compiled call writes exactly the bits its interpreter counterpart (fc_float_slice_eval, fc_grad_slice_eval,
+ *    fc_interval_eval_batch) writes on the same inputs -- for intervals the values, the choice bytes and the simplify
+ *    flags -- for every opcode and form, NaN payloads of rand / mix included.  NVRTC compiles the library's own device
+ *    arithmetic with the numeric flags the library is built with.
+ *  - Errors: kinds == 0, a kind that was not compiled, or an NVRTC compile error (log in fc_last_error):
+ *    FC_ERR_INVALID.  NVRTC that cannot be loaded: FC_ERR_UNSUPPORTED, and the message says where it looked.
+ *  - NVRTC is opened with dlopen at the first compile, never linked: the path in FIDGET_B200_NVRTC (a file, or the
+ *    directory holding libnvrtc.so.12) and nothing else if it is set; else libnvrtc.so.12 by soname; else
+ *    $CUDA_HOME/lib64 (default /usr/local/cuda).
+ *  - Lifetime: a compiled tape belongs to the context and must be released before fc_ctx_destroy, like a tape; it
+ *    retains its fc_tape.  Work goes on the context's stream (fc_ctx_set_stream).  Not cancellable (nor are the
+ *    calls it shadows). */
+typedef struct fc_compiled fc_compiled;     /* a tape compiled for some evaluator kinds; retains its fc_tape */
+#define FC_COMPILE_FLOAT 1u                 /* fc_compiled_float_slice_eval */
+#define FC_COMPILE_GRAD 2u                  /* fc_compiled_grad_slice_eval */
+#define FC_COMPILE_INTERVAL 4u              /* fc_compiled_interval_eval_batch */
+typedef struct fc_compiled_info {
+    uint32_t kinds;                 /* kinds compiled */
+    uint32_t nvrtc_version;         /* major * 1000 + minor * 10 of the NVRTC that compiled it */
+    uint32_t regs[3];               /* per kind (float, grad, interval): registers per thread, 0 if not compiled */
+    uint32_t local_bytes[3];        /* per kind: local memory (stack frame, spills included) per thread */
+    float compile_ms[3];            /* per kind: host wall time of source generation + NVRTC */
+    uint64_t cubin_bytes;
+} fc_compiled_info;
+int32_t fc_tape_compile(fc_ctx* ctx, const fc_tape* tape, uint32_t kinds, fc_compiled** out);
+int32_t fc_compiled_get_info(const fc_compiled* c, fc_compiled_info* info);
+int32_t fc_compiled_release(fc_compiled* c);
+/* Same arguments, layouts, host / device pointer rules and results as the interpreter calls they shadow */
+int32_t fc_compiled_float_slice_eval(fc_eval* e, const fc_compiled* c, const float* const* vars, float* const* out,
+                                     uint64_t n);
+int32_t fc_compiled_grad_slice_eval(fc_eval* e, const fc_compiled* c, const fc_grad* const* vars, fc_grad* const* out,
+                                    uint64_t n);
+int32_t fc_compiled_interval_eval_batch(fc_eval* e, const fc_compiled* c, const float* vars, uint64_t n, float* out,
+                                        uint8_t* choices, uint8_t* simplify);
+/* Host-only, no device needed (like fc_schedule_check): generate and compile the given bytecode for `kinds`, fill
+ * *info (regs / local_bytes read from the cubin), and optionally copy the generated source, NUL-terminated and cut
+ * to cap - 1 characters (source == NULL or cap == 0: only *n_source, the full length, is set). */
+int32_t fc_compile_check(const uint32_t* words, size_t n_words, uint8_t reg_count, uint32_t mem_count, uint32_t n_vars,
+                         uint32_t n_outputs, uint32_t kinds, char* source, size_t cap, size_t* n_source,
+                         fc_compiled_info* info);
+
 /* VmData::simplify (vm/data.rs:123-318) run on the device for one trace.
  * The child keeps the parent's register assignment (no re-allocation), is
  * value-identical to the reference's child, and reports the reference's

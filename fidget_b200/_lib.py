@@ -121,6 +121,16 @@ class FcMeshInfo(C.Structure):
                [("sampler_ms", C.c_float), ("mesh_ms", C.c_float)]
 
 
+class FcContourCfg(C.Structure):
+    _fields_ = [("depth", C.c_uint32), ("has_transform", C.c_uint32), ("world_to_model", C.c_float * 9), ("z", C.c_float),
+                ("flags", C.c_uint32), ("n_var_values", C.c_uint32), ("var_values", C.c_float * 16)]
+
+
+class FcContourInfo(C.Structure):
+    _fields_ = [(n, C.c_uint64) for n in ("n_leaves", "n_vertices", "n_polylines", "n_closed", "n_open")] + \
+               [("sampler_ms", C.c_float), ("contour_ms", C.c_float)]
+
+
 class FcSolveCfg(C.Structure):
     _fields_ = [("n_params", C.c_uint32), ("n_free", C.c_uint32), ("max_iters", C.c_uint32)]
 
@@ -158,6 +168,7 @@ FC_OUT_F32, FC_OUT_MASK_U8, FC_OUT_BITMAP_1BIT, FC_OUT_RGBA8 = 0, 1, 2, 3
 FC_ERR_CANCELLED = -6
 FC_FRAMES_PASS_BYTES = 512 << 20
 FC_MAX_VARS = 16
+FC_MAX_QUADTREE_DEPTH = 14
 FC_SCENE_MAX_SHAPES = 1024
 FC_SCENE_MAX_DEPTH = 262142
 FC_SCENE_MAX_ROOT_TILE = 1022
@@ -215,6 +226,8 @@ CUDA_API = {
     "fc_mesh_read": (_i32, [_vp, _vp, _vp]),
     "fc_mesh_read_cells": (_i32, [_vp, _vp, _u64, _P(_u64)]),
     "fc_mesh_write_stl": (_i32, [_vp, _vp, C.c_size_t, _P(C.c_size_t)]),
+    "fc_contour_build": (_i32, [_vp, _vp, _P(FcContourCfg), _P(FcContourInfo)]),
+    "fc_contour_read": (_i32, [_vp, _vp, _vp, _vp]),
     "fc_solve_batch": (_i32, [_vp, _P(_vp), _u32, _P(_P(_i32)), _P(FcSolveCfg), _vp, _u64, _vp]),
     "fc_schedule_check": (_i32, [_P(_u32), C.c_size_t, _u8, _u32, _u32, _u32, _P(FcScheduleInfo)]),
     "fc_denoise_normals": (_i32, [_vp, _vp, _u32, _u32, _vp]),

@@ -139,6 +139,9 @@ void fc_ctx_destroy(fc_ctx* c) {
     c->mesh_tree.release();
     c->mesh_herm.release();
     c->mesh_cells.release();
+    c->contour_leaves.release();
+    c->contour_scratch.release();
+    c->contour_out.release();
     c->tile_slots.release();
     c->fx_in.release();
     c->fx_out.release();
@@ -221,8 +224,13 @@ static int32_t cancel_site_of(const std::string& name) {
         if (name == "k_interval_level" + std::to_string(i)) return CS_LEVEL0 + i;
     for (int i = 0; i < CS_WAIT - CS_ROOT_COOP; ++i)
         if (name == names[i]) return CS_ROOT_COOP + i;
-    static_assert(CS_SCENE2D_RESOLVE + 1 == CS_COUNT, "one name per poll site");
+    static_assert(CS_SCENE2D_RESOLVE + 1 == CS_CONTOUR_LEAF, "one name per poll site");
     if (name == "k_scene2d_resolve") return CS_SCENE2D_RESOLVE;
+    static const char* const contour[] = {"k_contour_leaf", "k_contour_grads", "k_contour_vertices", "k_contour_segments",
+                                          "k_contour_link", "k_contour_emit"};
+    static_assert(sizeof(contour) / sizeof(contour[0]) == CS_COUNT - CS_CONTOUR_LEAF, "one name per poll site");
+    for (int i = 0; i < CS_COUNT - CS_CONTOUR_LEAF; ++i)
+        if (name == contour[i]) return CS_CONTOUR_LEAF + i;
     return -1;
 }
 

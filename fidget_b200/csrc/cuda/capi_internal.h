@@ -51,6 +51,25 @@ struct DevBuf {
     template <class T> T* as() { return static_cast<T*>(p); }
 };
 
+// Consecutive 256-byte-aligned arrays of one device buffer: take() points each at its place
+struct Carve {
+    char* base;
+    size_t used = 0;
+    template <class T> void take(T*& p, size_t bytes) {
+        p = base ? reinterpret_cast<T*>(base + used) : nullptr;
+        used += (bytes + 255) & ~size_t(255);
+    }
+};
+// Grows `buf` to the arrays lay_out(Carve&) takes, then points them into it
+template <class F> cudaError_t carve(DevBuf& buf, F lay_out) {
+    Carve size{nullptr};
+    lay_out(size);
+    if (cudaError_t e = buf.ensure(size.used)) return e;
+    Carve at{buf.as<char>()};
+    lay_out(at);
+    return cudaSuccess;
+}
+
 inline bool is_device_ptr(const void* p) {
     if (!p) return false;
     cudaPointerAttributes a;
@@ -132,6 +151,10 @@ struct fc_ctx {
     uint32_t mesh_n_verts = 0, mesh_n_tris = 0;
     DevBuf mesh_tree, mesh_herm, mesh_cells;                    // FC_FLAG_MESH_COLLAPSE: cell tree, Hermite records, final leaves
     uint32_t mesh_n_cells = 0;
+    DevBuf contour_leaves, contour_scratch, contour_out;        // fc_contour_build: sampler output, link scratch, polylines
+    uint32_t contour_n_verts = 0, contour_n_polys = 0;
+    uint32_t* contour_offsets = nullptr;                        // in contour_out, after the vertices
+    uint8_t* contour_closed = nullptr;
     DevBuf fx_in, fx_out, fx_tmp, fx_tables;  // effects: staged host images, intermediate maps, SSAO tables
     DevBuf solve_meta, solve_vals, solve_res; // fc_solve_batch: tape table + slot maps, staged host values / results
     // the batches (fc_render2d_frames, fc_render3d_frames, fc_render3d_scene): the frame or placement table, and the copy

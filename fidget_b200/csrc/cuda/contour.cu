@@ -1,0 +1,697 @@
+// 2D contours (fc_contour_build): dual contouring on a uniform quadtree of the [-1,1]^2 world square, linked into
+// polylines on the device.  The pipeline restricts the mesher's to two dimensions:
+//
+//   descent    k_contour_level: the interval levels of the octree sampler with Z fixed (level_job's QUAD mode), one
+//              launch per depth, four children per cell;
+//   leaves     k_contour_leaf: one warp per leaf, four corners, then the 16-ary edge search of k_octree_leaf -- four
+//              edges x 16 probes, two points per lane, in one pass; k_contour_grads: (dx, dy, v) at the intersections,
+//              one lane per edge, with the tape the leaf was sampled with;
+//   order      the surface leaves sorted by key (iy, ix): vertex ids come from a scan of the group counts in that
+//              order, so vertex id order is key order (iy, ix, group) and the sorted key list is the cell lookup;
+//   vertices   k_contour_vertices: one per connected group of inside corners, by the 2D QEF (qef2_vertex);
+//   segments   k_contour_segments: every interior sign-changing edge links the vertices owning it in its two cells,
+//              inside on the left.  Every vertex owns exactly two sign-changing edges, so it has at most one successor
+//              and one predecessor: next[] / prev[] are written directly, without a counting pass;
+//   linking    list ranking by pointer jumping over prev[]: pass 1 finds the smallest vertex of every cycle, pass 2
+//              cuts each cycle there and ranks every vertex from its polyline's head;
+//   emit       one scan over the heads in vertex order gives each polyline's place, and every vertex is scattered to
+//              head offset + rank.
+#include <cub/cub.cuh>
+
+#include "capi_internal.h"
+#include "level_job.cuh"
+
+namespace fdev {
+
+constexpr uint32_t NONE = ~0u;
+
+// One surface leaf of the quadtree.  Edge e: axis t = e >> 1 (0: along X, 1: along Y) at bit e & 1 of the other axis,
+// from corner c0 = (e & 1) << (1 - t) to c0 | 1 << t: edge 0 = corners 0-1, 1 = 2-3, 2 = 0-2, 3 = 1-3.
+struct ContourLeaf {
+    uint16_t ix, iy;
+    uint8_t mask, present;   // corner mask; bit e = edge e carries an intersection
+    uint16_t pad;
+    float pos[4][2];
+    float grad[4][3];        // dx, dy, v
+};
+
+struct ContourLeafParams {
+    const TileJob* jobs;
+    uint32_t cap_jobs;
+    Counters* ctr;
+    int list, cursor;
+    float cell_h, z;
+    uint32_t has_transform;
+    Mat4 mat;
+    VarBind vb;
+    ContourLeaf* out;
+    TapeRef* out_tapes;
+    uint32_t cap_out;
+    uint32_t* n_out;
+    CancelRef cancel;
+};
+
+// The quadtree levels: k_interval_level's claim loop around level_job's QUAD mode (one root cell)
+__global__ void __launch_bounds__(WARPS_PER_BLOCK * 32) k_contour_level(const __grid_constant__ LevelParams p) {
+    __shared__ uint32_t live_s[WARPS_PER_BLOCK][8][32];
+    const int lane = threadIdx.x & 31;
+    const int wib = threadIdx.x >> 5;
+    const uint32_t gw = blockIdx.x * WARPS_PER_BLOCK + wib;
+    uint32_t* cs = p.choice_scratch + size_t(gw) * p.choice_words * 32u + lane;
+    itv slots[REG_SLOTS];
+    const uint32_t n_jobs = p.root_mode ? 1u : min(p.ctr->n_jobs[p.level], p.cap_in);
+    for (;;) {
+        uint32_t j = 0;
+        if (lane == 0) {
+            j = atomicAdd(&p.ctr->cursor[p.level], 1u);
+            if (j < n_jobs && cancel_poll(p.cancel, CS_LEVEL0 + p.level, j)) j = ~0u;
+        }
+        j = __shfl_sync(FULL, j, 0);
+        if (j >= n_jobs) break;
+        level_job<2, false, false, false, true>(p, j, 1u, slots, cs, live_s[wib], lane, p.epoch);
+    }
+}
+
+__device__ __forceinline__ bool edge_setup2(uint32_t e, uint32_t mask, EdgeState& st) {
+    const uint32_t t = e >> 1, u = 1u - t, sv = e & 1u;
+    const uint32_t c0 = sv << u, c1 = c0 | (1u << t);
+    const bool in0 = (mask >> c0) & 1u, in1 = (mask >> c1) & 1u;
+    st.s[2] = st.e[2] = 0u;
+    if (in0 == in1) {
+        st.s[0] = st.e[0] = st.s[1] = st.e[1] = 0u;
+        return false;
+    }
+    st.s[u] = st.e[u] = sv ? 65535u : 0u;
+    st.s[t] = in0 ? 0u : 65535u;   // the search runs inside -> outside
+    st.e[t] = in0 ? 65535u : 0u;
+    return true;
+}
+
+// One warp per leaf job: corner mask, then the four edges' searches in one pass (lanes 0-15 follow edges 0 and 2, lanes
+// 16-31 edges 1 and 3, one probe each), with k_octree_leaf's rounds, fractions and bracket midpoint
+__global__ void __launch_bounds__(128) k_contour_leaf(const __grid_constant__ ContourLeafParams p) {
+    const int lane = threadIdx.x & 31;
+    float2 slots[REG_SLOTS];
+    const uint32_t n_jobs = min(p.ctr->n_jobs[p.list], p.cap_jobs);
+    for (;;) {
+        uint32_t j = 0;
+        if (lane == 0) {
+            j = atomicAdd(&p.ctr->cursor[p.cursor], 1u);
+            if (j < n_jobs && cancel_poll(p.cancel, CS_CONTOUR_LEAF, j)) j = ~0u;
+        }
+        j = __shfl_sync(FULL, j, 0);
+        if (j >= n_jobs) break;
+        const TileJob* job = p.jobs + j;
+        const uint32_t cx = job->x, cy = job->y;
+        const TapeRef tr = job->tape;
+        const float h = p.cell_h;
+        const float lo[2] = {float(cx) * h - 1.0f, float(cy) * h - 1.0f};
+        const float hi[2] = {float(cx + 1u) * h - 1.0f, float(cy + 1u) * h - 1.0f};
+        auto eval2 = [&](float x0, float y0, float x1, float y1) -> float2 {
+            float z0 = p.z, z1 = p.z;
+            if (p.has_transform) {
+                xform_f32(p.mat, x0, y0, z0, x0, y0, z0);
+                xform_f32(p.mat, x1, y1, z1, x1, y1, z1);
+            }
+            const float2 X = make_float2(x0, x1), Y = make_float2(y0, y1), Z = make_float2(z0, z1);
+            return run_f32x2(tr.ptr, tr.n_ops, slots, [&](uint32_t i) {
+                return pick_input(p.vb, i, X, Y, Z, [](float f) { return make_float2(f, f); });
+            });
+        };
+        const int c = lane & 3;
+        const float2 cv = eval2((c & 1) ? hi[0] : lo[0], (c & 2) ? hi[1] : lo[1], lo[0], lo[1]);
+        const uint32_t mask = __ballot_sync(FULL, cv.x < 0.0f) & 0xfu;
+        if (mask == 0u || mask == 15u) continue;
+        uint32_t slot = 0;
+        if (lane == 0) slot = atomicAdd(p.n_out, 1u);
+        slot = __shfl_sync(FULL, slot, 0);
+        if (slot >= p.cap_out) continue;   // counted: the host retries with the exact count
+        ContourLeaf* L = p.out + slot;
+        const int half = lane >> 4, jj = lane & 15;
+        EdgeState s0, s1;
+        const bool v0 = edge_setup2(uint32_t(half), mask, s0), v1 = edge_setup2(uint32_t(half) + 2u, mask, s1);
+        uint32_t present = 0;
+        for (uint32_t e = 0; e < 4u; ++e) {
+            EdgeState tmp;
+            if (edge_setup2(e, mask, tmp)) present |= 1u << e;
+        }
+        if (lane == 0) {
+            p.out_tapes[slot] = tr;
+            L->ix = uint16_t(cx); L->iy = uint16_t(cy);
+            L->mask = uint8_t(mask); L->present = uint8_t(present); L->pad = 0;
+        }
+        for (int round = 0; round < 4; ++round) {
+            uint32_t q0[2], q1[2];
+#pragma unroll
+            for (int a = 0; a < 2; ++a) {
+                q0[a] = (s0.s[a] * uint32_t(15 - jj) + s0.e[a] * uint32_t(jj)) / 15u;
+                q1[a] = (s1.s[a] * uint32_t(15 - jj) + s1.e[a] * uint32_t(jj)) / 15u;
+            }
+            const float2 v = eval2(lerp_u16(lo[0], hi[0], q0[0]), lerp_u16(lo[1], hi[1], q0[1]),
+                                   lerp_u16(lo[0], hi[0], q1[0]), lerp_u16(lo[1], hi[1], q1[1]));
+            const uint32_t b0 = (__ballot_sync(FULL, v.x >= 0.0f) >> (16 * half)) & 0xffffu;
+            const uint32_t b1 = (__ballot_sync(FULL, v.y >= 0.0f) >> (16 * half)) & 0xffffu;
+            auto narrow = [&](EdgeState& st, uint32_t bits) {
+                uint32_t frac = bits ? uint32_t(__ffs(bits) - 1) : 15u;
+                if (frac == 0u) frac = 1u;
+#pragma unroll
+                for (int a = 0; a < 2; ++a) {
+                    const uint32_t na = (st.s[a] * (16u - frac) + st.e[a] * (frac - 1u)) / 15u;
+                    const uint32_t nb = (st.s[a] * (15u - frac) + st.e[a] * frac) / 15u;
+                    st.s[a] = na & 0xffffu;
+                    st.e[a] = nb & 0xffffu;
+                }
+            };
+            narrow(s0, b0);
+            narrow(s1, b1);
+        }
+        if (jj == 0) {
+            if (v0) for (int a = 0; a < 2; ++a) L->pos[half][a] = lerp_u16(lo[a], hi[a], ((s0.s[a] + s0.e[a]) / 2u) & 0xffffu);
+            if (v1) for (int a = 0; a < 2; ++a) L->pos[half + 2][a] = lerp_u16(lo[a], hi[a], ((s1.s[a] + s1.e[a]) / 2u) & 0xffffu);
+        }
+    }
+}
+
+// Gradients at the intersections (as k_octree_grads, Z seeded at the slice): one warp per leaf, one lane per edge
+__global__ void __launch_bounds__(128) k_contour_grads(const __grid_constant__ ContourLeafParams p) {
+    grd slots[REG_SLOTS];
+    const int lane = threadIdx.x & 31;
+    const uint32_t warp = (blockIdx.x * blockDim.x + threadIdx.x) >> 5;
+    const uint32_t n_warps = (gridDim.x * blockDim.x) >> 5;
+    const uint32_t n = min(*p.n_out, p.cap_out);
+    for (uint32_t i = warp; i < n; i += n_warps) {
+        if (cancel_poll(p.cancel, CS_CONTOUR_GRADS, i)) break;   // (uniform over the warp)
+        ContourLeaf* L = p.out + i;
+        const TapeRef tr = p.out_tapes[i];
+        const uint32_t active = L->present;
+        const bool mine = lane < 4 && ((active >> lane) & 1u);
+        const int e = mine ? lane : (__ffs(active) - 1);
+        grd gx = gr(L->pos[e][0], 1.0f, 0.0f, 0.0f), gy = gr(L->pos[e][1], 0.0f, 1.0f, 0.0f), gz = gr(p.z, 0.0f, 0.0f, 1.0f);
+        if (p.has_transform) xform_gr(p.mat, gx, gy, gz, gx, gy, gz);
+        const grd r = run_grad(tr.ptr, tr.n_ops, slots, [&](uint32_t k) {
+            return pick_input(p.vb, k, gx, gy, gz, [](float f) { return gr1(f); });
+        });
+        if (mine) { L->grad[e][0] = r.y; L->grad[e][1] = r.z; L->grad[e][2] = r.x; }
+    }
+}
+
+// ---- QEF in 2D (QuadraticErrorSolver restricted to the plane) ---------------------------------------------------
+struct Qef2 { float ata[3], atb[2], btb, mp[3]; };   // ata = xx xy yy; mp = x, y, count
+
+__device__ inline void qef2_add_intersection(Qef2& q, const float p[2], const float g[3]) {
+    q.mp[0] += p[0]; q.mp[1] += p[1]; q.mp[2] += 1.0f;
+    const float nl = sqrtf(g[0] * g[0] + g[1] * g[1]);
+    const float n[2] = {g[0] / nl, g[1] / nl};
+    const float d = n[0] * p[0] + n[1] * p[1];
+    q.ata[0] += n[0] * n[0]; q.ata[1] += n[0] * n[1]; q.ata[2] += n[1] * n[1];
+    q.atb[0] += n[0] * d; q.atb[1] += n[1] * d;
+    q.btb += d * d;
+}
+
+// Symmetric 2x2 eigen-decomposition [[a, b], [b, c]] = V diag(w) V^T: one Jacobi rotation diagonalises it (the
+// rotation jacobi3 would apply to the pair, with the classic a - t b / c + t b update)
+__device__ inline void eigen2(float a, float b, float c, float w[2], float V[2][2]) {
+    if (fabsf(b) < 1e-37f) {
+        w[0] = a; w[1] = c;
+        V[0][0] = 1.0f; V[0][1] = 0.0f; V[1][0] = 0.0f; V[1][1] = 1.0f;
+        return;
+    }
+    const float theta = (c - a) / (2.0f * b);
+    const float t = (theta >= 0.0f ? 1.0f : -1.0f) / (fabsf(theta) + sqrtf(theta * theta + 1.0f));
+    const float cs = 1.0f / sqrtf(t * t + 1.0f), s = t * cs;
+    w[0] = a - t * b;
+    w[1] = c + t * b;
+    V[0][0] = cs; V[0][1] = s; V[1][0] = -s; V[1][1] = cs;
+}
+
+// QuadraticErrorSolver::solve in 2D: truncated pseudo-inverse about the mass point (relative cut-off 1e-3), the mass
+// point when the solve gives NaN
+__device__ inline void qef2_vertex(const Qef2& q, float pos[2]) {
+    const float ata[2][2] = {{q.ata[0], q.ata[1]}, {q.ata[1], q.ata[2]}};
+    const float center[2] = {q.mp[0] / q.mp[2], q.mp[1] / q.mp[2]};
+    float b[2];
+    for (int r = 0; r < 2; ++r) b[r] = q.atb[r] - (ata[r][0] * center[0] + ata[r][1] * center[1]);
+    float w[2], V[2][2];
+    eigen2(q.ata[0], q.ata[1], q.ata[2], w, V);
+    int order[2] = {0, 1};
+    if (fabsf(w[1]) > fabsf(w[0])) { order[0] = 1; order[1] = 0; }
+    const float cutoff = fabsf(w[order[0]]) * 1e-3f;
+    int rank = 2;
+    for (int k = 0; k < 2; ++k) if (fabsf(w[order[k]]) < cutoff) { rank = k; break; }
+    const float eps = rank < 2 ? fabsf(w[order[rank]]) : 0.0f;
+    float sol[2] = {0, 0};
+    for (int k = 0; k < 2; ++k) {
+        const int j = order[k];
+        if (!(fabsf(w[j]) > eps)) continue;
+        const float coef = (V[0][j] * b[0] + V[1][j] * b[1]) / w[j];
+        sol[0] += coef * V[0][j]; sol[1] += coef * V[1][j];
+    }
+    for (int r = 0; r < 2; ++r) pos[r] = sol[r] + center[r];
+    if (!(pos[0] == pos[0] && pos[1] == pos[1])) { pos[0] = center[0]; pos[1] = center[1]; }
+}
+
+// Connected groups of a 4-bit mask's inside corners along cell edges, numbered by their lowest corner: 2 bits per
+// corner, the group count in bits 8.. (two groups only for the diagonal masks 6 and 9)
+__device__ __forceinline__ uint32_t corner_groups2(uint32_t mask) {
+    if (mask == 6u) return (1u << 4) | (2u << 8);          // corners 1, 2
+    if (mask == 9u) return (1u << 6) | (2u << 8);          // corners 0, 3
+    return (mask == 0u ? 0u : 1u) << 8;
+}
+__device__ __forceinline__ uint32_t group_of(uint32_t packed, uint32_t corner) { return (packed >> (2u * corner)) & 3u; }
+
+__device__ __forceinline__ uint32_t leaf_key(const ContourLeaf& L) { return (uint32_t(L.iy) << 16) | L.ix; }
+
+struct ContourScratch {
+    const ContourLeaf* leaves;
+    uint32_t n_leaves, side;        // side: cells per axis
+    const uint32_t* keys;           // sorted leaf keys
+    const uint32_t* order;          // leaf index of each sorted position
+    uint32_t* packed;               // per sorted position: corner groups (corner_groups2)
+    uint32_t* n_groups;
+    const uint32_t* vbase;          // exclusive scan of n_groups: first vertex of each sorted position
+    float2* vpos;                   // [vertex] world position
+    uint32_t* next;
+    uint32_t* prev;
+    uint32_t* counts;               // [0] vertices [1] polylines [2] closed [3] open edges
+    CancelRef cancel;
+};
+
+__global__ void k_contour_keys(const ContourLeaf* leaves, uint32_t n, uint32_t* keys, uint32_t* idx) {
+    const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= n) return;
+    keys[i] = leaf_key(leaves[i]);
+    idx[i] = i;
+}
+
+__global__ void k_contour_groups(ContourScratch m) {
+    if (cancel_poll(m.cancel, CS_CONTOUR_VERTICES, blockIdx.x)) return;
+    const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= m.n_leaves) return;
+    const uint32_t packed = corner_groups2(m.leaves[m.order[i]].mask);
+    m.packed[i] = packed;
+    m.n_groups[i] = packed >> 8;
+}
+
+// One thread per sorted leaf: a QEF vertex per group; intersections enter in corner order, X-neighbour then Y
+__global__ void __launch_bounds__(128) k_contour_vertices(ContourScratch m) {
+    if (cancel_poll(m.cancel, CS_CONTOUR_VERTICES, blockIdx.x)) return;
+    const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= m.n_leaves) return;
+    const ContourLeaf& L = m.leaves[m.order[i]];
+    const uint32_t mask = L.mask, packed = m.packed[i], ng = packed >> 8, base = m.vbase[i];
+    if (i == m.n_leaves - 1u) m.counts[0] = base + ng;
+    for (uint32_t g = 0; g < ng; ++g) {
+        Qef2 q{};
+        bool forced = false;
+        float pos[2];
+        for (uint32_t s = 0; s < 4 && !forced; ++s) {
+            if (!((mask >> s) & 1u) || group_of(packed, s) != g) continue;
+            for (uint32_t t = 1; t < 4; t <<= 1) {
+                if ((mask >> (s ^ t)) & 1u) continue;   // not a transition
+                const uint32_t e = t == 1u ? ((s >> 1) & 1u) : 2u + (s & 1u);
+                const float p[2] = {L.pos[e][0], L.pos[e][1]};
+                const float gr3[3] = {L.grad[e][0], L.grad[e][1], L.grad[e][2]};
+                if (gr3[0] != gr3[0] || gr3[1] != gr3[1] || gr3[2] != gr3[2]) {   // a NaN gradient snaps to the intersection
+                    forced = true;
+                    pos[0] = p[0]; pos[1] = p[1];
+                    break;
+                }
+                qef2_add_intersection(q, p, gr3);
+            }
+        }
+        if (!forced) qef2_vertex(q, pos);
+        m.vpos[base + g] = make_float2(pos[0], pos[1]);
+    }
+}
+
+__device__ __forceinline__ uint32_t find_leaf(const ContourScratch& m, uint32_t key) {
+    uint32_t lo = 0, hi = m.n_leaves;
+    while (lo < hi) {
+        const uint32_t mid = (lo + hi) >> 1;
+        if (m.keys[mid] < key) lo = mid + 1u; else hi = mid;
+    }
+    return lo < m.n_leaves && m.keys[lo] == key ? lo : NONE;
+}
+
+// One thread per sorted leaf: its boundary edges are counted, its -X and -Y edges linked to the neighbours' vertices
+__global__ void __launch_bounds__(128) k_contour_segments(ContourScratch m) {
+    if (cancel_poll(m.cancel, CS_CONTOUR_SEGMENTS, blockIdx.x)) return;
+    const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= m.n_leaves) return;
+    const ContourLeaf& L = m.leaves[m.order[i]];
+    const uint32_t mask = L.mask, x = L.ix, y = L.iy, packed = m.packed[i], base = m.vbase[i];
+    auto in = [](uint32_t mk, uint32_t c) { return (mk >> c) & 1u; };
+    uint32_t open = 0;
+    if (x + 1u == m.side && in(mask, 1) != in(mask, 3)) ++open;
+    if (y + 1u == m.side && in(mask, 2) != in(mask, 3)) ++open;
+    // a: this cell's corners on the shared edge (low, high), b: the neighbour's; the neighbour is -X (d = 0) or -Y (d = 1)
+    const uint32_t ca[2][2] = {{0u, 2u}, {0u, 1u}}, cb[2][2] = {{1u, 3u}, {2u, 3u}};
+    for (uint32_t d = 0; d < 2; ++d) {
+        const uint32_t a0 = ca[d][0], a1 = ca[d][1];
+        if (in(mask, a0) == in(mask, a1)) continue;
+        if ((d == 0 ? x : y) == 0u) { ++open; continue; }
+        const uint32_t j = find_leaf(m, d == 0 ? ((y << 16) | (x - 1u)) : (((y - 1u) << 16) | x));
+        const uint32_t mj = j == NONE ? 0u : m.leaves[m.order[j]].mask;
+        if (j == NONE || in(mj, cb[d][0]) != in(mask, a0) || in(mj, cb[d][1]) != in(mask, a1)) { ++open; continue; }
+        // inside on the left: across a -X edge the path runs +X when the upper corner is inside; across a -Y edge it
+        // runs +Y when the left corner is inside
+        const bool up = d == 0 ? in(mask, a1) != 0u : in(mask, a0) != 0u;
+        const uint32_t ka = up ? (d == 0 ? a1 : a0) : (d == 0 ? a0 : a1);
+        const uint32_t kb = up ? (d == 0 ? cb[d][1] : cb[d][0]) : (d == 0 ? cb[d][0] : cb[d][1]);
+        const uint32_t va = base + group_of(packed, ka), vb = m.vbase[j] + group_of(m.packed[j], kb);
+        const uint32_t from = up ? vb : va, to = up ? va : vb;
+        m.next[from] = to;
+        m.prev[to] = from;
+    }
+    if (open) atomicAdd(&m.counts[3], open);
+}
+
+// List ranking by pointer jumping, one launch per round (ping-pong buffers).  After k rounds of pass 1, P[v] is the
+// vertex 2^k steps back (NONE past an open start) and A[v] the smallest vertex among the 2^k before and including v:
+// once 2^k reaches the vertex count, vertices with P[v] != NONE lie on cycles and A[v] is their cycle's minimum.  Pass 2
+// runs on prev[] with every cycle cut at that minimum: A[v] becomes the head 2^k - 1 steps back (or the polyline's
+// start) and R[v] the distance to it, capped at 2^k.
+struct LinkBufs { uint32_t *P[2], *A[2], *R[2]; uint8_t* closed; uint32_t* len; unsigned long long* scan; };
+
+template <int PASS>
+__global__ void k_link_init(ContourScratch m, LinkBufs b) {
+    if (cancel_poll(m.cancel, CS_CONTOUR_LINK, blockIdx.x)) return;
+    const uint32_t v = blockIdx.x * blockDim.x + threadIdx.x;
+    if (v >= m.counts[0]) return;
+    if (PASS == 1) {
+        b.P[0][v] = m.prev[v];
+        b.A[0][v] = v;
+    } else {   // (reads pass 1's final buffers, index 0 or 1 as the host passes them in P[1] / A[1])
+        const bool cyc = b.P[1][v] != NONE;
+        const uint32_t p = cyc && b.A[1][v] == v ? NONE : m.prev[v];
+        b.closed[v] = cyc;
+        b.P[0][v] = p;
+        b.A[0][v] = v;
+        b.R[0][v] = p != NONE;
+    }
+}
+template <int PASS>
+__global__ void k_link_round(ContourScratch m, LinkBufs b) {
+    if (cancel_poll(m.cancel, CS_CONTOUR_LINK, blockIdx.x)) return;
+    const uint32_t v = blockIdx.x * blockDim.x + threadIdx.x;
+    if (v >= m.counts[0]) return;
+    const uint32_t p = b.P[0][v];
+    if (p == NONE) {
+        b.P[1][v] = NONE;
+        b.A[1][v] = b.A[0][v];
+        if (PASS == 2) b.R[1][v] = b.R[0][v];
+        return;
+    }
+    b.P[1][v] = b.P[0][p];
+    if (PASS == 1) b.A[1][v] = min(b.A[0][v], b.A[0][p]);
+    else {
+        b.A[1][v] = b.A[0][p];
+        b.R[1][v] = b.R[0][v] + b.R[0][p];
+    }
+}
+// The last vertex of each polyline (no successor, or its head) writes the polyline's length at the head
+__global__ void k_link_lengths(ContourScratch m, LinkBufs b) {
+    if (cancel_poll(m.cancel, CS_CONTOUR_LINK, blockIdx.x)) return;
+    const uint32_t v = blockIdx.x * blockDim.x + threadIdx.x;
+    if (v >= m.counts[0]) return;
+    const uint32_t h = b.A[0][v], n = m.next[v];
+    if (n == NONE || n == h) b.len[h] = b.R[0][v] + 1u;
+}
+__global__ void k_link_heads(ContourScratch m, LinkBufs b, uint32_t cap) {
+    const uint32_t v = blockIdx.x * blockDim.x + threadIdx.x;
+    if (v >= cap) return;
+    b.scan[v] = v < m.counts[0] && b.A[0][v] == v ? (1ull << 32) | b.len[v] : 0ull;
+}
+
+// Every vertex to its place (head's offset + rank), in model space when `to_model`; heads write their polyline's record
+__global__ void k_contour_emit(ContourScratch m, LinkBufs b, const unsigned long long* scan, float2* out_v,
+                               uint32_t* out_off, uint8_t* out_closed, bool to_model, Mat4 M, float z) {
+    if (cancel_poll(m.cancel, CS_CONTOUR_EMIT, blockIdx.x)) return;
+    const uint32_t v = blockIdx.x * blockDim.x + threadIdx.x;
+    const uint32_t nv = m.counts[0];
+    if (v >= nv) return;
+    const uint32_t h = b.A[0][v];
+    float2 q = m.vpos[v];
+    if (to_model) {
+        float zz = z;
+        xform_f32(M, q.x, q.y, zz, q.x, q.y, zz);
+    }
+    out_v[uint32_t(scan[h]) + b.R[0][v]] = q;
+    if (h == v) {
+        const uint32_t k = uint32_t(scan[v] >> 32);
+        out_off[k] = uint32_t(scan[v]);
+        out_closed[k] = b.closed[v];
+        if (b.closed[v]) atomicAdd(&m.counts[2], 1u);
+    }
+    if (v == nv - 1u) {
+        const uint32_t n_poly = uint32_t(scan[v] >> 32) + (h == v ? 1u : 0u);
+        m.counts[1] = n_poly;
+        out_off[n_poly] = nv;
+    }
+}
+
+}  // namespace fdev
+
+// The quadtree sampler: interval levels, then the leaf and gradient kernels; *n_out = surface leaves found (more than
+// cap: FC_ERR_INVALID, nothing beyond cap written)
+static int32_t contour_sample(fc_ctx* c, const fc_tape* tape, const fc_contour_cfg* cfg, const VarBind& vb,
+                              const fdev::Mat4& mat, fdev::ContourLeaf* dout, uint64_t cap, uint32_t* n_out_p,
+                              const CallCancel& cc) {
+    using namespace fdev;
+    const uint32_t D = cfg->depth;
+    const int L = int(D) + 1;
+    cudaStream_t s = c->stream;
+    const int grid_blocks = c->sm_count * env_int("FIDGET_B200_BLOCKS_PER_SM", 6);
+    const uint32_t choice_words = (tape->info.choice_count + 15) / 16 + 1;
+    CU(c->choice_scratch.ensure(size_t(grid_blocks) * WARPS_PER_BLOCK * choice_words * 32 * 4));
+    CU(c->arena.ensure(c->arena_bytes));
+    CU(c->counters.ensure(sizeof(Counters) + 64));
+    CU(c->stats.ensure(sizeof(Stats)));
+    const uint64_t cap_limit = uint64_t(env_int("FIDGET_B200_MAX_TILES_M", 16)) << 20;
+    std::vector<uint64_t> level_cap(L + 1);
+    for (int l = 1; l <= L; ++l) {
+        level_cap[l] = std::min<uint64_t>(1ull << (2 * std::min(l, int(D))), cap_limit);
+        CU(c->jobs[l].ensure(level_cap[l] * sizeof(TileJob)));
+    }
+    CU(c->leaf_tapes.ensure(std::max<uint64_t>(cap, 1) * sizeof(TapeRef)));
+    CU(cudaMemsetAsync(c->counters.p, 0, sizeof(Counters) + 64, s));
+    uint32_t* d_n_out = reinterpret_cast<uint32_t*>(c->counters.as<char>() + sizeof(Counters));
+    for (int l = 0; l < L; ++l) {
+        LevelParams p{};
+        p.level = l;
+        p.tile = 1u << (D - uint32_t(l));
+        p.n_axis = l ? 2 : 0;
+        p.is_last = (l == L - 1);
+        p.root_mode = (l == 0);
+        p.roots_x = p.roots_y = p.roots_z = 1;
+        p.root_tape.ptr = tape->dev;
+        p.root_tape.n_ops = tape->info.n_ops;
+        p.root_tape.ref_len = tape->info.ref_len;
+        p.root_tape.n_choices = tape->info.choice_count;
+        p.width = p.height = 1u << D;
+        p.depth = 1;
+        p.z2d = cfg->z;
+        p.mat = mat;
+        p.jobs_in = l ? c->jobs[l].as<TileJob>() : nullptr;
+        p.cap_in = l ? uint32_t(level_cap[l]) : 0;
+        p.jobs_out = c->jobs[l + 1].as<TileJob>();
+        p.cap_out = uint32_t(level_cap[l + 1]);
+        p.arena = c->arena.as<uint2>();
+        p.arena_cap = std::min<uint64_t>(c->arena.cap, c->arena_bytes) / sizeof(uint2);
+        p.choice_scratch = c->choice_scratch.as<uint32_t>();
+        p.choice_words = choice_words;
+        p.ctr = c->counters.as<Counters>();
+        p.mode = 1;
+        p.has_transform = cfg->has_transform;
+        p.cell_h = 2.0f / float(1u << D);
+        p.vb = vb;
+        p.cancel = cc.ref;
+        const uint64_t warps = l ? std::max<uint64_t>(1, (1ull << (2 * l)) / 4) : 1;
+        const int blocks = int(std::min<uint64_t>((warps + WARPS_PER_BLOCK - 1) / WARPS_PER_BLOCK, uint64_t(grid_blocks)));
+        k_contour_level<<<std::max(blocks, 1), WARPS_PER_BLOCK * 32, 0, s>>>(p);
+    }
+    ContourLeafParams q{};
+    q.jobs = c->jobs[L].as<TileJob>();
+    q.cap_jobs = uint32_t(level_cap[L]);
+    q.ctr = c->counters.as<Counters>();
+    q.list = L; q.cursor = L;
+    q.cell_h = 2.0f / float(1u << D);
+    q.z = cfg->z;
+    q.has_transform = cfg->has_transform;
+    q.mat = mat;
+    q.vb = vb;
+    q.out = dout;
+    q.out_tapes = c->leaf_tapes.as<TapeRef>();
+    q.cap_out = uint32_t(cap);
+    q.n_out = d_n_out;
+    q.cancel = cc.ref;
+    k_contour_leaf<<<c->sm_count * 8, 128, 0, s>>>(q);
+    k_contour_grads<<<c->sm_count * 8, 128, 0, s>>>(q);
+    CU(cudaGetLastError());
+    uint32_t n_out = 0;
+    if (int32_t wrc = wait_read(c, s, cc, &n_out, d_n_out, 4)) return wrc;
+    *n_out_p = n_out;
+    if (int32_t rc = check_device_errors(c)) return rc;
+    if (n_out > cap) return fail(FC_ERR_INVALID, "contour leaf buffer too small: " + std::to_string(n_out) + " surface leaves");
+    return FC_OK;
+}
+
+// Vertices, segments, linking and the polylines, from n surface leaves in contour_leaves
+static int32_t contour_finish(fc_ctx* c, uint32_t n, const fc_contour_cfg* cfg, const fdev::Mat4& mat, bool to_model,
+                              fc_contour_info* info, const CallCancel& cc) {
+    using namespace fdev;
+    cudaStream_t s = c->stream;
+    const uint32_t V = 2u * n;   // at most two vertices per leaf
+    ContourScratch m{};
+    m.leaves = c->contour_leaves.as<ContourLeaf>();
+    m.n_leaves = n;
+    m.side = 1u << cfg->depth;
+    m.cancel = cc.ref;
+    LinkBufs b{};
+    uint32_t *keys_in, *idx_in, *keys, *order, *vbase;
+    unsigned long long* scan_out;
+    size_t t_sort = 0, t_scan32 = 0, t_scan64 = 0;
+    CU(cub::DeviceRadixSort::SortPairs(nullptr, t_sort, (uint32_t*)nullptr, (uint32_t*)nullptr, (uint32_t*)nullptr,
+                                       (uint32_t*)nullptr, int(n), 0, 32, s));
+    CU(cub::DeviceScan::ExclusiveSum(nullptr, t_scan32, (uint32_t*)nullptr, (uint32_t*)nullptr, int(n), s));
+    CU(cub::DeviceScan::ExclusiveSum(nullptr, t_scan64, (unsigned long long*)nullptr, (unsigned long long*)nullptr, int(V), s));
+    const size_t t_cub = std::max(t_sort, std::max(t_scan32, t_scan64));
+    void* cub_tmp;
+    const size_t w = size_t(n) * 4, wv = size_t(V) * 4;
+    CU(carve(c->contour_scratch, [&](Carve& cv) {
+        cv.take(keys_in, w); cv.take(idx_in, w); cv.take(keys, w); cv.take(order, w);
+        cv.take(m.packed, w); cv.take(m.n_groups, w); cv.take(vbase, w);
+        cv.take(m.vpos, size_t(V) * sizeof(float2));
+        cv.take(m.next, wv); cv.take(m.prev, wv);
+        for (int k = 0; k < 2; ++k) { cv.take(b.P[k], wv); cv.take(b.A[k], wv); cv.take(b.R[k], wv); }
+        cv.take(b.closed, V); cv.take(b.len, wv);
+        cv.take(b.scan, size_t(V) * 8); cv.take(scan_out, size_t(V) * 8);
+        cv.take(m.counts, 64);
+        cv.take(cub_tmp, t_cub);
+    }));
+    float2* out_v;
+    uint32_t* out_off;
+    uint8_t* out_closed;
+    CU(carve(c->contour_out, [&](Carve& cv) {
+        cv.take(out_v, size_t(V) * sizeof(float2)); cv.take(out_off, size_t(V + 1) * 4); cv.take(out_closed, V);
+    }));
+    c->contour_offsets = out_off;
+    c->contour_closed = out_closed;
+    m.keys = keys;
+    m.order = order;
+    m.vbase = vbase;
+    CU(cudaEventRecord(get_event(c, 2), s));
+    CU(cudaMemsetAsync(m.counts, 0, 64, s));
+    CU(cudaMemsetAsync(m.next, 0xff, wv, s));
+    CU(cudaMemsetAsync(m.prev, 0xff, wv, s));
+    const unsigned bl = (n + 127) / 128, bv = (V + 127) / 128;
+    k_contour_keys<<<bl, 128, 0, s>>>(m.leaves, n, keys_in, idx_in);
+    size_t t = t_cub;
+    CU(cub::DeviceRadixSort::SortPairs(cub_tmp, t, keys_in, keys, idx_in, order, int(n), 0, 32, s));
+    k_contour_groups<<<bl, 128, 0, s>>>(m);
+    t = t_cub;
+    CU(cub::DeviceScan::ExclusiveSum(cub_tmp, t, m.n_groups, vbase, int(n), s));
+    k_contour_vertices<<<bl, 128, 0, s>>>(m);
+    k_contour_segments<<<bl, 128, 0, s>>>(m);
+    // rounds: 2^K >= V covers every cycle and every distance to an open start
+    int K = 1;
+    while ((1ull << K) < V) ++K;
+    auto flip = [](LinkBufs x) { std::swap(x.P[0], x.P[1]); std::swap(x.A[0], x.A[1]); std::swap(x.R[0], x.R[1]); return x; };
+    k_link_init<1><<<bv, 128, 0, s>>>(m, b);
+    for (int r = 0; r < K; ++r) { k_link_round<1><<<bv, 128, 0, s>>>(m, b); b = flip(b); }
+    b = flip(b);   // pass 1's result, now in [1], is what k_link_init<2> reads; it writes [0]
+    k_link_init<2><<<bv, 128, 0, s>>>(m, b);
+    for (int r = 0; r < K; ++r) { k_link_round<2><<<bv, 128, 0, s>>>(m, b); b = flip(b); }
+    k_link_lengths<<<bv, 128, 0, s>>>(m, b);
+    k_link_heads<<<bv, 128, 0, s>>>(m, b, V);
+    t = t_cub;
+    CU(cub::DeviceScan::ExclusiveSum(cub_tmp, t, b.scan, scan_out, int(V), s));
+    k_contour_emit<<<bv, 128, 0, s>>>(m, b, scan_out, out_v, out_off, out_closed, to_model, mat, cfg->z);
+    cudaEvent_t e3 = get_event(c, 3);
+    CU(cudaEventRecord(e3, s));
+    CU(cudaGetLastError());
+    uint32_t cnt[4];
+    if (int32_t wrc = wait_read(c, s, cc, cnt, m.counts, sizeof cnt)) return wrc;
+    c->contour_n_verts = cnt[0];
+    c->contour_n_polys = cnt[1];
+    info->n_vertices = cnt[0];
+    info->n_polylines = cnt[1];
+    info->n_closed = cnt[2];
+    info->n_open = cnt[3];
+    if (cfg->flags & FC_FLAG_TIMING) cudaEventElapsedTime(&info->contour_ms, get_event(c, 2), e3);
+    return FC_OK;
+}
+
+extern "C" {
+
+int32_t fc_contour_build(fc_ctx* c, const fc_tape* tape, const fc_contour_cfg* cfg, fc_contour_info* info) {
+    if (!c || !tape || !cfg || !info) return fail(FC_ERR_INVALID, "null argument");
+    memset(info, 0, sizeof *info);
+    if (cfg->depth > FC_MAX_QUADTREE_DEPTH) return fail(FC_ERR_INVALID, "quadtree depth too large");
+    if (cfg->n_var_values > FC_MAX_VARS) return fail(FC_ERR_INVALID, "too many variable values");
+    if (tape->info.mem_count) return fail(FC_ERR_UNSUPPORTED, "contours need a tape without memory spills");
+    if (tape->info.n_outputs != 1) return fail(FC_ERR_INVALID, "ShapeTape has multiple outputs");
+    VarBind vb;
+    if (int32_t vrc = bind_vars(tape, cfg->var_values, cfg->n_var_values, vb)) return vrc;
+    CallCancel cc;
+    auto no_contour = [&](int32_t rc) {   // a cancelled build leaves no contour (a failed one keeps the previous)
+        std::lock_guard<std::mutex> guard(c->mu);
+        c->contour_n_verts = c->contour_n_polys = 0;
+        memset(info, 0, sizeof *info);
+        return rc;
+    };
+    if (int32_t crc = begin_call(c, cc)) return crc == FC_ERR_CANCELLED ? no_contour(crc) : crc;
+    // the 3x3 embedded as the 2D renderers embed it: (x, y, z, 1) -> (m0 x + m1 y + m2, m3 x + m4 y + m5, z, m6 x + m7 y + m8)
+    fdev::Mat4 mat{};
+    bool to_model = false;
+    const int idx[3] = {0, 1, 3};
+    for (int i = 0; i < 3; ++i)
+        for (int j = 0; j < 3; ++j) {
+            const float v = cfg->has_transform ? cfg->world_to_model[3 * i + j] : (i == j ? 1.0f : 0.0f);
+            mat.m[4 * idx[i] + idx[j]] = v;
+            to_model |= v != (i == j ? 1.0f : 0.0f);
+        }
+    mat.m[10] = 1.0f;
+    std::unique_lock<std::mutex> guard(c->mu);
+    CU(cudaSetDevice(c->device));
+    const bool timing = cfg->flags & FC_FLAG_TIMING;
+    // leaves: sized as fc_mesh_build sizes its own (the buffer of the last build, else the perimeter of the square in
+    // cells), and once more with the exact count
+    uint64_t cap = c->contour_leaves.cap / sizeof(fdev::ContourLeaf);
+    if (cap < 1024) cap = std::max<uint64_t>(1024, std::min<uint64_t>(1ull << (2 * cfg->depth), 8ull << cfg->depth));
+    uint32_t n = 0;
+    c->contour_n_verts = c->contour_n_polys = 0;
+    int32_t rc = FC_OK;
+    for (int attempt = 0; attempt < 2; ++attempt) {
+        CU(c->contour_leaves.ensure(cap * sizeof(fdev::ContourLeaf)));
+        if (timing) CU(cudaEventRecord(get_event(c, 0), c->stream));
+        rc = contour_sample(c, tape, cfg, vb, mat, c->contour_leaves.as<fdev::ContourLeaf>(), cap, &n, cc);
+        if (rc == FC_OK || rc == FC_ERR_CANCELLED) break;
+        if (n > cap && attempt == 0) { cap = n; continue; }
+        break;
+    }
+    if (rc == FC_OK && timing) {
+        CU(cudaEventRecord(get_event(c, 1), c->stream));
+        CU(cudaEventSynchronize(get_event(c, 1)));
+        cudaEventElapsedTime(&info->sampler_ms, get_event(c, 0), get_event(c, 1));
+    }
+    info->n_leaves = n;
+    if (rc == FC_OK && n) rc = contour_finish(c, n, cfg, mat, cfg->has_transform && to_model, info, cc);
+    guard.unlock();
+    return rc == FC_ERR_CANCELLED ? no_contour(rc) : rc;
+}
+
+int32_t fc_contour_read(fc_ctx* c, float* vertices, uint32_t* offsets, uint8_t* closed) {
+    if (!c) return fail(FC_ERR_INVALID, "null ctx");
+    std::lock_guard<std::mutex> guard(c->mu);
+    CU(cudaSetDevice(c->device));
+    const uint32_t nv = c->contour_n_verts, np = c->contour_n_polys;
+    static const uint32_t zero = 0;
+    if (vertices && nv) CU(cudaMemcpyAsync(vertices, c->contour_out.p, size_t(nv) * 8, cudaMemcpyDefault, c->stream));
+    if (offsets) CU(cudaMemcpyAsync(offsets, np ? c->contour_offsets : &zero, size_t(np + 1) * 4, cudaMemcpyDefault, c->stream));
+    if (closed && np) CU(cudaMemcpyAsync(closed, c->contour_closed, np, cudaMemcpyDefault, c->stream));
+    CU(cudaStreamSynchronize(c->stream));
+    return FC_OK;
+}
+
+}  // extern "C"

@@ -19,6 +19,15 @@ __device__ __forceinline__ uint32_t lanemask_lt() {
     return m;
 }
 
+// The edge searches of the octree and quadtree samplers: a point of a cell as u16 fractions of its bounds, and one
+// edge's bracket (start = inside end, end = outside end), per axis
+__device__ __forceinline__ float lerp_u16(float lo, float hi, uint32_t p) {
+    const float frac = float(p) / 65535.0f;   // CellBounds::pos (cell.rs:183-192), Interval::lerp
+    return lo * (1.0f - frac) + hi * frac;
+}
+
+struct EdgeState { uint32_t s[3], e[3]; };
+
 // INPUT clause -> value: the axes get coordinates, other slots their bound value
 template <class T, class F>
 __device__ __forceinline__ T pick_input(const VarBind& vb, uint32_t i, T X, T Y, T Z, F from_float) {

@@ -25,6 +25,7 @@ enum CancelSite : int32_t {
     CS_TREE_PARENTS, CS_TREE_COLLAPSE, CS_TREE_FINAL, CS_TREE_FACES0, CS_TREE_FACES1,
     CS_WAIT,                                              // polls inside spin waits: not a claim, never a trigger site
     CS_SCENE2D_RESOLVE,                                   // (after CS_WAIT: the ids the kernels above compare stay put)
+    CS_CONTOUR_LEAF, CS_CONTOUR_GRADS, CS_CONTOUR_VERTICES, CS_CONTOUR_SEGMENTS, CS_CONTOUR_LINK, CS_CONTOUR_EMIT,
     CS_COUNT
 };
 struct CancelRef {

@@ -42,7 +42,9 @@ __device__ __forceinline__ void store_fill(FillRec* dst, const FillRec& fr) {
     *reinterpret_cast<uint4*>(dst) = make_uint4(fr.x, fr.y, fr.value, fr.ready);
 }
 
-template <int DIM, bool FUSED, bool FRAMES = false, bool SCENE = false>
+// QUAD (2D only): the quadtree of fc_contour_build.  Coordinates are cells at the finest depth with world-square bounds
+// coord * cell_h - 1, seen through `mat` when has_transform, at Z = [z2d, z2d]; classified tiles are dropped (no fills).
+template <int DIM, bool FUSED, bool FRAMES = false, bool SCENE = false, bool QUAD = false>
 __device__ __forceinline__ void level_job(const LevelParams& p, uint32_t j, uint32_t n_roots, itv* slots, uint32_t* cs,
                                           uint32_t (*live)[32], int lane, uint32_t epoch) {
     const uint32_t T = p.tile;
@@ -118,6 +120,12 @@ __device__ __forceinline__ void level_job(const LevelParams& p, uint32_t j, uint
             Z = iv(float(cz) * h - 1.0f, float(cz + T) * h - 1.0f);
             if (p.has_transform) xform_iv(p.mat, X, Y, Z, vx, vy, vz);
             else { vx = X; vy = Y; vz = Z; }
+        } else if constexpr (QUAD) {
+            const float h = p.cell_h;
+            X = iv(float(cx) * h - 1.0f, float(cx + T) * h - 1.0f);
+            Y = iv(float(cy) * h - 1.0f, float(cy + T) * h - 1.0f);
+            if (p.has_transform) xform_iv(p.mat, X, Y, Z, vx, vy, vz);
+            else { vx = X; vy = Y; vz = Z; }
         } else {
             xform_iv(M, X, Y, Z, vx, vy, vz);
         }
@@ -188,7 +196,7 @@ __device__ __forceinline__ void level_job(const LevelParams& p, uint32_t j, uint
                     scene2d_cover(cover_out, p.occl_w, p.occl_h, p.cull, __shfl_sync(FULL, cx, src),
                                   __shfl_sync(FULL, cy, src), T, __shfl_sync(FULL, pl, src), lane, 32u);
                 }
-            } else {
+            } else if constexpr (!QUAD) {
                 uint32_t m = __ballot_sync(FULL, fill_in || fill_out);
                 if (m) {
                     uint32_t base = 0;

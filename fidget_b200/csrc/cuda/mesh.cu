@@ -683,24 +683,6 @@ __global__ void __launch_bounds__(128) k_tree_faces(MeshScratch m) {
 int32_t octree_sample_device(fc_ctx* c, const fc_tape* tape, const fc_octree_cfg* cfg, OctreeLeaf* dout, uint64_t cap,
                              uint32_t* n_out, fc_octree_stats* stats, const CallCancel& cc);
 
-// Consecutive 256-byte-aligned arrays of one device buffer: take() points each at its place
-struct Carve {
-    char* base;
-    size_t used = 0;
-    template <class T> void take(T*& p, size_t bytes) {
-        p = base ? reinterpret_cast<T*>(base + used) : nullptr;
-        used += (bytes + 255) & ~size_t(255);
-    }
-};
-// Grows `buf` to the arrays lay_out(Carve&) takes, then points them into it
-template <class F> static cudaError_t carve(DevBuf& buf, F lay_out) {
-    Carve size{nullptr};
-    lay_out(size);
-    if (cudaError_t e = buf.ensure(size.used)) return e;
-    Carve at{buf.as<char>()};
-    lay_out(at);
-    return cudaSuccess;
-}
 
 // The uniform mesh up to pass 0 of its face kernel (m: the surface leaves)
 static int32_t mesh_enqueue_uniform(fc_ctx* c, fdev::MeshScratch& m) {

@@ -9,13 +9,6 @@
 // edges (two half-warps x two points per lane), `frac` comes from a ballot.
 namespace fdev {
 
-__device__ __forceinline__ float lerp_u16(float lo, float hi, uint32_t p) {
-    const float frac = float(p) / 65535.0f;   // CellBounds::pos (cell.rs:183-192), Interval::lerp
-    return lo * (1.0f - frac) + hi * frac;
-}
-
-struct EdgeState { uint32_t s[3], e[3]; };
-
 // Edge `index` (= 4 t + 2 [start & v] + [start & u], types.rs:208-219) of a cell with corner `mask`
 __device__ __forceinline__ bool edge_setup(uint32_t index, uint32_t mask, EdgeState& st) {
     const uint32_t t = index >> 2, su = index & 1u, sv = (index >> 1) & 1u;

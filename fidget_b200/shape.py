@@ -991,6 +991,59 @@ def mesh_cells(cuda) -> np.ndarray:
 
 
 # ---------------------------------------------------------------------------
+# 2D contours (libfive's Contours::render): fc_contour_build / fc_contour_read
+def contour(shape: CudaShape, depth: int, z: float = 0.0, world_to_model=None, var_values=(),
+            cancel: CancelToken | None = None):
+    """Contours of the shape's Z slice over the [-1, 1]^2 world square, by dual contouring on a uniform quadtree of
+    ``depth`` (fc_contour_build): returns ``(vertices [n,2] float32, offsets [k+1] uint32, closed [k] bool, info dict)``,
+    polyline i being ``vertices[offsets[i]:offsets[i + 1]]``.  Inside regions lie on the left of the direction of travel
+    (counter-clockwise, y up) in the world square; a mirroring ``world_to_model`` (3x3, world -> model, as the 2D
+    renderers take it) reverses it in model space.  The order is canonical, so two builds give the same arrays.  None
+    when ``cancel`` cancelled the build (the context then holds no contour)."""
+    lib = shape._lib
+    c = _lib.FcContourCfg()
+    c.depth = depth
+    c.z = z
+    if world_to_model is not None:
+        c.has_transform = 1
+        c.world_to_model[:] = np.ascontiguousarray(world_to_model, dtype=np.float32).reshape(9).tolist()
+    c.flags = _lib.FC_FLAG_TIMING
+    c.n_var_values = len(var_values)          # (more than FC_MAX_VARS is refused by the library)
+    for i, v in enumerate(var_values[:_lib.FC_MAX_VARS]):
+        c.var_values[i] = float(v)
+    info = _lib.FcContourInfo()
+    rc = shape.cuda._cancellable(cancel, lambda: lib.fc_contour_build(shape.cuda._h, shape._h, C.byref(c), C.byref(info)))
+    if rc == _lib.FC_ERR_CANCELLED:
+        return None
+    _ck(rc)
+    verts = np.zeros((info.n_vertices, 2), dtype=np.float32)
+    offsets = np.zeros(info.n_polylines + 1, dtype=np.uint32)
+    closed = np.zeros(info.n_polylines, dtype=np.uint8)
+    _ck(lib.fc_contour_read(shape.cuda._h, _ptr(verts), _ptr(offsets), _ptr(closed)))
+    return verts, offsets, closed.astype(bool), {n: getattr(info, n) for n, _ in info._fields_}
+
+
+def contours_svg(vertices, offsets, closed, size: float = 512.0, stroke: str = "black", fill: str = "none",
+                 stroke_width: float = 1.0) -> str:
+    """An SVG document with one ``<path>`` per polyline of ``contour``'s output, closed ones ending in ``Z``.  The
+    view box is the [-1, 1]^2 square (``size`` pixels wide), y flipped to SVG's y-down frame.  Paths use
+    ``fill-rule="nonzero"``: the contours' consistent orientation makes a hole wind opposite to its outline."""
+    v = np.asarray(vertices, dtype=np.float32).reshape(-1, 2)
+    off = np.asarray(offsets, dtype=np.int64)
+    cl = np.asarray(closed, dtype=bool)
+    out = [f'<svg xmlns="http://www.w3.org/2000/svg" width="{size:g}" height="{size:g}" viewBox="-1 -1 2 2">']
+    for k in range(len(off) - 1):
+        pts = v[off[k]:off[k + 1]]
+        d = " ".join(("M" if i == 0 else "L") + f"{float(x)!r},{-float(y)!r}" for i, (x, y) in enumerate(pts))
+        if cl[k]:
+            d += " Z"
+        out.append(f'<path d="{d}" fill="{fill}" fill-rule="nonzero" stroke="{stroke}" '
+                   f'stroke-width="{stroke_width * 2.0 / size:g}"/>')
+    out.append("</svg>")
+    return "\n".join(out) + "\n"
+
+
+# ---------------------------------------------------------------------------
 # Constraint solver (fidget-solver/src/lib.rs): fc_solve_batch
 @dataclass(frozen=True)
 class Free:

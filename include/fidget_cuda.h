@@ -65,7 +65,7 @@ int32_t fc_ctx_set_arena_bytes(fc_ctx* ctx, uint64_t bytes);
  * layout of Rust's AtomicBool (CancelToken::into_raw() as *const u8): nonzero = cancelled.  The library reads it with
  * an acquire load, from any thread; NULL detaches it.  Context-wide, like fc_ctx_set_stream, and consulted only by
  * fc_render2d, fc_render2d_frames, fc_render2d_scene, fc_render3d, fc_render3d_frames, fc_render3d_scene, fc_octree_sample,
- * fc_mesh_build, and
+ * fc_mesh_build, fc_contour_build, and
  * fc_ctx_synchronize after the most recent FC_FLAG_ASYNC call of those.  With a flag attached:
  *  - set on entry: the call returns FC_ERR_CANCELLED before it allocates or launches anything;
  *  - set while the call runs: the kernels stop claiming work and the call returns FC_ERR_CANCELLED ("cancelled" in
@@ -512,6 +512,51 @@ int32_t fc_mesh_read_cells(fc_ctx* ctx, fc_mesh_cell* out, uint64_t cap, uint64_
 /* Mesh::write_stl (fidget-mesh/src/output.rs:7-38): binary STL of the last mesh, assembled on the device.
  * buf == NULL queries the size (84 + 50 * n_triangles). */
 int32_t fc_mesh_write_stl(fc_ctx* ctx, uint8_t* buf, size_t cap, size_t* n_bytes);
+
+/* ---- 2D contours (libfive's Contours::render, on the quadtree the mesher's octree restricts to) -------------------
+ * fc_contour_build extracts the contours of a 2D shape (a sketch, a cut profile, a Z slice of a 3D model) as closed or
+ * open polylines, by dual contouring on a uniform quadtree of the [-1,1]^2 world square, the result staying in HBM until
+ * it is read:
+ *  1. the quadtree is descended by interval evaluation, with the tape simplified at every cell, exactly as
+ *     fc_octree_sample does with Z fixed to [z, z]; cell bounds are float(i) * h - 1 with h = 2 / 2^depth, and a cell
+ *     proven inside (upper < 0) or outside (lower > 0) is dropped;
+ *  2. every remaining depth-level cell (ix, iy) gets a 4-bit corner mask (bit c = corner c inside, v < 0; bit 0 of c is
+ *     +X, bit 1 is +Y); masks 0 and 15 are not surface leaves.  On every edge whose corners differ, the intersection is
+ *     found by fc_octree_sample's 16-ary search, and the gradient there (dx, dy, v) in world coordinates;
+ *  3. one vertex per connected group of inside corners (adjacent along cell edges: two diagonal inside corners give two
+ *     vertices), placed by the 2D restriction of QuadraticErrorSolver::solve (fidget-mesh/src/qef.rs:67-168);
+ *  4. one segment per sign-changing edge inside the domain, between the vertices owning it in its two cells, directed so
+ *     that the inside lies on its left (counter-clockwise around inside regions, y up).  Edges on the domain boundary
+ *     give no segment and are counted in n_open;
+ *  5. segments are linked into polylines in a canonical order: an open polyline starts at its vertex without an incoming
+ *     segment, a closed one at its smallest vertex key (iy, ix, group); polylines are ordered by the key of their first
+ *     vertex.  The output is deterministic, bit for bit;
+ *  6. with has_transform, unless world_to_model is the identity, vertices are mapped to model space through the matrix
+ *     (f32, divided by the homogeneous term where that is not zero).  The direction of travel is the one in the world
+ *     square: a mirroring matrix reverses it in model space.
+ * world_to_model is a row-major 3x3, as the 2D renderers take it, applied to the world square (x, y, 1); Z is passed
+ * through.  Errors: depth above FC_MAX_QUADTREE_DEPTH, a multi-output tape or n_var_values above FC_MAX_VARS give
+ * FC_ERR_INVALID, a tape with memory slots FC_ERR_UNSUPPORTED.  The cancel flag (fc_ctx_set_cancel) stops the build; a
+ * cancelled build leaves no contour (fc_contour_read copies nothing, every count is 0). */
+#define FC_MAX_QUADTREE_DEPTH 14
+typedef struct fc_contour_cfg {
+    uint32_t depth;
+    uint32_t has_transform;     /* 0: world_to_model is ignored */
+    float world_to_model[9];    /* row-major 3x3 */
+    float z;                    /* the Z slice */
+    uint32_t flags;             /* FC_FLAG_TIMING: sampler_ms / contour_ms */
+    uint32_t n_var_values;      /* ShapeVars, as in fc_render2d_cfg */
+    float var_values[FC_MAX_VARS];
+} fc_contour_cfg;
+typedef struct fc_contour_info {
+    uint64_t n_leaves, n_vertices, n_polylines, n_closed, n_open;
+    float sampler_ms, contour_ms;   /* device time of the quadtree sampler / of vertices, segments and linking */
+} fc_contour_info;
+int32_t fc_contour_build(fc_ctx* ctx, const fc_tape* tape, const fc_contour_cfg* cfg, fc_contour_info* info);
+/* The last fc_contour_build's polylines: vertices (2 floats each, in polyline order), offsets (n_polylines + 1: polyline
+ * k is vertices offsets[k] .. offsets[k + 1] - 1) and closed (one byte per polyline, 1 = the last vertex joins the
+ * first).  Host or device pointers; any may be NULL. */
+int32_t fc_contour_read(fc_ctx* ctx, float* vertices, uint32_t* offsets, uint8_t* closed);
 
 /* ---- constraint solver (fidget-solver) ----------------------------------------------------------------------- */
 /* fidget_solver::solve (fidget-solver/src/lib.rs:191-289) for a batch of independent problems that share their

@@ -131,6 +131,11 @@ class FcContourInfo(C.Structure):
                [("sampler_ms", C.c_float), ("contour_ms", C.c_float)]
 
 
+class FcContourSlice(C.Structure):
+    _fields_ = [("z", C.c_float), ("has_transform", C.c_uint32), ("world_to_model", C.c_float * 9),
+                ("n_var_values", C.c_uint32), ("var_values", C.c_float * 16)]
+
+
 class FcSolveCfg(C.Structure):
     _fields_ = [("n_params", C.c_uint32), ("n_free", C.c_uint32), ("max_iters", C.c_uint32)]
 
@@ -228,6 +233,8 @@ CUDA_API = {
     "fc_mesh_write_stl": (_i32, [_vp, _vp, C.c_size_t, _P(C.c_size_t)]),
     "fc_contour_build": (_i32, [_vp, _vp, _P(FcContourCfg), _P(FcContourInfo)]),
     "fc_contour_read": (_i32, [_vp, _vp, _vp, _vp]),
+    "fc_contour_build_slices": (_i32, [_vp, _vp, _P(FcContourCfg), _P(FcContourSlice), _u32, _P(FcContourInfo),
+                                       _P(FcContourInfo)]),
     "fc_solve_batch": (_i32, [_vp, _P(_vp), _u32, _P(_P(_i32)), _P(FcSolveCfg), _vp, _u64, _vp]),
     "fc_schedule_check": (_i32, [_P(_u32), C.c_size_t, _u8, _u32, _u32, _u32, _P(FcScheduleInfo)]),
     "fc_denoise_normals": (_i32, [_vp, _vp, _u32, _u32, _vp]),

@@ -142,6 +142,9 @@ void fc_ctx_destroy(fc_ctx* c) {
     c->contour_leaves.release();
     c->contour_scratch.release();
     c->contour_out.release();
+    c->contour_offs.release();
+    c->contour_flags.release();
+    c->contour_slices.release();
     c->tile_slots.release();
     c->fx_in.release();
     c->fx_out.release();

@@ -151,10 +151,11 @@ struct fc_ctx {
     uint32_t mesh_n_verts = 0, mesh_n_tris = 0;
     DevBuf mesh_tree, mesh_herm, mesh_cells;                    // FC_FLAG_MESH_COLLAPSE: cell tree, Hermite records, final leaves
     uint32_t mesh_n_cells = 0;
-    DevBuf contour_leaves, contour_scratch, contour_out;        // fc_contour_build: sampler output, link scratch, polylines
+    DevBuf contour_leaves, contour_scratch, contour_out;        // fc_contour_build: sampler output, link scratch, vertices
+    DevBuf contour_offs, contour_flags, contour_slices;         // offsets, closed flags, a stack pass's slice table
     uint32_t contour_n_verts = 0, contour_n_polys = 0;
-    uint32_t* contour_offsets = nullptr;                        // in contour_out, after the vertices
-    uint8_t* contour_closed = nullptr;
+    uint32_t* contour_offsets = nullptr;                        // in contour_offs
+    uint8_t* contour_closed = nullptr;                          // in contour_flags
     DevBuf fx_in, fx_out, fx_tmp, fx_tables;  // effects: staged host images, intermediate maps, SSAO tables
     DevBuf solve_meta, solve_vals, solve_res; // fc_solve_batch: tape table + slot maps, staged host values / results
     // the batches (fc_render2d_frames, fc_render3d_frames, fc_render3d_scene): the frame or placement table, and the copy

@@ -16,7 +16,16 @@
 //              cuts each cycle there and ranks every vertex from its polyline's head;
 //   emit       one scan over the heads in vertex order gives each polyline's place, and every vertex is scattered to
 //              head offset + rank.
+//
+// A slice stack (fc_contour_build_slices) runs the same pipeline over the slices of a pass at once: slice k owns the cell
+// rows [k * 2^depth, (k + 1) * 2^depth) of one tall quadtree grid, level 0 evaluates one root cell per slice, and the
+// sort key is (slice, iy, ix), so vertex ids are slice-major, no search or segment leaves its slice, and every slice's
+// polylines come out in its own canonical order.  fc_contour_build is the stack of one slice; kernels with STACK = false
+// read that slice from their launch parameters, as the one-slice passes of a stack do.
 #include <cub/cub.cuh>
+
+#include <algorithm>
+#include <cmath>
 
 #include "capi_internal.h"
 #include "level_job.cuh"
@@ -28,9 +37,9 @@ constexpr uint32_t NONE = ~0u;
 // One surface leaf of the quadtree.  Edge e: axis t = e >> 1 (0: along X, 1: along Y) at bit e & 1 of the other axis,
 // from corner c0 = (e & 1) << (1 - t) to c0 | 1 << t: edge 0 = corners 0-1, 1 = 2-3, 2 = 0-2, 3 = 1-3.
 struct ContourLeaf {
-    uint16_t ix, iy;
+    uint16_t ix, iy;         // cell of its slice
     uint8_t mask, present;   // corner mask; bit e = edge e carries an intersection
-    uint16_t pad;
+    uint16_t slice;          // slice within the pass
     float pos[4][2];
     float grad[4][3];        // dx, dy, v
 };
@@ -49,17 +58,23 @@ struct ContourLeafParams {
     uint32_t cap_out;
     uint32_t* n_out;
     CancelRef cancel;
+    const ContourSlice* slices;   // STACK: the pass's slice table, `rows` cell rows per slice
+    uint32_t rows;
 };
 
-// The quadtree levels: k_interval_level's claim loop around level_job's QUAD mode (one root cell)
-__global__ void __launch_bounds__(WARPS_PER_BLOCK * 32) k_contour_level(const __grid_constant__ LevelParams p) {
+// The quadtree levels: k_interval_level's claim loop around level_job's QUAD mode (one root cell; STACK: one per slice,
+// roots_y slices, 32 to a warp at level 0)
+template <bool STACK>
+__global__ void __launch_bounds__(WARPS_PER_BLOCK * 32) k_contour_level(const __grid_constant__ LevelParams p,
+                                                                        const ContourSlice* slices) {
     __shared__ uint32_t live_s[WARPS_PER_BLOCK][8][32];
     const int lane = threadIdx.x & 31;
     const int wib = threadIdx.x >> 5;
     const uint32_t gw = blockIdx.x * WARPS_PER_BLOCK + wib;
     uint32_t* cs = p.choice_scratch + size_t(gw) * p.choice_words * 32u + lane;
     itv slots[REG_SLOTS];
-    const uint32_t n_jobs = p.root_mode ? 1u : min(p.ctr->n_jobs[p.level], p.cap_in);
+    const uint32_t n_roots = STACK ? p.roots_y : 1u;
+    const uint32_t n_jobs = p.root_mode ? (n_roots + 31u) / 32u : min(p.ctr->n_jobs[p.level], p.cap_in);
     for (;;) {
         uint32_t j = 0;
         if (lane == 0) {
@@ -68,7 +83,7 @@ __global__ void __launch_bounds__(WARPS_PER_BLOCK * 32) k_contour_level(const __
         }
         j = __shfl_sync(FULL, j, 0);
         if (j >= n_jobs) break;
-        level_job<2, false, false, false, true>(p, j, 1u, slots, cs, live_s[wib], lane, p.epoch);
+        level_job<2, false, STACK, false, true>(p, j, n_roots, slots, cs, live_s[wib], lane, p.epoch, slices);
     }
 }
 
@@ -89,6 +104,7 @@ __device__ __forceinline__ bool edge_setup2(uint32_t e, uint32_t mask, EdgeState
 
 // One warp per leaf job: corner mask, then the four edges' searches in one pass (lanes 0-15 follow edges 0 and 2, lanes
 // 16-31 edges 1 and 3, one probe each), with k_octree_leaf's rounds, fractions and bracket midpoint
+template <bool STACK>
 __global__ void __launch_bounds__(128) k_contour_leaf(const __grid_constant__ ContourLeafParams p) {
     const int lane = threadIdx.x & 31;
     float2 slots[REG_SLOTS];
@@ -102,20 +118,22 @@ __global__ void __launch_bounds__(128) k_contour_leaf(const __grid_constant__ Co
         j = __shfl_sync(FULL, j, 0);
         if (j >= n_jobs) break;
         const TileJob* job = p.jobs + j;
-        const uint32_t cx = job->x, cy = job->y;
+        // (STACK: the slice of the job's row supplies Z, matrix and vars, and cy is the row within the slice)
+        const uint32_t s = STACK ? job->y / p.rows : 0u;
+        const uint32_t cx = job->x, cy = STACK ? job->y - s * p.rows : job->y;
         const TapeRef tr = job->tape;
         const float h = p.cell_h;
         const float lo[2] = {float(cx) * h - 1.0f, float(cy) * h - 1.0f};
         const float hi[2] = {float(cx + 1u) * h - 1.0f, float(cy + 1u) * h - 1.0f};
         auto eval2 = [&](float x0, float y0, float x1, float y1) -> float2 {
-            float z0 = p.z, z1 = p.z;
-            if (p.has_transform) {
-                xform_f32(p.mat, x0, y0, z0, x0, y0, z0);
-                xform_f32(p.mat, x1, y1, z1, x1, y1, z1);
+            float z0 = STACK ? p.slices[s].z : p.z, z1 = z0;
+            if (STACK ? p.slices[s].has_transform : p.has_transform) {
+                xform_f32(STACK ? p.slices[s].mat : p.mat, x0, y0, z0, x0, y0, z0);
+                xform_f32(STACK ? p.slices[s].mat : p.mat, x1, y1, z1, x1, y1, z1);
             }
             const float2 X = make_float2(x0, x1), Y = make_float2(y0, y1), Z = make_float2(z0, z1);
             return run_f32x2(tr.ptr, tr.n_ops, slots, [&](uint32_t i) {
-                return pick_input(p.vb, i, X, Y, Z, [](float f) { return make_float2(f, f); });
+                return pick_input(STACK ? p.slices[s].vb : p.vb, i, X, Y, Z, [](float f) { return make_float2(f, f); });
             });
         };
         const int c = lane & 3;
@@ -138,7 +156,7 @@ __global__ void __launch_bounds__(128) k_contour_leaf(const __grid_constant__ Co
         if (lane == 0) {
             p.out_tapes[slot] = tr;
             L->ix = uint16_t(cx); L->iy = uint16_t(cy);
-            L->mask = uint8_t(mask); L->present = uint8_t(present); L->pad = 0;
+            L->mask = uint8_t(mask); L->present = uint8_t(present); L->slice = uint16_t(s);
         }
         for (int round = 0; round < 4; ++round) {
             uint32_t q0[2], q1[2];
@@ -173,6 +191,7 @@ __global__ void __launch_bounds__(128) k_contour_leaf(const __grid_constant__ Co
 }
 
 // Gradients at the intersections (as k_octree_grads, Z seeded at the slice): one warp per leaf, one lane per edge
+template <bool STACK>
 __global__ void __launch_bounds__(128) k_contour_grads(const __grid_constant__ ContourLeafParams p) {
     grd slots[REG_SLOTS];
     const int lane = threadIdx.x & 31;
@@ -186,10 +205,12 @@ __global__ void __launch_bounds__(128) k_contour_grads(const __grid_constant__ C
         const uint32_t active = L->present;
         const bool mine = lane < 4 && ((active >> lane) & 1u);
         const int e = mine ? lane : (__ffs(active) - 1);
-        grd gx = gr(L->pos[e][0], 1.0f, 0.0f, 0.0f), gy = gr(L->pos[e][1], 0.0f, 1.0f, 0.0f), gz = gr(p.z, 0.0f, 0.0f, 1.0f);
-        if (p.has_transform) xform_gr(p.mat, gx, gy, gz, gx, gy, gz);
+        const ContourSlice* sl = STACK ? p.slices + L->slice : nullptr;   // (STACK: the leaf's slice)
+        grd gx = gr(L->pos[e][0], 1.0f, 0.0f, 0.0f), gy = gr(L->pos[e][1], 0.0f, 1.0f, 0.0f),
+            gz = gr(STACK ? sl->z : p.z, 0.0f, 0.0f, 1.0f);
+        if (STACK ? sl->has_transform : p.has_transform) xform_gr(STACK ? sl->mat : p.mat, gx, gy, gz, gx, gy, gz);
         const grd r = run_grad(tr.ptr, tr.n_ops, slots, [&](uint32_t k) {
-            return pick_input(p.vb, k, gx, gy, gz, [](float f) { return gr1(f); });
+            return pick_input(STACK ? sl->vb : p.vb, k, gx, gy, gz, [](float f) { return gr1(f); });
         });
         if (mine) { L->grad[e][0] = r.y; L->grad[e][1] = r.z; L->grad[e][2] = r.x; }
     }
@@ -259,27 +280,36 @@ __device__ __forceinline__ uint32_t corner_groups2(uint32_t mask) {
 }
 __device__ __forceinline__ uint32_t group_of(uint32_t packed, uint32_t corner) { return (packed >> (2u * corner)) & 3u; }
 
-__device__ __forceinline__ uint32_t leaf_key(const ContourLeaf& L) { return (uint32_t(L.iy) << 16) | L.ix; }
+// Sort key (slice, iy, ix): 2 * depth bits of cell, the slice above them
+__device__ __forceinline__ unsigned long long leaf_key(const ContourLeaf& L, uint32_t depth) {
+    return ((unsigned long long)L.slice << (2u * depth)) | ((unsigned long long)L.iy << depth) | L.ix;
+}
+
+// Per slice of the pass (ContourScratch::per_slice, PS_WORDS words each): one past its last sorted leaf and its last
+// vertex (0: no leaves), its polylines, closed polylines and open edges
+enum { PS_LEAF_END, PS_VERT_END, PS_POLYS, PS_CLOSED, PS_OPEN, PS_WORDS };
 
 struct ContourScratch {
     const ContourLeaf* leaves;
-    uint32_t n_leaves, side;        // side: cells per axis
-    const uint32_t* keys;           // sorted leaf keys
-    const uint32_t* order;          // leaf index of each sorted position
-    uint32_t* packed;               // per sorted position: corner groups (corner_groups2)
+    uint32_t n_leaves, side, depth;  // side: cells per axis
+    const unsigned long long* keys;  // sorted leaf keys
+    const uint32_t* order;           // leaf index of each sorted position
+    uint32_t* packed;                // per sorted position: corner groups (corner_groups2)
     uint32_t* n_groups;
-    const uint32_t* vbase;          // exclusive scan of n_groups: first vertex of each sorted position
-    float2* vpos;                   // [vertex] world position
+    const uint32_t* vbase;           // exclusive scan of n_groups: first vertex of each sorted position
+    float2* vpos;                    // [vertex] world position
+    uint32_t* vslice;                // [vertex] its slice
     uint32_t* next;
     uint32_t* prev;
-    uint32_t* counts;               // [0] vertices [1] polylines [2] closed [3] open edges
+    uint32_t* counts;                // [0] vertices [1] polylines, then the per-slice words
+    uint32_t* per_slice;
     CancelRef cancel;
 };
 
-__global__ void k_contour_keys(const ContourLeaf* leaves, uint32_t n, uint32_t* keys, uint32_t* idx) {
+__global__ void k_contour_keys(const ContourLeaf* leaves, uint32_t n, uint32_t depth, unsigned long long* keys, uint32_t* idx) {
     const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= n) return;
-    keys[i] = leaf_key(leaves[i]);
+    keys[i] = leaf_key(leaves[i], depth);
     idx[i] = i;
 }
 
@@ -299,8 +329,14 @@ __global__ void __launch_bounds__(128) k_contour_vertices(ContourScratch m) {
     if (i >= m.n_leaves) return;
     const ContourLeaf& L = m.leaves[m.order[i]];
     const uint32_t mask = L.mask, packed = m.packed[i], ng = packed >> 8, base = m.vbase[i];
+    const uint32_t s = uint32_t(m.keys[i] >> (2u * m.depth));
     if (i == m.n_leaves - 1u) m.counts[0] = base + ng;
+    if (i == m.n_leaves - 1u || uint32_t(m.keys[i + 1u] >> (2u * m.depth)) != s) {   // the slice's last leaf
+        m.per_slice[PS_WORDS * s + PS_LEAF_END] = i + 1u;
+        m.per_slice[PS_WORDS * s + PS_VERT_END] = base + ng;
+    }
     for (uint32_t g = 0; g < ng; ++g) {
+        m.vslice[base + g] = s;
         Qef2 q{};
         bool forced = false;
         float pos[2];
@@ -324,7 +360,7 @@ __global__ void __launch_bounds__(128) k_contour_vertices(ContourScratch m) {
     }
 }
 
-__device__ __forceinline__ uint32_t find_leaf(const ContourScratch& m, uint32_t key) {
+__device__ __forceinline__ uint32_t find_leaf(const ContourScratch& m, unsigned long long key) {
     uint32_t lo = 0, hi = m.n_leaves;
     while (lo < hi) {
         const uint32_t mid = (lo + hi) >> 1;
@@ -340,6 +376,7 @@ __global__ void __launch_bounds__(128) k_contour_segments(ContourScratch m) {
     if (i >= m.n_leaves) return;
     const ContourLeaf& L = m.leaves[m.order[i]];
     const uint32_t mask = L.mask, x = L.ix, y = L.iy, packed = m.packed[i], base = m.vbase[i];
+    const unsigned long long key = m.keys[i];   // (the -X neighbour's key is key - 1, the -Y one's key - side)
     auto in = [](uint32_t mk, uint32_t c) { return (mk >> c) & 1u; };
     uint32_t open = 0;
     if (x + 1u == m.side && in(mask, 1) != in(mask, 3)) ++open;
@@ -350,7 +387,7 @@ __global__ void __launch_bounds__(128) k_contour_segments(ContourScratch m) {
         const uint32_t a0 = ca[d][0], a1 = ca[d][1];
         if (in(mask, a0) == in(mask, a1)) continue;
         if ((d == 0 ? x : y) == 0u) { ++open; continue; }
-        const uint32_t j = find_leaf(m, d == 0 ? ((y << 16) | (x - 1u)) : (((y - 1u) << 16) | x));
+        const uint32_t j = find_leaf(m, d == 0 ? key - 1u : key - m.side);
         const uint32_t mj = j == NONE ? 0u : m.leaves[m.order[j]].mask;
         if (j == NONE || in(mj, cb[d][0]) != in(mask, a0) || in(mj, cb[d][1]) != in(mask, a1)) { ++open; continue; }
         // inside on the left: across a -X edge the path runs +X when the upper corner is inside; across a -Y edge it
@@ -363,7 +400,7 @@ __global__ void __launch_bounds__(128) k_contour_segments(ContourScratch m) {
         m.next[from] = to;
         m.prev[to] = from;
     }
-    if (open) atomicAdd(&m.counts[3], open);
+    if (open) atomicAdd(&m.per_slice[PS_WORDS * uint32_t(key >> (2u * m.depth)) + PS_OPEN], open);
 }
 
 // List ranking by pointer jumping, one launch per round (ping-pong buffers).  After k rounds of pass 1, P[v] is the
@@ -423,43 +460,146 @@ __global__ void k_link_heads(ContourScratch m, LinkBufs b, uint32_t cap) {
     b.scan[v] = v < m.counts[0] && b.A[0][v] == v ? (1ull << 32) | b.len[v] : 0ull;
 }
 
-// Every vertex to its place (head's offset + rank), in model space when `to_model`; heads write their polyline's record
-__global__ void k_contour_emit(ContourScratch m, LinkBufs b, const unsigned long long* scan, float2* out_v,
-                               uint32_t* out_off, uint8_t* out_closed, bool to_model, Mat4 M, float z) {
+// Where a pass's polylines go: its first vertex and polyline in the stack's output (v, off, closed point there), and
+// the map to model space -- to_model / M / z of the one slice, or (STACK) each vertex's slice's
+struct EmitOut {
+    float2* v;
+    uint32_t* off;
+    uint8_t* closed;
+    uint32_t v0;            // vertices of the stack before this pass: added to every offset
+    bool to_model;
+    Mat4 M;
+    float z;
+    const ContourSlice* slices;
+};
+
+// Every vertex to its place (head's offset + rank), in model space when its slice asks; heads write their polyline's
+// record and count it for their slice
+template <bool STACK>
+__global__ void k_contour_emit(ContourScratch m, LinkBufs b, const unsigned long long* scan, const __grid_constant__ EmitOut o) {
     if (cancel_poll(m.cancel, CS_CONTOUR_EMIT, blockIdx.x)) return;
     const uint32_t v = blockIdx.x * blockDim.x + threadIdx.x;
     const uint32_t nv = m.counts[0];
     if (v >= nv) return;
-    const uint32_t h = b.A[0][v];
+    const uint32_t h = b.A[0][v], s = m.vslice[v];
     float2 q = m.vpos[v];
+    const bool to_model = STACK ? o.slices[s].to_model != 0u : o.to_model;
     if (to_model) {
-        float zz = z;
-        xform_f32(M, q.x, q.y, zz, q.x, q.y, zz);
+        float zz = STACK ? o.slices[s].z : o.z;
+        xform_f32(STACK ? o.slices[s].mat : o.M, q.x, q.y, zz, q.x, q.y, zz);
     }
-    out_v[uint32_t(scan[h]) + b.R[0][v]] = q;
+    o.v[uint32_t(scan[h]) + b.R[0][v]] = q;
     if (h == v) {
         const uint32_t k = uint32_t(scan[v] >> 32);
-        out_off[k] = uint32_t(scan[v]);
-        out_closed[k] = b.closed[v];
-        if (b.closed[v]) atomicAdd(&m.counts[2], 1u);
+        o.off[k] = o.v0 + uint32_t(scan[v]);
+        o.closed[k] = b.closed[v];
+        atomicAdd(&m.per_slice[PS_WORDS * s + PS_POLYS], 1u);
+        if (b.closed[v]) atomicAdd(&m.per_slice[PS_WORDS * s + PS_CLOSED], 1u);
     }
     if (v == nv - 1u) {
         const uint32_t n_poly = uint32_t(scan[v] >> 32) + (h == v ? 1u : 0u);
         m.counts[1] = n_poly;
-        out_off[n_poly] = nv;
+        o.off[n_poly] = o.v0 + nv;
     }
 }
 
 }  // namespace fdev
 
-// The quadtree sampler: interval levels, then the leaf and gradient kernels; *n_out = surface leaves found (more than
-// cap: FC_ERR_INVALID, nothing beyond cap written)
-static int32_t contour_sample(fc_ctx* c, const fc_tape* tape, const fc_contour_cfg* cfg, const VarBind& vb,
-                              const fdev::Mat4& mat, fdev::ContourLeaf* dout, uint64_t cap, uint32_t* n_out_p,
-                              const CallCancel& cc) {
+
+namespace {
+using fdev::ContourSlice;
+
+// Device bytes per surface leaf of a pass, for sizing passes: the leaf and its tape, the sort and group words of
+// contour_finish, and per vertex (at most two) its position, slice, links, list-ranking buffers, scans and output
+constexpr uint64_t CONTOUR_LEAF_BYTES = sizeof(fdev::ContourLeaf) + sizeof(fdev::TapeRef) + 7 * 4 + 12 +
+                                        2 * (8 + 4 + 2 * 4 + 6 * 4 + 1 + 4 + 2 * 8 + 8 + 4 + 1);
+
+// The passes of a slice stack, with the overflow policy of the 3D batches (PassPlan, render.cu): the first pass holds
+// one slice; later ones are sized from the largest per-slice use seen so far (arena clauses, jobs of the levels whose
+// list is capped, surface leaves against FC_FRAMES_PASS_BYTES) with headroom 1.5; a pass that overflows anyway is run
+// again as two halves, and only a one-slice pass returns the error.  FIDGET_B200_FRAMES_PER_PASS fixes the pass size.
+struct ContourPlan {
+    struct Range { uint32_t f0, n; };
+    uint32_t depth, n_items, n_max, next = 0;
+    int forced;
+    bool measured;
+    uint64_t arena_cap, cap_limit;
+    double use_arena = 0, use_leaves = 0, use_jobs[fdev::MAX_LEVELS + 1] = {};
+    std::vector<Range> redo;                    // halves of overflowed passes (a stack: the first half runs next)
+
+    ContourPlan(const fc_ctx* c, uint32_t d, uint32_t n) : depth(d), n_items(n) {
+        // (a pass's slice index is 16 bits in its leaves, and its cell rows must fit 32 bits)
+        n_max = uint32_t(std::min<uint64_t>({n, 0xffffu, (1ull << (32 - d)) - 1}));
+        forced = env_int("FIDGET_B200_FRAMES_PER_PASS", 0);
+        if (forced > 0) n_max = std::min<uint32_t>(n_max, uint32_t(forced));
+        measured = forced > 0;
+        arena_cap = std::min<uint64_t>(c->arena.cap, c->arena_bytes) / sizeof(uint2);
+        cap_limit = uint64_t(env_int("FIDGET_B200_MAX_TILES_M", 16)) << 20;
+    }
+    // the jobs of level l that every cell of n slices would queue, and the list's capacity
+    uint64_t worst(uint32_t n, int l) const { return uint64_t(n) << (2 * std::min<uint32_t>(uint32_t(l), depth)); }
+    uint64_t level_cap(uint32_t n, int l) const { return std::min(worst(n, l), cap_limit); }
+    bool more() const { return next < n_items || !redo.empty(); }
+    bool fits(uint32_t n) const {
+        const double h = 1.5 * n;
+        if (use_arena * h > double(arena_cap)) return false;
+        if (use_leaves * h * double(CONTOUR_LEAF_BYTES) > double(FC_FRAMES_PASS_BYTES)) return false;
+        for (int l = 1; l <= int(depth) + 1; ++l)
+            if (level_cap(n, l) < worst(n, l) && use_jobs[l] * h > double(level_cap(n, l))) return false;
+        return true;
+    }
+    Range take() {
+        if (!redo.empty()) { const Range r = redo.back(); redo.pop_back(); return r; }
+        uint32_t n = std::min(n_max, n_items - next);
+        if (!measured) n = 1;
+        else if (forced <= 0) while (n > 1 && !fits(n)) --n;
+        const Range r{next, n};
+        next += n;
+        return r;
+    }
+    // Records the use of the sampled pass r.  Its error if it fails; else `split` says that it overflowed and its
+    // halves are queued in its place.
+    int32_t observe(const fdev::Counters& ctr, const Range& r, uint32_t n_leaves, bool& split) {
+        const double n = double(r.n);
+        use_arena = std::max(use_arena, double(ctr.arena_top) / n);
+        use_leaves = std::max(use_leaves, double(n_leaves) / n);
+        for (int l = 1; l <= int(depth) + 1; ++l) use_jobs[l] = std::max(use_jobs[l], double(ctr.n_jobs[l]) / n);
+        measured = true;
+        split = false;
+        if (!ctr.error) return FC_OK;
+        if (r.n == 1 || (ctr.error & ~3u)) return device_error(ctr.error);
+        const uint32_t h = r.n / 2;
+        redo.push_back(Range{r.f0 + h, r.n - h});
+        redo.push_back(Range{r.f0, h});
+        split = true;
+        return FC_OK;
+    }
+};
+
+// Grows `b` to at least `need` bytes, keeping its first `keep` bytes (the polylines of the stack's earlier passes)
+int32_t grow_keep(fc_ctx* c, DevBuf& b, size_t need, size_t keep) {
+    if (need <= b.cap) return FC_OK;
+    const size_t cap = std::max(need, b.cap + b.cap / 2);
+    void* p = nullptr;
+    CU(cudaMalloc(&p, cap));
+    keep = std::min(keep, b.cap);
+    if (keep) CU(cudaMemcpyAsync(p, b.p, keep, cudaMemcpyDeviceToDevice, c->stream));
+    CU(cudaStreamSynchronize(c->stream));
+    b.release();
+    b.p = p;
+    b.cap = cap;
+    return FC_OK;
+}
+}  // namespace
+
+// The quadtree sampler over the n slices sl[0..n) (host; with n > 1 also d_sl on the device): interval levels, then the
+// leaf and gradient kernels.  *n_out = surface leaves found (nothing beyond cap written), ctr = the pass's counters.
+static int32_t contour_sample(fc_ctx* c, const fc_tape* tape, uint32_t D, const ContourSlice* sl, uint32_t n,
+                              const ContourSlice* d_sl, fdev::ContourLeaf* dout, uint64_t cap, uint32_t* n_out_p,
+                              fdev::Counters& ctr, const CallCancel& cc) {
     using namespace fdev;
-    const uint32_t D = cfg->depth;
     const int L = int(D) + 1;
+    const bool stack = n > 1;
     cudaStream_t s = c->stream;
     const int grid_blocks = c->sm_count * env_int("FIDGET_B200_BLOCKS_PER_SM", 6);
     const uint32_t choice_words = (tape->info.choice_count + 15) / 16 + 1;
@@ -470,7 +610,7 @@ static int32_t contour_sample(fc_ctx* c, const fc_tape* tape, const fc_contour_c
     const uint64_t cap_limit = uint64_t(env_int("FIDGET_B200_MAX_TILES_M", 16)) << 20;
     std::vector<uint64_t> level_cap(L + 1);
     for (int l = 1; l <= L; ++l) {
-        level_cap[l] = std::min<uint64_t>(1ull << (2 * std::min(l, int(D))), cap_limit);
+        level_cap[l] = std::min<uint64_t>(uint64_t(n) << (2 * std::min(l, int(D))), cap_limit);
         CU(c->jobs[l].ensure(level_cap[l] * sizeof(TileJob)));
     }
     CU(c->leaf_tapes.ensure(std::max<uint64_t>(cap, 1) * sizeof(TapeRef)));
@@ -483,15 +623,16 @@ static int32_t contour_sample(fc_ctx* c, const fc_tape* tape, const fc_contour_c
         p.n_axis = l ? 2 : 0;
         p.is_last = (l == L - 1);
         p.root_mode = (l == 0);
-        p.roots_x = p.roots_y = p.roots_z = 1;
+        p.roots_x = p.roots_z = 1;
+        p.roots_y = n;   // one root cell per slice, stacked along Y
         p.root_tape.ptr = tape->dev;
         p.root_tape.n_ops = tape->info.n_ops;
         p.root_tape.ref_len = tape->info.ref_len;
         p.root_tape.n_choices = tape->info.choice_count;
         p.width = p.height = 1u << D;
         p.depth = 1;
-        p.z2d = cfg->z;
-        p.mat = mat;
+        p.z2d = sl[0].z;
+        p.mat = sl[0].mat;
         p.jobs_in = l ? c->jobs[l].as<TileJob>() : nullptr;
         p.cap_in = l ? uint32_t(level_cap[l]) : 0;
         p.jobs_out = c->jobs[l + 1].as<TileJob>();
@@ -502,13 +643,15 @@ static int32_t contour_sample(fc_ctx* c, const fc_tape* tape, const fc_contour_c
         p.choice_words = choice_words;
         p.ctr = c->counters.as<Counters>();
         p.mode = 1;
-        p.has_transform = cfg->has_transform;
+        p.has_transform = sl[0].has_transform;
         p.cell_h = 2.0f / float(1u << D);
-        p.vb = vb;
+        p.vb = sl[0].vb;
         p.cancel = cc.ref;
-        const uint64_t warps = l ? std::max<uint64_t>(1, (1ull << (2 * l)) / 4) : 1;
+        p.frame_rows = 1u << D;
+        const uint64_t warps = l ? std::max<uint64_t>(1, (uint64_t(n) << (2 * l)) / 4) : (n + 31) / 32;
         const int blocks = int(std::min<uint64_t>((warps + WARPS_PER_BLOCK - 1) / WARPS_PER_BLOCK, uint64_t(grid_blocks)));
-        k_contour_level<<<std::max(blocks, 1), WARPS_PER_BLOCK * 32, 0, s>>>(p);
+        if (stack) k_contour_level<true><<<std::max(blocks, 1), WARPS_PER_BLOCK * 32, 0, s>>>(p, d_sl);
+        else k_contour_level<false><<<std::max(blocks, 1), WARPS_PER_BLOCK * 32, 0, s>>>(p, nullptr);
     }
     ContourLeafParams q{};
     q.jobs = c->jobs[L].as<TileJob>();
@@ -516,78 +659,98 @@ static int32_t contour_sample(fc_ctx* c, const fc_tape* tape, const fc_contour_c
     q.ctr = c->counters.as<Counters>();
     q.list = L; q.cursor = L;
     q.cell_h = 2.0f / float(1u << D);
-    q.z = cfg->z;
-    q.has_transform = cfg->has_transform;
-    q.mat = mat;
-    q.vb = vb;
+    q.z = sl[0].z;
+    q.has_transform = sl[0].has_transform;
+    q.mat = sl[0].mat;
+    q.vb = sl[0].vb;
     q.out = dout;
     q.out_tapes = c->leaf_tapes.as<TapeRef>();
     q.cap_out = uint32_t(cap);
     q.n_out = d_n_out;
     q.cancel = cc.ref;
-    k_contour_leaf<<<c->sm_count * 8, 128, 0, s>>>(q);
-    k_contour_grads<<<c->sm_count * 8, 128, 0, s>>>(q);
+    q.slices = stack ? d_sl : nullptr;
+    q.rows = 1u << D;
+    if (stack) {
+        k_contour_leaf<true><<<c->sm_count * 8, 128, 0, s>>>(q);
+        k_contour_grads<true><<<c->sm_count * 8, 128, 0, s>>>(q);
+    } else {
+        k_contour_leaf<false><<<c->sm_count * 8, 128, 0, s>>>(q);
+        k_contour_grads<false><<<c->sm_count * 8, 128, 0, s>>>(q);
+    }
     CU(cudaGetLastError());
     uint32_t n_out = 0;
     if (int32_t wrc = wait_read(c, s, cc, &n_out, d_n_out, 4)) return wrc;
     *n_out_p = n_out;
-    if (int32_t rc = check_device_errors(c)) return rc;
-    if (n_out > cap) return fail(FC_ERR_INVALID, "contour leaf buffer too small: " + std::to_string(n_out) + " surface leaves");
+    CU(cudaMemcpy(&ctr, c->counters.p, sizeof ctr, cudaMemcpyDeviceToHost));
     return FC_OK;
 }
 
-// Vertices, segments, linking and the polylines, from n surface leaves in contour_leaves
-static int32_t contour_finish(fc_ctx* c, uint32_t n, const fc_contour_cfg* cfg, const fdev::Mat4& mat, bool to_model,
-                              fc_contour_info* info, const CallCancel& cc) {
+// Vertices, segments, linking and the polylines of one pass, from its n surface leaves in contour_leaves: appended to
+// the stack's output after its v0 vertices and p0 polylines.  cnt receives the pass's vertex and polyline counts, then
+// PS_WORDS words per slice.
+static int32_t contour_finish(fc_ctx* c, uint32_t n, uint32_t D, const ContourSlice* sl, uint32_t n_sl,
+                              const ContourSlice* d_sl, uint64_t v0, uint64_t p0, std::vector<uint32_t>& cnt,
+                              float* ms, const CallCancel& cc) {
     using namespace fdev;
     cudaStream_t s = c->stream;
     const uint32_t V = 2u * n;   // at most two vertices per leaf
     ContourScratch m{};
     m.leaves = c->contour_leaves.as<ContourLeaf>();
     m.n_leaves = n;
-    m.side = 1u << cfg->depth;
+    m.side = 1u << D;
+    m.depth = D;
     m.cancel = cc.ref;
     LinkBufs b{};
-    uint32_t *keys_in, *idx_in, *keys, *order, *vbase;
+    unsigned long long *keys_in, *keys;
+    uint32_t *idx_in, *order, *vbase;
     unsigned long long* scan_out;
+    int key_bits = int(2 * D);   // (cell, then the slice's bits)
+    for (uint32_t k = n_sl - 1; k; k >>= 1) ++key_bits;
+    key_bits = std::max(key_bits, 1);
     size_t t_sort = 0, t_scan32 = 0, t_scan64 = 0;
-    CU(cub::DeviceRadixSort::SortPairs(nullptr, t_sort, (uint32_t*)nullptr, (uint32_t*)nullptr, (uint32_t*)nullptr,
-                                       (uint32_t*)nullptr, int(n), 0, 32, s));
+    CU(cub::DeviceRadixSort::SortPairs(nullptr, t_sort, (unsigned long long*)nullptr, (unsigned long long*)nullptr,
+                                       (uint32_t*)nullptr, (uint32_t*)nullptr, int(n), 0, key_bits, s));
     CU(cub::DeviceScan::ExclusiveSum(nullptr, t_scan32, (uint32_t*)nullptr, (uint32_t*)nullptr, int(n), s));
     CU(cub::DeviceScan::ExclusiveSum(nullptr, t_scan64, (unsigned long long*)nullptr, (unsigned long long*)nullptr, int(V), s));
     const size_t t_cub = std::max(t_sort, std::max(t_scan32, t_scan64));
     void* cub_tmp;
     const size_t w = size_t(n) * 4, wv = size_t(V) * 4;
+    const size_t cnt_bytes = (2 + size_t(PS_WORDS) * n_sl) * 4;
     CU(carve(c->contour_scratch, [&](Carve& cv) {
-        cv.take(keys_in, w); cv.take(idx_in, w); cv.take(keys, w); cv.take(order, w);
+        cv.take(keys_in, 2 * w); cv.take(idx_in, w); cv.take(keys, 2 * w); cv.take(order, w);
         cv.take(m.packed, w); cv.take(m.n_groups, w); cv.take(vbase, w);
-        cv.take(m.vpos, size_t(V) * sizeof(float2));
+        cv.take(m.vpos, size_t(V) * sizeof(float2)); cv.take(m.vslice, wv);
         cv.take(m.next, wv); cv.take(m.prev, wv);
         for (int k = 0; k < 2; ++k) { cv.take(b.P[k], wv); cv.take(b.A[k], wv); cv.take(b.R[k], wv); }
         cv.take(b.closed, V); cv.take(b.len, wv);
         cv.take(b.scan, size_t(V) * 8); cv.take(scan_out, size_t(V) * 8);
-        cv.take(m.counts, 64);
+        cv.take(m.counts, cnt_bytes);
         cv.take(cub_tmp, t_cub);
     }));
-    float2* out_v;
-    uint32_t* out_off;
-    uint8_t* out_closed;
-    CU(carve(c->contour_out, [&](Carve& cv) {
-        cv.take(out_v, size_t(V) * sizeof(float2)); cv.take(out_off, size_t(V + 1) * 4); cv.take(out_closed, V);
-    }));
-    c->contour_offsets = out_off;
-    c->contour_closed = out_closed;
+    m.per_slice = m.counts + 2;
+    if (int32_t rc = grow_keep(c, c->contour_out, size_t(v0 + V) * sizeof(float2), size_t(v0) * sizeof(float2))) return rc;
+    if (int32_t rc = grow_keep(c, c->contour_offs, size_t(p0 + V + 1) * 4, size_t(p0 + 1) * 4)) return rc;
+    if (int32_t rc = grow_keep(c, c->contour_flags, size_t(p0 + V), size_t(p0))) return rc;
+    EmitOut o{};
+    o.v = c->contour_out.as<float2>() + v0;
+    o.off = c->contour_offs.as<uint32_t>() + p0;
+    o.closed = c->contour_flags.as<uint8_t>() + p0;
+    o.v0 = uint32_t(v0);
+    o.to_model = sl[0].to_model != 0u;
+    o.M = sl[0].mat;
+    o.z = sl[0].z;
+    o.slices = n_sl > 1 ? d_sl : nullptr;
     m.keys = keys;
     m.order = order;
     m.vbase = vbase;
     CU(cudaEventRecord(get_event(c, 2), s));
-    CU(cudaMemsetAsync(m.counts, 0, 64, s));
+    CU(cudaMemsetAsync(m.counts, 0, cnt_bytes, s));
     CU(cudaMemsetAsync(m.next, 0xff, wv, s));
     CU(cudaMemsetAsync(m.prev, 0xff, wv, s));
     const unsigned bl = (n + 127) / 128, bv = (V + 127) / 128;
-    k_contour_keys<<<bl, 128, 0, s>>>(m.leaves, n, keys_in, idx_in);
+    k_contour_keys<<<bl, 128, 0, s>>>(m.leaves, n, D, keys_in, idx_in);
     size_t t = t_cub;
-    CU(cub::DeviceRadixSort::SortPairs(cub_tmp, t, keys_in, keys, idx_in, order, int(n), 0, 32, s));
+    CU(cub::DeviceRadixSort::SortPairs(cub_tmp, t, keys_in, keys, idx_in, order, int(n), 0, key_bits, s));
     k_contour_groups<<<bl, 128, 0, s>>>(m);
     t = t_cub;
     CU(cub::DeviceScan::ExclusiveSum(cub_tmp, t, m.n_groups, vbase, int(n), s));
@@ -606,79 +769,162 @@ static int32_t contour_finish(fc_ctx* c, uint32_t n, const fc_contour_cfg* cfg, 
     k_link_heads<<<bv, 128, 0, s>>>(m, b, V);
     t = t_cub;
     CU(cub::DeviceScan::ExclusiveSum(cub_tmp, t, b.scan, scan_out, int(V), s));
-    k_contour_emit<<<bv, 128, 0, s>>>(m, b, scan_out, out_v, out_off, out_closed, to_model, mat, cfg->z);
+    if (n_sl > 1) k_contour_emit<true><<<bv, 128, 0, s>>>(m, b, scan_out, o);
+    else k_contour_emit<false><<<bv, 128, 0, s>>>(m, b, scan_out, o);
     cudaEvent_t e3 = get_event(c, 3);
     CU(cudaEventRecord(e3, s));
     CU(cudaGetLastError());
-    uint32_t cnt[4];
-    if (int32_t wrc = wait_read(c, s, cc, cnt, m.counts, sizeof cnt)) return wrc;
-    c->contour_n_verts = cnt[0];
-    c->contour_n_polys = cnt[1];
-    info->n_vertices = cnt[0];
-    info->n_polylines = cnt[1];
-    info->n_closed = cnt[2];
-    info->n_open = cnt[3];
-    if (cfg->flags & FC_FLAG_TIMING) cudaEventElapsedTime(&info->contour_ms, get_event(c, 2), e3);
+    cnt.assign(cnt_bytes / 4, 0u);
+    if (int32_t wrc = wait_read(c, s, cc, cnt.data(), m.counts, cnt_bytes)) return wrc;
+    if (ms) cudaEventElapsedTime(ms, get_event(c, 2), e3);
     return FC_OK;
+}
+
+// The passes of a checked stack: every slice's polylines appended to the output in slice order, the per-slice counts
+// into per (when given) and their sums into info.  The caller holds the context's lock.
+static int32_t contour_stack(fc_ctx* c, const fc_tape* tape, uint32_t D, bool timing, const std::vector<ContourSlice>& sl,
+                             fc_contour_info* info, fc_contour_info* per, const CallCancel& cc) {
+    using namespace fdev;
+    const uint32_t N = uint32_t(sl.size());
+    ContourPlan plan(c, D, N);
+    uint64_t n_verts = 0, n_polys = 0;   // the stack's output so far
+    std::vector<uint32_t> cnt;
+    while (plan.more()) {
+        const ContourPlan::Range r = plan.take();
+        const ContourSlice* ps = sl.data() + r.f0;
+        ContourSlice* d_sl = nullptr;
+        if (r.n > 1) {
+            CU(c->contour_slices.ensure(size_t(r.n) * sizeof(ContourSlice)));
+            d_sl = c->contour_slices.as<ContourSlice>();
+            CU(cudaMemcpyAsync(d_sl, ps, size_t(r.n) * sizeof(ContourSlice), cudaMemcpyHostToDevice, c->stream));
+        }
+        // leaves: sized as fc_mesh_build sizes its own (the buffer of the last build, else the perimeter of the square
+        // in cells per slice, or the most per slice seen so far), and once more with the exact count
+        uint64_t cap = c->contour_leaves.cap / sizeof(ContourLeaf);
+        if (cap < 1024) cap = std::max<uint64_t>(1024, r.n * std::min<uint64_t>(1ull << (2 * D), 8ull << D));
+        if (plan.use_leaves > 0) cap = std::max<uint64_t>(cap, uint64_t(std::ceil(plan.use_leaves * 1.25 * r.n)));
+        cap = std::min<uint64_t>(cap, 0x7fffffffu);   // (cub's item counts are int)
+        uint32_t n = 0;
+        Counters ctr;
+        for (int attempt = 0; attempt < 2; ++attempt) {
+            CU(c->contour_leaves.ensure(cap * sizeof(ContourLeaf)));
+            if (timing) CU(cudaEventRecord(get_event(c, 0), c->stream));
+            if (int32_t rc = contour_sample(c, tape, D, ps, r.n, d_sl, c->contour_leaves.as<ContourLeaf>(), cap, &n, ctr, cc))
+                return rc;
+            if (n <= cap || ctr.error) break;
+            cap = n;
+        }
+        bool split = false;
+        if (int32_t rc = plan.observe(ctr, r, n, split)) return rc;
+        if (split) continue;
+        if (n > cap) return fail(FC_ERR_INVALID, "contour leaf buffer too small: " + std::to_string(n) + " surface leaves");
+        if (timing) {
+            float ms = 0;
+            CU(cudaEventRecord(get_event(c, 1), c->stream));
+            CU(cudaEventSynchronize(get_event(c, 1)));
+            cudaEventElapsedTime(&ms, get_event(c, 0), get_event(c, 1));
+            info->sampler_ms += ms;
+        }
+        if (!n) continue;
+        float ms = 0;
+        if (int32_t rc = contour_finish(c, n, D, ps, r.n, d_sl, n_verts, n_polys, cnt, timing ? &ms : nullptr, cc)) return rc;
+        info->contour_ms += ms;
+        uint32_t leaf_end = 0, vert_end = 0;
+        for (uint32_t k = 0; k < r.n; ++k) {
+            const uint32_t* wk = cnt.data() + 2 + PS_WORDS * k;
+            fc_contour_info si{};
+            if (wk[PS_LEAF_END]) {
+                si.n_leaves = wk[PS_LEAF_END] - leaf_end;
+                si.n_vertices = wk[PS_VERT_END] - vert_end;
+                leaf_end = wk[PS_LEAF_END];
+                vert_end = wk[PS_VERT_END];
+            }
+            si.n_polylines = wk[PS_POLYS];
+            si.n_closed = wk[PS_CLOSED];
+            si.n_open = wk[PS_OPEN];
+            if (per) per[r.f0 + k] = si;
+            info->n_leaves += si.n_leaves;
+            info->n_vertices += si.n_vertices;
+            info->n_polylines += si.n_polylines;
+            info->n_closed += si.n_closed;
+            info->n_open += si.n_open;
+        }
+        n_verts += cnt[0];
+        n_polys += cnt[1];
+        if (n_verts > 0xffffffffull)
+            return fail(FC_ERR_UNSUPPORTED, "contour stack has more vertices than 32-bit offsets can address");
+    }
+    c->contour_n_verts = uint32_t(n_verts);
+    c->contour_n_polys = uint32_t(n_polys);
+    c->contour_offsets = c->contour_offs.as<uint32_t>();
+    c->contour_closed = c->contour_flags.as<uint8_t>();
+    return FC_OK;
+}
+
+// fc_contour_build and fc_contour_build_slices: the checks of every slice, then the stack
+static int32_t contour_build(fc_ctx* c, const fc_tape* tape, const fc_contour_cfg* cfg, const fc_contour_slice* slices,
+                             uint32_t n_slices, fc_contour_info* info, fc_contour_info* per) {
+    memset(info, 0, sizeof *info);
+    if (per && n_slices) memset(per, 0, size_t(n_slices) * sizeof *per);
+    if (cfg->depth > FC_MAX_QUADTREE_DEPTH) return fail(FC_ERR_INVALID, "quadtree depth too large");
+    if (!slices && n_slices) return fail(FC_ERR_INVALID, "null slices");
+    for (uint32_t k = 0; k < n_slices; ++k)
+        if (slices[k].n_var_values > FC_MAX_VARS) return fail(FC_ERR_INVALID, "too many variable values");
+    if (tape->info.mem_count) return fail(FC_ERR_UNSUPPORTED, "contours need a tape without memory spills");
+    if (tape->info.n_outputs != 1) return fail(FC_ERR_INVALID, "ShapeTape has multiple outputs");
+    std::vector<ContourSlice> sl(n_slices);
+    for (uint32_t k = 0; k < n_slices; ++k) {
+        const fc_contour_slice& in = slices[k];
+        ContourSlice& out = sl[k];
+        if (int32_t vrc = bind_vars(tape, in.var_values, in.n_var_values, out.vb)) return vrc;
+        // the 3x3 embedded as the 2D renderers embed it: (x, y, z, 1) -> (m0 x + m1 y + m2, m3 x + m4 y + m5, z, m6 x + m7 y + m8)
+        bool to_model = false;
+        const int idx[3] = {0, 1, 3};
+        for (int i = 0; i < 3; ++i)
+            for (int j = 0; j < 3; ++j) {
+                const float v = in.has_transform ? in.world_to_model[3 * i + j] : (i == j ? 1.0f : 0.0f);
+                out.mat.m[4 * idx[i] + idx[j]] = v;
+                to_model |= v != (i == j ? 1.0f : 0.0f);
+            }
+        out.mat.m[10] = 1.0f;
+        out.z = in.z;
+        out.has_transform = in.has_transform;
+        out.to_model = in.has_transform && to_model;
+    }
+    CallCancel cc;
+    auto no_contour = [&](int32_t rc) {   // a failed or cancelled build leaves no contour
+        std::lock_guard<std::mutex> guard(c->mu);
+        c->contour_n_verts = c->contour_n_polys = 0;
+        memset(info, 0, sizeof *info);
+        if (per && n_slices) memset(per, 0, size_t(n_slices) * sizeof *per);
+        return rc;
+    };
+    if (int32_t crc = begin_call(c, cc)) return crc == FC_ERR_CANCELLED ? no_contour(crc) : crc;
+    std::unique_lock<std::mutex> guard(c->mu);
+    CU(cudaSetDevice(c->device));
+    c->contour_n_verts = c->contour_n_polys = 0;
+    const int32_t rc = n_slices ? contour_stack(c, tape, cfg->depth, cfg->flags & FC_FLAG_TIMING, sl, info, per, cc) : FC_OK;
+    guard.unlock();
+    return rc == FC_OK ? rc : no_contour(rc);
 }
 
 extern "C" {
 
 int32_t fc_contour_build(fc_ctx* c, const fc_tape* tape, const fc_contour_cfg* cfg, fc_contour_info* info) {
     if (!c || !tape || !cfg || !info) return fail(FC_ERR_INVALID, "null argument");
-    memset(info, 0, sizeof *info);
-    if (cfg->depth > FC_MAX_QUADTREE_DEPTH) return fail(FC_ERR_INVALID, "quadtree depth too large");
-    if (cfg->n_var_values > FC_MAX_VARS) return fail(FC_ERR_INVALID, "too many variable values");
-    if (tape->info.mem_count) return fail(FC_ERR_UNSUPPORTED, "contours need a tape without memory spills");
-    if (tape->info.n_outputs != 1) return fail(FC_ERR_INVALID, "ShapeTape has multiple outputs");
-    VarBind vb;
-    if (int32_t vrc = bind_vars(tape, cfg->var_values, cfg->n_var_values, vb)) return vrc;
-    CallCancel cc;
-    auto no_contour = [&](int32_t rc) {   // a cancelled build leaves no contour (a failed one keeps the previous)
-        std::lock_guard<std::mutex> guard(c->mu);
-        c->contour_n_verts = c->contour_n_polys = 0;
-        memset(info, 0, sizeof *info);
-        return rc;
-    };
-    if (int32_t crc = begin_call(c, cc)) return crc == FC_ERR_CANCELLED ? no_contour(crc) : crc;
-    // the 3x3 embedded as the 2D renderers embed it: (x, y, z, 1) -> (m0 x + m1 y + m2, m3 x + m4 y + m5, z, m6 x + m7 y + m8)
-    fdev::Mat4 mat{};
-    bool to_model = false;
-    const int idx[3] = {0, 1, 3};
-    for (int i = 0; i < 3; ++i)
-        for (int j = 0; j < 3; ++j) {
-            const float v = cfg->has_transform ? cfg->world_to_model[3 * i + j] : (i == j ? 1.0f : 0.0f);
-            mat.m[4 * idx[i] + idx[j]] = v;
-            to_model |= v != (i == j ? 1.0f : 0.0f);
-        }
-    mat.m[10] = 1.0f;
-    std::unique_lock<std::mutex> guard(c->mu);
-    CU(cudaSetDevice(c->device));
-    const bool timing = cfg->flags & FC_FLAG_TIMING;
-    // leaves: sized as fc_mesh_build sizes its own (the buffer of the last build, else the perimeter of the square in
-    // cells), and once more with the exact count
-    uint64_t cap = c->contour_leaves.cap / sizeof(fdev::ContourLeaf);
-    if (cap < 1024) cap = std::max<uint64_t>(1024, std::min<uint64_t>(1ull << (2 * cfg->depth), 8ull << cfg->depth));
-    uint32_t n = 0;
-    c->contour_n_verts = c->contour_n_polys = 0;
-    int32_t rc = FC_OK;
-    for (int attempt = 0; attempt < 2; ++attempt) {
-        CU(c->contour_leaves.ensure(cap * sizeof(fdev::ContourLeaf)));
-        if (timing) CU(cudaEventRecord(get_event(c, 0), c->stream));
-        rc = contour_sample(c, tape, cfg, vb, mat, c->contour_leaves.as<fdev::ContourLeaf>(), cap, &n, cc);
-        if (rc == FC_OK || rc == FC_ERR_CANCELLED) break;
-        if (n > cap && attempt == 0) { cap = n; continue; }
-        break;
-    }
-    if (rc == FC_OK && timing) {
-        CU(cudaEventRecord(get_event(c, 1), c->stream));
-        CU(cudaEventSynchronize(get_event(c, 1)));
-        cudaEventElapsedTime(&info->sampler_ms, get_event(c, 0), get_event(c, 1));
-    }
-    info->n_leaves = n;
-    if (rc == FC_OK && n) rc = contour_finish(c, n, cfg, mat, cfg->has_transform && to_model, info, cc);
-    guard.unlock();
-    return rc == FC_ERR_CANCELLED ? no_contour(rc) : rc;
+    fc_contour_slice one{};
+    one.z = cfg->z;
+    one.has_transform = cfg->has_transform;
+    memcpy(one.world_to_model, cfg->world_to_model, sizeof one.world_to_model);
+    one.n_var_values = cfg->n_var_values;
+    memcpy(one.var_values, cfg->var_values, sizeof one.var_values);
+    return contour_build(c, tape, cfg, &one, 1, info, nullptr);
+}
+
+int32_t fc_contour_build_slices(fc_ctx* c, const fc_tape* tape, const fc_contour_cfg* cfg, const fc_contour_slice* slices,
+                                uint32_t n_slices, fc_contour_info* info, fc_contour_info* per_slice) {
+    if (!c || !tape || !cfg || !info) return fail(FC_ERR_INVALID, "null argument");
+    return contour_build(c, tape, cfg, slices, n_slices, info, per_slice);
 }
 
 int32_t fc_contour_read(fc_ctx* c, float* vertices, uint32_t* offsets, uint8_t* closed) {

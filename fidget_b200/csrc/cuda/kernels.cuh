@@ -156,6 +156,18 @@ struct Frame2D {
     VarBind vb;
 };
 
+// One slice of a contour stack (fc_contour_build_slices): what fc_contour_build takes from its cfg per call.  The
+// stacked quadtree gives slice k the cell rows [k * 2^depth, (k + 1) * 2^depth), and a cell's rows are taken relative
+// to its slice.  has_transform stays a flag of its own: skipping the transform is not applying the identity (0 * z is
+// NaN for a non-finite z, and a sum can flip a signed zero).  to_model: vertices go back through `mat` (has_transform
+// and a matrix other than the identity).
+struct ContourSlice {
+    Mat4 mat;
+    float z;
+    uint32_t has_transform, to_model;
+    VarBind vb;
+};
+
 // Scene renders (fc_render3d_scene): K placements (a tape and its Frame2D) share one heightmap and one occlusion map.
 // Placement k's jobs carry k in TileJob::pad.  A heightmap key orders what the merged image keeps: the greater clamped
 // depth, then the lower placement, then, inside one placement, what fc_render3d orders by (raw depth, then a leaf id
@@ -316,6 +328,20 @@ template <bool FRAMES, bool SCENE, class P>
 __device__ __forceinline__ FrameView view_of(const P& p, uint32_t y, uint32_t pl) {
     if (SCENE) return FrameView{&p.frames[pl].mat, p.frames[pl].z, &p.frames[pl].vb, 0u, 0u};
     return frame_of<FRAMES>(p, y);
+}
+// QUAD (contours): the one slice of fc_contour_build in the launch parameters, or with STACK the slice of cell row y in
+// the table `slices` (a kernel argument of its own: LevelParams keeps the layout the other level kernels are built with),
+// frame_rows rows each
+template <bool STACK>
+__device__ __forceinline__ FrameView quad_view(const LevelParams& p, const ContourSlice* slices, uint32_t y) {
+    if (!STACK) return FrameView{&p.mat, p.z2d, &p.vb, 0u, 0u};
+    const uint32_t s = y / p.frame_rows;
+    const ContourSlice* sl = slices + s;
+    return FrameView{&sl->mat, sl->z, &sl->vb, s * p.frame_rows, 0u};
+}
+template <bool STACK>
+__device__ __forceinline__ uint32_t quad_has_transform(const LevelParams& p, const ContourSlice* slices, uint32_t y) {
+    return STACK ? slices[y / p.frame_rows].has_transform : p.has_transform;
 }
 #endif
 

@@ -44,9 +44,12 @@ __device__ __forceinline__ void store_fill(FillRec* dst, const FillRec& fr) {
 
 // QUAD (2D only): the quadtree of fc_contour_build.  Coordinates are cells at the finest depth with world-square bounds
 // coord * cell_h - 1, seen through `mat` when has_transform, at Z = [z2d, z2d]; classified tiles are dropped (no fills).
+// With FRAMES a contour slice stack: each cell's slice (`slices`, frame_rows rows each) supplies Z, the matrix, its
+// has_transform and the vars, and the cell's rows are relative to its slice.
 template <int DIM, bool FUSED, bool FRAMES = false, bool SCENE = false, bool QUAD = false>
 __device__ __forceinline__ void level_job(const LevelParams& p, uint32_t j, uint32_t n_roots, itv* slots, uint32_t* cs,
-                                          uint32_t (*live)[32], int lane, uint32_t epoch) {
+                                          uint32_t (*live)[32], int lane, uint32_t epoch,
+                                          const ContourSlice* slices = nullptr) {
     const uint32_t T = p.tile;
     bool cull_open = false, cull_check = false;
     TapeRef tr;
@@ -105,7 +108,7 @@ __device__ __forceinline__ void level_job(const LevelParams& p, uint32_t j, uint
         }
         // Region in screen coordinates -> model space (pixel.rs:325-342, voxel.rs:291-306); in a frame batch a
         // tile's coordinates are relative to its frame (per lane at level 0, whose 32 roots may span frames)
-        const FrameView fv = view_of<FRAMES, SCENE>(p, cy, pl);
+        const FrameView fv = QUAD ? quad_view<FRAMES>(p, slices, cy) : view_of<FRAMES, SCENE>(p, cy, pl);
         const Mat4& M = *fv.mat;
         const VarBind& vb = *fv.vb;
         itv X = iv(float(cx), float(cx) + float(T));
@@ -122,9 +125,10 @@ __device__ __forceinline__ void level_job(const LevelParams& p, uint32_t j, uint
             else { vx = X; vy = Y; vz = Z; }
         } else if constexpr (QUAD) {
             const float h = p.cell_h;
+            const uint32_t ry = cy - fv.y0;
             X = iv(float(cx) * h - 1.0f, float(cx + T) * h - 1.0f);
-            Y = iv(float(cy) * h - 1.0f, float(cy + T) * h - 1.0f);
-            if (p.has_transform) xform_iv(p.mat, X, Y, Z, vx, vy, vz);
+            Y = iv(float(ry) * h - 1.0f, float(ry + T) * h - 1.0f);
+            if (quad_has_transform<FRAMES>(p, slices, cy)) xform_iv(FRAMES ? M : p.mat, X, Y, Z, vx, vy, vz);
             else { vx = X; vy = Y; vz = Z; }
         } else {
             xform_iv(M, X, Y, Z, vx, vy, vz);

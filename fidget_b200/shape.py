@@ -1023,6 +1023,91 @@ def contour(shape: CudaShape, depth: int, z: float = 0.0, world_to_model=None, v
     return verts, offsets, closed.astype(bool), {n: getattr(info, n) for n, _ in info._fields_}
 
 
+def contour_slice_table(z=None, world_to_model=None, var_values=None):
+    """The ``fc_contour_slice`` table of ``contour_slices``: slice k's Z, ``world_to_model`` (3x3, world -> model) and
+    ShapeVars, each what ``contour`` puts into ``fc_contour_cfg`` for that slice's values.  Every argument given is per
+    slice (leading dimension n: ``z`` [n], ``world_to_model`` [n, 3, 3], ``var_values`` [n, k]); the others take
+    ``contour``'s defaults (z = 0, no transform, no values).  A ``world_to_model`` entry of None is a slice without a
+    transform, as ``contour``'s ``world_to_model=None`` (not the same as the identity flagged as a transform: a
+    non-finite z then becomes NaN).  Lengths that disagree raise ValueError, as in
+    ``frame_table``; with no per-slice argument at all there is one slice."""
+    per = {}
+    if z is not None:
+        per["z"] = np.asarray(z, dtype=np.float32).reshape(-1)
+    if var_values is not None:
+        vv = np.asarray(var_values, dtype=np.float32)
+        if vv.ndim != 2 or vv.shape[1] > _lib.FC_MAX_VARS:
+            raise ValueError(f"var_values must be [n, k] with k <= {_lib.FC_MAX_VARS}")
+        per["var_values"] = vv
+    if world_to_model is not None:
+        wm = [None if w is None else np.asarray(w, dtype=np.float32) for w in world_to_model]
+        if any(w is not None and w.shape != (3, 3) for w in wm):
+            raise ValueError("world_to_model must be [n, 3, 3] (an entry may be None: no transform)")
+        per["world_to_model"] = wm
+    lengths = {k: len(v) for k, v in per.items()}
+    if len(set(lengths.values())) > 1:
+        raise ValueError(f"per-slice arguments disagree in length: {lengths}")
+    n = next(iter(lengths.values())) if lengths else 1
+    table = (_lib.FcContourSlice * n)()
+    for k in range(n):
+        s = table[k]
+        s.z = float(per["z"][k]) if "z" in per else 0.0
+        if "world_to_model" in per and per["world_to_model"][k] is not None:
+            s.has_transform = 1
+            s.world_to_model[:] = per["world_to_model"][k].reshape(9).tolist()
+        values = per["var_values"][k] if "var_values" in per else ()
+        s.n_var_values = len(values)
+        for i, v in enumerate(values):
+            s.var_values[i] = float(v)
+    return table
+
+
+def split_contour_stack(vertices, offsets, closed, n_polylines):
+    """The per-slice ``(vertices, offsets, closed)`` of a stacked contour: slice k takes the next ``n_polylines[k]``
+    polylines, its offsets rebased to 0 -- each exactly what ``contour`` returns for that slice."""
+    v = np.asarray(vertices, dtype=np.float32).reshape(-1, 2)
+    off = np.asarray(offsets, dtype=np.uint32)
+    cl = np.asarray(closed).astype(bool)
+    out, p = [], 0
+    for npk in n_polylines:
+        npk = int(npk)
+        o = off[p:p + npk + 1]
+        out.append((v[int(o[0]):int(o[-1])], (o - o[0]).astype(np.uint32), cl[p:p + npk]))
+        p += npk
+    if p != len(cl) or len(off) != p + 1:
+        raise ValueError("per-slice polyline counts do not add up to the stack's")
+    return out
+
+
+def contour_slices(shape: CudaShape, depth: int, z=None, world_to_model=None, var_values=None,
+                   cancel: CancelToken | None = None):
+    """Contours of many slices in one call (``fc_contour_build_slices``): slice k is bit for bit ``contour`` of its
+    own ``z`` / ``world_to_model`` / ``var_values`` (see ``contour_slice_table``).  Returns ``(slices, info,
+    per_slice)``: ``slices[k] = (vertices, offsets, closed)`` as ``contour`` returns them, ``info`` the totals (device
+    times summed over passes) and ``per_slice[k]`` slice k's counts.  None when ``cancel`` cancelled the call (the
+    context then holds no contour)."""
+    lib = shape._lib
+    table = contour_slice_table(z=z, world_to_model=world_to_model, var_values=var_values)
+    n = len(table)
+    c = _lib.FcContourCfg()
+    c.depth = depth
+    c.flags = _lib.FC_FLAG_TIMING
+    info = _lib.FcContourInfo()
+    per = (_lib.FcContourInfo * n)()
+    rc = shape.cuda._cancellable(cancel, lambda: lib.fc_contour_build_slices(
+        shape.cuda._h, shape._h, C.byref(c), table, n, C.byref(info), per))
+    if rc == _lib.FC_ERR_CANCELLED:
+        return None
+    _ck(rc)
+    verts = np.zeros((info.n_vertices, 2), dtype=np.float32)
+    offsets = np.zeros(info.n_polylines + 1, dtype=np.uint32)
+    closed = np.zeros(info.n_polylines, dtype=np.uint8)
+    _ck(lib.fc_contour_read(shape.cuda._h, _ptr(verts), _ptr(offsets), _ptr(closed)))
+    as_dict = lambda x: {f: getattr(x, f) for f, _ in x._fields_}   # noqa: E731
+    per_slice = [as_dict(per[k]) for k in range(n)]
+    return split_contour_stack(verts, offsets, closed, [p["n_polylines"] for p in per_slice]), as_dict(info), per_slice
+
+
 def contours_svg(vertices, offsets, closed, size: float = 512.0, stroke: str = "black", fill: str = "none",
                  stroke_width: float = 1.0) -> str:
     """An SVG document with one ``<path>`` per polyline of ``contour``'s output, closed ones ending in ``Z``.  The

@@ -553,9 +553,38 @@ typedef struct fc_contour_info {
     float sampler_ms, contour_ms;   /* device time of the quadtree sampler / of vertices, segments and linking */
 } fc_contour_info;
 int32_t fc_contour_build(fc_ctx* ctx, const fc_tape* tape, const fc_contour_cfg* cfg, fc_contour_info* info);
-/* The last fc_contour_build's polylines: vertices (2 floats each, in polyline order), offsets (n_polylines + 1: polyline
- * k is vertices offsets[k] .. offsets[k + 1] - 1) and closed (one byte per polyline, 1 = the last vertex joins the
- * first).  Host or device pointers; any may be NULL. */
+/* Many slices of one tape contoured in one call: layers for a printer or a laser cutter, section drawings, a profile
+ * swept through a ShapeVars parameter.  Slice k's polylines are bit for bit those of fc_contour_build called with cfg's
+ * depth and flags plus slice k's z, has_transform, world_to_model and var_values (vertices, offsets relative to the
+ * slice, closed flags, canonical order).  The slices of a pass share each launch of the pipeline: one tall quadtree grid
+ * holds them, so every level launch holds the cells of all of them.
+ *  - cfg supplies depth and flags; its z, has_transform, world_to_model and var_values are ignored.
+ *  - fc_contour_read returns the whole stack: the slices in order, each slice's polylines in its canonical order, offsets
+ *    global over the stack.  Whichever of fc_contour_build and fc_contour_build_slices ran last is what it returns.
+ *  - per_slice (may be NULL, n_slices entries): slice k's n_leaves, n_vertices, n_polylines, n_closed and n_open; its
+ *    timing fields are 0.  info: the sums of those counts, and with FC_FLAG_TIMING sampler_ms and contour_ms summed
+ *    over passes.
+ *  - passes: the first pass holds one slice, later ones are sized from the largest per-slice arena, job-list and leaf
+ *    use seen so far (leaves and link scratch within FC_FRAMES_PASS_BYTES), and a pass that overflows anyway is run again
+ *    in halves: FC_ERR_ARENA or a work-list overflow comes back only where one slice alone would give it.
+ *  - Errors are fc_contour_build's, checked for every slice before anything is allocated or launched (depth, a
+ *    multi-output tape, more than FC_MAX_VARS values or a slice without a value for a bound variable: FC_ERR_INVALID; a
+ *    spilled tape: FC_ERR_UNSUPPORTED), and FC_ERR_INVALID for slices == NULL with n_slices > 0.  A stack of more than
+ *    2^32 - 1 vertices in all gives FC_ERR_UNSUPPORTED.  A failed or cancelled call (the cancel flag behaves as in
+ *    fc_contour_build) leaves no contour; n_slices == 0 launches nothing and leaves an empty contour. */
+typedef struct fc_contour_slice {
+    float z;                        /* as fc_contour_cfg.z */
+    uint32_t has_transform;         /* as fc_contour_cfg.has_transform */
+    float world_to_model[9];        /* as fc_contour_cfg.world_to_model */
+    uint32_t n_var_values;          /* ShapeVars of this slice, as fc_contour_cfg */
+    float var_values[FC_MAX_VARS];
+} fc_contour_slice;
+int32_t fc_contour_build_slices(fc_ctx* ctx, const fc_tape* tape, const fc_contour_cfg* cfg,
+                                const fc_contour_slice* slices /* host */, uint32_t n_slices,
+                                fc_contour_info* info /* totals */, fc_contour_info* per_slice /* may be NULL */);
+/* The polylines of the last fc_contour_build or fc_contour_build_slices: vertices (2 floats each, in polyline order),
+ * offsets (n_polylines + 1: polyline k is vertices offsets[k] .. offsets[k + 1] - 1) and closed (one byte per polyline,
+ * 1 = the last vertex joins the first).  Host or device pointers; any may be NULL. */
 int32_t fc_contour_read(fc_ctx* ctx, float* vertices, uint32_t* offsets, uint8_t* closed);
 
 /* ---- constraint solver (fidget-solver) ----------------------------------------------------------------------- */

@@ -14,6 +14,7 @@
 #include <vector>
 
 #include "../../../include/fidget_cuda.h"
+#include "env.h"
 #include "kernels.cuh"
 #include "effects.cuh"
 
@@ -92,41 +93,6 @@ inline void* pinned_device_alias(const void* p) {
         return nullptr;
     }
     return a.type == cudaMemoryTypeHost ? a.devicePointer : nullptr;
-}
-
-// Tuning knobs from the environment.  FIDGET_B200_ENV_LIVE=1 re-reads them on every call (tests flip knobs
-// between renders); otherwise each (name) is read once per process -- no getenv on the render path.
-inline int env_int(const char* name, int dflt) {
-    struct Slot { const char* name; int value; bool set; };
-    static Slot cache[32];
-    static std::mutex mu;
-    static const bool live = [] { const char* v = getenv("FIDGET_B200_ENV_LIVE"); return v && *v && atoi(v) != 0; }();
-    auto read = [&](int d) { const char* v = getenv(name); return v && *v ? atoi(v) : d; };
-    if (live) return read(dflt);
-    std::lock_guard<std::mutex> g(mu);
-    for (auto& sl : cache) {
-        if (sl.name == name) return sl.set ? sl.value : dflt;
-        if (!sl.name) {
-            const char* v = getenv(name);
-            sl.name = name;
-            sl.set = v && *v;
-            sl.value = sl.set ? atoi(v) : 0;
-            return sl.set ? sl.value : dflt;
-        }
-    }
-    return read(dflt);
-}
-// String knobs, read like env_int: once per process, or on every call with FIDGET_B200_ENV_LIVE=1
-inline std::string env_str(const char* name) {
-    static std::mutex mu;
-    static std::vector<std::pair<const char*, std::string>> cache;
-    static const bool live = [] { const char* v = getenv("FIDGET_B200_ENV_LIVE"); return v && *v && atoi(v) != 0; }();
-    auto read = [&] { const char* v = getenv(name); return std::string(v ? v : ""); };
-    if (live) return read();
-    std::lock_guard<std::mutex> g(mu);
-    for (auto& kv : cache) if (kv.first == name) return kv.second;
-    cache.emplace_back(name, read());
-    return cache.back().second;
 }
 
 // Cancellation of one call (fc_ctx_set_cancel): the flag attached when the call began and the device side's view
@@ -223,6 +189,15 @@ struct fc_tape {
     std::shared_ptr<struct Sched> sched;
 };
 
+// A tape as the kernels take it, its choice scratch words per lane (LevelParams::choice_words) and the arena a launch
+// may fill, in clauses
+inline TapeRef tape_ref(const fc_tape* t) { return TapeRef{t->dev, t->info.n_ops, t->info.ref_len, t->info.choice_count}; }
+inline uint32_t choice_words(const fc_tape* t) { return (t->info.choice_count + 15) / 16 + 1; }
+inline uint64_t arena_clauses(const fc_ctx* c) { return std::min<uint64_t>(c->arena.cap, c->arena_bytes) / sizeof(uint2); }
+// Work lists hold only ambiguous tiles (a surface-like set), so they are capped well below the N^3 tile count
+// (FIDGET_B200_MAX_TILES_M, 16 Mi jobs); overflow is reported, not ignored
+inline uint64_t list_cap_limit() { return uint64_t(env_int("FIDGET_B200_MAX_TILES_M", 16)) << 20; }
+
 struct Sched {
     int device = 0;
     uint64_t hash = 0;
@@ -267,6 +242,23 @@ int32_t bulk_eval(fc_eval* e, const fc_tape* t, const void* const* vars, void* c
                   const std::function<int32_t(BulkParams&, const std::vector<const void*>&)>& launch);
 int32_t transcode(const uint32_t* words, size_t n_words, uint8_t reg_count, uint32_t mem_count, uint32_t n_vars,
                   uint32_t n_outputs, std::vector<uint2>& out, uint32_t& n_choices);
+// octree_capi.cu
+// The uniform-tree samplers (octree_sample_device, contour_sample) over n_roots root cells, each with 2^dim children per
+// level down to depth D: their scratch (choice scratch, arena, counters with 64 zeroed bytes after them, stats, the
+// job lists, `cap` leaf tapes) and the LevelParams every level of both shares
+struct TreeScratch {
+    uint32_t D = 0;
+    int grid_blocks = 0;
+    uint32_t choice_words = 0;
+    uint64_t level_cap[MAX_LEVELS + 1] = {};   // level l's job list: the cells at depth min(l, D), capped
+    // blocks of a level launch of `warps` warps, within the grid
+    int blocks(uint64_t warps) const {
+        return std::max(int(std::min<uint64_t>((warps + WARPS_PER_BLOCK - 1) / WARPS_PER_BLOCK, uint64_t(grid_blocks))), 1);
+    }
+};
+int32_t tree_scratch(fc_ctx* c, const fc_tape* tape, uint32_t D, int dim, uint64_t n_roots, uint64_t cap, TreeScratch& t);
+LevelParams tree_level(fc_ctx* c, const fc_tape* tape, const TreeScratch& t, int l, uint32_t has_transform,
+                       const VarBind& vb, const CallCancel& cc);
 // render.cu
 int32_t pick_tile_sizes(const uint32_t* ts_in, uint32_t n_in, const uint32_t* dflt, uint32_t n_dflt, uint32_t max_size,
                         std::vector<uint32_t>& ts);

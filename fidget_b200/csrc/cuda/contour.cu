@@ -29,6 +29,7 @@
 
 #include "capi_internal.h"
 #include "level_job.cuh"
+#include "pass_plan.h"
 
 namespace fdev {
 
@@ -514,68 +515,6 @@ using fdev::ContourSlice;
 constexpr uint64_t CONTOUR_LEAF_BYTES = sizeof(fdev::ContourLeaf) + sizeof(fdev::TapeRef) + 7 * 4 + 12 +
                                         2 * (8 + 4 + 2 * 4 + 6 * 4 + 1 + 4 + 2 * 8 + 8 + 4 + 1);
 
-// The passes of a slice stack, with the overflow policy of the 3D batches (PassPlan, render.cu): the first pass holds
-// one slice; later ones are sized from the largest per-slice use seen so far (arena clauses, jobs of the levels whose
-// list is capped, surface leaves against FC_FRAMES_PASS_BYTES) with headroom 1.5; a pass that overflows anyway is run
-// again as two halves, and only a one-slice pass returns the error.  FIDGET_B200_FRAMES_PER_PASS fixes the pass size.
-struct ContourPlan {
-    struct Range { uint32_t f0, n; };
-    uint32_t depth, n_items, n_max, next = 0;
-    int forced;
-    bool measured;
-    uint64_t arena_cap, cap_limit;
-    double use_arena = 0, use_leaves = 0, use_jobs[fdev::MAX_LEVELS + 1] = {};
-    std::vector<Range> redo;                    // halves of overflowed passes (a stack: the first half runs next)
-
-    ContourPlan(const fc_ctx* c, uint32_t d, uint32_t n) : depth(d), n_items(n) {
-        // (a pass's slice index is 16 bits in its leaves, and its cell rows must fit 32 bits)
-        n_max = uint32_t(std::min<uint64_t>({n, 0xffffu, (1ull << (32 - d)) - 1}));
-        forced = env_int("FIDGET_B200_FRAMES_PER_PASS", 0);
-        if (forced > 0) n_max = std::min<uint32_t>(n_max, uint32_t(forced));
-        measured = forced > 0;
-        arena_cap = std::min<uint64_t>(c->arena.cap, c->arena_bytes) / sizeof(uint2);
-        cap_limit = uint64_t(env_int("FIDGET_B200_MAX_TILES_M", 16)) << 20;
-    }
-    // the jobs of level l that every cell of n slices would queue, and the list's capacity
-    uint64_t worst(uint32_t n, int l) const { return uint64_t(n) << (2 * std::min<uint32_t>(uint32_t(l), depth)); }
-    uint64_t level_cap(uint32_t n, int l) const { return std::min(worst(n, l), cap_limit); }
-    bool more() const { return next < n_items || !redo.empty(); }
-    bool fits(uint32_t n) const {
-        const double h = 1.5 * n;
-        if (use_arena * h > double(arena_cap)) return false;
-        if (use_leaves * h * double(CONTOUR_LEAF_BYTES) > double(FC_FRAMES_PASS_BYTES)) return false;
-        for (int l = 1; l <= int(depth) + 1; ++l)
-            if (level_cap(n, l) < worst(n, l) && use_jobs[l] * h > double(level_cap(n, l))) return false;
-        return true;
-    }
-    Range take() {
-        if (!redo.empty()) { const Range r = redo.back(); redo.pop_back(); return r; }
-        uint32_t n = std::min(n_max, n_items - next);
-        if (!measured) n = 1;
-        else if (forced <= 0) while (n > 1 && !fits(n)) --n;
-        const Range r{next, n};
-        next += n;
-        return r;
-    }
-    // Records the use of the sampled pass r.  Its error if it fails; else `split` says that it overflowed and its
-    // halves are queued in its place.
-    int32_t observe(const fdev::Counters& ctr, const Range& r, uint32_t n_leaves, bool& split) {
-        const double n = double(r.n);
-        use_arena = std::max(use_arena, double(ctr.arena_top) / n);
-        use_leaves = std::max(use_leaves, double(n_leaves) / n);
-        for (int l = 1; l <= int(depth) + 1; ++l) use_jobs[l] = std::max(use_jobs[l], double(ctr.n_jobs[l]) / n);
-        measured = true;
-        split = false;
-        if (!ctr.error) return FC_OK;
-        if (r.n == 1 || (ctr.error & ~3u)) return device_error(ctr.error);
-        const uint32_t h = r.n / 2;
-        redo.push_back(Range{r.f0 + h, r.n - h});
-        redo.push_back(Range{r.f0, h});
-        split = true;
-        return FC_OK;
-    }
-};
-
 // Grows `b` to at least `need` bytes, keeping its first `keep` bytes (the polylines of the stack's earlier passes)
 int32_t grow_keep(fc_ctx* c, DevBuf& b, size_t need, size_t keep) {
     if (need <= b.cap) return FC_OK;
@@ -601,61 +540,25 @@ static int32_t contour_sample(fc_ctx* c, const fc_tape* tape, uint32_t D, const 
     const int L = int(D) + 1;
     const bool stack = n > 1;
     cudaStream_t s = c->stream;
-    const int grid_blocks = c->sm_count * env_int("FIDGET_B200_BLOCKS_PER_SM", 6);
-    const uint32_t choice_words = (tape->info.choice_count + 15) / 16 + 1;
-    CU(c->choice_scratch.ensure(size_t(grid_blocks) * WARPS_PER_BLOCK * choice_words * 32 * 4));
-    CU(c->arena.ensure(c->arena_bytes));
-    CU(c->counters.ensure(sizeof(Counters) + 64));
-    CU(c->stats.ensure(sizeof(Stats)));
-    const uint64_t cap_limit = uint64_t(env_int("FIDGET_B200_MAX_TILES_M", 16)) << 20;
-    std::vector<uint64_t> level_cap(L + 1);
-    for (int l = 1; l <= L; ++l) {
-        level_cap[l] = std::min<uint64_t>(uint64_t(n) << (2 * std::min(l, int(D))), cap_limit);
-        CU(c->jobs[l].ensure(level_cap[l] * sizeof(TileJob)));
-    }
-    CU(c->leaf_tapes.ensure(std::max<uint64_t>(cap, 1) * sizeof(TapeRef)));
-    CU(cudaMemsetAsync(c->counters.p, 0, sizeof(Counters) + 64, s));
+    TreeScratch t;
+    if (int32_t trc = tree_scratch(c, tape, D, 2, n, cap, t)) return trc;
     uint32_t* d_n_out = reinterpret_cast<uint32_t*>(c->counters.as<char>() + sizeof(Counters));
     for (int l = 0; l < L; ++l) {
-        LevelParams p{};
-        p.level = l;
-        p.tile = 1u << (D - uint32_t(l));
-        p.n_axis = l ? 2 : 0;
-        p.is_last = (l == L - 1);
-        p.root_mode = (l == 0);
+        LevelParams p = tree_level(c, tape, t, l, sl[0].has_transform, sl[0].vb, cc);
         p.roots_x = p.roots_z = 1;
         p.roots_y = n;   // one root cell per slice, stacked along Y
-        p.root_tape.ptr = tape->dev;
-        p.root_tape.n_ops = tape->info.n_ops;
-        p.root_tape.ref_len = tape->info.ref_len;
-        p.root_tape.n_choices = tape->info.choice_count;
         p.width = p.height = 1u << D;
         p.depth = 1;
         p.z2d = sl[0].z;
         p.mat = sl[0].mat;
-        p.jobs_in = l ? c->jobs[l].as<TileJob>() : nullptr;
-        p.cap_in = l ? uint32_t(level_cap[l]) : 0;
-        p.jobs_out = c->jobs[l + 1].as<TileJob>();
-        p.cap_out = uint32_t(level_cap[l + 1]);
-        p.arena = c->arena.as<uint2>();
-        p.arena_cap = std::min<uint64_t>(c->arena.cap, c->arena_bytes) / sizeof(uint2);
-        p.choice_scratch = c->choice_scratch.as<uint32_t>();
-        p.choice_words = choice_words;
-        p.ctr = c->counters.as<Counters>();
-        p.mode = 1;
-        p.has_transform = sl[0].has_transform;
-        p.cell_h = 2.0f / float(1u << D);
-        p.vb = sl[0].vb;
-        p.cancel = cc.ref;
         p.frame_rows = 1u << D;
-        const uint64_t warps = l ? std::max<uint64_t>(1, (uint64_t(n) << (2 * l)) / 4) : (n + 31) / 32;
-        const int blocks = int(std::min<uint64_t>((warps + WARPS_PER_BLOCK - 1) / WARPS_PER_BLOCK, uint64_t(grid_blocks)));
-        if (stack) k_contour_level<true><<<std::max(blocks, 1), WARPS_PER_BLOCK * 32, 0, s>>>(p, d_sl);
-        else k_contour_level<false><<<std::max(blocks, 1), WARPS_PER_BLOCK * 32, 0, s>>>(p, nullptr);
+        const int blocks = t.blocks(l ? std::max<uint64_t>(1, (uint64_t(n) << (2 * l)) / 4) : (n + 31) / 32);
+        if (stack) k_contour_level<true><<<blocks, WARPS_PER_BLOCK * 32, 0, s>>>(p, d_sl);
+        else k_contour_level<false><<<blocks, WARPS_PER_BLOCK * 32, 0, s>>>(p, nullptr);
     }
     ContourLeafParams q{};
     q.jobs = c->jobs[L].as<TileJob>();
-    q.cap_jobs = uint32_t(level_cap[L]);
+    q.cap_jobs = uint32_t(t.level_cap[L]);
     q.ctr = c->counters.as<Counters>();
     q.list = L; q.cursor = L;
     q.cell_h = 2.0f / float(1u << D);
@@ -786,11 +689,25 @@ static int32_t contour_stack(fc_ctx* c, const fc_tape* tape, uint32_t D, bool ti
                              fc_contour_info* info, fc_contour_info* per, const CallCancel& cc) {
     using namespace fdev;
     const uint32_t N = uint32_t(sl.size());
-    ContourPlan plan(c, D, N);
+    // Passes as the 3D batches' (pass_plan.h), the measured quantity being surface leaves (with their link scratch)
+    // within FC_FRAMES_PASS_BYTES.  A pass's slice index is 16 bits in its leaves, and its cell rows must fit 32 bits.
+    const uint64_t cap_limit = list_cap_limit();
+    PassPlan plan(N, uint32_t(std::min<uint64_t>({N, 0xffffu, (1ull << (32 - D)) - 1})), [&](uint32_t n) {
+        PassLimits lim;
+        lim.arena_cap = arena_clauses(c);
+        for (int l = 1; l <= int(D) + 1; ++l) {   // every cell of n slices at depth min(l, D) queued
+            lim.worst[l] = uint64_t(n) << (2 * std::min<uint32_t>(uint32_t(l), D));
+            lim.cap[l] = std::min(lim.worst[l], cap_limit);
+        }
+        lim.extra_on = true;
+        lim.extra_scale = double(CONTOUR_LEAF_BYTES);
+        lim.extra_cap = FC_FRAMES_PASS_BYTES;
+        return lim;
+    });
     uint64_t n_verts = 0, n_polys = 0;   // the stack's output so far
     std::vector<uint32_t> cnt;
     while (plan.more()) {
-        const ContourPlan::Range r = plan.take();
+        const PassPlan::Range r = plan.take();
         const ContourSlice* ps = sl.data() + r.f0;
         ContourSlice* d_sl = nullptr;
         if (r.n > 1) {
@@ -802,7 +719,7 @@ static int32_t contour_stack(fc_ctx* c, const fc_tape* tape, uint32_t D, bool ti
         // in cells per slice, or the most per slice seen so far), and once more with the exact count
         uint64_t cap = c->contour_leaves.cap / sizeof(ContourLeaf);
         if (cap < 1024) cap = std::max<uint64_t>(1024, r.n * std::min<uint64_t>(1ull << (2 * D), 8ull << D));
-        if (plan.use_leaves > 0) cap = std::max<uint64_t>(cap, uint64_t(std::ceil(plan.use_leaves * 1.25 * r.n)));
+        if (plan.use_extra > 0) cap = std::max<uint64_t>(cap, uint64_t(std::ceil(plan.use_extra * 1.25 * r.n)));
         cap = std::min<uint64_t>(cap, 0x7fffffffu);   // (cub's item counts are int)
         uint32_t n = 0;
         Counters ctr;
@@ -815,7 +732,7 @@ static int32_t contour_stack(fc_ctx* c, const fc_tape* tape, uint32_t D, bool ti
             cap = n;
         }
         bool split = false;
-        if (int32_t rc = plan.observe(ctr, r, n, split)) return rc;
+        if (!plan.observe(ctr, n, r, split)) return device_error(ctr.error);
         if (split) continue;
         if (n > cap) return fail(FC_ERR_INVALID, "contour leaf buffer too small: " + std::to_string(n) + " surface leaves");
         if (timing) {

@@ -1,6 +1,50 @@
 // fc_octree_sample: the sampling half of fidget-mesh's Octree::build.
 #include "capi_internal.h"
 
+int32_t tree_scratch(fc_ctx* c, const fc_tape* tape, uint32_t D, int dim, uint64_t n_roots, uint64_t cap, TreeScratch& t) {
+    t.D = D;
+    t.grid_blocks = c->sm_count * env_int("FIDGET_B200_BLOCKS_PER_SM", 6);
+    t.choice_words = choice_words(tape);
+    CU(c->choice_scratch.ensure(size_t(t.grid_blocks) * WARPS_PER_BLOCK * t.choice_words * 32 * 4));
+    CU(c->arena.ensure(c->arena_bytes));
+    CU(c->counters.ensure(sizeof(Counters) + 64));
+    CU(c->stats.ensure(sizeof(Stats)));
+    const uint64_t cap_limit = list_cap_limit();
+    for (int l = 1; l <= int(D) + 1; ++l) {
+        t.level_cap[l] = std::min<uint64_t>(n_roots << (dim * std::min(l, int(D))), cap_limit);
+        CU(c->jobs[l].ensure(t.level_cap[l] * sizeof(TileJob)));
+    }
+    CU(c->leaf_tapes.ensure(std::max<uint64_t>(cap, 1) * sizeof(TapeRef)));
+    CU(cudaMemsetAsync(c->counters.p, 0, sizeof(Counters) + 64, c->stream));
+    return FC_OK;
+}
+
+LevelParams tree_level(fc_ctx* c, const fc_tape* tape, const TreeScratch& t, int l, uint32_t has_transform,
+                       const VarBind& vb, const CallCancel& cc) {
+    LevelParams p{};
+    p.level = l;
+    p.tile = 1u << (t.D - uint32_t(l));
+    p.n_axis = l ? 2 : 0;
+    p.is_last = (l == int(t.D));
+    p.root_mode = (l == 0);
+    p.root_tape = tape_ref(tape);
+    p.jobs_in = l ? c->jobs[l].as<TileJob>() : nullptr;
+    p.cap_in = l ? uint32_t(t.level_cap[l]) : 0;
+    p.jobs_out = c->jobs[l + 1].as<TileJob>();
+    p.cap_out = uint32_t(t.level_cap[l + 1]);
+    p.arena = c->arena.as<uint2>();
+    p.arena_cap = arena_clauses(c);
+    p.choice_scratch = c->choice_scratch.as<uint32_t>();
+    p.choice_words = t.choice_words;
+    p.ctr = c->counters.as<Counters>();
+    p.mode = 1;
+    p.has_transform = has_transform;
+    p.cell_h = 2.0f / float(1u << t.D);
+    p.vb = vb;
+    p.cancel = cc.ref;
+    return p;
+}
+
 // Device half: runs the sampler into `dout` (device memory, `cap` leaves); *n_out = surface leaves found
 // (FC_ERR_INVALID when it exceeds cap).  Takes the context lock.  `cc`: the call's cancellation (begin_call).
 int32_t octree_sample_device(fc_ctx* c, const fc_tape* tape, const fc_octree_cfg* cfg, OctreeLeaf* dout, uint64_t cap,
@@ -19,22 +63,8 @@ int32_t octree_sample_device(fc_ctx* c, const fc_tape* tape, const fc_octree_cfg
     const int L = int(D) + 1;   // interval levels: depth 0 (the root cell) .. D
     cudaStream_t s = c->stream;
     const bool timing = (cfg->flags & FC_FLAG_TIMING) != 0;
-    const int bps = env_int("FIDGET_B200_BLOCKS_PER_SM", 6);
-    const int grid_blocks = c->sm_count * bps;
-    const uint32_t choice_words = (tape->info.choice_count + 15) / 16 + 1;
-    CU(c->choice_scratch.ensure(size_t(grid_blocks) * WARPS_PER_BLOCK * choice_words * 32 * 4));
-    CU(c->arena.ensure(c->arena_bytes));
-    CU(c->counters.ensure(sizeof(Counters) + 64));
-    CU(c->stats.ensure(sizeof(Stats)));
-    const uint64_t cap_limit = uint64_t(env_int("FIDGET_B200_MAX_TILES_M", 16)) << 20;
-    std::vector<uint64_t> level_cap(L + 1);
-    for (int l = 1; l <= L; ++l) {
-        uint64_t cells = 1ull << (3 * std::min(l, int(D)));   // cells at depth l (the leaf list holds depth-D cells)
-        level_cap[l] = std::min<uint64_t>(cells, cap_limit);
-        CU(c->jobs[l].ensure(level_cap[l] * sizeof(TileJob)));
-    }
-    CU(c->leaf_tapes.ensure(std::max<uint64_t>(cap, 1) * sizeof(TapeRef)));
-    CU(cudaMemsetAsync(c->counters.p, 0, sizeof(Counters) + 64, s));
+    TreeScratch t;
+    if (int32_t trc = tree_scratch(c, tape, D, 3, 1, cap, t)) return trc;
     CU(cudaMemsetAsync(c->stats.p, 0, sizeof(Stats), s));
     // extra device words after Counters: [0] n_out, then 5 u64 leaf statistics (8-byte aligned)
     uint32_t* d_n_out = reinterpret_cast<uint32_t*>(c->counters.as<char>() + sizeof(Counters));
@@ -42,43 +72,18 @@ int32_t octree_sample_device(fc_ctx* c, const fc_tape* tape, const fc_octree_cfg
     if (timing) CU(cudaEventRecord(get_event(c, 0), s));
     uint32_t launches = 0;
     for (int l = 0; l < L; ++l) {
-        LevelParams p{};
-        p.level = l;
-        p.tile = 1u << (D - uint32_t(l));
-        p.n_axis = l ? 2 : 0;
-        p.is_last = (l == L - 1);
-        p.root_mode = (l == 0);
+        LevelParams p = tree_level(c, tape, t, l, cfg->has_transform, vb, cc);
         p.roots_x = p.roots_y = p.roots_z = 1;
-        p.root_tape.ptr = tape->dev;
-        p.root_tape.n_ops = tape->info.n_ops;
-        p.root_tape.ref_len = tape->info.ref_len;
-        p.root_tape.n_choices = tape->info.choice_count;
         p.width = p.height = p.depth = 1u << D;
         memcpy(p.mat.m, cfg->world_to_model, sizeof p.mat.m);
-        p.jobs_in = l ? c->jobs[l].as<TileJob>() : nullptr;
-        p.cap_in = l ? uint32_t(level_cap[l]) : 0;
-        p.jobs_out = c->jobs[l + 1].as<TileJob>();
-        p.cap_out = uint32_t(level_cap[l + 1]);
-        p.arena = c->arena.as<uint2>();
-        p.arena_cap = std::min<uint64_t>(c->arena.cap, c->arena_bytes) / sizeof(uint2);
-        p.choice_scratch = c->choice_scratch.as<uint32_t>();
-        p.choice_words = choice_words;
-        p.ctr = c->counters.as<Counters>();
         p.stats = c->stats.as<Stats>();
-        p.mode = 1;
-        p.has_transform = cfg->has_transform;
-        p.cell_h = 2.0f / float(1u << D);
-        p.vb = vb;
-        p.cancel = cc.ref;
-        uint64_t cells = 1ull << (3 * l);
-        uint64_t warps = l ? std::max<uint64_t>(1, cells / 8) : 1;
-        int blocks = int(std::min<uint64_t>((warps + WARPS_PER_BLOCK - 1) / WARPS_PER_BLOCK, uint64_t(grid_blocks)));
-        launch_interval_level_3d(p, std::max(blocks, 1), s);
+        const uint64_t cells = 1ull << (3 * l);
+        launch_interval_level_3d(p, t.blocks(l ? std::max<uint64_t>(1, cells / 8) : 1), s);
         ++launches;
     }
     OctreeLeafParams q{};
     q.jobs = c->jobs[L].as<TileJob>();
-    q.cap_jobs = uint32_t(level_cap[L]);
+    q.cap_jobs = uint32_t(t.level_cap[L]);
     q.ctr = c->counters.as<Counters>();
     q.list = L; q.cursor = L;
     q.cell_h = 2.0f / float(1u << D);

@@ -5,6 +5,7 @@
 #include <functional>
 
 #include "capi_internal.h"
+#include "pass_plan.h"
 
 // TileSizesRef::new (fidget-raster/src/lib.rs:59-66)
 int32_t pick_tile_sizes(const uint32_t* ts_in, uint32_t n_in, const uint32_t* dflt, uint32_t n_dflt,
@@ -158,10 +159,7 @@ static int32_t enqueue_tiles_2d(fc_ctx* c, const fc_tape* tape, const fc_render2
         p.roots_x = g.roots_x; p.roots_y = g.roots_y; p.roots_z = 1;
         p.root_x0 = 0; p.root_y0 = g.row0 * ts[0]; p.root_z0 = 0;
         p.root_list = g.d_roots; p.n_root_list = g.n_list;
-        p.root_tape.ptr = tape->dev;
-        p.root_tape.n_ops = tape->info.n_ops;
-        p.root_tape.ref_len = tape->info.ref_len;
-        p.root_tape.n_choices = tape->info.choice_count;
+        p.root_tape = tape_ref(tape);
         p.width = cfg->width; p.height = cfg->height; p.depth = 1;
         p.z2d = cfg->z;
         memcpy(p.mat.m, cfg->mat, sizeof p.mat.m);
@@ -172,7 +170,7 @@ static int32_t enqueue_tiles_2d(fc_ctx* c, const fc_tape* tape, const fc_render2
         p.fills = c->fills[l].as<FillRec>();
         p.cap_fills = uint32_t(g.level_tiles[l + 1]);
         p.arena = c->arena.as<uint2>();
-        p.arena_cap = std::min<uint64_t>(c->arena.cap, c->arena_bytes) / sizeof(uint2);
+        p.arena_cap = arena_clauses(c);
         p.choice_scratch = c->choice_scratch.as<uint32_t>();
         p.choice_words = g.choice_words;
         p.ctr = c->counters.as<Counters>();
@@ -220,10 +218,7 @@ static int32_t enqueue_tiles_2d(fc_ctx* c, const fc_tape* tape, const fc_render2
             // level 0 of a scene: one launch per distinct tape over the root tiles of its placements, as in a 3D scene
             for (size_t k = 0; k < g.groups.size(); ++k) {
                 const SceneGroup& gr = g.groups[k];
-                p.root_tape.ptr = gr.tape->dev;
-                p.root_tape.n_ops = gr.tape->info.n_ops;
-                p.root_tape.ref_len = gr.tape->info.ref_len;
-                p.root_tape.n_choices = gr.tape->info.choice_count;
+                p.root_tape = tape_ref(gr.tape);
                 p.scene_pl = g.d_pl + gr.first;
                 p.n_scene_pl = gr.n;
                 if (k) CU(cudaMemsetAsync(&c->counters.as<Counters>()->cursor[0], 0, sizeof(uint32_t), s));
@@ -401,7 +396,7 @@ static int32_t prepare_2d(fc_ctx* c, const fc_tape* tape, const fc_render2d_cfg*
     // (enqueue_tiles_2d caps a level's grid by its list's capacity)
     const int bps = env_int("FIDGET_B200_BLOCKS_PER_SM", 8);
     g.grid_blocks = c->sm_count * bps;
-    g.choice_words = (tape->info.choice_count + 15) / 16 + 1;
+    g.choice_words = choice_words(tape);
     return FC_OK;
 }
 // scratch of a pipeline over n_roots root tiles (level_tiles sized by the caller)
@@ -526,7 +521,7 @@ static int32_t prepare_3d(fc_ctx* c, const fc_tape* tape, const fc_render3d_cfg*
     const int bps_last = std::max(bps, env_int("FIDGET_B200_LAST_LEVEL_BLOCKS_PER_SM", 8));
     g.grid_blocks = c->sm_count * bps;
     g.grid_blocks_last = c->sm_count * bps_last;
-    g.choice_words = (tape->info.choice_count + 15) / 16 + 1;
+    g.choice_words = choice_words(tape);
     // occlusion map (16 x 16 pixel blocks); used when every tile size down to 16 is a multiple of 16
     g.occl_w = (cfg->width + 15) / 16;
     g.occl_h = (cfg->height + 15) / 16;
@@ -535,9 +530,7 @@ static int32_t prepare_3d(fc_ctx* c, const fc_tape* tape, const fc_render3d_cfg*
     g.exact_census = (cfg->flags & FC_FLAG_EXACT_CENSUS) != 0;
     return FC_OK;
 }
-// Work lists hold only ambiguous tiles (a surface-like set), so they are capped well below the N^3 tile count
-// (FIDGET_B200_MAX_TILES_M, 16 Mi jobs); overflow is reported, not ignored.  The exact census is capped at 64 Mi records.
-static uint64_t list_cap_limit() { return uint64_t(env_int("FIDGET_B200_MAX_TILES_M", 16)) << 20; }
+// Job lists capped at list_cap_limit(); the exact census is capped at 64 Mi records
 static void size_lists_3d(Tiles3D& g) {
     const std::vector<uint32_t>& ts = g.ts;
     const int L = int(ts.size());
@@ -594,10 +587,7 @@ static int32_t enqueue_tiles_3d(fc_ctx* c, const fc_tape* tape, const fc_render3
         p.roots_x = g.roots_x; p.roots_y = g.roots_y; p.roots_z = g.roots_z;
         p.root_x0 = 0; p.root_y0 = g.row0 * T0; p.root_z0 = g.z_begin;
         p.root_list = g.d_roots; p.n_root_list = g.n_list;
-        p.root_tape.ptr = tape->dev;
-        p.root_tape.n_ops = tape->info.n_ops;
-        p.root_tape.ref_len = tape->info.ref_len;
-        p.root_tape.n_choices = tape->info.choice_count;
+        p.root_tape = tape_ref(tape);
         p.width = cfg->width; p.height = cfg->height; p.depth = cfg->depth;
         memcpy(p.mat.m, cfg->mat, sizeof p.mat.m);
         p.jobs_in = l ? c->jobs[l].as<TileJob>() : nullptr;
@@ -605,7 +595,7 @@ static int32_t enqueue_tiles_3d(fc_ctx* c, const fc_tape* tape, const fc_render3
         p.jobs_out = c->jobs[l + 1].as<TileJob>();
         p.cap_out = uint32_t(g.level_cap[l + 1]);
         p.arena = c->arena.as<uint2>();
-        p.arena_cap = std::min<uint64_t>(c->arena.cap, c->arena_bytes) / sizeof(uint2);
+        p.arena_cap = arena_clauses(c);
         p.choice_scratch = c->choice_scratch.as<uint32_t>();
         p.choice_words = g.choice_words;
         p.ctr = c->counters.as<Counters>();
@@ -648,10 +638,7 @@ static int32_t enqueue_tiles_3d(fc_ctx* c, const fc_tape* tape, const fc_render3
             const uint64_t per = uint64_t(g.roots_x) * g.roots_y * g.roots_z;
             for (size_t k = 0; k < g.groups.size(); ++k) {
                 const SceneGroup& gr = g.groups[k];
-                p.root_tape.ptr = gr.tape->dev;
-                p.root_tape.n_ops = gr.tape->info.n_ops;
-                p.root_tape.ref_len = gr.tape->info.ref_len;
-                p.root_tape.n_choices = gr.tape->info.choice_count;
+                p.root_tape = tape_ref(gr.tape);
                 p.scene_pl = g.d_pl + gr.first;
                 p.n_scene_pl = gr.n;
                 if (k) CU(cudaMemsetAsync(&c->counters.as<Counters>()->cursor[0], 0, sizeof(uint32_t), s));
@@ -757,84 +744,39 @@ static void add_stage_ms_3d(fc_ctx* c, size_t first, int L, float* stage_ms) {
 }
 
 // ---- passes of the 3D batches (fc_render3d_frames: frames; fc_render3d_scene: placements) ----
-// Overflow policy: a pass fails (FC_ERR_ARENA, list overflow) only where one of its items alone would.  The first pass
-// holds one item; later ones are sized from the largest per-item use seen so far (arena clauses, jobs per level, census
-// records) with headroom 1.5; a pass that still overflows is run again as two halves (the kernels report overflow, they
-// do not fault), and only a one-item pass returns the error.  Only capped lists can overflow: a job list whose cap is
-// the worst case of the pass (every tile of the level queued) never does, so the headroom applies to the arena, to the
-// job lists clamped by FIDGET_B200_MAX_TILES_M and to a clamped census.  The caller runs the passes: take() the next
-// one, observe() its counters once it is done, until more() is false.
-namespace {
-struct PassPlan {
-    struct Range { uint32_t f0, n; };
-    const fc_ctx* c;
-    std::function<Tiles3D(uint32_t)> grid_of;   // the tile grid of a pass of n items, lists and census capped
-    uint32_t n_items, n_max = 1, next = 0;      // next: the first item no pass has taken yet
-    int L = 0, forced = 0;
-    double use_arena = 0, use_census = 0, use_jobs[MAX_LEVELS + 1] = {};
-    bool measured = false;
-    std::vector<Range> redo;                    // halves of overflowed passes (a stack: the first half runs next)
-
-    // n_max: the most items a pass may hold: FC_FRAMES_PASS_BYTES (at least one item) for its lists, census, z-sort
-    // order and item_bytes per item, 32-bit root ids and the caller's own limit n_cap
-    PassPlan(const fc_ctx* ctx, std::function<Tiles3D(uint32_t)> grid, uint32_t n, uint64_t item_bytes, uint32_t n_cap)
-        : c(ctx), grid_of(std::move(grid)), n_items(n) {
-        L = int(grid_of(1).ts.size());
-        auto allowed = [&](uint32_t k) {
-            const Tiles3D gp = grid_of(k);
-            uint64_t b = uint64_t(k) * item_bytes + gp.level_cap[L] * 4 + gp.cap_census * sizeof(CensusRec);
-            for (int l = 1; l <= L; ++l) b += gp.level_cap[l] * sizeof(TileJob);
-            return b <= FC_FRAMES_PASS_BYTES && gp.n_roots <= 0xfffffff0ull;
-        };
-        while (n_max < std::min(n_items, n_cap) && allowed(n_max + 1)) ++n_max;
-        // (diagnostic: passes of this size, at most the limits above, neither measured first nor shrunk to fit)
-        forced = env_int("FIDGET_B200_FRAMES_PER_PASS", 0);
-        if (forced > 0) n_max = std::min<uint32_t>(n_max, uint32_t(forced));
-        measured = forced > 0;
-    }
-    bool more() const { return next < n_items || !redo.empty(); }
-    bool fits(uint32_t n) const {
+// The planner (pass_plan.h) of a batch of n_items whose pass of n items is the tile grid grid_of(n), lists and census
+// capped.  n_max: FC_FRAMES_PASS_BYTES (at least one item) for its lists, census, z-sort order and item_bytes per item,
+// 32-bit root ids and the caller's own limit n_cap.  A list's worst case is every tile of its level queued; the exact
+// census counts (as the planner's measured quantity) when it is capped below every tile of every level evaluated.
+static PassPlan plan_3d(const fc_ctx* c, const std::function<Tiles3D(uint32_t)>& grid_of, uint32_t n_items,
+                        uint64_t item_bytes, uint32_t n_cap) {
+    const int L = int(grid_of(1).ts.size());
+    auto allowed = [&](uint32_t k) {
+        const Tiles3D gp = grid_of(k);
+        uint64_t b = uint64_t(k) * item_bytes + gp.level_cap[L] * 4 + gp.cap_census * sizeof(CensusRec);
+        for (int l = 1; l <= L; ++l) b += gp.level_cap[l] * sizeof(TileJob);
+        return b <= FC_FRAMES_PASS_BYTES && gp.n_roots <= 0xfffffff0ull;
+    };
+    uint32_t n_max = 1;
+    while (n_max < std::min(n_items, n_cap) && allowed(n_max + 1)) ++n_max;
+    return PassPlan(n_items, n_max, [c, grid_of, L](uint32_t n) {
         const Tiles3D gp = grid_of(n);
-        const double h = 1.5 * n;
-        if (use_arena * h > double(std::min<uint64_t>(c->arena.cap, c->arena_bytes) / sizeof(uint2))) return false;
+        PassLimits lim;
+        lim.arena_cap = arena_clauses(c);
         uint64_t census_worst = gp.n_roots;
         for (int l = 1; l <= L; ++l) {
             const uint64_t r = gp.ts[0] / gp.ts[l - 1];
-            const bool clamped = gp.level_cap[l] < gp.n_roots * r * r * r;
-            if (clamped && use_jobs[l] * h > double(gp.level_cap[l])) return false;
+            lim.cap[l] = gp.level_cap[l];
+            lim.worst[l] = gp.n_roots * r * r * r;
             if (l < L) { const uint64_t q = gp.ts[l - 1] / gp.ts[l]; census_worst += gp.level_cap[l] * q * q * q; }
         }
-        const bool census_clamped = gp.exact_census && gp.cap_census < census_worst;
-        return !census_clamped || use_census * h <= double(gp.cap_census);
-    }
-    Range take() {
-        if (!redo.empty()) { const Range r = redo.back(); redo.pop_back(); return r; }
-        uint32_t n = std::min(n_max, n_items - next);
-        if (!measured) n = 1;
-        else if (forced <= 0) while (n > 1 && !fits(n)) --n;
-        const Range r{next, n};
-        next += n;
-        return r;
-    }
-    // Records the use of the finished pass r from its counters.  Its error if it fails; else `split` says that it
-    // overflowed and its halves are queued in its place.
-    int32_t observe(const Counters& ctr, const Range& r, bool& split) {
-        const double n = double(r.n);
-        use_arena = std::max(use_arena, double(ctr.arena_top) / n);
-        use_census = std::max(use_census, double(ctr.n_census) / n);
-        for (int l = 1; l <= L; ++l) use_jobs[l] = std::max(use_jobs[l], double(ctr.n_jobs[l]) / n);
-        measured = true;
-        split = false;
-        if (!ctr.error) return FC_OK;
-        if (r.n == 1 || (ctr.error & ~3u)) return device_error(ctr.error);
-        const uint32_t h = r.n / 2;
-        redo.push_back(Range{r.f0 + h, r.n - h});
-        redo.push_back(Range{r.f0, h});
-        split = true;
-        return FC_OK;
-    }
-};
+        lim.extra_on = gp.exact_census && gp.cap_census < census_worst;
+        lim.extra_cap = gp.cap_census;
+        return lim;
+    });
+}
 
+namespace {
 // The stats of a 3D batch, summed over the passes that stand: census, pixels, grads, the largest arena use and
 // (FC_FLAG_TIMING) the stage times
 struct PassStats {
@@ -1161,7 +1103,7 @@ int32_t fc_render2d_scene(fc_ctx* c, const fc_tape* const* tapes, const fc_frame
     const uint32_t W = cfg->width, H = cfg->height;
     g.roots_y = (H + T0 - 1) / T0;
     for (uint32_t k = 0; k < n_shapes; ++k)   // choice scratch for the largest choice_count
-        g.choice_words = std::max(g.choice_words, (tapes[k]->info.choice_count + 15) / 16 + 1);
+        g.choice_words = std::max(g.choice_words, choice_words(tapes[k]));
     g.scene = true;
     g.blocks_x = (W + leaf - 1) / leaf;
     g.blocks_y = (H + leaf - 1) / leaf;
@@ -1447,8 +1389,9 @@ int32_t fc_render3d_frames(fc_ctx* c, const fc_tape* tape, const fc_render3d_cfg
         return gp;
     };
     // (exact census: a pass keeps its census rows within 16 bits)
-    PassPlan plan(c, grid_of, n_frames, size_t(frame_rows) * W * 8 + occl_frame * 4 + (host_out ? 2 * img_px * 16 : 0),
-                  g.exact_census ? 65536 / frame_rows : 0xffffffffu);
+    PassPlan plan = plan_3d(c, grid_of, n_frames,
+                            size_t(frame_rows) * W * 8 + occl_frame * 4 + (host_out ? 2 * img_px * 16 : 0),
+                            g.exact_census ? 65536 / frame_rows : 0xffffffffu);
     const uint32_t n_max = plan.n_max;
     if (int32_t erc = ensure_scratch_3d(c, grid_of(n_max), size_t(W) * frame_rows * n_max, occl_frame * n_max)) return erc;
     CU(c->frame_table.ensure(size_t(n_frames) * sizeof(Frame2D)));
@@ -1495,7 +1438,7 @@ int32_t fc_render3d_frames(fc_ctx* c, const fc_tape* tape, const fc_render3d_cfg
         if (int32_t wrc = wait_pass(c, f.b, cc, true)) return wrc;
         const PassStatus& ps = c->pass_pin[f.b];
         bool split = false;
-        if (int32_t orc = plan.observe(ps.ctr, f.r, split)) return orc;
+        if (!plan.observe(ps.ctr, ps.ctr.n_census, f.r, split)) return device_error(ps.ctr.error);
         if (split) return FC_OK;
         if (want_stats) sum.add(c, ps, timing, f.ev0, L);
         if (host_out) {
@@ -1593,7 +1536,7 @@ int32_t fc_render3d_scene(fc_ctx* c, const fc_tape* const* tapes, const fc_frame
     const uint64_t vol_roots = uint64_t(g.roots_x) * g.roots_y * g.roots_z;
     if (vol_roots > 0xfffffff0ull) return fail(FC_ERR_UNSUPPORTED, "volume too large");
     for (uint32_t k = 0; k < n_shapes; ++k)   // choice scratch for the largest choice_count
-        g.choice_words = std::max(g.choice_words, (tapes[k]->info.choice_count + 15) / 16 + 1);
+        g.choice_words = std::max(g.choice_words, choice_words(tapes[k]));
     g.scene = true;
     g.clamp_at = clamp ? cfg->depth - 1u : 0xffffffffu;
     const bool timing = (cfg->flags & FC_FLAG_TIMING) != 0;
@@ -1612,7 +1555,7 @@ int32_t fc_render3d_scene(fc_ctx* c, const fc_tape* const* tapes, const fc_frame
         gp.level_cap[L] = std::min<uint64_t>(gp.level_cap[L], FC_SCENE_MAX_LEAF_JOBS);
         return gp;
     };
-    PassPlan plan(c, grid_of, n_shapes, 0, 0xffffffffu);
+    PassPlan plan = plan_3d(c, grid_of, n_shapes, 0, 0xffffffffu);
     if (int32_t erc = ensure_scratch_3d(c, grid_of(plan.n_max), npix, occl_blocks * 2)) return erc;
     CU(c->frame_table.ensure(size_t(n_shapes) * sizeof(Frame2D)));
     CU(c->scene_pl.ensure(size_t(n_shapes) * 4));
@@ -1688,7 +1631,7 @@ int32_t fc_render3d_scene(fc_ctx* c, const fc_tape* const* tapes, const fc_frame
             CU(cudaStreamSynchronize(s));
         }
         bool split = false;
-        if (int32_t orc = plan.observe(hs->ctr, r, split)) return abandon(orc);
+        if (!plan.observe(hs->ctr, hs->ctr.n_census, r, split)) return abandon(device_error(hs->ctr.error));
         if (split) {
             if (int32_t brc = snapshot(true)) return abandon(brc);
             continue;

@@ -184,12 +184,13 @@ def grad(op, form, a, b=None, imm=None):
             x = va.astype(np.float64)
             dv = {"sin": lambda: np.cos(x), "cos": lambda: -np.sin(x), "tan": lambda: 1.0 / np.cos(x) ** 2,
                   "asin": lambda: 1.0 / np.sqrt(1.0 - x * x), "acos": lambda: -1.0 / np.sqrt(1.0 - x * x),
-                  "atan": lambda: 1.0 / (x * x + 1.0), "exp": lambda: np.exp(x), "ln": lambda: 1.0 / x}[op]()
+                  "atan": lambda: 1.0 / (x * x + 1.0), "exp": lambda: v.astype(np.float64),   # the VM's own f32 value
+                  "ln": lambda: 1.0 / x}[op]()
             return _pack(v, (da.astype(np.float64) * col(dv)).astype(F))
         if op == "atan2":
-            y, x = va.astype(np.float64), vb.astype(np.float64)
-            d = x * x + y * y
-            return _pack(f32("atan2", va, vb), ((col(x) * da - col(y) * db) / col(d)).astype(F))
+            # IEEE steps in the VM's order, in f32: d = x * x + y * y underflows and overflows where the VM's does
+            d = vb * vb + va * va
+            return _pack(f32("atan2", va, vb), (col(vb) * da - col(va) * db) / col(d))
         if op == "add":
             return _pack(va + vb, da + db)
         if op == "sub":

@@ -121,6 +121,15 @@ class FcMeshInfo(C.Structure):
                [("sampler_ms", C.c_float), ("mesh_ms", C.c_float)]
 
 
+class FcMeshFrame(C.Structure):
+    _fields_ = [("has_transform", C.c_uint32), ("world_to_model", C.c_float * 16), ("n_var_values", C.c_uint32),
+                ("var_values", C.c_float * 16)]
+
+
+class FcMeshFrameInfo(C.Structure):
+    _fields_ = [(n, C.c_uint64) for n in ("n_leaves", "n_vertices", "n_triangles", "open_edges", "n_cells")]
+
+
 class FcContourCfg(C.Structure):
     _fields_ = [("depth", C.c_uint32), ("has_transform", C.c_uint32), ("world_to_model", C.c_float * 9), ("z", C.c_float),
                 ("flags", C.c_uint32), ("n_var_values", C.c_uint32), ("var_values", C.c_float * 16)]
@@ -174,6 +183,8 @@ FC_ERR_CANCELLED = -6
 FC_FRAMES_PASS_BYTES = 512 << 20
 FC_MAX_VARS = 16
 FC_MAX_QUADTREE_DEPTH = 14
+FC_MAX_OCTREE_DEPTH = 12
+FC_MESH_MAX_PASS_FRAMES = 4096
 FC_SCENE_MAX_SHAPES = 1024
 FC_SCENE_MAX_DEPTH = 262142
 FC_SCENE_MAX_ROOT_TILE = 1022
@@ -231,6 +242,8 @@ CUDA_API = {
     "fc_mesh_read": (_i32, [_vp, _vp, _vp]),
     "fc_mesh_read_cells": (_i32, [_vp, _vp, _u64, _P(_u64)]),
     "fc_mesh_write_stl": (_i32, [_vp, _vp, C.c_size_t, _P(C.c_size_t)]),
+    "fc_mesh_build_frames": (_i32, [_vp, _vp, _P(FcOctreeCfg), _P(FcMeshFrame), _u32, _P(FcMeshInfo),
+                                    _P(FcMeshFrameInfo)]),
     "fc_contour_build": (_i32, [_vp, _vp, _P(FcContourCfg), _P(FcContourInfo)]),
     "fc_contour_read": (_i32, [_vp, _vp, _vp, _vp]),
     "fc_contour_build_slices": (_i32, [_vp, _vp, _P(FcContourCfg), _P(FcContourSlice), _u32, _P(FcContourInfo),

@@ -117,6 +117,10 @@ struct fc_ctx {
     uint32_t mesh_n_verts = 0, mesh_n_tris = 0;
     DevBuf mesh_tree, mesh_herm, mesh_cells;                    // FC_FLAG_MESH_COLLAPSE: cell tree, Hermite records, final leaves
     uint32_t mesh_n_cells = 0;
+    // fc_mesh_build_frames: a pass's frame table, and each frame's first vertex and triangle in the mesh (uint2 per frame,
+    // for fc_mesh_write_stl; unused with one frame).  No mesh is one frame of nothing.
+    DevBuf mesh_frames, mesh_ranges;
+    uint32_t mesh_n_frames = 1;
     DevBuf contour_leaves, contour_scratch, contour_out;        // fc_contour_build: sampler output, link scratch, vertices
     DevBuf contour_offs, contour_flags, contour_slices;         // offsets, closed flags, a stack pass's slice table
     uint32_t contour_n_verts = 0, contour_n_polys = 0;
@@ -259,6 +263,11 @@ struct TreeScratch {
 int32_t tree_scratch(fc_ctx* c, const fc_tape* tape, uint32_t D, int dim, uint64_t n_roots, uint64_t cap, TreeScratch& t);
 LevelParams tree_level(fc_ctx* c, const fc_tape* tape, const TreeScratch& t, int l, uint32_t has_transform,
                        const VarBind& vb, const CallCancel& cc);
+int32_t octree_enqueue(fc_ctx* c, const fc_tape* tape, uint32_t D, const MeshFrame* fr, uint32_t n, const MeshFrame* d_fr,
+                       OctreeLeaf* dout, uint64_t cap, bool stats, cudaEvent_t t0, const CallCancel& cc, uint32_t* launches);
+// contour.cu
+// Grows `b` to at least `need` bytes, keeping its first `keep` bytes (the output of a batch's earlier passes)
+int32_t grow_keep(fc_ctx* c, DevBuf& b, size_t need, size_t keep);
 // render.cu
 int32_t pick_tile_sizes(const uint32_t* ts_in, uint32_t n_in, const uint32_t* dflt, uint32_t n_dflt, uint32_t max_size,
                         std::vector<uint32_t>& ts);

@@ -1,7 +1,7 @@
 // 2D contours (fc_contour_build): dual contouring on a uniform quadtree of the [-1,1]^2 world square, linked into
 // polylines on the device.  The pipeline restricts the mesher's to two dimensions:
 //
-//   descent    k_contour_level: the interval levels of the octree sampler with Z fixed (level_job's QUAD mode), one
+//   descent    k_contour_level: the interval levels of the octree sampler with Z fixed (level_job's TREE mode), one
 //              launch per depth, four children per cell;
 //   leaves     k_contour_leaf: one warp per leaf, four corners, then the 16-ary edge search of k_octree_leaf -- four
 //              edges x 16 probes, two points per lane, in one pass; k_contour_grads: (dx, dy, v) at the intersections,
@@ -63,7 +63,7 @@ struct ContourLeafParams {
     uint32_t rows;
 };
 
-// The quadtree levels: k_interval_level's claim loop around level_job's QUAD mode (one root cell; STACK: one per slice,
+// The quadtree levels: k_interval_level's claim loop around level_job's TREE mode (one root cell; STACK: one per slice,
 // roots_y slices, 32 to a warp at level 0)
 template <bool STACK>
 __global__ void __launch_bounds__(WARPS_PER_BLOCK * 32) k_contour_level(const __grid_constant__ LevelParams p,
@@ -514,8 +514,8 @@ using fdev::ContourSlice;
 // contour_finish, and per vertex (at most two) its position, slice, links, list-ranking buffers, scans and output
 constexpr uint64_t CONTOUR_LEAF_BYTES = sizeof(fdev::ContourLeaf) + sizeof(fdev::TapeRef) + 7 * 4 + 12 +
                                         2 * (8 + 4 + 2 * 4 + 6 * 4 + 1 + 4 + 2 * 8 + 8 + 4 + 1);
+}  // namespace
 
-// Grows `b` to at least `need` bytes, keeping its first `keep` bytes (the polylines of the stack's earlier passes)
 int32_t grow_keep(fc_ctx* c, DevBuf& b, size_t need, size_t keep) {
     if (need <= b.cap) return FC_OK;
     const size_t cap = std::max(need, b.cap + b.cap / 2);
@@ -529,7 +529,6 @@ int32_t grow_keep(fc_ctx* c, DevBuf& b, size_t need, size_t keep) {
     b.cap = cap;
     return FC_OK;
 }
-}  // namespace
 
 // The quadtree sampler over the n slices sl[0..n) (host; with n > 1 also d_sl on the device): interval levels, then the
 // leaf and gradient kernels.  *n_out = surface leaves found (nothing beyond cap written), ctr = the pass's counters.

@@ -167,6 +167,10 @@ struct ContourSlice {
     uint32_t has_transform, to_model;
     VarBind vb;
 };
+// One frame of a mesh frame batch (fc_mesh_build_frames) is the same record with z unused: the stacked octree gives frame
+// k the cell rows [k * 2^depth, (k + 1) * 2^depth), a cell's rows are taken relative to its frame, and to_model sends the
+// frame's vertices back through `mat`.
+using MeshFrame = ContourSlice;
 
 // Scene renders (fc_render3d_scene): K placements (a tape and its Frame2D) share one heightmap and one occlusion map.
 // Placement k's jobs carry k in TileJob::pad.  A heightmap key orders what the merged image keeps: the greater clamped
@@ -329,7 +333,7 @@ __device__ __forceinline__ FrameView view_of(const P& p, uint32_t y, uint32_t pl
     if (SCENE) return FrameView{&p.frames[pl].mat, p.frames[pl].z, &p.frames[pl].vb, 0u, 0u};
     return frame_of<FRAMES>(p, y);
 }
-// QUAD (contours): the one slice of fc_contour_build in the launch parameters, or with STACK the slice of cell row y in
+// TREE (contours): the one slice of fc_contour_build in the launch parameters, or with STACK the slice of cell row y in
 // the table `slices` (a kernel argument of its own: LevelParams keeps the layout the other level kernels are built with),
 // frame_rows rows each
 template <bool STACK>
@@ -474,8 +478,14 @@ struct OctreeLeafParams {
 };
 
 // launchers (kernels.cu)
-void launch_octree_leaf(const OctreeLeafParams& p, int blocks, cudaStream_t s);
-void launch_octree_grads(const OctreeLeafParams& p, int blocks, cudaStream_t s);
+// frames == null: the one frame in the launch parameters (fc_octree_sample, fc_mesh_build); else a mesh frame batch's
+// table, `rows` cell rows per frame (the leaves record their frame in OctreeLeaf::pad)
+void launch_octree_leaf(const OctreeLeafParams& p, int blocks, cudaStream_t s, const MeshFrame* frames = nullptr,
+                        uint32_t rows = 0);
+void launch_octree_grads(const OctreeLeafParams& p, int blocks, cudaStream_t s, const MeshFrame* frames = nullptr,
+                         uint32_t rows = 0);
+// the interval levels of a mesh frame batch's stacked octree (one root cell per frame, p.roots_y frames)
+void launch_octree_level_frames(const LevelParams& p, const MeshFrame* frames, int blocks, cudaStream_t s);
 void launch_interval_level_3d(const LevelParams& p, int blocks, cudaStream_t s);
 void launch_voxels_3d(const VoxelParams& p, int blocks, cudaStream_t s);
 // Counting sort of the leaf jobs by descending Z layer: hist/offsets are device scratch of n_layers+1 words

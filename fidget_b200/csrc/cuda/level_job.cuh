@@ -42,11 +42,14 @@ __device__ __forceinline__ void store_fill(FillRec* dst, const FillRec& fr) {
     *reinterpret_cast<uint4*>(dst) = make_uint4(fr.x, fr.y, fr.value, fr.ready);
 }
 
-// QUAD (2D only): the quadtree of fc_contour_build.  Coordinates are cells at the finest depth with world-square bounds
-// coord * cell_h - 1, seen through `mat` when has_transform, at Z = [z2d, z2d]; classified tiles are dropped (no fills).
-// With FRAMES a contour slice stack: each cell's slice (`slices`, frame_rows rows each) supplies Z, the matrix, its
-// has_transform and the vars, and the cell's rows are relative to its slice.
-template <int DIM, bool FUSED, bool FRAMES = false, bool SCENE = false, bool QUAD = false>
+// TREE: the samplers' trees whose cells read their view from a ContourSlice table (a MeshFrame is the same record, z
+// unused), not from the render parameters.  DIM 2: the quadtree of
+// fc_contour_build.  Coordinates are cells at the finest depth with world-square bounds coord * cell_h - 1, seen through
+// `mat` when has_transform, at Z = [z2d, z2d]; classified tiles are dropped (no fills).  With FRAMES a contour slice
+// stack: each cell's slice (`slices`, frame_rows rows each) supplies Z, the matrix, its has_transform and the vars, and
+// the cell's rows are relative to its slice.  DIM 3 with FRAMES (octree mode 1): the stacked octree of a mesh frame
+// batch, each cell's frame read the same way (its Z is the cell's own).
+template <int DIM, bool FUSED, bool FRAMES = false, bool SCENE = false, bool TREE = false>
 __device__ __forceinline__ void level_job(const LevelParams& p, uint32_t j, uint32_t n_roots, itv* slots, uint32_t* cs,
                                           uint32_t (*live)[32], int lane, uint32_t epoch,
                                           const ContourSlice* slices = nullptr) {
@@ -108,7 +111,7 @@ __device__ __forceinline__ void level_job(const LevelParams& p, uint32_t j, uint
         }
         // Region in screen coordinates -> model space (pixel.rs:325-342, voxel.rs:291-306); in a frame batch a
         // tile's coordinates are relative to its frame (per lane at level 0, whose 32 roots may span frames)
-        const FrameView fv = QUAD ? quad_view<FRAMES>(p, slices, cy) : view_of<FRAMES, SCENE>(p, cy, pl);
+        const FrameView fv = TREE ? quad_view<FRAMES>(p, slices, cy) : view_of<FRAMES, SCENE>(p, cy, pl);
         const Mat4& M = *fv.mat;
         const VarBind& vb = *fv.vb;
         itv X = iv(float(cx), float(cx) + float(T));
@@ -117,13 +120,15 @@ __device__ __forceinline__ void level_job(const LevelParams& p, uint32_t j, uint
         itv vx, vy, vz;
         if (DIM == 3 && p.mode == 1u) {
             // octree cell bounds in world space (CellBounds::child, cell.rs:155-166): dyadic, exact in f32
+            // (TREE: a mesh frame batch -- the rows are the frame's, and the frame supplies matrix and has_transform)
             const float h = p.cell_h;
+            const uint32_t ry = TREE ? cy - fv.y0 : cy;
             X = iv(float(cx) * h - 1.0f, float(cx + T) * h - 1.0f);
-            Y = iv(float(cy) * h - 1.0f, float(cy + T) * h - 1.0f);
+            Y = iv(float(ry) * h - 1.0f, float(ry + T) * h - 1.0f);
             Z = iv(float(cz) * h - 1.0f, float(cz + T) * h - 1.0f);
-            if (p.has_transform) xform_iv(p.mat, X, Y, Z, vx, vy, vz);
+            if (TREE ? quad_has_transform<FRAMES>(p, slices, cy) : p.has_transform) xform_iv(TREE ? M : p.mat, X, Y, Z, vx, vy, vz);
             else { vx = X; vy = Y; vz = Z; }
-        } else if constexpr (QUAD) {
+        } else if constexpr (TREE) {
             const float h = p.cell_h;
             const uint32_t ry = cy - fv.y0;
             X = iv(float(cx) * h - 1.0f, float(cx + T) * h - 1.0f);
@@ -200,7 +205,7 @@ __device__ __forceinline__ void level_job(const LevelParams& p, uint32_t j, uint
                     scene2d_cover(cover_out, p.occl_w, p.occl_h, p.cull, __shfl_sync(FULL, cx, src),
                                   __shfl_sync(FULL, cy, src), T, __shfl_sync(FULL, pl, src), lane, 32u);
                 }
-            } else if constexpr (!QUAD) {
+            } else if constexpr (!TREE) {
                 uint32_t m = __ballot_sync(FULL, fill_in || fill_out);
                 if (m) {
                     uint32_t base = 0;

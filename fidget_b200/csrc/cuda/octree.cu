@@ -1,5 +1,5 @@
 // Octree sampler leaves of fidget-mesh's Manifold Dual Contouring (sampling half).
-#include "interp.cuh"
+#include "level_job.cuh"
 
 // ---------------------------------------------------------------------------
 // Octree sampler leaves (OctreeBuilder::leaf, fidget-mesh/src/octree.rs:590-808):
@@ -23,7 +23,11 @@ __device__ __forceinline__ bool edge_setup(uint32_t index, uint32_t mask, EdgeSt
     return true;
 }
 
-__global__ void __launch_bounds__(128) k_octree_leaf(const __grid_constant__ OctreeLeafParams p) {
+// STACK: a mesh frame batch's stacked octree -- the frame of the job's row supplies matrix, has_transform and vars, the
+// cell's rows are the frame's, and the leaf records its frame in `pad` (0 for the one frame of a single build)
+template <bool STACK>
+__global__ void __launch_bounds__(128) k_octree_leaf(const __grid_constant__ OctreeLeafParams p, const MeshFrame* frames,
+                                                     uint32_t rows) {
     const int lane = threadIdx.x & 31;
     float2 slots[REG_SLOTS];
     const uint32_t n_jobs = min(p.ctr->n_jobs[p.list], p.cap_jobs);
@@ -37,19 +41,20 @@ __global__ void __launch_bounds__(128) k_octree_leaf(const __grid_constant__ Oct
         j = __shfl_sync(FULL, j, 0);
         if (j >= n_jobs) break;
         const TileJob* job = p.jobs + j;
-        const uint32_t cx = job->x, cy = job->y, cz = job->z;
+        const uint32_t f = STACK ? job->y / rows : 0u;
+        const uint32_t cx = job->x, cy = STACK ? job->y - f * rows : job->y, cz = job->z;
         const TapeRef tr = job->tape;
         const float h = p.cell_h;
         const float lo[3] = {float(cx) * h - 1.0f, float(cy) * h - 1.0f, float(cz) * h - 1.0f};
         const float hi[3] = {float(cx + 1u) * h - 1.0f, float(cy + 1u) * h - 1.0f, float(cz + 1u) * h - 1.0f};
         auto eval2 = [&](float x0, float y0, float z0, float x1, float y1, float z1) -> float2 {
-            if (p.has_transform) {
-                xform_f32(p.mat, x0, y0, z0, x0, y0, z0);
-                xform_f32(p.mat, x1, y1, z1, x1, y1, z1);
+            if (STACK ? frames[f].has_transform : p.has_transform) {
+                xform_f32(STACK ? frames[f].mat : p.mat, x0, y0, z0, x0, y0, z0);
+                xform_f32(STACK ? frames[f].mat : p.mat, x1, y1, z1, x1, y1, z1);
             }
             const float2 X = make_float2(x0, x1), Y = make_float2(y0, y1), Z = make_float2(z0, z1);
             return run_f32x2(tr.ptr, tr.n_ops, slots, [&](uint32_t i) {
-                return pick_input(p.vb, i, X, Y, Z, [](float f) { return make_float2(f, f); });
+                return pick_input(STACK ? frames[f].vb : p.vb, i, X, Y, Z, [](float v) { return make_float2(v, v); });
             });
         };
         // corners (CellBounds::corner: bit i of the corner index selects the upper bound on axis i)
@@ -81,7 +86,7 @@ __global__ void __launch_bounds__(128) k_octree_leaf(const __grid_constant__ Oct
             n_pts += 64ull * ne;
             L->ix = uint16_t(cx); L->iy = uint16_t(cy); L->iz = uint16_t(cz);
             L->mask = uint8_t(mask); L->n_edges = uint8_t(ne);
-            L->present = uint16_t(active); L->pad = 0;
+            L->present = uint16_t(active); L->pad = uint16_t(f);
         }
         const int half = lane >> 4, jj = lane & 15;
         for (uint32_t pass = 0; pass * 4u < ne; ++pass) {
@@ -137,11 +142,15 @@ __global__ void __launch_bounds__(128) k_octree_leaf(const __grid_constant__ Oct
         }
     }
 }
-void launch_octree_leaf(const OctreeLeafParams& p, int blocks, cudaStream_t s) { k_octree_leaf<<<blocks, 128, 0, s>>>(p); }
+void launch_octree_leaf(const OctreeLeafParams& p, int blocks, cudaStream_t s, const MeshFrame* frames, uint32_t rows) {
+    if (frames) k_octree_leaf<true><<<blocks, 128, 0, s>>>(p, frames, rows);
+    else k_octree_leaf<false><<<blocks, 128, 0, s>>>(p, nullptr, 0);
+}
 
 // Gradients at the intersections (octree.rs:780-808): one warp per surface leaf, one lane per edge,
 // with the tape k_octree_leaf recorded for that leaf.
-__global__ void __launch_bounds__(128) k_octree_grads(const __grid_constant__ OctreeLeafParams p) {
+template <bool STACK>
+__global__ void __launch_bounds__(128) k_octree_grads(const __grid_constant__ OctreeLeafParams p, const MeshFrame* frames) {
     grd slots[REG_SLOTS];
     const int lane = threadIdx.x & 31;
     const uint32_t warp = (blockIdx.x * blockDim.x + threadIdx.x) >> 5;
@@ -155,11 +164,12 @@ __global__ void __launch_bounds__(128) k_octree_grads(const __grid_constant__ Oc
         const uint32_t active = L->present;
         const bool mine = lane < 12 && ((active >> lane) & 1u);
         const int e = mine ? lane : (__ffs(active) - 1);
+        const MeshFrame* fr = STACK ? frames + L->pad : nullptr;   // (STACK: the leaf's frame)
         grd gx = gr(L->pos[e][0], 1.0f, 0.0f, 0.0f), gy = gr(L->pos[e][1], 0.0f, 1.0f, 0.0f),
             gz = gr(L->pos[e][2], 0.0f, 0.0f, 1.0f);
-        if (p.has_transform) xform_gr(p.mat, gx, gy, gz, gx, gy, gz);
+        if (STACK ? fr->has_transform : p.has_transform) xform_gr(STACK ? fr->mat : p.mat, gx, gy, gz, gx, gy, gz);
         const grd r = run_grad(tr.ptr, tr.n_ops, slots, [&](uint32_t k) {
-            return pick_input(p.vb, k, gx, gy, gz, [](float f) { return gr1(f); });
+            return pick_input(STACK ? fr->vb : p.vb, k, gx, gy, gz, [](float f) { return gr1(f); });
         });
         if (mine) {
             L->grad[e][0] = r.y; L->grad[e][1] = r.z; L->grad[e][2] = r.w; L->grad[e][3] = r.x;
@@ -171,6 +181,36 @@ __global__ void __launch_bounds__(128) k_octree_grads(const __grid_constant__ Oc
         if (lane == 0 && n_pts) atomicAdd(&p.stats[4], n_pts);
     }
 }
-void launch_octree_grads(const OctreeLeafParams& p, int blocks, cudaStream_t s) { k_octree_grads<<<blocks, 128, 0, s>>>(p); }
+void launch_octree_grads(const OctreeLeafParams& p, int blocks, cudaStream_t s, const MeshFrame* frames, uint32_t) {
+    if (frames) k_octree_grads<true><<<blocks, 128, 0, s>>>(p, frames);
+    else k_octree_grads<false><<<blocks, 128, 0, s>>>(p, nullptr);
+}
+
+// The levels of a mesh frame batch's stacked octree: k_interval_level's claim loop around level_job's octree mode with
+// the frame table (one root cell per frame, 32 to a warp at level 0)
+__global__ void __launch_bounds__(WARPS_PER_BLOCK * 32) k_octree_level(const __grid_constant__ LevelParams p,
+                                                                       const MeshFrame* frames) {
+    __shared__ uint32_t live_s[WARPS_PER_BLOCK][8][32];
+    const int lane = threadIdx.x & 31;
+    const int wib = threadIdx.x >> 5;
+    const uint32_t gw = blockIdx.x * WARPS_PER_BLOCK + wib;
+    uint32_t* cs = p.choice_scratch + size_t(gw) * p.choice_words * 32u + lane;
+    itv slots[REG_SLOTS];
+    const uint32_t n_roots = p.roots_y;
+    const uint32_t n_jobs = p.root_mode ? (n_roots + 31u) / 32u : min(p.ctr->n_jobs[p.level], p.cap_in);
+    for (;;) {
+        uint32_t j = 0;
+        if (lane == 0) {
+            j = atomicAdd(&p.ctr->cursor[p.level], 1u);
+            if (j < n_jobs && cancel_poll(p.cancel, CS_LEVEL0 + p.level, j)) j = ~0u;
+        }
+        j = __shfl_sync(FULL, j, 0);
+        if (j >= n_jobs) break;
+        level_job<3, false, true, false, true>(p, j, n_roots, slots, cs, live_s[wib], lane, p.epoch, frames);
+    }
+}
+void launch_octree_level_frames(const LevelParams& p, const MeshFrame* frames, int blocks, cudaStream_t s) {
+    k_octree_level<<<blocks, WARPS_PER_BLOCK * 32, 0, s>>>(p, frames);
+}
 
 }  // namespace fdev

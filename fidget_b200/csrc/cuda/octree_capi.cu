@@ -45,6 +45,58 @@ LevelParams tree_level(fc_ctx* c, const fc_tape* tape, const TreeScratch& t, int
     return p;
 }
 
+// The sampler's launches over n frames (fr: host; with n > 1 also d_fr on the device): the interval levels of one root
+// cell per frame, the frames stacked along Y (frame k owns the cell rows [k * 2^D, (k + 1) * 2^D)), then the leaf and
+// gradient kernels into `dout` (`cap` leaves; *d_n_out counts the surface leaves, beyond cap too).  One frame takes the
+// single-frame kernels with the frame in the launch parameters.  stats: the level and leaf statistics of
+// fc_octree_stats (c->stats and the words after the counters).  t0 (or null) is recorded once the scratch is set up.
+int32_t octree_enqueue(fc_ctx* c, const fc_tape* tape, uint32_t D, const MeshFrame* fr, uint32_t n, const MeshFrame* d_fr,
+                       OctreeLeaf* dout, uint64_t cap, bool stats, cudaEvent_t t0, const CallCancel& cc, uint32_t* launches) {
+    const int L = int(D) + 1;   // interval levels: depth 0 (the root cell) .. D
+    cudaStream_t s = c->stream;
+    const bool stack = n > 1;
+    TreeScratch t;
+    if (int32_t trc = tree_scratch(c, tape, D, 3, n, cap, t)) return trc;
+    if (stats) CU(cudaMemsetAsync(c->stats.p, 0, sizeof(Stats), s));
+    // extra device words after Counters: [0] n_out, then 5 u64 leaf statistics (8-byte aligned)
+    uint32_t* d_n_out = reinterpret_cast<uint32_t*>(c->counters.as<char>() + sizeof(Counters));
+    unsigned long long* d_leaf_stats = reinterpret_cast<unsigned long long*>(c->counters.as<char>() + sizeof(Counters) + 8);
+    if (t0) CU(cudaEventRecord(t0, s));
+    for (int l = 0; l < L; ++l) {
+        LevelParams p = tree_level(c, tape, t, l, fr[0].has_transform, fr[0].vb, cc);
+        p.roots_x = p.roots_z = 1;
+        p.roots_y = n;   // one root cell per frame, stacked along Y
+        p.width = p.depth = 1u << D;
+        p.height = n << D;
+        p.mat = fr[0].mat;
+        p.frame_rows = 1u << D;
+        p.stats = stats ? c->stats.as<Stats>() : nullptr;
+        const uint64_t cells = uint64_t(n) << (3 * l);
+        if (stack) launch_octree_level_frames(p, d_fr, t.blocks(l ? std::max<uint64_t>(1, cells / 8) : (n + 31) / 32), s);
+        else launch_interval_level_3d(p, t.blocks(l ? std::max<uint64_t>(1, cells / 8) : 1), s);
+    }
+    OctreeLeafParams q{};
+    q.jobs = c->jobs[L].as<TileJob>();
+    q.cap_jobs = uint32_t(t.level_cap[L]);
+    q.ctr = c->counters.as<Counters>();
+    q.list = L; q.cursor = L;
+    q.cell_h = 2.0f / float(1u << D);
+    q.has_transform = fr[0].has_transform;
+    q.mat = fr[0].mat;
+    q.vb = fr[0].vb;
+    q.out = dout;
+    q.out_tapes = c->leaf_tapes.as<TapeRef>();
+    q.cap_out = uint32_t(cap);
+    q.n_out = d_n_out;
+    q.stats = stats ? d_leaf_stats : nullptr;
+    q.cancel = cc.ref;
+    launch_octree_leaf(q, c->sm_count * 8, s, stack ? d_fr : nullptr, 1u << D);
+    launch_octree_grads(q, c->sm_count * 8, s, stack ? d_fr : nullptr, 1u << D);
+    if (launches) *launches = uint32_t(L) + 2;
+    CU(cudaGetLastError());
+    return FC_OK;
+}
+
 // Device half: runs the sampler into `dout` (device memory, `cap` leaves); *n_out = surface leaves found
 // (FC_ERR_INVALID when it exceeds cap).  Takes the context lock.  `cc`: the call's cancellation (begin_call).
 int32_t octree_sample_device(fc_ctx* c, const fc_tape* tape, const fc_octree_cfg* cfg, OctreeLeaf* dout, uint64_t cap,
@@ -57,50 +109,20 @@ int32_t octree_sample_device(fc_ctx* c, const fc_tape* tape, const fc_octree_cfg
     if (cap > 0xfffffff0ull) return fail(FC_ERR_INVALID, "leaf capacity too large");
     std::lock_guard<std::mutex> guard(c->mu);
     CU(cudaSetDevice(c->device));
-    VarBind vb;
-    if (int32_t vrc = bind_vars(tape, cfg->var_values, cfg->n_var_values, vb)) return vrc;
+    MeshFrame one{};
+    if (int32_t vrc = bind_vars(tape, cfg->var_values, cfg->n_var_values, one.vb)) return vrc;
+    memcpy(one.mat.m, cfg->world_to_model, sizeof one.mat.m);
+    one.has_transform = cfg->has_transform;
     const uint32_t D = cfg->depth;
-    const int L = int(D) + 1;   // interval levels: depth 0 (the root cell) .. D
     cudaStream_t s = c->stream;
     const bool timing = (cfg->flags & FC_FLAG_TIMING) != 0;
-    TreeScratch t;
-    if (int32_t trc = tree_scratch(c, tape, D, 3, 1, cap, t)) return trc;
-    CU(cudaMemsetAsync(c->stats.p, 0, sizeof(Stats), s));
-    // extra device words after Counters: [0] n_out, then 5 u64 leaf statistics (8-byte aligned)
+    uint32_t launches = 0;
+    if (int32_t rc = octree_enqueue(c, tape, D, &one, 1, nullptr, dout, cap, true, timing ? get_event(c, 0) : nullptr, cc,
+                                    &launches))
+        return rc;
+    if (timing) CU(cudaEventRecord(get_event(c, 1), s));
     uint32_t* d_n_out = reinterpret_cast<uint32_t*>(c->counters.as<char>() + sizeof(Counters));
     unsigned long long* d_leaf_stats = reinterpret_cast<unsigned long long*>(c->counters.as<char>() + sizeof(Counters) + 8);
-    if (timing) CU(cudaEventRecord(get_event(c, 0), s));
-    uint32_t launches = 0;
-    for (int l = 0; l < L; ++l) {
-        LevelParams p = tree_level(c, tape, t, l, cfg->has_transform, vb, cc);
-        p.roots_x = p.roots_y = p.roots_z = 1;
-        p.width = p.height = p.depth = 1u << D;
-        memcpy(p.mat.m, cfg->world_to_model, sizeof p.mat.m);
-        p.stats = c->stats.as<Stats>();
-        const uint64_t cells = 1ull << (3 * l);
-        launch_interval_level_3d(p, t.blocks(l ? std::max<uint64_t>(1, cells / 8) : 1), s);
-        ++launches;
-    }
-    OctreeLeafParams q{};
-    q.jobs = c->jobs[L].as<TileJob>();
-    q.cap_jobs = uint32_t(t.level_cap[L]);
-    q.ctr = c->counters.as<Counters>();
-    q.list = L; q.cursor = L;
-    q.cell_h = 2.0f / float(1u << D);
-    q.has_transform = cfg->has_transform;
-    memcpy(q.mat.m, cfg->world_to_model, sizeof q.mat.m);
-    q.vb = vb;
-    q.out = dout;
-    q.out_tapes = c->leaf_tapes.as<TapeRef>();
-    q.cap_out = uint32_t(cap);
-    q.n_out = d_n_out;
-    q.stats = d_leaf_stats;
-    q.cancel = cc.ref;
-    launch_octree_leaf(q, c->sm_count * 8, s);
-    launch_octree_grads(q, c->sm_count * 8, s);
-    launches += 2;
-    if (timing) CU(cudaEventRecord(get_event(c, 1), s));
-    CU(cudaGetLastError());
     uint32_t n_out = 0;
     if (int32_t wrc = wait_read(c, s, cc, &n_out, d_n_out, 4)) {
         *n_out_p = 0;

@@ -987,7 +987,126 @@ def mesh_cells(cuda) -> np.ndarray:
     _ck(lib.fc_mesh_read_cells(cuda._h, None, 0, C.byref(n)))
     out = np.zeros(n.value, dtype=MESH_CELL)
     _ck(lib.fc_mesh_read_cells(cuda._h, _ptr(out), n.value, C.byref(n)))
-    return out[np.lexsort((out["ix"], out["iy"], out["iz"], out["depth"]))]
+    return _sorted_cells(out)
+
+
+def mesh_frame_table(world_to_model=None, var_values=None):
+    """The ``fc_mesh_frame`` table of ``mesh_frames``: frame k's ``world_to_model`` (4x4, world -> model) and ShapeVars,
+    each what ``mesh`` puts into ``fc_octree_cfg`` for that frame's values.  Every argument given is per frame (leading
+    dimension n: ``world_to_model`` [n, 4, 4], ``var_values`` [n, k]); the other takes ``mesh``'s default (no transform,
+    no values).  A ``world_to_model`` entry of None is a frame without a transform, as ``mesh``'s
+    ``world_to_model=None``.  Lengths that disagree raise ValueError, as in ``contour_slice_table``; with no per-frame
+    argument at all there is one frame."""
+    per = {}
+    if var_values is not None:
+        vv = np.asarray(var_values, dtype=np.float32)
+        if vv.ndim != 2 or vv.shape[1] > _lib.FC_MAX_VARS:
+            raise ValueError(f"var_values must be [n, k] with k <= {_lib.FC_MAX_VARS}")
+        per["var_values"] = vv
+    if world_to_model is not None:
+        wm = [None if w is None else np.asarray(w, dtype=np.float32) for w in world_to_model]
+        if any(w is not None and w.shape != (4, 4) for w in wm):
+            raise ValueError("world_to_model must be [n, 4, 4] (an entry may be None: no transform)")
+        per["world_to_model"] = wm
+    lengths = {k: len(v) for k, v in per.items()}
+    if len(set(lengths.values())) > 1:
+        raise ValueError(f"per-frame arguments disagree in length: {lengths}")
+    n = next(iter(lengths.values())) if lengths else 1
+    table = (_lib.FcMeshFrame * n)()
+    for k in range(n):
+        f = table[k]
+        if "world_to_model" in per and per["world_to_model"][k] is not None:
+            f.has_transform = 1
+            f.world_to_model[:] = per["world_to_model"][k].reshape(16).tolist()
+        values = per["var_values"][k] if "var_values" in per else ()
+        f.n_var_values = len(values)
+        for i, v in enumerate(values):
+            f.var_values[i] = float(v)
+    return table
+
+
+def split_mesh_frames(vertices, triangles, per_frame, cells=None):
+    """The per-frame ``(vertices, triangles)`` (and final leaves, with ``cells``) of a batch's read buffers: frame k
+    takes the next ``n_vertices`` / ``n_triangles`` / ``n_cells`` rows of ``per_frame[k]``; its triangle indices are
+    already local to its vertices.  Counts that do not add up to the buffers' lengths raise ValueError."""
+    v = np.asarray(vertices, dtype=np.float32).reshape(-1, 3)
+    t = np.asarray(triangles, dtype=np.uint32).reshape(-1, 3)
+    out, pv, pt, pc = [], 0, 0, 0
+    for p in per_frame:
+        nv, nt = int(p["n_vertices"]), int(p["n_triangles"])
+        part = [v[pv:pv + nv], t[pt:pt + nt]]
+        if cells is not None:
+            nc = int(p["n_cells"])
+            part.append(cells[pc:pc + nc])
+            pc += nc
+        out.append(tuple(part))
+        pv, pt = pv + nv, pt + nt
+    if pv != len(v) or pt != len(t) or (cells is not None and pc != len(cells)):
+        raise ValueError("per-frame counts do not add up to the batch's")
+    return out
+
+
+def split_mesh_stl(buf, n_triangles):
+    """The per-frame binary STL files of a batch's ``fc_mesh_write_stl`` output: frame k's takes 84 + 50 n_k bytes.
+    Counts that do not add up to the buffer's length raise ValueError."""
+    b = bytes(buf)
+    out, p = [], 0
+    for nt in n_triangles:
+        size = 84 + 50 * int(nt)
+        out.append(b[p:p + size])
+        p += size
+    if p != len(b):
+        raise ValueError("per-frame triangle counts do not add up to the STL's length")
+    return out
+
+
+def _sorted_cells(cells):
+    return cells[np.lexsort((cells["ix"], cells["iy"], cells["iz"], cells["depth"]))]
+
+
+def mesh_frames(shape: CudaShape, depth: int, world_to_model=None, var_values=None, collapse: bool = False,
+                stl: bool = False, cells: bool = False, cancel: CancelToken | None = None):
+    """Meshes of many frames in one call (``fc_mesh_build_frames``): frame k is ``mesh`` of its own
+    ``world_to_model`` / ``var_values`` (see ``mesh_frame_table``), the same vertices bit for bit and the same
+    triangles.  Returns ``(frames, info, per_frame)``: ``frames[k] = (vertices, triangles)``, plus frame k's binary STL
+    bytes when ``stl`` and its final leaves (sorted as ``mesh_cells`` sorts them) when ``cells``; ``info`` the totals
+    (device times summed over passes) and ``per_frame[k]`` frame k's counts.  None when ``cancel`` cancelled the call
+    (the context then holds no mesh)."""
+    lib = shape._lib
+    table = mesh_frame_table(world_to_model=world_to_model, var_values=var_values)
+    n = len(table)
+    c = _lib.FcOctreeCfg()
+    c.depth = depth
+    c.flags = _lib.FC_FLAG_TIMING | (_lib.FC_FLAG_MESH_COLLAPSE if collapse else 0)
+    info = _lib.FcMeshInfo()
+    per = (_lib.FcMeshFrameInfo * n)()
+    rc = shape.cuda._cancellable(cancel, lambda: lib.fc_mesh_build_frames(
+        shape.cuda._h, shape._h, C.byref(c), table, n, C.byref(info), per))
+    if rc == _lib.FC_ERR_CANCELLED:
+        return None
+    _ck(rc)
+    verts = np.zeros((info.n_vertices, 3), dtype=np.float32)
+    tris = np.zeros((info.n_triangles, 3), dtype=np.uint32)
+    _ck(lib.fc_mesh_read(shape.cuda._h, _ptr(verts), _ptr(tris)))
+    as_dict = lambda x: {f: getattr(x, f) for f, _ in x._fields_}   # noqa: E731
+    per_frame = [as_dict(per[k]) for k in range(n)]
+    all_cells = None
+    if cells:
+        nc = C.c_uint64()
+        _ck(lib.fc_mesh_read_cells(shape.cuda._h, None, 0, C.byref(nc)))
+        all_cells = np.zeros(nc.value, dtype=MESH_CELL)
+        _ck(lib.fc_mesh_read_cells(shape.cuda._h, _ptr(all_cells), nc.value, C.byref(nc)))
+    frames = split_mesh_frames(verts, tris, per_frame, all_cells)
+    if cells:
+        frames = [(v, t, _sorted_cells(cl)) for v, t, cl in frames]
+    if stl:
+        nb = C.c_size_t()
+        _ck(lib.fc_mesh_write_stl(shape.cuda._h, None, 0, C.byref(nb)))
+        buf = np.zeros(nb.value, dtype=np.uint8)
+        _ck(lib.fc_mesh_write_stl(shape.cuda._h, _ptr(buf), nb.value, C.byref(nb)))
+        files = split_mesh_stl(buf, [p["n_triangles"] for p in per_frame])
+        frames = [(f[0], f[1], files[k]) + tuple(f[2:]) for k, f in enumerate(frames)]
+    return frames, as_dict(info), per_frame
 
 
 # ---------------------------------------------------------------------------

@@ -65,7 +65,7 @@ int32_t fc_ctx_set_arena_bytes(fc_ctx* ctx, uint64_t bytes);
  * layout of Rust's AtomicBool (CancelToken::into_raw() as *const u8): nonzero = cancelled.  The library reads it with
  * an acquire load, from any thread; NULL detaches it.  Context-wide, like fc_ctx_set_stream, and consulted only by
  * fc_render2d, fc_render2d_frames, fc_render2d_scene, fc_render3d, fc_render3d_frames, fc_render3d_scene, fc_octree_sample,
- * fc_mesh_build, fc_contour_build, and
+ * fc_mesh_build, fc_mesh_build_frames, fc_contour_build, and
  * fc_ctx_synchronize after the most recent FC_FLAG_ASYNC call of those.  With a flag attached:
  *  - set on entry: the call returns FC_ERR_CANCELLED before it allocates or launches anything;
  *  - set while the call runs: the kernels stop claiming work and the call returns FC_ERR_CANCELLED ("cancelled" in
@@ -510,8 +510,46 @@ typedef struct fc_mesh_cell {
  * without FC_FLAG_MESH_COLLAPSE).  out == NULL queries the count. */
 int32_t fc_mesh_read_cells(fc_ctx* ctx, fc_mesh_cell* out, uint64_t cap, uint64_t* n);
 /* Mesh::write_stl (fidget-mesh/src/output.rs:7-38): binary STL of the last mesh, assembled on the device.
- * buf == NULL queries the size (84 + 50 * n_triangles). */
+ * buf == NULL queries the size (84 + 50 * n_triangles; after fc_mesh_build_frames one file per frame, back to back). */
 int32_t fc_mesh_write_stl(fc_ctx* ctx, uint8_t* buf, size_t cap, size_t* n_bytes);
+/* Many meshes of one tape in one call: an animation through a ShapeVars parameter, a design sweep, one part under several
+ * placements or views.  Frame k's mesh is what fc_mesh_build gives for cfg's depth and flags (FC_FLAG_MESH_COLLAPSE,
+ * FC_FLAG_TIMING) plus frame k's has_transform, world_to_model and var_values: the same vertices bit for bit and the same
+ * triangles as triples of vertex positions with their winding (both compared as multisets, since fc_mesh_build writes
+ * in atomic order), the same n_leaves, n_vertices, n_triangles and open_edges, and with collapse the same final leaves
+ * and cell vertices.  The frames of a pass share each launch: one tall octree grid holds them (frame k owns the cell
+ * rows [k * 2^depth, (k + 1) * 2^depth)), and the mesher keys every cell by its frame, so nothing crosses frames.
+ *  - cfg supplies depth and flags; its has_transform, world_to_model and var_values are ignored.
+ *  - fc_mesh_read returns the whole batch: vertices and triangles frame-contiguous in frame order, each frame's
+ *    triangle indices relative to its first vertex, so frame k's rows of the two arrays are a complete mesh on their own
+ *    (per_frame gives the row counts).  fc_mesh_read_cells lists the final leaves frame by frame (n_cells each), and
+ *    fc_mesh_write_stl writes one complete binary STL per frame, back to back: frame k's file takes
+ *    84 + 50 * n_triangles_k bytes.  After a single fc_mesh_build the reads give what a batch of its one frame would;
+ *    whichever of the two ran last is what they return.
+ *  - per_frame (may be NULL, n_frames entries): frame k's counts.  info: their sums (n_cells has no field there), and
+ *    sampler_ms (with FC_FLAG_TIMING) and mesh_ms summed over passes.
+ *  - passes: the first pass holds one frame, later ones are sized from the largest per-frame arena, job-list and
+ *    surface-leaf use seen so far (leaves and mesh scratch within FC_FRAMES_PASS_BYTES, at most
+ *    FC_MESH_MAX_PASS_FRAMES frames), and a pass that overflows anyway is run again in halves: FC_ERR_ARENA, a work-list
+ *    overflow or "mesh too large for cell collapse" comes back only where one frame alone would give it.
+ *  - Errors are fc_mesh_build's, checked for every frame before anything is allocated or launched (depth above
+ *    FC_MAX_OCTREE_DEPTH, a multi-output tape, more than FC_MAX_VARS values or a frame without a value for a bound
+ *    variable: FC_ERR_INVALID; a tape with memory slots: FC_ERR_UNSUPPORTED), and FC_ERR_INVALID for frames == NULL
+ *    with n_frames > 0.  A failed or cancelled call (the cancel flag behaves as in fc_mesh_build) leaves no mesh, as
+ *    does n_frames == 0, which launches nothing. */
+#define FC_MESH_MAX_PASS_FRAMES 4096u
+typedef struct fc_mesh_frame {
+    uint32_t has_transform;         /* as fc_octree_cfg.has_transform */
+    float world_to_model[16];       /* as fc_octree_cfg.world_to_model (row-major 4x4) */
+    uint32_t n_var_values;          /* ShapeVars of this frame, as fc_octree_cfg */
+    float var_values[FC_MAX_VARS];
+} fc_mesh_frame;
+typedef struct fc_mesh_frame_info {
+    uint64_t n_leaves, n_vertices, n_triangles, open_edges, n_cells;
+} fc_mesh_frame_info;
+int32_t fc_mesh_build_frames(fc_ctx* ctx, const fc_tape* tape, const fc_octree_cfg* cfg /* depth, flags */,
+                             const fc_mesh_frame* frames /* host */, uint32_t n_frames,
+                             fc_mesh_info* info /* totals */, fc_mesh_frame_info* per_frame /* may be NULL */);
 
 /* ---- 2D contours (libfive's Contours::render, on the quadtree the mesher's octree restricts to) -------------------
  * fc_contour_build extracts the contours of a 2D shape (a sketch, a cut profile, a Z slice of a 3D model) as closed or

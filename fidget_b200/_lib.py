@@ -165,6 +165,7 @@ class FcCompiledInfo(C.Structure):
 
 FC_COMPILE_FLOAT, FC_COMPILE_GRAD, FC_COMPILE_INTERVAL = 1, 2, 4
 FC_SOLVE_MAX_FREE, FC_SOLVE_MAX_CONSTRAINTS, FC_SOLVE_MAX_PARAMS = 64, 256, 1024
+FC_SOLVE_LARGE_MAX_FREE, FC_SOLVE_LARGE_MAX_CONSTRAINTS, FC_SOLVE_LARGE_MAX_PARAMS = 1024, 4096, 16384
 FC_SOLVE_ZERO_RESIDUAL = 0
 FC_SOLVE_UNCHANGED = 1
 FC_SOLVE_ZERO_ERR = 2
@@ -249,6 +250,7 @@ CUDA_API = {
     "fc_contour_build_slices": (_i32, [_vp, _vp, _P(FcContourCfg), _P(FcContourSlice), _u32, _P(FcContourInfo),
                                        _P(FcContourInfo)]),
     "fc_solve_batch": (_i32, [_vp, _P(_vp), _u32, _P(_P(_i32)), _P(FcSolveCfg), _vp, _u64, _vp]),
+    "fc_solve_large_batch": (_i32, [_vp, _P(_vp), _u32, _P(_P(_i32)), _P(FcSolveCfg), _vp, _u64, _vp]),
     "fc_schedule_check": (_i32, [_P(_u32), C.c_size_t, _u8, _u32, _u32, _u32, _P(FcScheduleInfo)]),
     "fc_denoise_normals": (_i32, [_vp, _vp, _u32, _u32, _vp]),
     "fc_compute_ssao": (_i32, [_vp, _vp, _u32, _u32, _u32, _vp, _u32, _vp, _u32, _vp]),

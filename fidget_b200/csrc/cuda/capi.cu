@@ -153,6 +153,7 @@ void fc_ctx_destroy(fc_ctx* c) {
     c->solve_meta.release();
     c->solve_vals.release();
     c->solve_res.release();
+    c->solve_work.release();
     c->frame_table.release();
     c->frame_tops.release();
     c->scene_pl.release();
@@ -231,9 +232,13 @@ static int32_t cancel_site_of(const std::string& name) {
     if (name == "k_scene2d_resolve") return CS_SCENE2D_RESOLVE;
     static const char* const contour[] = {"k_contour_leaf", "k_contour_grads", "k_contour_vertices", "k_contour_segments",
                                           "k_contour_link", "k_contour_emit"};
-    static_assert(sizeof(contour) / sizeof(contour[0]) == CS_COUNT - CS_CONTOUR_LEAF, "one name per poll site");
-    for (int i = 0; i < CS_COUNT - CS_CONTOUR_LEAF; ++i)
+    static_assert(sizeof(contour) / sizeof(contour[0]) == CS_SOLVE - CS_CONTOUR_LEAF, "one name per poll site");
+    for (int i = 0; i < CS_SOLVE - CS_CONTOUR_LEAF; ++i)
         if (name == contour[i]) return CS_CONTOUR_LEAF + i;
+    static const char* const solve[] = {"k_solve", "k_solve_large"};
+    static_assert(sizeof(solve) / sizeof(solve[0]) == CS_COUNT - CS_SOLVE, "one name per poll site");
+    for (int i = 0; i < CS_COUNT - CS_SOLVE; ++i)
+        if (name == solve[i]) return CS_SOLVE + i;
     return -1;
 }
 

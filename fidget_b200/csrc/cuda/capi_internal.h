@@ -127,7 +127,8 @@ struct fc_ctx {
     uint32_t* contour_offsets = nullptr;                        // in contour_offs
     uint8_t* contour_closed = nullptr;                          // in contour_flags
     DevBuf fx_in, fx_out, fx_tmp, fx_tables;  // effects: staged host images, intermediate maps, SSAO tables
-    DevBuf solve_meta, solve_vals, solve_res; // fc_solve_batch: tape table + slot maps, staged host values / results
+    DevBuf solve_meta, solve_vals, solve_res; // the solvers: tape table + slot maps, staged host values / results
+    DevBuf solve_work;                        // fc_solve_large_batch: one workspace slice per cluster in flight
     // the batches (fc_render2d_frames, fc_render3d_frames, fc_render3d_scene): the frame or placement table, and the copy
     // stream that returns a frame batch's pass to a host `out` while the next pass runs (ev_pass: the pass in staging
     // buffer b is complete; ev_copied: copied back).  fc_render2d_frames: each pass's arena high-water mark.

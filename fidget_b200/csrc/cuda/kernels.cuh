@@ -26,6 +26,7 @@ enum CancelSite : int32_t {
     CS_WAIT,                                              // polls inside spin waits: not a claim, never a trigger site
     CS_SCENE2D_RESOLVE,                                   // (after CS_WAIT: the ids the kernels above compare stay put)
     CS_CONTOUR_LEAF, CS_CONTOUR_GRADS, CS_CONTOUR_VERTICES, CS_CONTOUR_SEGMENTS, CS_CONTOUR_LINK, CS_CONTOUR_EMIT,
+    CS_SOLVE, CS_SOLVE_LARGE,                             // the solvers: item = problem index (claim and every iteration)
     CS_COUNT
 };
 struct CancelRef {

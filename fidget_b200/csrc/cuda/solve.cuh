@@ -1,6 +1,8 @@
-// Batched Levenberg-Marquardt solver (fc_solve_batch): launch parameters shared by solve.cu and solve_capi.cu.
+// Batched Levenberg-Marquardt solvers (fc_solve_batch, fc_solve_large_batch): launch parameters shared by solve.cu and
+// solve_capi.cu.
 #pragma once
 #include "kernels.cuh"
+#include "solve_plan.h"
 
 namespace fdev {
 
@@ -20,6 +22,9 @@ struct SolveParams {
     float* values;                 // [n_problems][n_params], free entries overwritten with the solution
     SolveResultDev* results;       // [n_problems] or null
     uint64_t n_problems;
+    CancelRef cancel;              // polled before a problem is claimed and at the top of every iteration
+    float* work;                   // k_solve_large: [clusters][slice_floats] workspace (solve_plan.h)
+    size_t slice_floats;
 };
 
 // Dynamic shared memory of one block (bytes)
@@ -28,5 +33,10 @@ uint32_t solve_threads(uint32_t n_free);
 // Sets the kernel's shared-memory limit and returns its resident blocks per SM for this shape (0: does not fit)
 int solve_blocks_per_sm(uint32_t m, uint32_t n_params, uint32_t n_free);
 void launch_solve(const SolveParams& p, int blocks, cudaStream_t s);
+
+// k_solve_large: one problem per cluster of `cluster` CTAs.  Sets the kernel's attributes and returns the device's
+// resident clusters of that size (cudaOccupancyMaxActiveClusters; 0: none fits), or a negative CUDA error
+int solve_large_max_clusters(uint32_t cluster);
+cudaError_t launch_solve_large(const SolveParams& p, uint32_t cluster, uint64_t clusters, cudaStream_t s);
 
 }  // namespace fdev

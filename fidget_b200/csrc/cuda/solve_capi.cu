@@ -1,24 +1,31 @@
-// fc_solve_batch (include/fidget_cuda.h, "constraint solver"): argument checks, the tape table and slot maps, staging
-// of host values / results, and the launch of k_solve (solve.cu).
+// fc_solve_batch and fc_solve_large_batch (include/fidget_cuda.h, "constraint solver"): argument checks, the tape table
+// and slot maps, staging of host values / results, cancellation, and the launch of k_solve or k_solve_large (solve.cu).
 #include "capi_internal.h"
 #include "solve.cuh"
 
 static_assert(sizeof(fc_solve_result) == sizeof(SolveResultDev), "fc_solve_result layout");
+static_assert(FC_SOLVE_LARGE_MAX_FREE == SOLVE_LARGE_MAX_FREE &&
+                  FC_SOLVE_LARGE_MAX_CONSTRAINTS == SOLVE_LARGE_MAX_CONSTRAINTS &&
+                  FC_SOLVE_LARGE_MAX_PARAMS == SOLVE_LARGE_MAX_PARAMS, "fc_solve_large_batch limits");
 
-extern "C" int32_t fc_solve_batch(fc_ctx* c, const fc_tape* const* constraints, uint32_t n_constraints,
-                                  const int32_t* const* slot_param, const fc_solve_cfg* cfg, float* values,
-                                  uint64_t n_problems, fc_solve_result* results) {
+static int32_t solve_call(fc_ctx* c, const fc_tape* const* constraints, uint32_t n_constraints,
+                          const int32_t* const* slot_param, const fc_solve_cfg* cfg, float* values, uint64_t n_problems,
+                          fc_solve_result* results, bool large) {
+    const std::string fn = large ? "fc_solve_large_batch" : "fc_solve_batch";
     if (!c || !cfg || (n_constraints && (!constraints || !slot_param)) || (n_problems && !values))
         return fail(FC_ERR_INVALID, "null argument");
     const uint32_t n_params = cfg->n_params, n_free = cfg->n_free;
-    if (n_free == 0) return fail(FC_ERR_INVALID, "fc_solve_batch: no free parameter");
-    if (n_free > n_params) return fail(FC_ERR_INVALID, "fc_solve_batch: n_free > n_params");
-    if (n_free > SOLVE_MAX_FREE)
-        return fail(FC_ERR_UNSUPPORTED, "fc_solve_batch: more than " + std::to_string(SOLVE_MAX_FREE) + " free parameters");
-    if (n_constraints > SOLVE_MAX_CONSTRAINTS)
-        return fail(FC_ERR_UNSUPPORTED, "fc_solve_batch: more than " + std::to_string(SOLVE_MAX_CONSTRAINTS) + " constraints");
-    if (n_params > SOLVE_MAX_PARAMS)
-        return fail(FC_ERR_UNSUPPORTED, "fc_solve_batch: more than " + std::to_string(SOLVE_MAX_PARAMS) + " parameters");
+    const uint32_t max_free = large ? SOLVE_LARGE_MAX_FREE : SOLVE_MAX_FREE;
+    const uint32_t max_constraints = large ? SOLVE_LARGE_MAX_CONSTRAINTS : SOLVE_MAX_CONSTRAINTS;
+    const uint32_t max_params = large ? SOLVE_LARGE_MAX_PARAMS : SOLVE_MAX_PARAMS;
+    if (n_free == 0) return fail(FC_ERR_INVALID, fn + ": no free parameter");
+    if (n_free > n_params) return fail(FC_ERR_INVALID, fn + ": n_free > n_params");
+    if (n_free > max_free)
+        return fail(FC_ERR_UNSUPPORTED, fn + ": more than " + std::to_string(max_free) + " free parameters");
+    if (n_constraints > max_constraints)
+        return fail(FC_ERR_UNSUPPORTED, fn + ": more than " + std::to_string(max_constraints) + " constraints");
+    if (n_params > max_params)
+        return fail(FC_ERR_UNSUPPORTED, fn + ": more than " + std::to_string(max_params) + " parameters");
 
     // tape table [m] | slot offsets [m + 1] | slot -> parameter
     std::vector<TapeRef> refs(n_constraints);
@@ -26,7 +33,7 @@ extern "C" int32_t fc_solve_batch(fc_ctx* c, const fc_tape* const* constraints, 
     std::vector<int32_t> slots;
     for (uint32_t k = 0; k < n_constraints; ++k) {
         const fc_tape* t = constraints[k];
-        const std::string who = "fc_solve_batch: constraint " + std::to_string(k);
+        const std::string who = fn + ": constraint " + std::to_string(k);
         if (!t) return fail(FC_ERR_INVALID, who + " is null");
         if (t->ctx != c) return fail(FC_ERR_INVALID, who + " belongs to another context");
         if (t->info.mem_count) return fail(FC_ERR_UNSUPPORTED, who + " uses memory slots");
@@ -43,10 +50,35 @@ extern "C" int32_t fc_solve_batch(fc_ctx* c, const fc_tape* const* constraints, 
     }
     if (n_problems == 0) return FC_OK;
 
+    CallCancel cc;
+    if (int32_t rc = begin_call(c, cc)) return rc;
     std::lock_guard<std::mutex> guard(c->mu);
     CU(cudaSetDevice(c->device));
-    const int per_sm = solve_blocks_per_sm(n_constraints, n_params, n_free);
-    if (per_sm <= 0) return fail(FC_ERR_UNSUPPORTED, "fc_solve_batch: problem too large for one thread block's shared memory");
+    // launch shape: k_solve's blocks per SM, or k_solve_large's cluster size and clusters in flight (solve_plan.h)
+    int per_sm = 0;
+    uint32_t cluster = 1;
+    uint64_t clusters = 0;
+    size_t slice = 0;
+    if (!large) {
+        per_sm = solve_blocks_per_sm(n_constraints, n_params, n_free);
+        if (per_sm <= 0) return fail(FC_ERR_UNSUPPORTED, fn + ": problem too large for one thread block's shared memory");
+    } else {
+        const int forced = env_int("FIDGET_B200_SOLVE_CLUSTER", 0);
+        cluster = solve_cluster_size(n_free, forced);
+        int resident = solve_large_max_clusters(cluster);
+        // without a forced size, a cluster the device cannot place is halved: every size gives the same bits
+        while (resident == 0 && forced <= 0 && cluster > 1) resident = solve_large_max_clusters(cluster /= 2);
+        if (resident < 0) CU(cudaError_t(-resident));
+        if (resident == 0)
+            return fail(FC_ERR_UNSUPPORTED, fn + ": the device cannot place a cluster of " + std::to_string(cluster) + " CTAs");
+        int device_sms = 0;
+        CU(cudaDeviceGetAttribute(&device_sms, cudaDevAttrMultiProcessorCount, c->device));
+        slice = solve_large_slice_bytes(n_constraints, n_params, n_free);
+        clusters = solve_large_clusters(n_problems, resident, c->sm_count, device_sms, slice, FC_FRAMES_PASS_BYTES);
+        if (cudaError_t e = c->solve_work.ensure(slice * clusters))
+            return fail(FC_ERR_CUDA, fn + ": cannot allocate the " + std::to_string(slice * clusters >> 20) +
+                                         " MiB solver workspace: " + cudaGetErrorString(e));
+    }
 
     const size_t b_refs = refs.size() * sizeof(TapeRef), b_offs = offs.size() * 4, b_slots = slots.size() * 4;
     const size_t o_offs = (b_refs + 15) & ~size_t(15), o_slots = (o_offs + b_offs + 15) & ~size_t(15);
@@ -66,6 +98,9 @@ extern "C" int32_t fc_solve_batch(fc_ctx* c, const fc_tape* const* constraints, 
     p.n_free = n_free;
     p.max_iters = cfg->max_iters ? cfg->max_iters : 1000u;
     p.n_problems = n_problems;
+    p.cancel = cc.ref;
+    p.work = large ? c->solve_work.as<float>() : nullptr;
+    p.slice_floats = slice / 4;
 
     const size_t b_vals = size_t(n_problems) * n_params * 4, b_res = size_t(n_problems) * sizeof(fc_solve_result);
     const bool dvals = is_device_ptr(values), dres = is_device_ptr(results);
@@ -83,11 +118,30 @@ extern "C" int32_t fc_solve_batch(fc_ctx* c, const fc_tape* const* constraints, 
             p.results = c->solve_res.as<SolveResultDev>();
         }
     }
-    const uint64_t cap = uint64_t(per_sm) * uint64_t(c->sm_count);
-    launch_solve(p, int(n_problems < cap ? n_problems : cap), c->stream);
+    if (large) {
+        CU(launch_solve_large(p, cluster, clusters, c->stream));
+    } else {
+        const uint64_t cap = uint64_t(per_sm) * uint64_t(c->sm_count);
+        launch_solve(p, int(n_problems < cap ? n_problems : cap), c->stream);
+    }
     CU(cudaGetLastError());
+    // with a cancel flag attached the (cancellable) wait comes first, and a cancelled call copies nothing back
+    if (cc.flag)
+        if (int32_t rc = wait_call(c, c->stream, cc)) return rc;
     if (!dvals) CU(cudaMemcpyAsync(values, p.values, b_vals, cudaMemcpyDeviceToHost, c->stream));
     if (results && !dres) CU(cudaMemcpyAsync(results, p.results, b_res, cudaMemcpyDeviceToHost, c->stream));
     CU(cudaStreamSynchronize(c->stream));
     return FC_OK;
+}
+
+extern "C" int32_t fc_solve_batch(fc_ctx* c, const fc_tape* const* constraints, uint32_t n_constraints,
+                                  const int32_t* const* slot_param, const fc_solve_cfg* cfg, float* values,
+                                  uint64_t n_problems, fc_solve_result* results) {
+    return solve_call(c, constraints, n_constraints, slot_param, cfg, values, n_problems, results, false);
+}
+
+extern "C" int32_t fc_solve_large_batch(fc_ctx* c, const fc_tape* const* constraints, uint32_t n_constraints,
+                                        const int32_t* const* slot_param, const fc_solve_cfg* cfg, float* values,
+                                        uint64_t n_problems, fc_solve_result* results) {
+    return solve_call(c, constraints, n_constraints, slot_param, cfg, values, n_problems, results, true);
 }

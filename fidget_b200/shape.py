@@ -57,8 +57,8 @@ def schedule_check(tape: TapeData) -> dict:
 
 
 class CancelToken:
-    """``CancelToken``: a flag another thread sets to stop a render, ``octree_sample`` or ``mesh`` in flight (the call
-    then returns ``None``).  One byte, read by the library with an acquire load (``fc_ctx_set_cancel``)."""
+    """``CancelToken``: a flag another thread sets to stop a render, ``octree_sample``, ``mesh``, ``contour`` or solve in
+    flight (the call then returns ``None``).  One byte, read by the library with an acquire load (``fc_ctx_set_cancel``)."""
 
     def __init__(self):
         self._flag = C.c_uint8(0)
@@ -1248,7 +1248,7 @@ def contours_svg(vertices, offsets, closed, size: float = 512.0, stroke: str = "
 
 
 # ---------------------------------------------------------------------------
-# Constraint solver (fidget-solver/src/lib.rs): fc_solve_batch
+# Constraint solver (fidget-solver/src/lib.rs): fc_solve_batch, fc_solve_large_batch
 @dataclass(frozen=True)
 class Free:
     """``Parameter::Free``: a variable the solver moves, starting at ``value``."""
@@ -1261,17 +1261,11 @@ class Fixed:
     value: float
 
 
-def solve_batch(constraints, free, fixed, values, max_iters=None):
-    """Levenberg-Marquardt least squares on the constraints' output 0, for many problems at once
-    (``fc_solve_batch``).  ``free`` / ``fixed``: the variable keys ("x", "y", "z" or ``Context.var()`` ids); the free
-    ones are the Jacobian's columns, in this order.  ``values``: [n_problems, len(free) + len(fixed)] starting values
-    of the free variables followed by the fixed ones -- a numpy array, or a CUDA torch tensor (the work and the
-    results then stay on the device).  ``max_iters``: step cap (default 1000).
-    Returns ``(values, status, iterations, err)``: a copy of ``values`` with the free entries solved, and per problem
-    the exit (``FC_SOLVE_*``), the number of steps and the final squared error."""
+def _solve_call(fn, constraints, free, fixed, values, max_iters, cancel):
+    """fc_solve_batch / fc_solve_large_batch (``fn``): the shared staging of solve_batch and solve_large_batch"""
     constraints = list(constraints)
     if not constraints:
-        raise ValueError("solve_batch needs at least one constraint")
+        raise ValueError(f"{fn[3:]} needs at least one constraint")
     cuda = constraints[0].cuda
     lib = cuda._lib
     free, fixed = list(free), list(fixed)
@@ -1292,25 +1286,54 @@ def solve_batch(constraints, free, fixed, values, max_iters=None):
     tapes = (C.c_void_p * len(constraints))(*[c._h for c in constraints])
     sp = (C.POINTER(C.c_int32) * len(maps))(*[m.ctypes.data_as(C.POINTER(C.c_int32)) for m in maps])
     cfg = _lib.FcSolveCfg(len(keys), len(free), 0 if max_iters is None else int(max_iters))
-    _ck(lib.fc_solve_batch(cuda._h, tapes, len(constraints), sp, C.byref(cfg), _ptr(vals), int(vals.shape[0]),
-                           _ptr(res)))
+    call = getattr(lib, fn)
+    rc = cuda._cancellable(cancel, lambda: call(cuda._h, tapes, len(constraints), sp, C.byref(cfg), _ptr(vals),
+                                                int(vals.shape[0]), _ptr(res)))
+    if rc == _lib.FC_ERR_CANCELLED:
+        return None
+    _ck(rc)
     if device:
         import torch
         return vals, res[:, 0].clone(), res[:, 1].clone(), res.view(torch.float32)[:, 2].clone()
     return vals, res[:, 0].astype(np.uint32), res[:, 1].astype(np.uint32), res.view(np.float32)[:, 2].copy()
 
 
-def solve(constraints, params: dict, max_iters=None) -> dict:
+def solve_batch(constraints, free, fixed, values, max_iters=None, cancel: CancelToken | None = None):
+    """Levenberg-Marquardt least squares on the constraints' output 0, for many problems at once
+    (``fc_solve_batch``).  ``free`` / ``fixed``: the variable keys ("x", "y", "z" or ``Context.var()`` ids); the free
+    ones are the Jacobian's columns, in this order.  ``values``: [n_problems, len(free) + len(fixed)] starting values
+    of the free variables followed by the fixed ones -- a numpy array, or a CUDA torch tensor (the work and the
+    results then stay on the device).  ``max_iters``: step cap (default 1000).
+    Returns ``(values, status, iterations, err)``: a copy of ``values`` with the free entries solved, and per problem
+    the exit (``FC_SOLVE_*``), the number of steps and the final squared error.  None when ``cancel`` cancelled it."""
+    return _solve_call("fc_solve_batch", constraints, free, fixed, values, max_iters, cancel)
+
+
+def solve_large_batch(constraints, free, fixed, values, max_iters=None, cancel: CancelToken | None = None):
+    """``solve_batch`` for problems of up to 1024 free variables, 4096 constraints and 16384 variables in all
+    (``fc_solve_large_batch``: one problem per thread-block cluster).  Same arguments and return; on every problem
+    ``solve_batch`` accepts, the same bits.  None when ``cancel`` cancelled it."""
+    return _solve_call("fc_solve_large_batch", constraints, free, fixed, values, max_iters, cancel)
+
+
+def solve(constraints, params: dict, max_iters=None, cancel: CancelToken | None = None) -> dict | None:
     """``fidget_solver::solve``: ``params`` maps variable keys ("x", "y", "z" or ``Context.var()`` ids) to
-    ``Free(start)`` / ``Fixed(value)``; returns {key: solved value} for the free ones."""
+    ``Free(start)`` / ``Fixed(value)``; returns {key: solved value} for the free ones, or None when ``cancel``
+    cancelled it.  Problems beyond ``solve_batch``'s limits go to ``solve_large_batch``."""
     for k, p in params.items():
         if not isinstance(p, (Free, Fixed)):
             raise TypeError(f"parameter {k!r} must be Free(..) or Fixed(..), not {p!r}")
     free = [k for k, p in params.items() if isinstance(p, Free)]
     fixed = [k for k, p in params.items() if isinstance(p, Fixed)]
     row = [params[k].value for k in free] + [params[k].value for k in fixed]
-    vals, _, _, _ = solve_batch(constraints, free, fixed, np.array([row], dtype=np.float32), max_iters)
-    return {k: float(vals[0, i]) for i, k in enumerate(free)}
+    constraints = list(constraints)
+    small = (len(free) <= _lib.FC_SOLVE_MAX_FREE and len(constraints) <= _lib.FC_SOLVE_MAX_CONSTRAINTS
+             and len(free) + len(fixed) <= _lib.FC_SOLVE_MAX_PARAMS)
+    out = (solve_batch if small else solve_large_batch)(constraints, free, fixed, np.array([row], dtype=np.float32),
+                                                        max_iters, cancel)
+    if out is None:
+        return None
+    return {k: float(out[0][0, i]) for i, k in enumerate(free)}
 
 
 def pixel_inside(img: np.ndarray) -> np.ndarray:

@@ -65,7 +65,7 @@ int32_t fc_ctx_set_arena_bytes(fc_ctx* ctx, uint64_t bytes);
  * layout of Rust's AtomicBool (CancelToken::into_raw() as *const u8): nonzero = cancelled.  The library reads it with
  * an acquire load, from any thread; NULL detaches it.  Context-wide, like fc_ctx_set_stream, and consulted only by
  * fc_render2d, fc_render2d_frames, fc_render2d_scene, fc_render3d, fc_render3d_frames, fc_render3d_scene, fc_octree_sample,
- * fc_mesh_build, fc_mesh_build_frames, fc_contour_build, and
+ * fc_mesh_build, fc_mesh_build_frames, fc_contour_build, fc_solve_batch, fc_solve_large_batch, and
  * fc_ctx_synchronize after the most recent FC_FLAG_ASYNC call of those.  With a flag attached:
  *  - set on entry: the call returns FC_ERR_CANCELLED before it allocates or launches anything;
  *  - set while the call runs: the kernels stop claiming work and the call returns FC_ERR_CANCELLED ("cancelled" in
@@ -639,7 +639,10 @@ int32_t fc_contour_read(fc_ctx* ctx, float* vertices, uint32_t* offsets, uint8_t
  *  - the pseudo-inverse is a cyclic Jacobi eigen-solve in f32 with a fixed operation order (the reference calls
  *    nalgebra's SVD): results agree with the reference to rounding, and bit for bit with the project's CPU oracle.
  * Limits (FC_ERR_UNSUPPORTED beyond them): n_free <= 64, n_constraints <= 256, n_params <= 1024, constraint tapes
- * without memory slots.  n_free == 0 is FC_ERR_INVALID (the reference indexes an empty Jacobian).  Not cancellable. */
+ * without memory slots; fc_solve_large_batch takes larger problems.  n_free == 0 is FC_ERR_INVALID (the reference
+ * indexes an empty Jacobian).  Cancellable (fc_ctx_set_cancel): the solver stops claiming problems and stops each
+ * problem in flight at its next iteration; a cancelled call returns FC_ERR_CANCELLED and copies nothing back to host
+ * values / results, and a row in device memory is either untouched or fully solved. */
 #define FC_SOLVE_MAX_FREE 64
 #define FC_SOLVE_MAX_CONSTRAINTS 256
 #define FC_SOLVE_MAX_PARAMS 1024
@@ -662,6 +665,19 @@ typedef struct fc_solve_result { uint32_t status, iterations; float err; uint32_
 int32_t fc_solve_batch(fc_ctx* ctx, const fc_tape* const* constraints, uint32_t n_constraints,
                        const int32_t* const* slot_param, const fc_solve_cfg* cfg, float* values, uint64_t n_problems,
                        fc_solve_result* results);
+/* fc_solve_batch for larger problems: one problem per thread-block cluster of up to 16 CTAs, its matrices in a
+ * context-owned device workspace (about 28 MiB per problem in flight at the limits; the problems in flight are capped
+ * so that it stays within FC_FRAMES_PASS_BYTES, but a lone problem always gets its workspace).  Arguments, exits and
+ * cancellation as in fc_solve_batch; it accepts every problem fc_solve_batch accepts, and its result is bit for bit
+ * what fc_solve_batch gives there.  Limits (FC_ERR_UNSUPPORTED beyond them): n_free <= 1024, n_constraints <= 4096,
+ * n_params <= 16384, constraint tapes without memory slots.  FC_ERR_CUDA if the workspace cannot be allocated. */
+/* a cluster of up to 16 CTAs: 16 times fc_solve_batch's limits (1024, 4096, 16384) */
+#define FC_SOLVE_LARGE_MAX_FREE (16 * FC_SOLVE_MAX_FREE)
+#define FC_SOLVE_LARGE_MAX_CONSTRAINTS (16 * FC_SOLVE_MAX_CONSTRAINTS)
+#define FC_SOLVE_LARGE_MAX_PARAMS (16 * FC_SOLVE_MAX_PARAMS)
+int32_t fc_solve_large_batch(fc_ctx* ctx, const fc_tape* const* constraints, uint32_t n_constraints,
+                             const int32_t* const* slot_param, const fc_solve_cfg* cfg, float* values,
+                             uint64_t n_problems, fc_solve_result* results);
 
 /* ---- diagnostics ---------------------------------------------------------- */
 /* Host-only (no device needed): builds the level-0 schedule fc_tape_create would build for this

@@ -248,22 +248,27 @@ int32_t bulk_eval(fc_eval* e, const fc_tape* t, const void* const* vars, void* c
 int32_t transcode(const uint32_t* words, size_t n_words, uint8_t reg_count, uint32_t mem_count, uint32_t n_vars,
                   uint32_t n_outputs, std::vector<uint2>& out, uint32_t& n_choices);
 // octree_capi.cu
-// The uniform-tree samplers (octree_sample_device, contour_sample) over n_roots root cells, each with 2^dim children per
-// level down to depth D: their scratch (choice scratch, arena, counters with 64 zeroed bytes after them, stats, the
-// job lists, `cap` leaf tapes) and the LevelParams every level of both shares
+// The uniform-tree samplers (octree_enqueue, contour_sample) over n_roots root cells stacked along Y (one per frame or
+// slice), each with 2^dim children per level down to depth D: their scratch (choice scratch, arena, counters with 64
+// zeroed bytes after them, stats, the job lists, `cap` leaf tapes), the LevelParams every level of both shares, and the
+// size of each level's launch
 struct TreeScratch {
     uint32_t D = 0;
+    int dim = 0;
+    uint64_t n_roots = 0;
     int grid_blocks = 0;
     uint32_t choice_words = 0;
     uint64_t level_cap[MAX_LEVELS + 1] = {};   // level l's job list: the cells at depth min(l, D), capped
-    // blocks of a level launch of `warps` warps, within the grid
-    int blocks(uint64_t warps) const {
+    // blocks of level l's launch, within the grid: a warp per parent cell, or per 32 root cells at level 0
+    int blocks(int l) const {
+        const uint64_t warps = l ? std::max<uint64_t>(1, (n_roots << (dim * l)) >> dim) : (n_roots + 31) / 32;
         return std::max(int(std::min<uint64_t>((warps + WARPS_PER_BLOCK - 1) / WARPS_PER_BLOCK, uint64_t(grid_blocks))), 1);
     }
 };
 int32_t tree_scratch(fc_ctx* c, const fc_tape* tape, uint32_t D, int dim, uint64_t n_roots, uint64_t cap, TreeScratch& t);
-LevelParams tree_level(fc_ctx* c, const fc_tape* tape, const TreeScratch& t, int l, uint32_t has_transform,
-                       const VarBind& vb, const CallCancel& cc);
+// level l's launch parameters, with the matrix, transform flag and vars of the first frame or slice, f0
+LevelParams tree_level(fc_ctx* c, const fc_tape* tape, const TreeScratch& t, int l, const ContourSlice& f0,
+                       const CallCancel& cc);
 int32_t octree_enqueue(fc_ctx* c, const fc_tape* tape, uint32_t D, const MeshFrame* fr, uint32_t n, const MeshFrame* d_fr,
                        OctreeLeaf* dout, uint64_t cap, bool stats, cudaEvent_t t0, const CallCancel& cc, uint32_t* launches);
 // contour.cu

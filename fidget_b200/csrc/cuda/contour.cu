@@ -1,11 +1,11 @@
 // 2D contours (fc_contour_build): dual contouring on a uniform quadtree of the [-1,1]^2 world square, linked into
 // polylines on the device.  The pipeline restricts the mesher's to two dimensions:
 //
-//   descent    k_contour_level: the interval levels of the octree sampler with Z fixed (level_job's TREE mode), one
-//              launch per depth, four children per cell;
-//   leaves     k_contour_leaf: one warp per leaf, four corners, then the 16-ary edge search of k_octree_leaf -- four
-//              edges x 16 probes, two points per lane, in one pass; k_contour_grads: (dx, dy, v) at the intersections,
-//              one lane per edge, with the tape the leaf was sampled with;
+//   descent    k_tree_level<2, *> (octree.cu): the octree sampler's interval levels with Z fixed (level_job's TREE
+//              mode), one launch per depth, four children per cell;
+//   leaves     k_contour_leaf: one warp per leaf, four corners, then the samplers' 16-ary edge search (edge_search) --
+//              four edges x 16 probes, two points per lane, in one pass; k_contour_grads: (dx, dy, v) at the
+//              intersections (grad_at), one lane per edge, with the tape the leaf was sampled with;
 //   order      the surface leaves sorted by key (iy, ix): vertex ids come from a scan of the group counts in that
 //              order, so vertex id order is key order (iy, ix, group) and the sorted key list is the cell lookup;
 //   vertices   k_contour_vertices: one per connected group of inside corners, by the 2D QEF (qef2_vertex);
@@ -63,31 +63,6 @@ struct ContourLeafParams {
     uint32_t rows;
 };
 
-// The quadtree levels: k_interval_level's claim loop around level_job's TREE mode (one root cell; STACK: one per slice,
-// roots_y slices, 32 to a warp at level 0)
-template <bool STACK>
-__global__ void __launch_bounds__(WARPS_PER_BLOCK * 32) k_contour_level(const __grid_constant__ LevelParams p,
-                                                                        const ContourSlice* slices) {
-    __shared__ uint32_t live_s[WARPS_PER_BLOCK][8][32];
-    const int lane = threadIdx.x & 31;
-    const int wib = threadIdx.x >> 5;
-    const uint32_t gw = blockIdx.x * WARPS_PER_BLOCK + wib;
-    uint32_t* cs = p.choice_scratch + size_t(gw) * p.choice_words * 32u + lane;
-    itv slots[REG_SLOTS];
-    const uint32_t n_roots = STACK ? p.roots_y : 1u;
-    const uint32_t n_jobs = p.root_mode ? (n_roots + 31u) / 32u : min(p.ctr->n_jobs[p.level], p.cap_in);
-    for (;;) {
-        uint32_t j = 0;
-        if (lane == 0) {
-            j = atomicAdd(&p.ctr->cursor[p.level], 1u);
-            if (j < n_jobs && cancel_poll(p.cancel, CS_LEVEL0 + p.level, j)) j = ~0u;
-        }
-        j = __shfl_sync(FULL, j, 0);
-        if (j >= n_jobs) break;
-        level_job<2, false, STACK, false, true>(p, j, n_roots, slots, cs, live_s[wib], lane, p.epoch, slices);
-    }
-}
-
 __device__ __forceinline__ bool edge_setup2(uint32_t e, uint32_t mask, EdgeState& st) {
     const uint32_t t = e >> 1, u = 1u - t, sv = e & 1u;
     const uint32_t c0 = sv << u, c1 = c0 | (1u << t);
@@ -103,8 +78,8 @@ __device__ __forceinline__ bool edge_setup2(uint32_t e, uint32_t mask, EdgeState
     return true;
 }
 
-// One warp per leaf job: corner mask, then the four edges' searches in one pass (lanes 0-15 follow edges 0 and 2, lanes
-// 16-31 edges 1 and 3, one probe each), with k_octree_leaf's rounds, fractions and bracket midpoint
+// One warp per leaf job: corner mask, then the four edges' searches in one pass of edge_search (lanes 0-15 follow edges
+// 0 and 2, lanes 16-31 edges 1 and 3, one probe each)
 template <bool STACK>
 __global__ void __launch_bounds__(128) k_contour_leaf(const __grid_constant__ ContourLeafParams p) {
     const int lane = threadIdx.x & 31;
@@ -146,7 +121,7 @@ __global__ void __launch_bounds__(128) k_contour_leaf(const __grid_constant__ Co
         slot = __shfl_sync(FULL, slot, 0);
         if (slot >= p.cap_out) continue;   // counted: the host retries with the exact count
         ContourLeaf* L = p.out + slot;
-        const int half = lane >> 4, jj = lane & 15;
+        const int half = lane >> 4;
         EdgeState s0, s1;
         const bool v0 = edge_setup2(uint32_t(half), mask, s0), v1 = edge_setup2(uint32_t(half) + 2u, mask, s1);
         uint32_t present = 0;
@@ -159,39 +134,11 @@ __global__ void __launch_bounds__(128) k_contour_leaf(const __grid_constant__ Co
             L->ix = uint16_t(cx); L->iy = uint16_t(cy);
             L->mask = uint8_t(mask); L->present = uint8_t(present); L->slice = uint16_t(s);
         }
-        for (int round = 0; round < 4; ++round) {
-            uint32_t q0[2], q1[2];
-#pragma unroll
-            for (int a = 0; a < 2; ++a) {
-                q0[a] = (s0.s[a] * uint32_t(15 - jj) + s0.e[a] * uint32_t(jj)) / 15u;
-                q1[a] = (s1.s[a] * uint32_t(15 - jj) + s1.e[a] * uint32_t(jj)) / 15u;
-            }
-            const float2 v = eval2(lerp_u16(lo[0], hi[0], q0[0]), lerp_u16(lo[1], hi[1], q0[1]),
-                                   lerp_u16(lo[0], hi[0], q1[0]), lerp_u16(lo[1], hi[1], q1[1]));
-            const uint32_t b0 = (__ballot_sync(FULL, v.x >= 0.0f) >> (16 * half)) & 0xffffu;
-            const uint32_t b1 = (__ballot_sync(FULL, v.y >= 0.0f) >> (16 * half)) & 0xffffu;
-            auto narrow = [&](EdgeState& st, uint32_t bits) {
-                uint32_t frac = bits ? uint32_t(__ffs(bits) - 1) : 15u;
-                if (frac == 0u) frac = 1u;
-#pragma unroll
-                for (int a = 0; a < 2; ++a) {
-                    const uint32_t na = (st.s[a] * (16u - frac) + st.e[a] * (frac - 1u)) / 15u;
-                    const uint32_t nb = (st.s[a] * (15u - frac) + st.e[a] * frac) / 15u;
-                    st.s[a] = na & 0xffffu;
-                    st.e[a] = nb & 0xffffu;
-                }
-            };
-            narrow(s0, b0);
-            narrow(s1, b1);
-        }
-        if (jj == 0) {
-            if (v0) for (int a = 0; a < 2; ++a) L->pos[half][a] = lerp_u16(lo[a], hi[a], ((s0.s[a] + s0.e[a]) / 2u) & 0xffffu);
-            if (v1) for (int a = 0; a < 2; ++a) L->pos[half + 2][a] = lerp_u16(lo[a], hi[a], ((s1.s[a] + s1.e[a]) / 2u) & 0xffffu);
-        }
+        edge_search<2>(s0, s1, lo, hi, eval2, L->pos, v0, uint32_t(half), v1, uint32_t(half) + 2u);
     }
 }
 
-// Gradients at the intersections (as k_octree_grads, Z seeded at the slice): one warp per leaf, one lane per edge
+// Gradients at the intersections (grad_at, Z at the slice's): one warp per leaf, one lane per edge
 template <bool STACK>
 __global__ void __launch_bounds__(128) k_contour_grads(const __grid_constant__ ContourLeafParams p) {
     grd slots[REG_SLOTS];
@@ -207,12 +154,8 @@ __global__ void __launch_bounds__(128) k_contour_grads(const __grid_constant__ C
         const bool mine = lane < 4 && ((active >> lane) & 1u);
         const int e = mine ? lane : (__ffs(active) - 1);
         const ContourSlice* sl = STACK ? p.slices + L->slice : nullptr;   // (STACK: the leaf's slice)
-        grd gx = gr(L->pos[e][0], 1.0f, 0.0f, 0.0f), gy = gr(L->pos[e][1], 0.0f, 1.0f, 0.0f),
-            gz = gr(STACK ? sl->z : p.z, 0.0f, 0.0f, 1.0f);
-        if (STACK ? sl->has_transform : p.has_transform) xform_gr(STACK ? sl->mat : p.mat, gx, gy, gz, gx, gy, gz);
-        const grd r = run_grad(tr.ptr, tr.n_ops, slots, [&](uint32_t k) {
-            return pick_input(STACK ? sl->vb : p.vb, k, gx, gy, gz, [](float f) { return gr1(f); });
-        });
+        const grd r = grad_at(tr, slots, L->pos[e][0], L->pos[e][1], STACK ? sl->z : p.z,
+                              STACK ? sl->has_transform : p.has_transform, STACK ? sl->mat : p.mat, STACK ? sl->vb : p.vb);
         if (mine) { L->grad[e][0] = r.y; L->grad[e][1] = r.z; L->grad[e][2] = r.x; }
     }
 }
@@ -543,17 +486,9 @@ static int32_t contour_sample(fc_ctx* c, const fc_tape* tape, uint32_t D, const 
     if (int32_t trc = tree_scratch(c, tape, D, 2, n, cap, t)) return trc;
     uint32_t* d_n_out = reinterpret_cast<uint32_t*>(c->counters.as<char>() + sizeof(Counters));
     for (int l = 0; l < L; ++l) {
-        LevelParams p = tree_level(c, tape, t, l, sl[0].has_transform, sl[0].vb, cc);
-        p.roots_x = p.roots_z = 1;
-        p.roots_y = n;   // one root cell per slice, stacked along Y
-        p.width = p.height = 1u << D;
-        p.depth = 1;
+        LevelParams p = tree_level(c, tape, t, l, sl[0], cc);
         p.z2d = sl[0].z;
-        p.mat = sl[0].mat;
-        p.frame_rows = 1u << D;
-        const int blocks = t.blocks(l ? std::max<uint64_t>(1, (uint64_t(n) << (2 * l)) / 4) : (n + 31) / 32);
-        if (stack) k_contour_level<true><<<blocks, WARPS_PER_BLOCK * 32, 0, s>>>(p, d_sl);
-        else k_contour_level<false><<<blocks, WARPS_PER_BLOCK * 32, 0, s>>>(p, nullptr);
+        launch_tree_level(p, 2, stack ? d_sl : nullptr, t.blocks(l), s);
     }
     ContourLeafParams q{};
     q.jobs = c->jobs[L].as<TileJob>();

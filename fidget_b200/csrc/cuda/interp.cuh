@@ -28,6 +28,52 @@ __device__ __forceinline__ float lerp_u16(float lo, float hi, uint32_t p) {
 
 struct EdgeState { uint32_t s[3], e[3]; };
 
+// The 16-ary edge search (OctreeBuilder::leaf) on the first AXES axes of two edges per lane, in a cell with bounds lo /
+// hi: each half-warp follows its own pair of edges (s0, s1), and lane jj of it probes fraction jj / 15 of both brackets
+// through eval2 (x0, y0[, z0], x1, y1[, z1]) -> (v0, v1).  Each of four rounds narrows a bracket to the step that ends
+// at its first probe at or outside the surface.  The half-warp's lane 0 then writes the bracket midpoint of each valid
+// edge (v0, v1) to its intersection, pos[e0] / pos[e1].
+template <int AXES, class Eval2>
+__device__ __forceinline__ void edge_search(EdgeState& s0, EdgeState& s1, const float* lo, const float* hi,
+                                            const Eval2& eval2, float (*pos)[AXES], bool v0, uint32_t e0, bool v1,
+                                            uint32_t e1) {
+    const int lane = threadIdx.x & 31, half = lane >> 4, jj = lane & 15;
+    for (int round = 0; round < 4; ++round) {
+        uint32_t q0[AXES], q1[AXES];
+#pragma unroll
+        for (int a = 0; a < AXES; ++a) {
+            q0[a] = (s0.s[a] * uint32_t(15 - jj) + s0.e[a] * uint32_t(jj)) / 15u;
+            q1[a] = (s1.s[a] * uint32_t(15 - jj) + s1.e[a] * uint32_t(jj)) / 15u;
+        }
+        float2 v;
+        if constexpr (AXES == 3)
+            v = eval2(lerp_u16(lo[0], hi[0], q0[0]), lerp_u16(lo[1], hi[1], q0[1]), lerp_u16(lo[2], hi[2], q0[2]),
+                      lerp_u16(lo[0], hi[0], q1[0]), lerp_u16(lo[1], hi[1], q1[1]), lerp_u16(lo[2], hi[2], q1[2]));
+        else
+            v = eval2(lerp_u16(lo[0], hi[0], q0[0]), lerp_u16(lo[1], hi[1], q0[1]),
+                      lerp_u16(lo[0], hi[0], q1[0]), lerp_u16(lo[1], hi[1], q1[1]));
+        const uint32_t b0 = (__ballot_sync(FULL, v.x >= 0.0f) >> (16 * half)) & 0xffffu;
+        const uint32_t b1 = (__ballot_sync(FULL, v.y >= 0.0f) >> (16 * half)) & 0xffffu;
+        auto narrow = [&](EdgeState& st, uint32_t bits) {
+            uint32_t frac = bits ? uint32_t(__ffs(bits) - 1) : 15u;
+            if (frac == 0u) frac = 1u;
+#pragma unroll
+            for (int a = 0; a < AXES; ++a) {
+                const uint32_t na = (st.s[a] * (16u - frac) + st.e[a] * (frac - 1u)) / 15u;
+                const uint32_t nb = (st.s[a] * (15u - frac) + st.e[a] * frac) / 15u;
+                st.s[a] = na & 0xffffu;
+                st.e[a] = nb & 0xffffu;
+            }
+        };
+        narrow(s0, b0);
+        narrow(s1, b1);
+    }
+    if (jj == 0) {
+        if (v0) for (int a = 0; a < AXES; ++a) pos[e0][a] = lerp_u16(lo[a], hi[a], ((s0.s[a] + s0.e[a]) / 2u) & 0xffffu);
+        if (v1) for (int a = 0; a < AXES; ++a) pos[e1][a] = lerp_u16(lo[a], hi[a], ((s1.s[a] + s1.e[a]) / 2u) & 0xffffu);
+    }
+}
+
 // INPUT clause -> value: the axes get coordinates, other slots their bound value
 template <class T, class F>
 __device__ __forceinline__ T pick_input(const VarBind& vb, uint32_t i, T X, T Y, T Z, F from_float) {
@@ -535,6 +581,17 @@ __device__ __forceinline__ grd run_grad(const uint2* __restrict__ tape, uint32_t
         slots[(x >> 8) & 0xffu] = r;
     }
     return result;
+}
+
+// The samplers' gradient probe (octree.rs:780-808): (v, dv/dx, dv/dy, dv/dz) of a tape at the world point (x, y, z),
+// seen through `mat` when has_transform
+__device__ __forceinline__ grd grad_at(const TapeRef& tr, grd* slots, float x, float y, float z, uint32_t has_transform,
+                                       const Mat4& mat, const VarBind& vb) {
+    grd gx = gr(x, 1.0f, 0.0f, 0.0f), gy = gr(y, 0.0f, 1.0f, 0.0f), gz = gr(z, 0.0f, 0.0f, 1.0f);
+    if (has_transform) xform_gr(mat, gx, gy, gz, gx, gy, gz);
+    return run_grad(tr.ptr, tr.n_ops, slots, [&](uint32_t k) {
+        return pick_input(vb, k, gx, gy, gz, [](float f) { return gr1(f); });
+    });
 }
 
 }  // namespace fdev

@@ -485,8 +485,10 @@ void launch_octree_leaf(const OctreeLeafParams& p, int blocks, cudaStream_t s, c
                         uint32_t rows = 0);
 void launch_octree_grads(const OctreeLeafParams& p, int blocks, cudaStream_t s, const MeshFrame* frames = nullptr,
                          uint32_t rows = 0);
-// the interval levels of a mesh frame batch's stacked octree (one root cell per frame, p.roots_y frames)
-void launch_octree_level_frames(const LevelParams& p, const MeshFrame* frames, int blocks, cudaStream_t s);
+// the interval levels of the samplers' trees (octree.cu, k_tree_level): dim 3, a mesh frame batch's stacked octree (one
+// root cell per frame, p.roots_y frames); dim 2, a contour's quadtree (frames == null: one root cell, the slice in the
+// launch parameters; else a slice stack's table, one root cell per slice)
+void launch_tree_level(const LevelParams& p, int dim, const ContourSlice* frames, int blocks, cudaStream_t s);
 void launch_interval_level_3d(const LevelParams& p, int blocks, cudaStream_t s);
 void launch_voxels_3d(const VoxelParams& p, int blocks, cudaStream_t s);
 // Counting sort of the leaf jobs by descending Z layer: hist/offsets are device scratch of n_layers+1 words

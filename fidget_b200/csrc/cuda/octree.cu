@@ -1,4 +1,5 @@
-// Octree sampler leaves of fidget-mesh's Manifold Dual Contouring (sampling half).
+// Octree sampler leaves of fidget-mesh's Manifold Dual Contouring (sampling half), and the level kernel of the octree
+// and quadtree samplers' trees.
 #include "level_job.cuh"
 
 // ---------------------------------------------------------------------------
@@ -88,7 +89,7 @@ __global__ void __launch_bounds__(128) k_octree_leaf(const __grid_constant__ Oct
             L->mask = uint8_t(mask); L->n_edges = uint8_t(ne);
             L->present = uint16_t(active); L->pad = uint16_t(f);
         }
-        const int half = lane >> 4, jj = lane & 15;
+        const int half = lane >> 4;
         for (uint32_t pass = 0; pass * 4u < ne; ++pass) {
             // this lane follows edges k0 (component x) and k1 (component y) of the pass
             const uint32_t k0 = pass * 4u + uint32_t(half), k1 = k0 + 2u;
@@ -102,35 +103,7 @@ __global__ void __launch_bounds__(128) k_octree_leaf(const __grid_constant__ Oct
             EdgeState s0, s1;
             edge_setup(e0, mask, s0);
             edge_setup(e1, mask, s1);
-            for (int round = 0; round < 4; ++round) {
-                uint32_t q0[3], q1[3];
-#pragma unroll
-                for (int a = 0; a < 3; ++a) {
-                    q0[a] = (s0.s[a] * uint32_t(15 - jj) + s0.e[a] * uint32_t(jj)) / 15u;
-                    q1[a] = (s1.s[a] * uint32_t(15 - jj) + s1.e[a] * uint32_t(jj)) / 15u;
-                }
-                const float2 v = eval2(lerp_u16(lo[0], hi[0], q0[0]), lerp_u16(lo[1], hi[1], q0[1]), lerp_u16(lo[2], hi[2], q0[2]),
-                                       lerp_u16(lo[0], hi[0], q1[0]), lerp_u16(lo[1], hi[1], q1[1]), lerp_u16(lo[2], hi[2], q1[2]));
-                const uint32_t b0 = (__ballot_sync(FULL, v.x >= 0.0f) >> (16 * half)) & 0xffffu;
-                const uint32_t b1 = (__ballot_sync(FULL, v.y >= 0.0f) >> (16 * half)) & 0xffffu;
-                auto narrow = [&](EdgeState& st, uint32_t bits) {
-                    uint32_t frac = bits ? uint32_t(__ffs(bits) - 1) : 15u;
-                    if (frac == 0u) frac = 1u;
-#pragma unroll
-                    for (int a = 0; a < 3; ++a) {
-                        const uint32_t na = (st.s[a] * (16u - frac) + st.e[a] * (frac - 1u)) / 15u;
-                        const uint32_t nb = (st.s[a] * (15u - frac) + st.e[a] * frac) / 15u;
-                        st.s[a] = na & 0xffffu;
-                        st.e[a] = nb & 0xffffu;
-                    }
-                };
-                narrow(s0, b0);
-                narrow(s1, b1);
-            }
-            if (jj == 0) {
-                if (v0) for (int a = 0; a < 3; ++a) L->pos[e0][a] = lerp_u16(lo[a], hi[a], ((s0.s[a] + s0.e[a]) / 2u) & 0xffffu);
-                if (v1) for (int a = 0; a < 3; ++a) L->pos[e1][a] = lerp_u16(lo[a], hi[a], ((s1.s[a] + s1.e[a]) / 2u) & 0xffffu);
-            }
+            edge_search<3>(s0, s1, lo, hi, eval2, L->pos, v0, e0, v1, e1);
         }
     }
     if (p.stats) {
@@ -165,12 +138,8 @@ __global__ void __launch_bounds__(128) k_octree_grads(const __grid_constant__ Oc
         const bool mine = lane < 12 && ((active >> lane) & 1u);
         const int e = mine ? lane : (__ffs(active) - 1);
         const MeshFrame* fr = STACK ? frames + L->pad : nullptr;   // (STACK: the leaf's frame)
-        grd gx = gr(L->pos[e][0], 1.0f, 0.0f, 0.0f), gy = gr(L->pos[e][1], 0.0f, 1.0f, 0.0f),
-            gz = gr(L->pos[e][2], 0.0f, 0.0f, 1.0f);
-        if (STACK ? fr->has_transform : p.has_transform) xform_gr(STACK ? fr->mat : p.mat, gx, gy, gz, gx, gy, gz);
-        const grd r = run_grad(tr.ptr, tr.n_ops, slots, [&](uint32_t k) {
-            return pick_input(STACK ? fr->vb : p.vb, k, gx, gy, gz, [](float f) { return gr1(f); });
-        });
+        const grd r = grad_at(tr, slots, L->pos[e][0], L->pos[e][1], L->pos[e][2],
+                              STACK ? fr->has_transform : p.has_transform, STACK ? fr->mat : p.mat, STACK ? fr->vb : p.vb);
         if (mine) {
             L->grad[e][0] = r.y; L->grad[e][1] = r.z; L->grad[e][2] = r.w; L->grad[e][3] = r.x;
             ++n_pts;
@@ -186,17 +155,19 @@ void launch_octree_grads(const OctreeLeafParams& p, int blocks, cudaStream_t s, 
     else k_octree_grads<false><<<blocks, 128, 0, s>>>(p, nullptr);
 }
 
-// The levels of a mesh frame batch's stacked octree: k_interval_level's claim loop around level_job's octree mode with
-// the frame table (one root cell per frame, 32 to a warp at level 0)
-__global__ void __launch_bounds__(WARPS_PER_BLOCK * 32) k_octree_level(const __grid_constant__ LevelParams p,
-                                                                       const MeshFrame* frames) {
+// The levels of the samplers' trees: k_interval_level's claim loop around level_job's TREE mode.  DIM 3: a mesh frame
+// batch's stacked octree, one root cell per frame; DIM 2: the quadtree of a contour, one root cell, or with STACK one per
+// slice of a stack.  `frames` is the frame or slice table (STACK); root cells go 32 to a warp at level 0.
+template <int DIM, bool STACK>
+__global__ void __launch_bounds__(WARPS_PER_BLOCK * 32) k_tree_level(const __grid_constant__ LevelParams p,
+                                                                     const ContourSlice* frames) {
     __shared__ uint32_t live_s[WARPS_PER_BLOCK][8][32];
     const int lane = threadIdx.x & 31;
     const int wib = threadIdx.x >> 5;
     const uint32_t gw = blockIdx.x * WARPS_PER_BLOCK + wib;
     uint32_t* cs = p.choice_scratch + size_t(gw) * p.choice_words * 32u + lane;
     itv slots[REG_SLOTS];
-    const uint32_t n_roots = p.roots_y;
+    const uint32_t n_roots = STACK ? p.roots_y : 1u;
     const uint32_t n_jobs = p.root_mode ? (n_roots + 31u) / 32u : min(p.ctr->n_jobs[p.level], p.cap_in);
     for (;;) {
         uint32_t j = 0;
@@ -206,11 +177,13 @@ __global__ void __launch_bounds__(WARPS_PER_BLOCK * 32) k_octree_level(const __g
         }
         j = __shfl_sync(FULL, j, 0);
         if (j >= n_jobs) break;
-        level_job<3, false, true, false, true>(p, j, n_roots, slots, cs, live_s[wib], lane, p.epoch, frames);
+        level_job<DIM, false, STACK, false, true>(p, j, n_roots, slots, cs, live_s[wib], lane, p.epoch, frames);
     }
 }
-void launch_octree_level_frames(const LevelParams& p, const MeshFrame* frames, int blocks, cudaStream_t s) {
-    k_octree_level<<<blocks, WARPS_PER_BLOCK * 32, 0, s>>>(p, frames);
+void launch_tree_level(const LevelParams& p, int dim, const ContourSlice* frames, int blocks, cudaStream_t s) {
+    if (dim == 3) k_tree_level<3, true><<<blocks, WARPS_PER_BLOCK * 32, 0, s>>>(p, frames);
+    else if (frames) k_tree_level<2, true><<<blocks, WARPS_PER_BLOCK * 32, 0, s>>>(p, frames);
+    else k_tree_level<2, false><<<blocks, WARPS_PER_BLOCK * 32, 0, s>>>(p, nullptr);
 }
 
 }  // namespace fdev

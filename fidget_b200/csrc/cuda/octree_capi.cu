@@ -3,6 +3,8 @@
 
 int32_t tree_scratch(fc_ctx* c, const fc_tape* tape, uint32_t D, int dim, uint64_t n_roots, uint64_t cap, TreeScratch& t) {
     t.D = D;
+    t.dim = dim;
+    t.n_roots = n_roots;
     t.grid_blocks = c->sm_count * env_int("FIDGET_B200_BLOCKS_PER_SM", 6);
     t.choice_words = choice_words(tape);
     CU(c->choice_scratch.ensure(size_t(t.grid_blocks) * WARPS_PER_BLOCK * t.choice_words * 32 * 4));
@@ -19,8 +21,8 @@ int32_t tree_scratch(fc_ctx* c, const fc_tape* tape, uint32_t D, int dim, uint64
     return FC_OK;
 }
 
-LevelParams tree_level(fc_ctx* c, const fc_tape* tape, const TreeScratch& t, int l, uint32_t has_transform,
-                       const VarBind& vb, const CallCancel& cc) {
+LevelParams tree_level(fc_ctx* c, const fc_tape* tape, const TreeScratch& t, int l, const ContourSlice& f0,
+                       const CallCancel& cc) {
     LevelParams p{};
     p.level = l;
     p.tile = 1u << (t.D - uint32_t(l));
@@ -38,10 +40,18 @@ LevelParams tree_level(fc_ctx* c, const fc_tape* tape, const TreeScratch& t, int
     p.choice_words = t.choice_words;
     p.ctr = c->counters.as<Counters>();
     p.mode = 1;
-    p.has_transform = has_transform;
+    p.has_transform = f0.has_transform;
     p.cell_h = 2.0f / float(1u << t.D);
-    p.vb = vb;
+    p.vb = f0.vb;
     p.cancel = cc.ref;
+    p.roots_x = p.roots_z = 1;
+    p.roots_y = uint32_t(t.n_roots);   // one root cell per frame or slice, stacked along Y
+    p.frame_rows = 1u << t.D;
+    p.mat = f0.mat;
+    // the extents: the octree's stacked grid (2^D x n 2^D x 2^D cells), one slice of the quadtree (2^D x 2^D x 1)
+    p.width = 1u << t.D;
+    p.height = t.dim == 3 ? uint32_t(t.n_roots) << t.D : 1u << t.D;
+    p.depth = t.dim == 3 ? 1u << t.D : 1u;
     return p;
 }
 
@@ -63,17 +73,10 @@ int32_t octree_enqueue(fc_ctx* c, const fc_tape* tape, uint32_t D, const MeshFra
     unsigned long long* d_leaf_stats = reinterpret_cast<unsigned long long*>(c->counters.as<char>() + sizeof(Counters) + 8);
     if (t0) CU(cudaEventRecord(t0, s));
     for (int l = 0; l < L; ++l) {
-        LevelParams p = tree_level(c, tape, t, l, fr[0].has_transform, fr[0].vb, cc);
-        p.roots_x = p.roots_z = 1;
-        p.roots_y = n;   // one root cell per frame, stacked along Y
-        p.width = p.depth = 1u << D;
-        p.height = n << D;
-        p.mat = fr[0].mat;
-        p.frame_rows = 1u << D;
+        LevelParams p = tree_level(c, tape, t, l, fr[0], cc);
         p.stats = stats ? c->stats.as<Stats>() : nullptr;
-        const uint64_t cells = uint64_t(n) << (3 * l);
-        if (stack) launch_octree_level_frames(p, d_fr, t.blocks(l ? std::max<uint64_t>(1, cells / 8) : (n + 31) / 32), s);
-        else launch_interval_level_3d(p, t.blocks(l ? std::max<uint64_t>(1, cells / 8) : 1), s);
+        if (stack) launch_tree_level(p, 3, d_fr, t.blocks(l), s);
+        else launch_interval_level_3d(p, t.blocks(l), s);
     }
     OctreeLeafParams q{};
     q.jobs = c->jobs[L].as<TileJob>();

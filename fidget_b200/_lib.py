@@ -130,6 +130,14 @@ class FcMeshFrameInfo(C.Structure):
     _fields_ = [(n, C.c_uint64) for n in ("n_leaves", "n_vertices", "n_triangles", "open_edges", "n_cells")]
 
 
+class FcMeasureResult(C.Structure):
+    _fields_ = [(n, C.c_uint64) for n in ("n_inside", "n_proven", "n_undecided")] + \
+               [("s1", C.c_uint64 * 3), ("s2", C.c_uint64 * 6), ("lo", C.c_uint32 * 3), ("hi", C.c_uint32 * 3)] + \
+               [(n, C.c_double) for n in ("volume", "volume_lo", "volume_hi")] + \
+               [("centroid", C.c_double * 3), ("inertia", C.c_double * 6), ("bbox_min", C.c_double * 3),
+                ("bbox_max", C.c_double * 3)]
+
+
 class FcContourCfg(C.Structure):
     _fields_ = [("depth", C.c_uint32), ("has_transform", C.c_uint32), ("world_to_model", C.c_float * 9), ("z", C.c_float),
                 ("flags", C.c_uint32), ("n_var_values", C.c_uint32), ("var_values", C.c_float * 16)]
@@ -245,6 +253,7 @@ CUDA_API = {
     "fc_mesh_write_stl": (_i32, [_vp, _vp, C.c_size_t, _P(C.c_size_t)]),
     "fc_mesh_build_frames": (_i32, [_vp, _vp, _P(FcOctreeCfg), _P(FcMeshFrame), _u32, _P(FcMeshInfo),
                                     _P(FcMeshFrameInfo)]),
+    "fc_measure": (_i32, [_vp, _vp, _P(FcOctreeCfg), _P(FcMeshFrame), _u32, _vp, _P(C.c_float)]),
     "fc_contour_build": (_i32, [_vp, _vp, _P(FcContourCfg), _P(FcContourInfo)]),
     "fc_contour_read": (_i32, [_vp, _vp, _vp, _vp]),
     "fc_contour_build_slices": (_i32, [_vp, _vp, _P(FcContourCfg), _P(FcContourSlice), _u32, _P(FcContourInfo),

@@ -236,9 +236,11 @@ static int32_t cancel_site_of(const std::string& name) {
     for (int i = 0; i < CS_SOLVE - CS_CONTOUR_LEAF; ++i)
         if (name == contour[i]) return CS_CONTOUR_LEAF + i;
     static const char* const solve[] = {"k_solve", "k_solve_large"};
-    static_assert(sizeof(solve) / sizeof(solve[0]) == CS_COUNT - CS_SOLVE, "one name per poll site");
-    for (int i = 0; i < CS_COUNT - CS_SOLVE; ++i)
+    static_assert(sizeof(solve) / sizeof(solve[0]) == CS_MEASURE_BRICK - CS_SOLVE, "one name per poll site");
+    for (int i = 0; i < CS_MEASURE_BRICK - CS_SOLVE; ++i)
         if (name == solve[i]) return CS_SOLVE + i;
+    static_assert(CS_MEASURE_BRICK + 1 == CS_COUNT, "one name per poll site");
+    if (name == "k_measure_brick") return CS_MEASURE_BRICK;
     return -1;
 }
 

@@ -27,6 +27,7 @@ enum CancelSite : int32_t {
     CS_SCENE2D_RESOLVE,                                   // (after CS_WAIT: the ids the kernels above compare stay put)
     CS_CONTOUR_LEAF, CS_CONTOUR_GRADS, CS_CONTOUR_VERTICES, CS_CONTOUR_SEGMENTS, CS_CONTOUR_LINK, CS_CONTOUR_EMIT,
     CS_SOLVE, CS_SOLVE_LARGE,                             // the solvers: item = problem index (claim and every iteration)
+    CS_MEASURE_BRICK,                                     // fc_measure's brick kernel: item = brick
     CS_COUNT
 };
 struct CancelRef {
@@ -259,6 +260,30 @@ struct LevelParams {
     uint32_t n_scene_pl;
     uint32_t clamp_at;
     uint32_t fused_tail;           // the fused 2D tail consumes this level's jobs: count them in Counters::outstanding
+    // fc_measure (k_tree_level with MEASURE): one accumulator per frame of the pass, which the frame's proven-inside
+    // cells are folded into
+    struct MeasureAcc* measure;
+};
+
+// fc_measure's exact per-frame sums (fc_measure_result's integer fields, in its order).  Over the inside cells (i, j, k)
+// at depth D, with u = 2i + 1, v = 2j + 1, w = 2k + 1: the counts, s1 = (Σu, Σv, Σw), s2 = (Σuu, Σvv, Σww, Σuv, Σuw,
+// Σvw) and the inclusive cell-index box (lo starts at 0xffffffff, hi at 0).  Every word only ever grows by atomic adds,
+// minima and maxima of integers, so the result does not depend on the order of the work.
+struct MeasureAcc {
+    unsigned long long n_inside, n_proven, n_undecided;
+    unsigned long long s1[3], s2[6];
+    uint32_t lo[3], hi[3];
+};
+// The brick kernel (measure.cu): every ambiguous cell of edge `brick` in list `list`, its brick^3 cell centres evaluated
+// with the cell's simplified tape; frame f owns the cell rows [f * rows, (f + 1) * rows) and accumulator acc[f]
+struct MeasureBrickParams {
+    const TileJob* jobs;
+    uint32_t cap_jobs;
+    Counters* ctr;
+    int list, cursor;
+    uint32_t depth, brick, rows;
+    MeasureAcc* acc;
+    CancelRef cancel;
 };
 
 #ifdef __CUDACC__
@@ -489,6 +514,9 @@ void launch_octree_grads(const OctreeLeafParams& p, int blocks, cudaStream_t s, 
 // root cell per frame, p.roots_y frames); dim 2, a contour's quadtree (frames == null: one root cell, the slice in the
 // launch parameters; else a slice stack's table, one root cell per slice)
 void launch_tree_level(const LevelParams& p, int dim, const ContourSlice* frames, int blocks, cudaStream_t s);
+// fc_measure's levels: the stacked octree of dim 3 with its proven-inside cells folded into p.measure
+void launch_tree_level_measure(const LevelParams& p, const MeshFrame* frames, int blocks, cudaStream_t s);
+void launch_measure_bricks(const MeasureBrickParams& p, const MeshFrame* frames, int blocks, cudaStream_t s);
 void launch_interval_level_3d(const LevelParams& p, int blocks, cudaStream_t s);
 void launch_voxels_3d(const VoxelParams& p, int blocks, cudaStream_t s);
 // Counting sort of the leaf jobs by descending Z layer: hist/offsets are device scratch of n_layers+1 words

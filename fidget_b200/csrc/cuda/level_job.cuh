@@ -42,14 +42,82 @@ __device__ __forceinline__ void store_fill(FillRec* dst, const FillRec& fr) {
     *reinterpret_cast<uint4*>(dst) = make_uint4(fr.x, fr.y, fr.value, fr.ready);
 }
 
+// fc_measure's sums of one lane (MeasureAcc's fields but the brick count), folded over a warp and into a frame's
+// accumulator.  A cell of edge T at (x0, y0, z0) (depth-D cell indices) holds T^3 cells; along one axis its odd numbers
+// 2i + 1 sum to (x0 + T)^2 - x0^2 and their squares to F(x0 + T) - F(x0), F(m) = m (4 m^2 - 1) / 3.  Every term fits
+// u64 up to depth 12 (T <= 2^12, sums of one axis <= 2^24, F <= 2^36.5).
+struct MeasureSums {
+    unsigned long long n, s1[3], s2[6];
+    uint32_t lo[3], hi[3];
+    __device__ __forceinline__ void clear() {
+        n = 0;
+        for (int a = 0; a < 3; ++a) { s1[a] = 0; s2[a] = 0; s2[a + 3] = 0; lo[a] = 0xffffffffu; hi[a] = 0u; }
+    }
+    __device__ __forceinline__ static unsigned long long odd_sq(unsigned long long m) { return m * (4ull * m * m - 1ull) / 3ull; }
+    __device__ __forceinline__ void add_block(uint32_t x0, uint32_t y0, uint32_t z0, uint32_t T) {
+        const uint32_t c[3] = {x0, y0, z0};
+        const unsigned long long t = T, t2 = t * t;
+        unsigned long long a1[3];
+        for (int a = 0; a < 3; ++a) {
+            const unsigned long long e = c[a] + t;
+            a1[a] = e * e - (unsigned long long)c[a] * c[a];
+            s1[a] += t2 * a1[a];
+            s2[a] += t2 * (odd_sq(e) - odd_sq(c[a]));
+            lo[a] = min(lo[a], c[a]);
+            hi[a] = max(hi[a], c[a] + T - 1u);
+        }
+        n += t2 * t;
+        s2[3] += t * a1[0] * a1[1];
+        s2[4] += t * a1[0] * a1[2];
+        s2[5] += t * a1[1] * a1[2];
+    }
+    __device__ __forceinline__ void add_cell(uint32_t i, uint32_t j, uint32_t k) {
+        const unsigned long long u = 2u * i + 1u, v = 2u * j + 1u, w = 2u * k + 1u;
+        ++n;
+        s1[0] += u; s1[1] += v; s1[2] += w;
+        s2[0] += u * u; s2[1] += v * v; s2[2] += w * w;
+        s2[3] += u * v; s2[4] += u * w; s2[5] += v * w;
+        lo[0] = min(lo[0], i); lo[1] = min(lo[1], j); lo[2] = min(lo[2], k);
+        hi[0] = max(hi[0], i); hi[1] = max(hi[1], j); hi[2] = max(hi[2], k);
+    }
+    // the sums of the whole warp, in every lane
+    __device__ __forceinline__ void warp_fold() {
+        for (int o = 16; o > 0; o >>= 1) {
+            n += __shfl_xor_sync(FULL, n, o);
+            for (int a = 0; a < 3; ++a) {
+                s1[a] += __shfl_xor_sync(FULL, s1[a], o);
+                lo[a] = min(lo[a], __shfl_xor_sync(FULL, lo[a], o));
+                hi[a] = max(hi[a], __shfl_xor_sync(FULL, hi[a], o));
+            }
+            for (int a = 0; a < 6; ++a) s2[a] += __shfl_xor_sync(FULL, s2[a], o);
+        }
+    }
+    // into a frame's accumulator (one thread): n inside cells, of which `proven` in proven-inside cells, and `undecided`
+    // brick cells
+    __device__ __forceinline__ void flush(MeasureAcc* acc, bool proven, unsigned long long undecided) const {
+        if (undecided) atomicAdd(&acc->n_undecided, undecided);
+        if (!n) return;
+        atomicAdd(&acc->n_inside, n);
+        if (proven) atomicAdd(&acc->n_proven, n);
+        for (int a = 0; a < 3; ++a) {
+            atomicAdd(&acc->s1[a], s1[a]);
+            atomicMin(&acc->lo[a], lo[a]);
+            atomicMax(&acc->hi[a], hi[a]);
+        }
+        for (int a = 0; a < 6; ++a) atomicAdd(&acc->s2[a], s2[a]);
+    }
+};
+
 // TREE: the samplers' trees whose cells read their view from a ContourSlice table (a MeshFrame is the same record, z
 // unused), not from the render parameters.  DIM 2: the quadtree of
 // fc_contour_build.  Coordinates are cells at the finest depth with world-square bounds coord * cell_h - 1, seen through
 // `mat` when has_transform, at Z = [z2d, z2d]; classified tiles are dropped (no fills).  With FRAMES a contour slice
 // stack: each cell's slice (`slices`, frame_rows rows each) supplies Z, the matrix, its has_transform and the vars, and
 // the cell's rows are relative to its slice.  DIM 3 with FRAMES (octree mode 1): the stacked octree of a mesh frame
-// batch, each cell's frame read the same way (its Z is the cell's own).
-template <int DIM, bool FUSED, bool FRAMES = false, bool SCENE = false, bool TREE = false>
+// batch, each cell's frame read the same way (its Z is the cell's own).  MEASURE (DIM 3, TREE, FRAMES: fc_measure): the
+// block moments and box of the lanes' proven-inside cells go into their frame's accumulator, p.measure[cell row /
+// frame_rows]; a warp's children share one frame, the root cells of level 0 each have their own.
+template <int DIM, bool FUSED, bool FRAMES = false, bool SCENE = false, bool TREE = false, bool MEASURE = false>
 __device__ __forceinline__ void level_job(const LevelParams& p, uint32_t j, uint32_t n_roots, itv* slots, uint32_t* cs,
                                           uint32_t (*live)[32], int lane, uint32_t epoch,
                                           const ContourSlice* slices = nullptr) {
@@ -158,6 +226,20 @@ __device__ __forceinline__ void level_job(const LevelParams& p, uint32_t j, uint
         const bool fill_out = valid && !p.pixel_perfect && !fill_in && r.x > 0.0f;
         const bool amb = valid && !fill_in && !fill_out;
 
+        if constexpr (MEASURE) {
+            static_assert(DIM == 3 && TREE && FRAMES, "fc_measure's levels are the stacked octree's");
+            if (__any_sync(FULL, fill_in)) {
+                MeasureSums ms;
+                ms.clear();
+                if (fill_in) ms.add_block(cx, cy - fv.y0, cz, T);
+                if (p.root_mode) {
+                    if (fill_in) ms.flush(p.measure + cy / p.frame_rows, true, 0);
+                } else {
+                    ms.warp_fold();
+                    if (lane == 0) ms.flush(p.measure + cy / p.frame_rows, true, 0);
+                }
+            }
+        }
         if (DIM == 3) {
             // full tile: depth = max(depth, top + 1) over its footprint (voxel.rs:310-317)
             uint32_t m = p.mode == 1u ? 0u : __ballot_sync(FULL, fill_in);

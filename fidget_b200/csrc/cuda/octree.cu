@@ -157,8 +157,9 @@ void launch_octree_grads(const OctreeLeafParams& p, int blocks, cudaStream_t s, 
 
 // The levels of the samplers' trees: k_interval_level's claim loop around level_job's TREE mode.  DIM 3: a mesh frame
 // batch's stacked octree, one root cell per frame; DIM 2: the quadtree of a contour, one root cell, or with STACK one per
-// slice of a stack.  `frames` is the frame or slice table (STACK); root cells go 32 to a warp at level 0.
-template <int DIM, bool STACK>
+// slice of a stack.  `frames` is the frame or slice table (STACK); root cells go 32 to a warp at level 0.  MEASURE:
+// fc_measure's levels of the stacked octree, proven-inside cells folded into p.measure (level_job).
+template <int DIM, bool STACK, bool MEASURE = false>
 __global__ void __launch_bounds__(WARPS_PER_BLOCK * 32) k_tree_level(const __grid_constant__ LevelParams p,
                                                                      const ContourSlice* frames) {
     __shared__ uint32_t live_s[WARPS_PER_BLOCK][8][32];
@@ -177,13 +178,16 @@ __global__ void __launch_bounds__(WARPS_PER_BLOCK * 32) k_tree_level(const __gri
         }
         j = __shfl_sync(FULL, j, 0);
         if (j >= n_jobs) break;
-        level_job<DIM, false, STACK, false, true>(p, j, n_roots, slots, cs, live_s[wib], lane, p.epoch, frames);
+        level_job<DIM, false, STACK, false, true, MEASURE>(p, j, n_roots, slots, cs, live_s[wib], lane, p.epoch, frames);
     }
 }
 void launch_tree_level(const LevelParams& p, int dim, const ContourSlice* frames, int blocks, cudaStream_t s) {
     if (dim == 3) k_tree_level<3, true><<<blocks, WARPS_PER_BLOCK * 32, 0, s>>>(p, frames);
     else if (frames) k_tree_level<2, true><<<blocks, WARPS_PER_BLOCK * 32, 0, s>>>(p, frames);
     else k_tree_level<2, false><<<blocks, WARPS_PER_BLOCK * 32, 0, s>>>(p, nullptr);
+}
+void launch_tree_level_measure(const LevelParams& p, const MeshFrame* frames, int blocks, cudaStream_t s) {
+    k_tree_level<3, true, true><<<blocks, WARPS_PER_BLOCK * 32, 0, s>>>(p, frames);
 }
 
 }  // namespace fdev

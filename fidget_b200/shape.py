@@ -1109,6 +1109,42 @@ def mesh_frames(shape: CudaShape, depth: int, world_to_model=None, var_values=No
     return frames, as_dict(info), per_frame
 
 
+# fc_measure_result as a numpy record (one row per frame)
+MEASURE_RESULT = np.dtype([("n_inside", np.uint64), ("n_proven", np.uint64), ("n_undecided", np.uint64),
+                           ("s1", np.uint64, 3), ("s2", np.uint64, 6), ("lo", np.uint32, 3), ("hi", np.uint32, 3),
+                           ("volume", np.float64), ("volume_lo", np.float64), ("volume_hi", np.float64),
+                           ("centroid", np.float64, 3), ("inertia", np.float64, 6), ("bbox_min", np.float64, 3),
+                           ("bbox_max", np.float64, 3)])
+
+
+def measure(shape: CudaShape, depth: int, world_to_model=None, var_values=None, cancel: CancelToken | None = None,
+            timing: bool = False):
+    """Volume, centroid, inertia and bounding box of the shape's voxel solid at ``depth`` (``fc_measure``), per frame:
+    ``world_to_model`` / ``var_values`` are per-frame as in ``mesh_frame_table`` (a single 4x4 matrix or a 1-D value
+    list is one frame; with neither there is one frame).  Returns a ``MEASURE_RESULT`` array with one row per frame --
+    the exact integer sums and counts, and the float64 results in model space -- and with ``timing`` also the device
+    time in ms.  None when ``cancel`` cancelled the call."""
+    lib = shape._lib
+    if world_to_model is not None and not isinstance(world_to_model, (list, tuple)) and \
+            np.asarray(world_to_model).shape == (4, 4):
+        world_to_model = [world_to_model]
+    if var_values is not None and np.asarray(var_values, dtype=np.float32).ndim == 1:
+        var_values = [var_values]
+    table = mesh_frame_table(world_to_model=world_to_model, var_values=var_values)
+    n = len(table)
+    c = _lib.FcOctreeCfg()
+    c.depth = depth
+    c.flags = _lib.FC_FLAG_TIMING if timing else 0
+    out = np.zeros(n, dtype=MEASURE_RESULT)
+    ms = C.c_float()
+    rc = shape.cuda._cancellable(cancel, lambda: lib.fc_measure(shape.cuda._h, shape._h, C.byref(c), table, n, _ptr(out),
+                                                                C.byref(ms)))
+    if rc == _lib.FC_ERR_CANCELLED:
+        return None
+    _ck(rc)
+    return (out, ms.value) if timing else out
+
+
 # ---------------------------------------------------------------------------
 # 2D contours (libfive's Contours::render): fc_contour_build / fc_contour_read
 def contour(shape: CudaShape, depth: int, z: float = 0.0, world_to_model=None, var_values=(),

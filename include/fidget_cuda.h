@@ -538,6 +538,7 @@ int32_t fc_mesh_write_stl(fc_ctx* ctx, uint8_t* buf, size_t cap, size_t* n_bytes
  *    with n_frames > 0.  A failed or cancelled call (the cancel flag behaves as in fc_mesh_build) leaves no mesh, as
  *    does n_frames == 0, which launches nothing. */
 #define FC_MESH_MAX_PASS_FRAMES 4096u
+
 typedef struct fc_mesh_frame {
     uint32_t has_transform;         /* as fc_octree_cfg.has_transform */
     float world_to_model[16];       /* as fc_octree_cfg.world_to_model (row-major 4x4) */
@@ -550,6 +551,58 @@ typedef struct fc_mesh_frame_info {
 int32_t fc_mesh_build_frames(fc_ctx* ctx, const fc_tape* tape, const fc_octree_cfg* cfg /* depth, flags */,
                              const fc_mesh_frame* frames /* host */, uint32_t n_frames,
                              fc_mesh_info* info /* totals */, fc_mesh_frame_info* per_frame /* may be NULL */);
+
+/* ---- Measurement: volume, centre of mass, inertia and bounding box ------------------------------------------------
+ * fc_measure measures the voxel solid of a shape at depth D (0 <= D <= FC_MAX_OCTREE_DEPTH): the world cube [-1,1]^3 is
+ * split into 2^D cells per axis, cell (i, j, k) spanning [-1 + i h, -1 + (i + 1) h] on X (likewise Y, Z), h = 2 / 2^D,
+ * and the solid is the union of the cells that count as inside, as solid cubes of unit density.  With has_transform the
+ * field is seen through world_to_model, as fc_mesh_build sees it.  Which cells count as inside is fixed by the descent:
+ *  - with B = min(4, 2^D) the brick edge, interval levels run from the root cell down to cells of edge B, one octree
+ *    depth per level, with fc_octree_sample's bounds, transform, tape simplification and classification: upper < 0
+ *    proves the cell inside (all its depth-D cells count), lower > 0 proves it outside (dropped), anything else is
+ *    split further;
+ *  - every ambiguous cell of edge B is a brick: each of its B^3 depth-D cells counts as inside iff the f32 value at its
+ *    centre (-1 + (2i + 1) 2^-D, ...; exact in f32), through world_to_model as the octree leaf's corners are, with the
+ *    brick's own simplified tape, is < 0.
+ * For tapes of IEEE operations an interval never contradicts a point value in its box, so the result should equal a
+ * classification of every cell centre.
+ * Exact results (integers, independent of the launch grid, the order of the work and the passes), with u = 2i + 1,
+ * v = 2j + 1, w = 2k + 1 over the inside cells: n_inside; n_proven, those in interval-proven-inside cells; n_undecided,
+ * B^3 times the number of bricks; s1 = (Σu, Σv, Σw); s2 = (Σuu, Σvv, Σww, Σuv, Σuw, Σvw); lo / hi, the inclusive
+ * cell-index box (0xFFFFFFFF and 0 when n_inside is 0).  Every sum fits u64 up to depth 12 (Σuv <= 2^62).
+ * Derived results, float64, computed from the integers on the host.  In world space the volume is N h^3, the centroid
+ * -1 + s1 / (N 2^D), the covariance (N s2 - s1 s1^T) / (N^2 4^D) plus h^2 / 12 on the diagonal (the numerators formed
+ * exactly), and [volume_lo, volume_hi] = [n_proven, n_proven + n_undecided] h^3 encloses the shape's true volume inside
+ * the cube, up to rounding (the intervals are not outward-rounded).  The fields below are in model space: with
+ * has_transform and a matrix other than the identity, world_to_model = [A t; 0 1] scales the volumes by |det A|, maps
+ * the centroid, and turns the covariance C into A C A^T; inertia = volume (tr(C) I - C) about the centroid (Ixx, Iyy,
+ * Izz, Ixy, Ixz, Iyz; the products of inertia are -∫xy dV); bbox is the box of the 8 mapped corners of the world box
+ * [lo h - 1, (hi + 1) h - 1].  An empty frame has volume 0 and NaN centroid, inertia and box.
+ *  - frames (host, n_frames entries): each frame's has_transform, world_to_model and var_values; cfg supplies depth and
+ *    flags (FC_FLAG_TIMING: *device_ms, when not NULL, receives the device time summed over passes).
+ *  - passes: the frames of a pass share each launch in one stacked octree (frame k owns the cell rows
+ *    [k 2^D, (k + 1) 2^D)); the first pass holds one frame, later ones are sized from the largest per-frame arena and
+ *    job-list use seen so far, and a pass that overflows anyway is run again in halves: FC_ERR_ARENA or a work-list
+ *    overflow comes back only where one frame alone gives it.
+ *  - Checked for every frame before anything is allocated or launched: depth above FC_MAX_OCTREE_DEPTH, a multi-output
+ *    tape, more than FC_MAX_VARS values, a frame without a value for a bound variable, and NULL frames or out with
+ *    n_frames > 0 give FC_ERR_INVALID; a tape with memory slots or a projective world_to_model (last row other than
+ *    0 0 0 1, with has_transform) gives FC_ERR_UNSUPPORTED.  n_frames == 0 launches nothing and returns FC_OK.
+ *  - The cancel flag behaves as in fc_mesh_build: a cancelled call returns FC_ERR_CANCELLED with out zeroed, and the
+ *    context stays usable.  A failed call zeroes out too. */
+typedef struct fc_measure_result {
+    uint64_t n_inside, n_proven, n_undecided;
+    uint64_t s1[3];                 /* Σu, Σv, Σw */
+    uint64_t s2[6];                 /* Σuu, Σvv, Σww, Σuv, Σuw, Σvw */
+    uint32_t lo[3], hi[3];          /* inclusive cell-index box of the inside cells */
+    double volume, volume_lo, volume_hi;
+    double centroid[3];
+    double inertia[6];              /* Ixx, Iyy, Izz, Ixy, Ixz, Iyz about the centroid */
+    double bbox_min[3], bbox_max[3];
+} fc_measure_result;
+int32_t fc_measure(fc_ctx* ctx, const fc_tape* tape, const fc_octree_cfg* cfg /* depth, flags */,
+                   const fc_mesh_frame* frames /* host */, uint32_t n_frames, fc_measure_result* out /* host */,
+                   float* device_ms /* FC_FLAG_TIMING, may be NULL */);
 
 /* ---- 2D contours (libfive's Contours::render, on the quadtree the mesher's octree restricts to) -------------------
  * fc_contour_build extracts the contours of a 2D shape (a sketch, a cut profile, a Z slice of a 3D model) as closed or

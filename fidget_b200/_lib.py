@@ -49,6 +49,13 @@ def load() -> C.CDLL:
     return _LIB
 
 
+class _Record(C.Structure):
+    """A C struct whose fields read back as a dict (arrays as lists)"""
+
+    def as_dict(self):
+        return {n: list(v) if isinstance(v, C.Array) else v for n, _ in self._fields_ for v in [getattr(self, n)]}
+
+
 class FcTapeInfo(C.Structure):
     _fields_ = [(n, C.c_uint32) for n in
                 ("n_ops", "ref_len", "choice_count", "reg_count", "mem_count", "n_vars", "n_outputs")]
@@ -70,7 +77,7 @@ class FcFrame3d(C.Structure):
     _fields_ = [("mat", C.c_float * 16), ("n_var_values", C.c_uint32), ("var_values", C.c_float * 16)]
 
 
-class FcScheduleInfo(C.Structure):
+class FcScheduleInfo(_Record):
     _fields_ = [(n, C.c_uint32) for n in ("suitable", "n_clauses", "n_waves", "widest_wave", "n_tail", "n_segments",
                                           "n_chain_clauses", "n_slots")]
 
@@ -83,18 +90,11 @@ class FcRender3dCfg(C.Structure):
                 ("root_stride", C.c_uint32), ("root_offset", C.c_uint32)]
 
 
-class FcRenderStats(C.Structure):
+class FcRenderStats(_Record):
     _fields_ = [(n, C.c_uint64 * 8) for n in
                 ("evaluated", "filled_inside", "filled_outside", "ambiguous", "simplified")] + \
                [("pixels", C.c_uint64), ("grads", C.c_uint64), ("arena_bytes_used", C.c_uint64),
                 ("kernel_launches", C.c_uint32), ("stage_ms", C.c_float * 16)]
-
-    def as_dict(self):
-        d = {n: list(getattr(self, n)) for n in
-             ("evaluated", "filled_inside", "filled_outside", "ambiguous", "simplified")}
-        d.update(pixels=int(self.pixels), grads=int(self.grads), arena_bytes_used=int(self.arena_bytes_used),
-                 kernel_launches=int(self.kernel_launches), stage_ms=list(self.stage_ms))
-        return d
 
 
 class FcOctreeCfg(C.Structure):
@@ -102,21 +102,14 @@ class FcOctreeCfg(C.Structure):
                 ("flags", C.c_uint32), ("n_var_values", C.c_uint32), ("var_values", C.c_float * 16)]
 
 
-class FcOctreeStats(C.Structure):
+class FcOctreeStats(_Record):
     _fields_ = [(n, C.c_uint64 * 16) for n in ("evaluated", "full", "empty", "ambiguous")] + \
                [(n, C.c_uint64) for n in ("leaf_empty", "leaf_full", "leaf_surface", "float_points", "grad_points",
                                           "arena_bytes_used")] + \
                [("kernel_launches", C.c_uint32), ("total_ms", C.c_float)]
 
-    def as_dict(self):
-        d = {n: list(getattr(self, n)) for n in ("evaluated", "full", "empty", "ambiguous")}
-        for n in ("leaf_empty", "leaf_full", "leaf_surface", "float_points", "grad_points", "arena_bytes_used",
-                  "kernel_launches", "total_ms"):
-            d[n] = getattr(self, n)
-        return d
 
-
-class FcMeshInfo(C.Structure):
+class FcMeshInfo(_Record):
     _fields_ = [(n, C.c_uint64) for n in ("n_leaves", "n_vertices", "n_triangles", "open_edges")] + \
                [("sampler_ms", C.c_float), ("mesh_ms", C.c_float)]
 
@@ -126,7 +119,7 @@ class FcMeshFrame(C.Structure):
                 ("var_values", C.c_float * 16)]
 
 
-class FcMeshFrameInfo(C.Structure):
+class FcMeshFrameInfo(_Record):
     _fields_ = [(n, C.c_uint64) for n in ("n_leaves", "n_vertices", "n_triangles", "open_edges", "n_cells")]
 
 
@@ -143,7 +136,7 @@ class FcContourCfg(C.Structure):
                 ("flags", C.c_uint32), ("n_var_values", C.c_uint32), ("var_values", C.c_float * 16)]
 
 
-class FcContourInfo(C.Structure):
+class FcContourInfo(_Record):
     _fields_ = [(n, C.c_uint64) for n in ("n_leaves", "n_vertices", "n_polylines", "n_closed", "n_open")] + \
                [("sampler_ms", C.c_float), ("contour_ms", C.c_float)]
 
@@ -161,14 +154,9 @@ class FcSolveResult(C.Structure):
     _fields_ = [("status", C.c_uint32), ("iterations", C.c_uint32), ("err", C.c_float), ("pad", C.c_uint32)]
 
 
-class FcCompiledInfo(C.Structure):
+class FcCompiledInfo(_Record):
     _fields_ = [("kinds", C.c_uint32), ("nvrtc_version", C.c_uint32), ("regs", C.c_uint32 * 3),
                 ("local_bytes", C.c_uint32 * 3), ("compile_ms", C.c_float * 3), ("cubin_bytes", C.c_uint64)]
-
-    def as_dict(self):
-        return {"kinds": int(self.kinds), "nvrtc_version": int(self.nvrtc_version), "regs": list(self.regs),
-                "local_bytes": list(self.local_bytes), "compile_ms": list(self.compile_ms),
-                "cubin_bytes": int(self.cubin_bytes)}
 
 
 FC_COMPILE_FLOAT, FC_COMPILE_GRAD, FC_COMPILE_INTERVAL = 1, 2, 4

@@ -248,6 +248,25 @@ int32_t bulk_eval(fc_eval* e, const fc_tape* t, const void* const* vars, void* c
 int32_t transcode(const uint32_t* words, size_t n_words, uint8_t reg_count, uint32_t mem_count, uint32_t n_vars,
                   uint32_t n_outputs, std::vector<uint2>& out, uint32_t& n_choices);
 // octree_capi.cu
+// The refusals every uniform-tree call (octree sample, mesh frames, contours, fc_measure) makes before it begins, locks
+// or allocates: a depth above the tree's limit (FC_MAX_OCTREE_DEPTH for dim 3, FC_MAX_QUADTREE_DEPTH for 2), a null
+// `table` of n > 0 frames or slices, more than FC_MAX_VARS values in one, a tape with memory slots (`what` names the
+// caller), a multi-output tape.  F: fc_mesh_frame or fc_contour_slice.
+template <class F>
+int32_t check_tree_call(const fc_tape* tape, int dim, uint32_t depth, const F* table, uint32_t n, const char* what);
+// A frame or slice as the tree kernels take it, its vars bound (bind_vars' refusals).  to_model: map the vertices back
+// through world_to_model (row-major 4x4) unless it is the identity, as Octree::build does (octree.rs:58-65).  The
+// kernels read the matrix only with has_transform.
+int32_t bind_frame(const fc_tape* tape, uint32_t has_transform, const float* world_to_model, float z, const float* values,
+                   uint32_t n_values, MeshFrame& f);
+// Level l's job list over n root cells of 2^dim children per level: every cell at depth min(l, D), at most `limit`
+inline uint64_t tree_list(uint64_t n, int dim, uint32_t D, int l, uint64_t limit) {
+    return std::min(n << (dim * std::min(l, int(D))), limit);
+}
+// The passes of a batch of n frames or slices (pass_plan.h), at most n_max each: the job lists of levels 1 .. `levels`
+// as tree_scratch sizes them, and with leaf_bytes > 0 the surface leaves within FC_FRAMES_PASS_BYTES
+struct PassPlan;
+PassPlan tree_passes(fc_ctx* c, uint32_t n, uint32_t n_max, uint32_t D, int dim, int levels, double leaf_bytes);
 // The uniform-tree samplers (octree_enqueue, contour_sample) over n_roots root cells stacked along Y (one per frame or
 // slice), each with 2^dim children per level down to depth D: their scratch (choice scratch, arena, counters with 64
 // zeroed bytes after them, stats, the job lists, `cap` leaf tapes), the LevelParams every level of both shares, and the

@@ -625,19 +625,8 @@ static int32_t contour_stack(fc_ctx* c, const fc_tape* tape, uint32_t D, bool ti
     const uint32_t N = uint32_t(sl.size());
     // Passes as the 3D batches' (pass_plan.h), the measured quantity being surface leaves (with their link scratch)
     // within FC_FRAMES_PASS_BYTES.  A pass's slice index is 16 bits in its leaves, and its cell rows must fit 32 bits.
-    const uint64_t cap_limit = list_cap_limit();
-    PassPlan plan(N, uint32_t(std::min<uint64_t>({N, 0xffffu, (1ull << (32 - D)) - 1})), [&](uint32_t n) {
-        PassLimits lim;
-        lim.arena_cap = arena_clauses(c);
-        for (int l = 1; l <= int(D) + 1; ++l) {   // every cell of n slices at depth min(l, D) queued
-            lim.worst[l] = uint64_t(n) << (2 * std::min<uint32_t>(uint32_t(l), D));
-            lim.cap[l] = std::min(lim.worst[l], cap_limit);
-        }
-        lim.extra_on = true;
-        lim.extra_scale = double(CONTOUR_LEAF_BYTES);
-        lim.extra_cap = FC_FRAMES_PASS_BYTES;
-        return lim;
-    });
+    PassPlan plan = tree_passes(c, N, uint32_t(std::min<uint64_t>({N, 0xffffu, (1ull << (32 - D)) - 1})), D, 2, int(D) + 1,
+                                double(CONTOUR_LEAF_BYTES));
     uint64_t n_verts = 0, n_polys = 0;   // the stack's output so far
     std::vector<uint32_t> cnt;
     while (plan.more()) {
@@ -717,30 +706,17 @@ static int32_t contour_build(fc_ctx* c, const fc_tape* tape, const fc_contour_cf
                              uint32_t n_slices, fc_contour_info* info, fc_contour_info* per) {
     memset(info, 0, sizeof *info);
     if (per && n_slices) memset(per, 0, size_t(n_slices) * sizeof *per);
-    if (cfg->depth > FC_MAX_QUADTREE_DEPTH) return fail(FC_ERR_INVALID, "quadtree depth too large");
-    if (!slices && n_slices) return fail(FC_ERR_INVALID, "null slices");
-    for (uint32_t k = 0; k < n_slices; ++k)
-        if (slices[k].n_var_values > FC_MAX_VARS) return fail(FC_ERR_INVALID, "too many variable values");
-    if (tape->info.mem_count) return fail(FC_ERR_UNSUPPORTED, "contours need a tape without memory spills");
-    if (tape->info.n_outputs != 1) return fail(FC_ERR_INVALID, "ShapeTape has multiple outputs");
+    if (int32_t rc = check_tree_call(tape, 2, cfg->depth, slices, n_slices, "the contour sampler")) return rc;
     std::vector<ContourSlice> sl(n_slices);
     for (uint32_t k = 0; k < n_slices; ++k) {
         const fc_contour_slice& in = slices[k];
-        ContourSlice& out = sl[k];
-        if (int32_t vrc = bind_vars(tape, in.var_values, in.n_var_values, out.vb)) return vrc;
         // the 3x3 embedded as the 2D renderers embed it: (x, y, z, 1) -> (m0 x + m1 y + m2, m3 x + m4 y + m5, z, m6 x + m7 y + m8)
-        bool to_model = false;
+        float m[16] = {};
         const int idx[3] = {0, 1, 3};
         for (int i = 0; i < 3; ++i)
-            for (int j = 0; j < 3; ++j) {
-                const float v = in.has_transform ? in.world_to_model[3 * i + j] : (i == j ? 1.0f : 0.0f);
-                out.mat.m[4 * idx[i] + idx[j]] = v;
-                to_model |= v != (i == j ? 1.0f : 0.0f);
-            }
-        out.mat.m[10] = 1.0f;
-        out.z = in.z;
-        out.has_transform = in.has_transform;
-        out.to_model = in.has_transform && to_model;
+            for (int j = 0; j < 3; ++j) m[4 * idx[i] + idx[j]] = in.world_to_model[3 * i + j];
+        m[10] = 1.0f;
+        if (int32_t vrc = bind_frame(tape, in.has_transform, m, in.z, in.var_values, in.n_var_values, sl[k])) return vrc;
     }
     CallCancel cc;
     auto no_contour = [&](int32_t rc) {   // a failed or cancelled build leaves no contour

@@ -153,18 +153,10 @@ int32_t measure_passes(fc_ctx* c, const fc_tape* tape, uint32_t D, bool timing, 
     const uint32_t N = uint32_t(fr.size());
     const uint32_t b = std::min<uint32_t>(D, 2), B = 1u << b;
     const int Lb = int(D - b) + 1;   // interval levels 0 .. D - b; the bricks are list Lb
-    const uint64_t cap_limit = list_cap_limit();
     cudaStream_t s = c->stream;
     // a pass's cell rows must fit 32 bits
-    PassPlan plan(N, uint32_t(std::min<uint64_t>({N, FC_MESH_MAX_PASS_FRAMES, 0xffffffffull >> D})), [&](uint32_t n) {
-        PassLimits lim;
-        lim.arena_cap = arena_clauses(c);
-        for (int l = 1; l <= Lb; ++l) {   // as tree_scratch sizes them
-            lim.worst[l] = uint64_t(n) << (3 * std::min<uint32_t>(uint32_t(l), D));
-            lim.cap[l] = std::min(lim.worst[l], cap_limit);
-        }
-        return lim;
-    });
+    PassPlan plan = tree_passes(c, N, uint32_t(std::min<uint64_t>({N, FC_MESH_MAX_PASS_FRAMES, 0xffffffffull >> D})), D, 3,
+                                Lb, 0);
     MeasureAcc init{};
     for (int i = 0; i < 3; ++i) init.lo[i] = 0xffffffffu;
     std::vector<MeasureAcc> h_acc;
@@ -225,19 +217,15 @@ int32_t fc_measure(fc_ctx* c, const fc_tape* tape, const fc_octree_cfg* cfg, con
     if (!c || !tape || !cfg) return fail(FC_ERR_INVALID, "null argument");
     if (n_frames && (!frames || !out)) return fail(FC_ERR_INVALID, "null frames or out");
     if (out && n_frames) memset(out, 0, size_t(n_frames) * sizeof *out);
-    if (cfg->depth > FC_MAX_OCTREE_DEPTH) return fail(FC_ERR_INVALID, "octree depth too large");
-    if (tape->info.n_outputs != 1) return fail(FC_ERR_INVALID, "ShapeTape has multiple outputs");
-    if (tape->info.mem_count) return fail(FC_ERR_UNSUPPORTED, "fc_measure needs a tape without memory spills");
+    if (int32_t rc = check_tree_call(tape, 3, cfg->depth, frames, n_frames, "fc_measure")) return rc;
     std::vector<MeshFrame> fr(n_frames);
     for (uint32_t k = 0; k < n_frames; ++k) {
         const fc_mesh_frame& in = frames[k];
-        if (in.n_var_values > FC_MAX_VARS) return fail(FC_ERR_INVALID, "too many variable values");
         if (in.has_transform && (in.world_to_model[12] != 0.0f || in.world_to_model[13] != 0.0f ||
                                  in.world_to_model[14] != 0.0f || in.world_to_model[15] != 1.0f))
             return fail(FC_ERR_UNSUPPORTED, "fc_measure needs an affine world_to_model (last row 0 0 0 1)");
-        if (int32_t vrc = bind_vars(tape, in.var_values, in.n_var_values, fr[k].vb)) return vrc;
-        memcpy(fr[k].mat.m, in.world_to_model, sizeof fr[k].mat.m);
-        fr[k].has_transform = in.has_transform;
+        if (int32_t vrc = bind_frame(tape, in.has_transform, in.world_to_model, 0.0f, in.var_values, in.n_var_values, fr[k]))
+            return vrc;
     }
     if (!n_frames) return FC_OK;
     const uint32_t D = cfg->depth;

@@ -1063,20 +1063,9 @@ static int32_t mesh_passes(fc_ctx* c, const fc_tape* tape, uint32_t D, uint32_t 
     const bool collapse = (flags & FC_FLAG_MESH_COLLAPSE) != 0, timing = (flags & FC_FLAG_TIMING) != 0;
     // Passes as the 3D batches' (pass_plan.h), the measured quantity being surface leaves (with their mesh scratch)
     // within FC_FRAMES_PASS_BYTES.  A pass's frame index is 12 bits in the cell keys, and its cell rows must fit 32 bits.
-    const uint64_t cap_limit = list_cap_limit();
     const double leaf_bytes = double(collapse ? MESH_COLLAPSE_LEAF_BYTES : MESH_LEAF_BYTES);
-    PassPlan plan(N, uint32_t(std::min<uint64_t>({N, MESH_MAX_PASS_FRAMES, 0xffffffffull >> D})), [&](uint32_t n) {
-        PassLimits lim;
-        lim.arena_cap = arena_clauses(c);
-        for (int l = 1; l <= int(D) + 1; ++l) {   // every cell of n frames at depth min(l, D) queued
-            lim.worst[l] = uint64_t(n) << (3 * std::min<uint32_t>(uint32_t(l), D));
-            lim.cap[l] = std::min(lim.worst[l], cap_limit);
-        }
-        lim.extra_on = true;
-        lim.extra_scale = leaf_bytes;
-        lim.extra_cap = FC_FRAMES_PASS_BYTES;
-        return lim;
-    });
+    PassPlan plan = tree_passes(c, N, uint32_t(std::min<uint64_t>({N, MESH_MAX_PASS_FRAMES, 0xffffffffull >> D})), D, 3,
+                                int(D) + 1, leaf_bytes);
     const uint64_t first_guess = std::min<uint64_t>(1ull << (3 * D), 6ull << (2 * D));   // leaves of one frame
     uint64_t v0 = 0, t0 = 0, c0 = 0;   // the batch's output so far
     std::vector<uint2> ranges(N);
@@ -1183,23 +1172,12 @@ static int32_t mesh_build_frames(fc_ctx* c, const fc_tape* tape, const fc_octree
         if (per && n_frames) memset(per, 0, size_t(n_frames) * sizeof *per);
         return rc;
     };
-    if (cfg->depth > FC_MAX_OCTREE_DEPTH) return no_mesh(fail(FC_ERR_INVALID, "octree depth too large"));
-    if (!frames && n_frames) return no_mesh(fail(FC_ERR_INVALID, "null frames"));
-    for (uint32_t k = 0; k < n_frames; ++k)
-        if (frames[k].n_var_values > FC_MAX_VARS) return no_mesh(fail(FC_ERR_INVALID, "too many variable values"));
-    if (tape->info.mem_count) return no_mesh(fail(FC_ERR_UNSUPPORTED, "the octree sampler needs a tape without memory spills"));
-    if (tape->info.n_outputs != 1) return no_mesh(fail(FC_ERR_INVALID, "ShapeTape has multiple outputs"));
+    if (int32_t rc = check_tree_call(tape, 3, cfg->depth, frames, n_frames, "the octree sampler")) return no_mesh(rc);
     std::vector<MeshFrame> fr(n_frames);
     for (uint32_t k = 0; k < n_frames; ++k) {
         const fc_mesh_frame& in = frames[k];
-        MeshFrame& out = fr[k];
-        if (int32_t vrc = bind_vars(tape, in.var_values, in.n_var_values, out.vb)) return no_mesh(vrc);
-        memcpy(out.mat.m, in.world_to_model, sizeof out.mat.m);
-        // Octree::build maps the vertices through Settings::world_to_model unless that is the identity (octree.rs:58-65)
-        bool to_model = false;
-        for (int i = 0; i < 16 && in.has_transform; ++i) to_model |= out.mat.m[i] != (i % 5 == 0 ? 1.0f : 0.0f);
-        out.has_transform = in.has_transform;
-        out.to_model = to_model;
+        if (int32_t vrc = bind_frame(tape, in.has_transform, in.world_to_model, 0.0f, in.var_values, in.n_var_values, fr[k]))
+            return no_mesh(vrc);
     }
     CallCancel cc;
     if (int32_t crc = begin_call(c, cc)) return no_mesh(crc);
@@ -1245,16 +1223,15 @@ int32_t fc_mesh_build(fc_ctx* c, const fc_tape* tape, const fc_octree_cfg* cfg, 
         if (n > cap && attempt == 0) { cap = n; continue; }   // retry once with the exact count
         return rc;
     }
+    MeshFrame view;   // the frame octree_sample_device bound, for its to_model
+    if (int32_t vrc = bind_frame(tape, cfg->has_transform, cfg->world_to_model, 0.0f, cfg->var_values, cfg->n_var_values,
+                                 view))
+        return vrc;
     std::unique_lock<std::mutex> guard(c->mu);
     info->n_leaves = n;
     info->sampler_ms = ost.total_ms;
     mesh_clear(c);
     if (n == 0) return FC_OK;
-    // Octree::build maps the vertices through Settings::world_to_model unless that is the identity (octree.rs:58-65)
-    fdev::Mat4 view;
-    memcpy(view.m, cfg->world_to_model, sizeof view.m);
-    bool to_model = false;
-    for (int i = 0; i < 16 && cfg->has_transform; ++i) to_model |= view.m[i] != (i % 5 == 0 ? 1.0f : 0.0f);
     fdev::MeshScratch m{};
     m.leaves = c->mesh_leaves.as<OctreeLeaf>();
     m.n_leaves = m.n_nodes = n;
@@ -1263,7 +1240,7 @@ int32_t fc_mesh_build(fc_ctx* c, const fc_tape* tape, const fc_octree_cfg* cfg, 
     m.n_frames = 1;
     const bool collapse = cfg->flags & FC_FLAG_MESH_COLLAPSE;
     int32_t rc = collapse ? mesh_enqueue_collapse(c, m, 0, cc) : mesh_enqueue_uniform(c, m);
-    if (rc == FC_OK) rc = mesh_finish(c, m, collapse, to_model ? &view : nullptr, info, cc);
+    if (rc == FC_OK) rc = mesh_finish(c, m, collapse, view.to_model ? &view.mat : nullptr, info, cc);
     guard.unlock();
     return rc == FC_ERR_CANCELLED ? no_mesh(rc) : rc;
 }

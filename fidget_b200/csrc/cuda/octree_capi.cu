@@ -1,5 +1,47 @@
 // fc_octree_sample: the sampling half of fidget-mesh's Octree::build.
 #include "capi_internal.h"
+#include "pass_plan.h"
+
+template <class F>
+int32_t check_tree_call(const fc_tape* tape, int dim, uint32_t depth, const F* table, uint32_t n, const char* what) {
+    if (depth > uint32_t(dim == 3 ? FC_MAX_OCTREE_DEPTH : FC_MAX_QUADTREE_DEPTH))
+        return fail(FC_ERR_INVALID, dim == 3 ? "octree depth too large" : "quadtree depth too large");
+    if (!table && n) return fail(FC_ERR_INVALID, dim == 3 ? "null frames" : "null slices");
+    for (uint32_t k = 0; k < n; ++k)
+        if (table[k].n_var_values > FC_MAX_VARS) return fail(FC_ERR_INVALID, "too many variable values");
+    if (tape->info.mem_count) return fail(FC_ERR_UNSUPPORTED, std::string(what) + " needs a tape without memory spills");
+    if (tape->info.n_outputs != 1) return fail(FC_ERR_INVALID, "ShapeTape has multiple outputs");
+    return FC_OK;
+}
+template int32_t check_tree_call(const fc_tape*, int, uint32_t, const fc_mesh_frame*, uint32_t, const char*);
+template int32_t check_tree_call(const fc_tape*, int, uint32_t, const fc_contour_slice*, uint32_t, const char*);
+
+int32_t bind_frame(const fc_tape* tape, uint32_t has_transform, const float* world_to_model, float z, const float* values,
+                   uint32_t n_values, MeshFrame& f) {
+    memcpy(f.mat.m, world_to_model, sizeof f.mat.m);
+    f.z = z;
+    f.has_transform = has_transform;
+    bool identity = true;
+    for (int i = 0; i < 16; ++i) identity &= f.mat.m[i] == (i % 5 == 0 ? 1.0f : 0.0f);
+    f.to_model = has_transform && !identity;
+    return bind_vars(tape, values, n_values, f.vb);
+}
+
+PassPlan tree_passes(fc_ctx* c, uint32_t n, uint32_t n_max, uint32_t D, int dim, int levels, double leaf_bytes) {
+    const uint64_t cap_limit = list_cap_limit();
+    return PassPlan(n, n_max, [=](uint32_t k) {
+        PassLimits lim;
+        lim.arena_cap = arena_clauses(c);
+        for (int l = 1; l <= levels; ++l) {   // the worst case: every cell of k trees at depth min(l, D) queued
+            lim.worst[l] = tree_list(k, dim, D, l, ~0ull);
+            lim.cap[l] = tree_list(k, dim, D, l, cap_limit);
+        }
+        lim.extra_on = leaf_bytes > 0;
+        lim.extra_scale = leaf_bytes;
+        lim.extra_cap = FC_FRAMES_PASS_BYTES;
+        return lim;
+    });
+}
 
 int32_t tree_scratch(fc_ctx* c, const fc_tape* tape, uint32_t D, int dim, uint64_t n_roots, uint64_t cap, TreeScratch& t) {
     t.D = D;
@@ -13,7 +55,7 @@ int32_t tree_scratch(fc_ctx* c, const fc_tape* tape, uint32_t D, int dim, uint64
     CU(c->stats.ensure(sizeof(Stats)));
     const uint64_t cap_limit = list_cap_limit();
     for (int l = 1; l <= int(D) + 1; ++l) {
-        t.level_cap[l] = std::min<uint64_t>(n_roots << (dim * std::min(l, int(D))), cap_limit);
+        t.level_cap[l] = tree_list(n_roots, dim, D, l, cap_limit);
         CU(c->jobs[l].ensure(t.level_cap[l] * sizeof(TileJob)));
     }
     CU(c->leaf_tapes.ensure(std::max<uint64_t>(cap, 1) * sizeof(TapeRef)));
@@ -106,16 +148,14 @@ int32_t octree_sample_device(fc_ctx* c, const fc_tape* tape, const fc_octree_cfg
                              uint32_t* n_out_p, fc_octree_stats* stats, const CallCancel& cc) {
     static_assert(sizeof(fc_octree_leaf) == sizeof(OctreeLeaf) && sizeof(OctreeLeaf) == 348, "leaf layout");
     if (!c || !tape || !cfg || !n_out_p) return fail(FC_ERR_INVALID, "null argument");
-    if (cfg->depth > FC_MAX_OCTREE_DEPTH) return fail(FC_ERR_INVALID, "octree depth too large");
-    if (tape->info.mem_count) return fail(FC_ERR_UNSUPPORTED, "the octree sampler needs a tape without memory spills");
-    if (tape->info.n_outputs != 1) return fail(FC_ERR_INVALID, "ShapeTape has multiple outputs");
+    if (int32_t rc = check_tree_call<fc_mesh_frame>(tape, 3, cfg->depth, nullptr, 0, "the octree sampler")) return rc;
     if (cap > 0xfffffff0ull) return fail(FC_ERR_INVALID, "leaf capacity too large");
     std::lock_guard<std::mutex> guard(c->mu);
     CU(cudaSetDevice(c->device));
     MeshFrame one{};
-    if (int32_t vrc = bind_vars(tape, cfg->var_values, cfg->n_var_values, one.vb)) return vrc;
-    memcpy(one.mat.m, cfg->world_to_model, sizeof one.mat.m);
-    one.has_transform = cfg->has_transform;
+    if (int32_t vrc = bind_frame(tape, cfg->has_transform, cfg->world_to_model, 0.0f, cfg->var_values, cfg->n_var_values,
+                                 one))
+        return vrc;
     const uint32_t D = cfg->depth;
     cudaStream_t s = c->stream;
     const bool timing = (cfg->flags & FC_FLAG_TIMING) != 0;

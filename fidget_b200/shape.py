@@ -53,7 +53,7 @@ def schedule_check(tape: TapeData) -> dict:
     info = _lib.FcScheduleInfo()
     _ck(lib.fc_schedule_check(bc.words.ctypes.data_as(C.POINTER(C.c_uint32)), len(bc.words), bc.reg_count, bc.mem_count,
                               tape.n_vars, tape.output_count, C.byref(info)))
-    return {n: getattr(info, n) for n, _ in info._fields_}
+    return info.as_dict()
 
 
 class CancelToken:
@@ -590,14 +590,11 @@ def render2d(shape: CudaShape, cfg: RenderConfig2D, out=None, stats: bool = Fals
     return (out, st.as_dict()) if stats else out
 
 
-def frame_table(cfg: RenderConfig2D, z=None, var_values=None, world_to_model=None, mats=None):
-    """The ``fc_frame2d`` table of ``render2d_frames``: frame k's matrix, Z and ShapeVars, each exactly what
-    ``render2d`` puts into ``fc_render2d_cfg`` for the config ``cfg`` with that frame's values.  Every argument
-    given is per frame (leading dimension n: ``z`` [n], ``var_values`` [n, k], ``world_to_model`` [n, 3, 3],
-    ``mats`` [n, 4, 4]); the others come from ``cfg``.  Lengths that disagree raise ValueError; with no per-frame
-    argument at all there is one frame.  ``mats`` and ``world_to_model`` are exclusive."""
-    if mats is not None and world_to_model is not None:
-        raise ValueError("give mats or world_to_model, not both")
+def _per_frame(what: str, z=None, var_values=None, mats=(), none_ok: bool = False):
+    """The per-frame (per-``what``) arguments of a table builder that are given, checked and converted: ``z`` [n],
+    ``var_values`` [n, k] with k <= FC_MAX_VARS, and each ``(name, value, r)`` of ``mats`` an [n, r, r] stack of
+    matrices -- with ``none_ok`` a sequence whose entries may also be None.  Returns ``(per, n)``: ``per`` maps each
+    given name to its values; lengths that disagree raise ValueError, and with nothing given n is 1."""
     per = {}
     if z is not None:
         per["z"] = np.asarray(z, dtype=np.float32).reshape(-1)
@@ -606,20 +603,41 @@ def frame_table(cfg: RenderConfig2D, z=None, var_values=None, world_to_model=Non
         if vv.ndim != 2 or vv.shape[1] > _lib.FC_MAX_VARS:
             raise ValueError(f"var_values must be [n, k] with k <= {_lib.FC_MAX_VARS}")
         per["var_values"] = vv
-    if world_to_model is not None:
-        wm = np.asarray(world_to_model, dtype=np.float32)
-        if wm.ndim != 3 or wm.shape[1:] != (3, 3):
-            raise ValueError("world_to_model must be [n, 3, 3]")
-        per["world_to_model"] = wm
-    if mats is not None:
-        m = np.asarray(mats, dtype=np.float32)
-        if m.ndim != 3 or m.shape[1:] != (4, 4):
-            raise ValueError("mats must be [n, 4, 4]")
-        per["mats"] = m
+    for name, m, r in mats:
+        if m is None:
+            continue
+        if none_ok:
+            m = [None if w is None else np.asarray(w, dtype=np.float32) for w in m]
+            if any(w is not None and w.shape != (r, r) for w in m):
+                raise ValueError(f"{name} must be [n, {r}, {r}] (an entry may be None: no transform)")
+        else:
+            m = np.asarray(m, dtype=np.float32)
+            if m.ndim != 3 or m.shape[1:] != (r, r):
+                raise ValueError(f"{name} must be [n, {r}, {r}]")
+        per[name] = m
     lengths = {k: len(v) for k, v in per.items()}
     if len(set(lengths.values())) > 1:
-        raise ValueError(f"per-frame arguments disagree in length: {lengths}")
-    n = next(iter(lengths.values())) if lengths else 1
+        raise ValueError(f"per-{what} arguments disagree in length: {lengths}")
+    return per, next(iter(lengths.values()), 1)
+
+
+def _set_vars(rec, values):
+    """``n_var_values`` and ``var_values`` of a C record"""
+    rec.n_var_values = len(values)
+    for i, v in enumerate(values):
+        rec.var_values[i] = float(v)
+
+
+def frame_table(cfg: RenderConfig2D, z=None, var_values=None, world_to_model=None, mats=None):
+    """The ``fc_frame2d`` table of ``render2d_frames``: frame k's matrix, Z and ShapeVars, each exactly what
+    ``render2d`` puts into ``fc_render2d_cfg`` for the config ``cfg`` with that frame's values.  Every argument
+    given is per frame (leading dimension n: ``z`` [n], ``var_values`` [n, k], ``world_to_model`` [n, 3, 3],
+    ``mats`` [n, 4, 4]); the others come from ``cfg``.  Lengths that disagree raise ValueError; with no per-frame
+    argument at all there is one frame.  ``mats`` and ``world_to_model`` are exclusive."""
+    if mats is not None and world_to_model is not None:
+        raise ValueError("give mats or world_to_model, not both")
+    per, n = _per_frame("frame", z=z, var_values=var_values, mats=(("world_to_model", world_to_model, 3),
+                                                                    ("mats", mats, 4)))
     table = (_lib.FcFrame2d * n)()
     base = None if ("mats" in per or "world_to_model" in per) else \
         np.ascontiguousarray(cfg.matrix(), dtype=np.float32).reshape(16).tolist()
@@ -632,10 +650,7 @@ def frame_table(cfg: RenderConfig2D, z=None, var_values=None, world_to_model=Non
         else:
             f.mat[:] = base
         f.z = float(per["z"][k]) if "z" in per else cfg.z
-        values = per["var_values"][k] if "var_values" in per else cfg.var_values
-        f.n_var_values = len(values)
-        for i, v in enumerate(values):
-            f.var_values[i] = float(v)
+        _set_vars(f, per["var_values"][k] if "var_values" in per else cfg.var_values)
     return table
 
 
@@ -707,22 +722,7 @@ def frame_table_3d(cfg: RenderConfig3D, var_values=None, world_to_model=None, ma
     ``world_to_model`` are exclusive."""
     if mats is not None and world_to_model is not None:
         raise ValueError("give mats or world_to_model, not both")
-    per = {}
-    if var_values is not None:
-        vv = np.asarray(var_values, dtype=np.float32)
-        if vv.ndim != 2 or vv.shape[1] > _lib.FC_MAX_VARS:
-            raise ValueError(f"var_values must be [n, k] with k <= {_lib.FC_MAX_VARS}")
-        per["var_values"] = vv
-    for name, m in (("world_to_model", world_to_model), ("mats", mats)):
-        if m is not None:
-            m = np.asarray(m, dtype=np.float32)
-            if m.ndim != 3 or m.shape[1:] != (4, 4):
-                raise ValueError(f"{name} must be [n, 4, 4]")
-            per[name] = m
-    lengths = {k: len(v) for k, v in per.items()}
-    if len(set(lengths.values())) > 1:
-        raise ValueError(f"per-frame arguments disagree in length: {lengths}")
-    n = next(iter(lengths.values())) if lengths else 1
+    per, n = _per_frame("frame", var_values=var_values, mats=(("world_to_model", world_to_model, 4), ("mats", mats, 4)))
     table = (_lib.FcFrame3d * n)()
     base = None if ("mats" in per or "world_to_model" in per) else \
         np.ascontiguousarray(cfg.matrix(), dtype=np.float32).reshape(16).tolist()
@@ -734,10 +734,7 @@ def frame_table_3d(cfg: RenderConfig3D, var_values=None, world_to_model=None, ma
             f.mat[:] = voxel_mat(cfg.width, cfg.height, cfg.depth, per["world_to_model"][k]).reshape(16).tolist()
         else:
             f.mat[:] = base
-        values = per["var_values"][k] if "var_values" in per else cfg.var_values
-        f.n_var_values = len(values)
-        for i, v in enumerate(values):
-            f.var_values[i] = float(v)
+        _set_vars(f, per["var_values"][k] if "var_values" in per else cfg.var_values)
     return table
 
 
@@ -768,18 +765,22 @@ def scene_table(cfg: RenderConfig3D, n: int, var_values=None, world_to_model=Non
     """The ``fc_frame3d`` placement table of ``render3d_scene`` for ``n`` shapes: entry k is what ``frame_table_3d``
     gives for placement k's values (``world_to_model`` [n, 4, 4], ``mats`` [n, 4, 4], ``var_values`` [n, k]).  What is
     not given per placement comes from ``cfg``, for all n; lengths other than n raise ValueError."""
-    per = {name: v for name, v in (("var_values", var_values), ("world_to_model", world_to_model), ("mats", mats))
-           if v is not None}
+    return _scene_table(lambda **per: frame_table_3d(cfg, **per), n, var_values=var_values,
+                        world_to_model=world_to_model, mats=mats)
+
+
+def _scene_table(build, n: int, **given):
+    """The placement table of a scene of n shapes: ``build(**per)`` (``frame_table`` or ``frame_table_3d`` of the
+    scene's config) of the per-placement arguments given, each of length n; with none given, n copies of its one
+    frame."""
+    per = {name: v for name, v in given.items() if v is not None}
     for name, v in per.items():
         if len(v) != n:
             raise ValueError(f"{name} has {len(v)} entries for {n} shapes")
-    if not per:   # every placement is cfg's own view and vars
-        one = frame_table_3d(cfg)[0]
-        table = (_lib.FcFrame3d * n)()
-        for k in range(n):
-            C.memmove(C.byref(table[k]), C.byref(one), C.sizeof(one))
-        return table
-    return frame_table_3d(cfg, **per)
+    if not per:   # every placement is cfg's own view (Z) and vars
+        one = build()[0]
+        return (type(one) * n)(*[one] * n)
+    return build(**per)
 
 
 def render3d_scene(shapes, cfg: RenderConfig3D, var_values=None, world_to_model=None, mats=None, out=None,
@@ -828,18 +829,8 @@ def scene_table_2d(cfg: RenderConfig2D, n: int, z=None, var_values=None, world_t
     """The ``fc_frame2d`` placement table of ``render2d_scene`` for ``n`` shapes: entry k is what ``frame_table`` gives
     for placement k's values (``z`` [n], ``var_values`` [n, k], ``world_to_model`` [n, 3, 3], ``mats`` [n, 4, 4]).  What
     is not given per placement comes from ``cfg``, for all n; lengths other than n raise ValueError."""
-    per = {name: v for name, v in (("z", z), ("var_values", var_values), ("world_to_model", world_to_model),
-                                   ("mats", mats)) if v is not None}
-    for name, v in per.items():
-        if len(v) != n:
-            raise ValueError(f"{name} has {len(v)} entries for {n} shapes")
-    if not per:   # every placement is cfg's own view, Z and vars
-        one = frame_table(cfg)[0]
-        table = (_lib.FcFrame2d * n)()
-        for k in range(n):
-            C.memmove(C.byref(table[k]), C.byref(one), C.sizeof(one))
-        return table
-    return frame_table(cfg, **per)
+    return _scene_table(lambda **per: frame_table(cfg, **per), n, z=z, var_values=var_values,
+                        world_to_model=world_to_model, mats=mats)
 
 
 def scene_colors(colors, n: int) -> np.ndarray:
@@ -907,20 +898,24 @@ OCTREE_LEAF =np.dtype([("ix", np.uint16), ("iy", np.uint16), ("iz", np.uint16), 
                         ("pos", np.float32, (12, 3)), ("grad", np.float32, (12, 4))])
 
 
+def _octree_cfg(depth: int, timing: bool, collapse: bool = False, world_to_model=None, var_values=()):
+    """The ``fc_octree_cfg`` of ``octree_sample``, ``mesh``, ``mesh_frames`` and ``measure``"""
+    c = _lib.FcOctreeCfg()
+    c.depth = depth
+    c.flags = (_lib.FC_FLAG_TIMING if timing else 0) | (_lib.FC_FLAG_MESH_COLLAPSE if collapse else 0)
+    if world_to_model is not None:
+        c.has_transform = 1
+        c.world_to_model[:] = np.ascontiguousarray(world_to_model, dtype=np.float32).reshape(16).tolist()
+    _set_vars(c, var_values)
+    return c
+
+
 def octree_sample(shape: CudaShape, depth: int, world_to_model=None, capacity: int | None = None,
                   stats: bool = False, timing: bool = False, var_values=(), cancel: CancelToken | None = None):
     """Sampler half of ``fidget_mesh::Octree::build`` (octree.rs:521-808): surface leaves with their
     corner mask and per-edge Hermite data, sorted by (iz, iy, ix).  None when ``cancel`` cancelled it."""
     lib = shape._lib
-    c = _lib.FcOctreeCfg()
-    c.depth = depth
-    if world_to_model is not None:
-        c.has_transform = 1
-        c.world_to_model[:] = np.ascontiguousarray(world_to_model, dtype=np.float32).reshape(16).tolist()
-    c.flags = _lib.FC_FLAG_TIMING if timing else 0
-    c.n_var_values = len(var_values)
-    for i, v in enumerate(var_values):
-        c.var_values[i] = float(v)
+    c = _octree_cfg(depth, timing, world_to_model=world_to_model, var_values=var_values)
     cap = capacity if capacity is not None else max(1024, min(8 ** depth, 6 * 4 ** depth))
     st = _lib.FcOctreeStats()
     while True:
@@ -948,46 +943,51 @@ def mesh(shape: CudaShape, depth: int, world_to_model=None, var_values=(), stl: 
     dual is walked over leaves of different depths (``mesh_cells`` then lists the final leaves).  None when
     ``cancel`` cancelled the build (the context then holds no mesh)."""
     lib = shape._lib
-    c = _lib.FcOctreeCfg()
-    c.depth = depth
-    if world_to_model is not None:
-        c.has_transform = 1
-        c.world_to_model[:] = np.ascontiguousarray(world_to_model, dtype=np.float32).reshape(16).tolist()
-    c.flags = _lib.FC_FLAG_TIMING | (_lib.FC_FLAG_MESH_COLLAPSE if collapse else 0)
-    c.n_var_values = len(var_values)
-    for i, v in enumerate(var_values):
-        c.var_values[i] = float(v)
+    c = _octree_cfg(depth, True, collapse, world_to_model=world_to_model, var_values=var_values)
     info = _lib.FcMeshInfo()
     rc = shape.cuda._cancellable(cancel, lambda: lib.fc_mesh_build(shape.cuda._h, shape._h, C.byref(c), C.byref(info)))
     if rc == _lib.FC_ERR_CANCELLED:
         return None
     _ck(rc)
-    verts = np.zeros((info.n_vertices, 3), dtype=np.float32)
-    tris = np.zeros((info.n_triangles, 3), dtype=np.uint32)
-    _ck(lib.fc_mesh_read(shape.cuda._h, _ptr(verts), _ptr(tris)))
-    d = {n: getattr(info, n) for n, _ in info._fields_}
-    if not stl:
-        return verts, tris, d
-    n = C.c_size_t()
-    _ck(lib.fc_mesh_write_stl(shape.cuda._h, None, 0, C.byref(n)))
-    buf = np.zeros(n.value, dtype=np.uint8)
-    _ck(lib.fc_mesh_write_stl(shape.cuda._h, _ptr(buf), n.value, C.byref(n)))
-    return verts, tris, d, buf.tobytes()
+    verts, tris, _, buf = _mesh_read(shape.cuda, info, stl=stl)
+    return (verts, tris, info.as_dict(), buf) if stl else (verts, tris, info.as_dict())
 
 
 MESH_CELL = np.dtype([("ix", np.uint16), ("iy", np.uint16), ("iz", np.uint16), ("depth", np.uint8), ("mask", np.uint8),
                       ("vertex", np.float32, 3)])
 
 
-def mesh_cells(cuda) -> np.ndarray:
-    """Final leaves of the octree of the context's last ``mesh(..., collapse=True)``: depth, cell coordinates at
-    that depth, corner mask and first cell vertex, sorted by (depth, iz, iy, ix).  Empty after a uniform mesh."""
+def _mesh_read(cuda, info, cells: bool = False, stl: bool = False):
+    """The context's mesh of ``info``'s counts: ``(vertices [n, 3], triangles [m, 3], final leaves, binary STL bytes)``,
+    the leaves (in the library's order) with ``cells`` and the STL with ``stl``, else None"""
+    lib = cuda._lib
+    verts = np.zeros((info.n_vertices, 3), dtype=np.float32)
+    tris = np.zeros((info.n_triangles, 3), dtype=np.uint32)
+    _ck(lib.fc_mesh_read(cuda._h, _ptr(verts), _ptr(tris)))
+    buf = None
+    if stl:
+        n = C.c_size_t()
+        _ck(lib.fc_mesh_write_stl(cuda._h, None, 0, C.byref(n)))
+        buf = np.zeros(n.value, dtype=np.uint8)
+        _ck(lib.fc_mesh_write_stl(cuda._h, _ptr(buf), n.value, C.byref(n)))
+        buf = buf.tobytes()
+    return verts, tris, _read_cells(cuda) if cells else None, buf
+
+
+def _read_cells(cuda) -> np.ndarray:
+    """The final leaves of the context's mesh, in the library's order (frame by frame)"""
     lib = cuda._lib
     n = C.c_uint64()
     _ck(lib.fc_mesh_read_cells(cuda._h, None, 0, C.byref(n)))
     out = np.zeros(n.value, dtype=MESH_CELL)
     _ck(lib.fc_mesh_read_cells(cuda._h, _ptr(out), n.value, C.byref(n)))
-    return _sorted_cells(out)
+    return out
+
+
+def mesh_cells(cuda) -> np.ndarray:
+    """Final leaves of the octree of the context's last ``mesh(..., collapse=True)``: depth, cell coordinates at
+    that depth, corner mask and first cell vertex, sorted by (depth, iz, iy, ix).  Empty after a uniform mesh."""
+    return _sorted_cells(_read_cells(cuda))
 
 
 def mesh_frame_table(world_to_model=None, var_values=None):
@@ -997,31 +997,14 @@ def mesh_frame_table(world_to_model=None, var_values=None):
     no values).  A ``world_to_model`` entry of None is a frame without a transform, as ``mesh``'s
     ``world_to_model=None``.  Lengths that disagree raise ValueError, as in ``contour_slice_table``; with no per-frame
     argument at all there is one frame."""
-    per = {}
-    if var_values is not None:
-        vv = np.asarray(var_values, dtype=np.float32)
-        if vv.ndim != 2 or vv.shape[1] > _lib.FC_MAX_VARS:
-            raise ValueError(f"var_values must be [n, k] with k <= {_lib.FC_MAX_VARS}")
-        per["var_values"] = vv
-    if world_to_model is not None:
-        wm = [None if w is None else np.asarray(w, dtype=np.float32) for w in world_to_model]
-        if any(w is not None and w.shape != (4, 4) for w in wm):
-            raise ValueError("world_to_model must be [n, 4, 4] (an entry may be None: no transform)")
-        per["world_to_model"] = wm
-    lengths = {k: len(v) for k, v in per.items()}
-    if len(set(lengths.values())) > 1:
-        raise ValueError(f"per-frame arguments disagree in length: {lengths}")
-    n = next(iter(lengths.values())) if lengths else 1
+    per, n = _per_frame("frame", var_values=var_values, mats=(("world_to_model", world_to_model, 4),), none_ok=True)
     table = (_lib.FcMeshFrame * n)()
     for k in range(n):
         f = table[k]
         if "world_to_model" in per and per["world_to_model"][k] is not None:
             f.has_transform = 1
             f.world_to_model[:] = per["world_to_model"][k].reshape(16).tolist()
-        values = per["var_values"][k] if "var_values" in per else ()
-        f.n_var_values = len(values)
-        for i, v in enumerate(values):
-            f.var_values[i] = float(v)
+        _set_vars(f, per["var_values"][k] if "var_values" in per else ())
     return table
 
 
@@ -1075,9 +1058,7 @@ def mesh_frames(shape: CudaShape, depth: int, world_to_model=None, var_values=No
     lib = shape._lib
     table = mesh_frame_table(world_to_model=world_to_model, var_values=var_values)
     n = len(table)
-    c = _lib.FcOctreeCfg()
-    c.depth = depth
-    c.flags = _lib.FC_FLAG_TIMING | (_lib.FC_FLAG_MESH_COLLAPSE if collapse else 0)
+    c = _octree_cfg(depth, True, collapse)
     info = _lib.FcMeshInfo()
     per = (_lib.FcMeshFrameInfo * n)()
     rc = shape.cuda._cancellable(cancel, lambda: lib.fc_mesh_build_frames(
@@ -1085,28 +1066,15 @@ def mesh_frames(shape: CudaShape, depth: int, world_to_model=None, var_values=No
     if rc == _lib.FC_ERR_CANCELLED:
         return None
     _ck(rc)
-    verts = np.zeros((info.n_vertices, 3), dtype=np.float32)
-    tris = np.zeros((info.n_triangles, 3), dtype=np.uint32)
-    _ck(lib.fc_mesh_read(shape.cuda._h, _ptr(verts), _ptr(tris)))
-    as_dict = lambda x: {f: getattr(x, f) for f, _ in x._fields_}   # noqa: E731
-    per_frame = [as_dict(per[k]) for k in range(n)]
-    all_cells = None
-    if cells:
-        nc = C.c_uint64()
-        _ck(lib.fc_mesh_read_cells(shape.cuda._h, None, 0, C.byref(nc)))
-        all_cells = np.zeros(nc.value, dtype=MESH_CELL)
-        _ck(lib.fc_mesh_read_cells(shape.cuda._h, _ptr(all_cells), nc.value, C.byref(nc)))
+    verts, tris, all_cells, buf = _mesh_read(shape.cuda, info, cells=cells, stl=stl)
+    per_frame = [p.as_dict() for p in per]
     frames = split_mesh_frames(verts, tris, per_frame, all_cells)
     if cells:
         frames = [(v, t, _sorted_cells(cl)) for v, t, cl in frames]
     if stl:
-        nb = C.c_size_t()
-        _ck(lib.fc_mesh_write_stl(shape.cuda._h, None, 0, C.byref(nb)))
-        buf = np.zeros(nb.value, dtype=np.uint8)
-        _ck(lib.fc_mesh_write_stl(shape.cuda._h, _ptr(buf), nb.value, C.byref(nb)))
         files = split_mesh_stl(buf, [p["n_triangles"] for p in per_frame])
         frames = [(f[0], f[1], files[k]) + tuple(f[2:]) for k, f in enumerate(frames)]
-    return frames, as_dict(info), per_frame
+    return frames, info.as_dict(), per_frame
 
 
 # fc_measure_result as a numpy record (one row per frame)
@@ -1132,9 +1100,7 @@ def measure(shape: CudaShape, depth: int, world_to_model=None, var_values=None, 
         var_values = [var_values]
     table = mesh_frame_table(world_to_model=world_to_model, var_values=var_values)
     n = len(table)
-    c = _lib.FcOctreeCfg()
-    c.depth = depth
-    c.flags = _lib.FC_FLAG_TIMING if timing else 0
+    c = _octree_cfg(depth, timing)
     out = np.zeros(n, dtype=MEASURE_RESULT)
     ms = C.c_float()
     rc = shape.cuda._cancellable(cancel, lambda: lib.fc_measure(shape.cuda._h, shape._h, C.byref(c), table, n, _ptr(out),
@@ -1171,11 +1137,16 @@ def contour(shape: CudaShape, depth: int, z: float = 0.0, world_to_model=None, v
     if rc == _lib.FC_ERR_CANCELLED:
         return None
     _ck(rc)
+    return _contour_read(shape.cuda, info) + (info.as_dict(),)
+
+
+def _contour_read(cuda, info):
+    """The context's contour of ``info``'s counts: ``(vertices [n, 2], offsets [k + 1], closed [k] bool)``"""
     verts = np.zeros((info.n_vertices, 2), dtype=np.float32)
     offsets = np.zeros(info.n_polylines + 1, dtype=np.uint32)
     closed = np.zeros(info.n_polylines, dtype=np.uint8)
-    _ck(lib.fc_contour_read(shape.cuda._h, _ptr(verts), _ptr(offsets), _ptr(closed)))
-    return verts, offsets, closed.astype(bool), {n: getattr(info, n) for n, _ in info._fields_}
+    _ck(cuda._lib.fc_contour_read(cuda._h, _ptr(verts), _ptr(offsets), _ptr(closed)))
+    return verts, offsets, closed.astype(bool)
 
 
 def contour_slice_table(z=None, world_to_model=None, var_values=None):
@@ -1186,23 +1157,7 @@ def contour_slice_table(z=None, world_to_model=None, var_values=None):
     transform, as ``contour``'s ``world_to_model=None`` (not the same as the identity flagged as a transform: a
     non-finite z then becomes NaN).  Lengths that disagree raise ValueError, as in
     ``frame_table``; with no per-slice argument at all there is one slice."""
-    per = {}
-    if z is not None:
-        per["z"] = np.asarray(z, dtype=np.float32).reshape(-1)
-    if var_values is not None:
-        vv = np.asarray(var_values, dtype=np.float32)
-        if vv.ndim != 2 or vv.shape[1] > _lib.FC_MAX_VARS:
-            raise ValueError(f"var_values must be [n, k] with k <= {_lib.FC_MAX_VARS}")
-        per["var_values"] = vv
-    if world_to_model is not None:
-        wm = [None if w is None else np.asarray(w, dtype=np.float32) for w in world_to_model]
-        if any(w is not None and w.shape != (3, 3) for w in wm):
-            raise ValueError("world_to_model must be [n, 3, 3] (an entry may be None: no transform)")
-        per["world_to_model"] = wm
-    lengths = {k: len(v) for k, v in per.items()}
-    if len(set(lengths.values())) > 1:
-        raise ValueError(f"per-slice arguments disagree in length: {lengths}")
-    n = next(iter(lengths.values())) if lengths else 1
+    per, n = _per_frame("slice", z=z, var_values=var_values, mats=(("world_to_model", world_to_model, 3),), none_ok=True)
     table = (_lib.FcContourSlice * n)()
     for k in range(n):
         s = table[k]
@@ -1210,10 +1165,7 @@ def contour_slice_table(z=None, world_to_model=None, var_values=None):
         if "world_to_model" in per and per["world_to_model"][k] is not None:
             s.has_transform = 1
             s.world_to_model[:] = per["world_to_model"][k].reshape(9).tolist()
-        values = per["var_values"][k] if "var_values" in per else ()
-        s.n_var_values = len(values)
-        for i, v in enumerate(values):
-            s.var_values[i] = float(v)
+        _set_vars(s, per["var_values"][k] if "var_values" in per else ())
     return table
 
 
@@ -1254,13 +1206,9 @@ def contour_slices(shape: CudaShape, depth: int, z=None, world_to_model=None, va
     if rc == _lib.FC_ERR_CANCELLED:
         return None
     _ck(rc)
-    verts = np.zeros((info.n_vertices, 2), dtype=np.float32)
-    offsets = np.zeros(info.n_polylines + 1, dtype=np.uint32)
-    closed = np.zeros(info.n_polylines, dtype=np.uint8)
-    _ck(lib.fc_contour_read(shape.cuda._h, _ptr(verts), _ptr(offsets), _ptr(closed)))
-    as_dict = lambda x: {f: getattr(x, f) for f, _ in x._fields_}   # noqa: E731
-    per_slice = [as_dict(per[k]) for k in range(n)]
-    return split_contour_stack(verts, offsets, closed, [p["n_polylines"] for p in per_slice]), as_dict(info), per_slice
+    per_slice = [p.as_dict() for p in per]
+    slices = split_contour_stack(*_contour_read(shape.cuda, info), [p["n_polylines"] for p in per_slice])
+    return slices, info.as_dict(), per_slice
 
 
 def contours_svg(vertices, offsets, closed, size: float = 512.0, stroke: str = "black", fill: str = "none",

@@ -131,6 +131,24 @@ class FcMeasureResult(C.Structure):
                 ("bbox_max", C.c_double * 3)]
 
 
+class FcRay(C.Structure):
+    _fields_ = [("origin", C.c_float * 3), ("dir", C.c_float * 3), ("t0", C.c_float), ("dt", C.c_float)]
+
+
+class FcRayHit(C.Structure):
+    _fields_ = [("k", C.c_uint32), ("flags", C.c_uint32), ("t", C.c_float), ("pos", C.c_float * 3), ("value", C.c_float),
+                ("grad", C.c_float * 3)]
+
+
+class FcRaycastCfg(C.Structure):
+    _fields_ = [("steps", C.c_uint32), ("flags", C.c_uint32), ("n_var_values", C.c_uint32), ("var_values", C.c_float * 16)]
+
+
+class FcRaycastInfo(_Record):
+    _fields_ = [("n_hits", C.c_uint64), ("n_proven", C.c_uint64), ("evaluated", C.c_uint64 * 8),
+                ("leaf_samples", C.c_uint64), ("passes", C.c_uint32), ("device_ms", C.c_float)]
+
+
 class FcContourCfg(C.Structure):
     _fields_ = [("depth", C.c_uint32), ("has_transform", C.c_uint32), ("world_to_model", C.c_float * 9), ("z", C.c_float),
                 ("flags", C.c_uint32), ("n_var_values", C.c_uint32), ("var_values", C.c_float * 16)]
@@ -187,6 +205,9 @@ FC_SCENE_MAX_DEPTH = 262142
 FC_SCENE_MAX_ROOT_TILE = 1022
 FC_SCENE_MAX_LEAF_JOBS = 67108863
 FC_SCENE2D_NONE = 0xFFFF
+FC_RAY_MISS = 0xFFFFFFFF
+FC_RAY_PROVEN = 1
+FC_RAY_MAX_STEPS = 1 << 24
 
 # name -> (restype, argtypes); mirrors include/fidget_cuda.h one to one
 _vp, _u32, _i32, _u64, _u8 = C.c_void_p, C.c_uint32, C.c_int32, C.c_uint64, C.c_uint8
@@ -242,6 +263,7 @@ CUDA_API = {
     "fc_mesh_build_frames": (_i32, [_vp, _vp, _P(FcOctreeCfg), _P(FcMeshFrame), _u32, _P(FcMeshInfo),
                                     _P(FcMeshFrameInfo)]),
     "fc_measure": (_i32, [_vp, _vp, _P(FcOctreeCfg), _P(FcMeshFrame), _u32, _vp, _P(C.c_float)]),
+    "fc_raycast": (_i32, [_vp, _vp, _P(FcRaycastCfg), _vp, _u64, _vp, _P(FcRaycastInfo)]),
     "fc_contour_build": (_i32, [_vp, _vp, _P(FcContourCfg), _P(FcContourInfo)]),
     "fc_contour_read": (_i32, [_vp, _vp, _vp, _vp]),
     "fc_contour_build_slices": (_i32, [_vp, _vp, _P(FcContourCfg), _P(FcContourSlice), _u32, _P(FcContourInfo),

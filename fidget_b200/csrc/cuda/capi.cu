@@ -239,8 +239,10 @@ static int32_t cancel_site_of(const std::string& name) {
     static_assert(sizeof(solve) / sizeof(solve[0]) == CS_MEASURE_BRICK - CS_SOLVE, "one name per poll site");
     for (int i = 0; i < CS_MEASURE_BRICK - CS_SOLVE; ++i)
         if (name == solve[i]) return CS_SOLVE + i;
-    static_assert(CS_MEASURE_BRICK + 1 == CS_COUNT, "one name per poll site");
+    static_assert(CS_RAY_HITS + 1 == CS_COUNT, "one name per poll site");
     if (name == "k_measure_brick") return CS_MEASURE_BRICK;
+    if (name == "k_ray_leaf") return CS_RAY_LEAF;
+    if (name == "k_ray_hits") return CS_RAY_HITS;
     return -1;
 }
 

@@ -251,7 +251,7 @@ int32_t transcode(const uint32_t* words, size_t n_words, uint8_t reg_count, uint
 // The refusals every uniform-tree call (octree sample, mesh frames, contours, fc_measure) makes before it begins, locks
 // or allocates: a depth above the tree's limit (FC_MAX_OCTREE_DEPTH for dim 3, FC_MAX_QUADTREE_DEPTH for 2), a null
 // `table` of n > 0 frames or slices, more than FC_MAX_VARS values in one, a tape with memory slots (`what` names the
-// caller), a multi-output tape.  F: fc_mesh_frame or fc_contour_slice.
+// caller), a multi-output tape.  F: fc_mesh_frame or fc_contour_slice (fc_raycast: its cfg, depth 0).
 template <class F>
 int32_t check_tree_call(const fc_tape* tape, int dim, uint32_t depth, const F* table, uint32_t n, const char* what);
 // A frame or slice as the tree kernels take it, its vars bound (bind_vars' refusals).  to_model: map the vertices back

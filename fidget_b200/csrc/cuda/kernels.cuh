@@ -28,6 +28,7 @@ enum CancelSite : int32_t {
     CS_CONTOUR_LEAF, CS_CONTOUR_GRADS, CS_CONTOUR_VERTICES, CS_CONTOUR_SEGMENTS, CS_CONTOUR_LINK, CS_CONTOUR_EMIT,
     CS_SOLVE, CS_SOLVE_LARGE,                             // the solvers: item = problem index (claim and every iteration)
     CS_MEASURE_BRICK,                                     // fc_measure's brick kernel: item = brick
+    CS_RAY_LEAF, CS_RAY_HITS,                             // fc_raycast's leaf (item = segment) and hit (item = warp) kernels
     CS_COUNT
 };
 struct CancelRef {
@@ -285,6 +286,26 @@ struct MeasureBrickParams {
     MeasureAcc* acc;
     CancelRef cancel;
 };
+
+// fc_raycast (ray.cu).  A ray and a hit as fc_ray and fc_ray_hit lay them out.  The interval levels take their lists,
+// arena, tape and vars from LevelParams and the pass from RayPass: a job is a segment of ray x starting at sample y,
+// whose 32 children (seg samples each) are the lanes of one warp; level 0 takes 32 rays per warp, whole.  best[r] is ray
+// r's smallest candidate so far, (k << 1) | proven (0xffffffff: none), lowered with atomicMin.
+struct Ray { float o[3], d[3], t0, dt; };
+struct RayHit { uint32_t k, flags; float t, pos[3], value, grad[3]; };
+struct RayPass {
+    const Ray* rays;
+    RayHit* hits;
+    uint32_t* best;
+    unsigned long long* tally;   // [0] hits, [1] proven hits, [2] samples evaluated by the leaf launch
+    uint32_t n_rays, steps;
+    uint32_t seg;                // samples per segment this launch evaluates (level 0: 32^L, the whole ray)
+};
+void launch_ray_level(const LevelParams& p, const RayPass& r, int blocks, cudaStream_t s);
+// the ambiguous 32-sample segments of list p.level, one warp each (p.jobs_in, p.cap_in, cursor p.level)
+void launch_ray_leaf(const LevelParams& p, const RayPass& r, int blocks, cudaStream_t s);
+void launch_ray_hits(const RayPass& r, const TapeRef& root, const VarBind& vb, const CancelRef& cancel, cudaStream_t s);
+void launch_ray_clear(RayHit* hits, uint64_t n, cudaStream_t s);
 
 #ifdef __CUDACC__
 __device__ __forceinline__ uint32_t root_count(const LevelParams& p, bool with_z) {

@@ -108,6 +108,54 @@ struct MeasureSums {
     }
 };
 
+// The simplification of a warp's ambiguous children (render/mod.rs:96-152: keep the child only if it is shorter): the
+// lanes whose choices (`pk`, packed at `cs` by the interval walk of `tr`) trace something claim one arena slot each and
+// simplify `tr` into it.  Returns this lane's child tape, `tr` itself when it is not simplified or not shorter; `kept`
+// says which.  An exhausted arena sets error bit 0 and keeps every parent tape.  Shared by level_job and the ray
+// levels (ray.cu); the warp calls it together.
+template <bool FUSED>
+__device__ __forceinline__ TapeRef simplify_children(const LevelParams& p, const TapeRef& tr, bool amb, const ChoicePacker& pk,
+                                                     uint32_t* cs, uint32_t (*live)[32], int lane, bool& kept) {
+    TapeRef child = tr;
+    kept = false;
+    const bool need = amb && pk.any_nonboth;
+    const uint32_t mneed = __ballot_sync(FULL, need);
+    if (mneed) {
+        const uint32_t total = __popc(mneed);
+        // worst-case slot per child; in the fused kernel slots are whole 128-byte lines, so that a line
+        // written for one tape is never one an SM may already hold in L1 for another
+        const uint32_t slot_ops = FUSED ? ((tr.n_ops + 15u) & ~15u) : tr.n_ops;
+        unsigned long long base = 0;
+        if (lane == 0) base = atomicAdd(&p.ctr->arena_top, (unsigned long long)total * slot_ops + (FUSED ? 15u : 0u));
+        base = __shfl_sync(FULL, base, 0);
+        if (FUSED) base = (base + 15ull) & ~15ull;   // (the root level's tapes end anywhere)
+        if (base + (unsigned long long)total * slot_ops > p.arena_cap) {
+            if (lane == 0) atomicOr(&p.ctr->error, 1u);
+        } else {
+            const uint32_t rank = __popc(mneed & lanemask_lt());
+            unsigned long long end = base + (unsigned long long)(rank + 1u) * slot_ops;
+            ChoiceUnpacker cu;
+            cu.base = cs;
+            cu.ci = tr.n_choices;
+            uint32_t n_dev, ref_len, nch;
+            simplify_lane<!FUSED>(tr.ptr, tr.n_ops, need, live, lane, cu, p.arena + end, n_dev, ref_len, nch);
+            bool keep = need && ref_len < tr.ref_len;
+            kept = keep;
+            if (keep) {
+                child.ptr = p.arena + (end - n_dev);
+                child.n_ops = n_dev;
+                child.ref_len = ref_len;
+                child.n_choices = nch;
+            }
+            if (p.stats) {
+                uint32_t mk = __ballot_sync(FULL, keep);
+                if (lane == 0 && mk) atomicAdd(&p.stats->simplified[p.level], (unsigned long long)__popc(mk));
+            }
+        }
+    }
+    return child;
+}
+
 // TREE: the samplers' trees whose cells read their view from a ContourSlice table (a MeshFrame is the same record, z
 // unused), not from the render parameters.  DIM 2: the quadtree of
 // fc_contour_build.  Coordinates are cells at the finest depth with world-square bounds coord * cell_h - 1, seen through
@@ -320,44 +368,8 @@ __device__ __forceinline__ void level_job(const LevelParams& p, uint32_t j, uint
             }
         }
 
-        // simplification (render/mod.rs:96-152: keep the child only if it is shorter)
-        TapeRef child = tr;
         bool kept = false;
-        const bool need = amb && pk.any_nonboth;
-        const uint32_t mneed = __ballot_sync(FULL, need);
-        if (mneed) {
-            const uint32_t total = __popc(mneed);
-            // worst-case slot per child; in the fused kernel slots are whole 128-byte lines, so that a line
-            // written for one tape is never one an SM may already hold in L1 for another
-            const uint32_t slot_ops = FUSED ? ((tr.n_ops + 15u) & ~15u) : tr.n_ops;
-            unsigned long long base = 0;
-            if (lane == 0) base = atomicAdd(&p.ctr->arena_top, (unsigned long long)total * slot_ops + (FUSED ? 15u : 0u));
-            base = __shfl_sync(FULL, base, 0);
-            if (FUSED) base = (base + 15ull) & ~15ull;   // (the root level's tapes end anywhere)
-            if (base + (unsigned long long)total * slot_ops > p.arena_cap) {
-                if (lane == 0) atomicOr(&p.ctr->error, 1u);
-            } else {
-                const uint32_t rank = __popc(mneed & lanemask_lt());
-                unsigned long long end = base + (unsigned long long)(rank + 1u) * slot_ops;
-                ChoiceUnpacker cu;
-                cu.base = cs;
-                cu.ci = tr.n_choices;
-                uint32_t n_dev, ref_len, nch;
-                simplify_lane<!FUSED>(tape, tr.n_ops, need, live, lane, cu, p.arena + end, n_dev, ref_len, nch);
-                bool keep = need && ref_len < tr.ref_len;
-                kept = keep;
-                if (keep) {
-                    child.ptr = p.arena + (end - n_dev);
-                    child.n_ops = n_dev;
-                    child.ref_len = ref_len;
-                    child.n_choices = nch;
-                }
-                if (p.stats) {
-                    uint32_t mk = __ballot_sync(FULL, keep);
-                    if (lane == 0 && mk) atomicAdd(&p.stats->simplified[p.level], (unsigned long long)__popc(mk));
-                }
-            }
-        }
+        const TapeRef child = simplify_children<FUSED>(p, tr, amb, pk, cs, live, lane, kept);
 
         if (DIM == 3 && p.census) {   // exact census: what this launch evaluated, judged later against the final heightmap
             const uint32_t mv = __ballot_sync(FULL, valid);

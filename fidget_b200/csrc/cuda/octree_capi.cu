@@ -15,6 +15,7 @@ int32_t check_tree_call(const fc_tape* tape, int dim, uint32_t depth, const F* t
 }
 template int32_t check_tree_call(const fc_tape*, int, uint32_t, const fc_mesh_frame*, uint32_t, const char*);
 template int32_t check_tree_call(const fc_tape*, int, uint32_t, const fc_contour_slice*, uint32_t, const char*);
+template int32_t check_tree_call(const fc_tape*, int, uint32_t, const fc_raycast_cfg*, uint32_t, const char*);
 
 int32_t bind_frame(const fc_tape* tape, uint32_t has_transform, const float* world_to_model, float z, const float* values,
                    uint32_t n_values, MeshFrame& f) {

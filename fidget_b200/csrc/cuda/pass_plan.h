@@ -1,5 +1,5 @@
 // The passes of the batches whose work lists are capped (fc_render3d_frames: frames; fc_render3d_scene: placements;
-// fc_contour_build_slices: slices).  Overflow policy: a pass fails (FC_ERR_ARENA, list overflow) only where one of its
+// fc_contour_build_slices: slices; fc_raycast: rays).  Overflow policy: a pass fails (FC_ERR_ARENA, list overflow) only where one of its
 // items alone would.  The first pass holds one item; later ones are sized from the largest per-item use seen so far
 // (arena clauses, jobs per level, and one more measured quantity of the caller's: census records, surface leaves) with
 // headroom 1.5; a pass that still overflows is run again as two halves (the kernels report overflow, they do not
@@ -59,7 +59,17 @@ struct PassPlan {
         if (!redo.empty()) { const Range r = redo.back(); redo.pop_back(); return r; }
         uint32_t n = std::min(n_max, n_items - next);
         if (!measured) n = 1;
-        else if (forced <= 0) while (n > 1 && !fits(n)) --n;
+        else if (forced <= 0 && !fits(n)) {
+            // the largest pass that fits, by bisection: fits() holds for every size up to some bound and for none above
+            // (the uses and the capped limits grow with n, and a limit at its worst case never binds); one item always
+            // runs
+            uint32_t lo = 1, hi = n;
+            while (hi - lo > 1) {
+                const uint32_t mid = lo + (hi - lo) / 2;
+                (fits(mid) ? lo : hi) = mid;
+            }
+            n = lo;
+        }
         const Range r{next, n};
         next += n;
         return r;

@@ -1112,6 +1112,106 @@ def measure(shape: CudaShape, depth: int, world_to_model=None, var_values=None, 
 
 
 # ---------------------------------------------------------------------------
+# Ray casts: fc_raycast
+RAY = np.dtype([("origin", np.float32, 3), ("dir", np.float32, 3), ("t0", np.float32), ("dt", np.float32)])
+RAY_HIT = np.dtype([("k", np.uint32), ("flags", np.uint32), ("t", np.float32), ("pos", np.float32, 3),
+                    ("value", np.float32), ("grad", np.float32, 3)])
+
+
+def _ray_columns(origins, dirs, t0, dt, n, torch_dev):
+    """The [n, 8] float32 rows of fc_ray (origin, dir, t0, dt), numpy or on the tensors' device"""
+    if torch_dev is not None:
+        import torch
+
+        def col(v):
+            v = torch.as_tensor(v, dtype=torch.float32, device=torch_dev)
+            return (v.reshape(-1) if v.numel() == n else v.reshape(()).expand(n)).reshape(n, 1)
+        return torch.cat([origins.reshape(n, 3).float(), dirs.reshape(n, 3).float(), col(t0), col(dt)], 1).contiguous()
+    rays = np.zeros(n, dtype=RAY)
+    rays["origin"] = np.asarray(origins, dtype=np.float32).reshape(n, 3)
+    rays["dir"] = np.asarray(dirs, dtype=np.float32).reshape(n, 3)
+    rays["t0"] = np.broadcast_to(np.asarray(t0, dtype=np.float32).reshape(-1), (n,))
+    rays["dt"] = np.broadcast_to(np.asarray(dt, dtype=np.float32).reshape(-1), (n,))
+    return rays
+
+
+def raycast(shape: CudaShape, origins, dirs, t0, dt, steps: int, var_values=(), cancel: CancelToken | None = None,
+            timing: bool = False):
+    """The first inside sample of each ray (``fc_raycast``): ray i samples ``origins[i] + t_k * dirs[i]`` at
+    ``t_k = t0 + k * dt``, k < ``steps``, in model space, f32 with one rounding per operation.  ``origins`` and ``dirs``
+    are [n, 3]; ``t0`` and ``dt`` scalars or [n].  numpy inputs give numpy outputs; CUDA torch tensors stay on the device
+    and give tensors there.  Returns ``(k, t, pos, value, grad, proven, info)``: k (``FC_RAY_MISS`` = 0xFFFFFFFF for a
+    miss, as int64 for tensors), t, pos [n, 3], the root tape's value and gradient [n, 3] at pos, proven (the hit is
+    the first sample of an interval-proven-inside segment) and the info dict of ``fc_raycast_info``.  ``var_values``
+    bind the tape's other inputs (ShapeVars).  None when ``cancel`` cancelled the call."""
+    lib = shape._lib
+    torch_dev = origins.device if hasattr(origins, "data_ptr") and getattr(origins, "is_cuda", False) else None
+    n = int(origins.shape[0]) if hasattr(origins, "shape") else len(origins)
+    rays = _ray_columns(origins, dirs, t0, dt, n, torch_dev)
+    if torch_dev is not None:
+        import torch
+        hits = torch.empty((n, 10), dtype=torch.float32, device=torch_dev)
+        torch.cuda.synchronize(torch_dev)   # (the rays are built on torch's stream; the call runs on the context's)
+    else:
+        hits = np.zeros(n, dtype=RAY_HIT)
+    c = _lib.FcRaycastCfg()
+    c.steps = steps
+    c.flags = _lib.FC_FLAG_TIMING if timing else 0
+    _set_vars(c, var_values)
+    info = _lib.FcRaycastInfo()
+    rc = shape.cuda._cancellable(cancel, lambda: lib.fc_raycast(shape.cuda._h, shape._h, C.byref(c), _ptr(rays), n,
+                                                                _ptr(hits), C.byref(info)))
+    if rc == _lib.FC_ERR_CANCELLED:
+        return None
+    _ck(rc)
+    if torch_dev is not None:
+        import torch
+        words = hits.view(torch.int32)
+        k = words[:, 0].to(torch.int64) & 0xFFFFFFFF
+        proven = (words[:, 1] & _lib.FC_RAY_PROVEN) != 0
+        return k, hits[:, 2], hits[:, 3:6], hits[:, 6], hits[:, 7:10], proven, info.as_dict()
+    return (hits["k"], hits["t"], hits["pos"], hits["value"], hits["grad"], (hits["flags"] & _lib.FC_RAY_PROVEN) != 0,
+            info.as_dict())
+
+
+def pick_rays(cfg: RenderConfig3D, pixels):
+    """The model-space rays of ``pick``: for screen pixel (x, y), origin = the voxel (x, y, depth - 1) under
+    ``cfg.matrix()`` (f32, as the renderer maps voxels: ((m0 x + m1 y) + m2 z) + m3), dir = minus the matrix's Z column,
+    t0 = 0, dt = 1, so that sample k lies on voxel (x, y, depth - 1 - k).  Returns ``(origins [n, 3], dirs [n, 3])``;
+    ValueError for a projective matrix (last row other than 0 0 0 1)."""
+    m = np.asarray(cfg.matrix(), dtype=np.float32).reshape(4, 4)
+    if not np.array_equal(m[3], np.array([0, 0, 0, 1], dtype=np.float32)):
+        raise ValueError("pick needs an affine view (the matrix's last row 0 0 0 1)")
+    px = np.asarray(pixels).reshape(-1, 2)
+    x, y = px[:, 0].astype(np.float32), px[:, 1].astype(np.float32)
+    z = np.float32(cfg.depth - 1)
+    origins = np.stack([((m[i, 0] * x + m[i, 1] * y) + m[i, 2] * z) + m[i, 3] for i in range(3)], 1).astype(np.float32)
+    dirs = np.broadcast_to(-m[:3, 2], origins.shape).astype(np.float32)
+    return origins, dirs
+
+
+def pick(shape: CudaShape, cfg: RenderConfig3D, pixels, cancel: CancelToken | None = None):
+    """What lies under screen pixels (x, y) of a 3D view (``pixels`` [n, 2]): each pixel's ray runs down its voxel column
+    from z = depth - 1 to 0 (``pick_rays``, ``steps`` = depth) through ``fc_raycast``.  Returns ``(depth, pos, normal)``:
+    the depth ``fc_render3d`` stores for the pixel (depth - k for a hit at sample k, 0 for a miss, and with
+    ``cfg.clamp`` depth for anything at depth - 1 or above, voxel.rs:535-546), the model-space position of the hit and
+    the root tape's model-space gradient there (0 for a miss).  Affine views only.  The samples are the renderer's voxel
+    positions bit for bit, and the depth equals ``render3d``'s, when every coordinate is exact in f32: an identity
+    view (no ``world_to_model``) of power-of-two sizes.  Other views sample the same column up to rounding.  None when
+    ``cancel`` cancelled the call."""
+    origins, dirs = pick_rays(cfg, pixels)
+    r = raycast(shape, origins, dirs, 0.0, 1.0, cfg.depth, var_values=cfg.var_values, cancel=cancel)
+    if r is None:
+        return None
+    k, _, pos, _, grad, _, _ = r
+    hit = k != _lib.FC_RAY_MISS
+    depth = np.where(hit, np.uint32(cfg.depth) - np.where(hit, k, 0), 0).astype(np.uint32)
+    if cfg.clamp:
+        depth = np.where(depth >= cfg.depth - 1, cfg.depth, depth).astype(np.uint32)
+    return depth, pos, grad
+
+
+# ---------------------------------------------------------------------------
 # 2D contours (libfive's Contours::render): fc_contour_build / fc_contour_read
 def contour(shape: CudaShape, depth: int, z: float = 0.0, world_to_model=None, var_values=(),
             cancel: CancelToken | None = None):

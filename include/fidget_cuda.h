@@ -65,7 +65,7 @@ int32_t fc_ctx_set_arena_bytes(fc_ctx* ctx, uint64_t bytes);
  * layout of Rust's AtomicBool (CancelToken::into_raw() as *const u8): nonzero = cancelled.  The library reads it with
  * an acquire load, from any thread; NULL detaches it.  Context-wide, like fc_ctx_set_stream, and consulted only by
  * fc_render2d, fc_render2d_frames, fc_render2d_scene, fc_render3d, fc_render3d_frames, fc_render3d_scene, fc_octree_sample,
- * fc_mesh_build, fc_mesh_build_frames, fc_contour_build, fc_solve_batch, fc_solve_large_batch, and
+ * fc_mesh_build, fc_mesh_build_frames, fc_contour_build, fc_raycast, fc_solve_batch, fc_solve_large_batch, and
  * fc_ctx_synchronize after the most recent FC_FLAG_ASYNC call of those.  With a flag attached:
  *  - set on entry: the call returns FC_ERR_CANCELLED before it allocates or launches anything;
  *  - set while the call runs: the kernels stop claiming work and the call returns FC_ERR_CANCELLED ("cancelled" in
@@ -603,6 +603,72 @@ typedef struct fc_measure_result {
 int32_t fc_measure(fc_ctx* ctx, const fc_tape* tape, const fc_octree_cfg* cfg /* depth, flags */,
                    const fc_mesh_frame* frames /* host */, uint32_t n_frames, fc_measure_result* out /* host */,
                    float* device_ms /* FC_FLAG_TIMING, may be NULL */);
+
+/* ---- Ray casts: the first inside sample along each ray --------------------------------------------------------------
+ * fc_raycast answers, for each of n_rays rays, where the ray first enters the shape (picking, line of sight, depth
+ * sensors, placing a point on a surface).  Ray r has `steps` samples k = 0 .. steps - 1, each computed in f32 with one
+ * round-to-nearest per operation, in model space (no transform):
+ *     t_k = t0 + float(k) * dt,    x_k = origin + t_k * dir   (per axis)
+ * With dt > 0 each of these steps is monotone in k (t_k non-decreasing; t * d non-decreasing or non-increasing in t by
+ * the sign of d; o + s non-decreasing in s), so on every axis the samples of a segment [a, b] lie between x_a and x_b:
+ * the box spanned by a segment's two end samples encloses every sample in it.  Which samples count is fixed by the
+ * descent:
+ *  - L = max(1, ceil(log2(steps) / 5)) interval levels l = 0 .. L - 1 of segments 32^(L - l) samples long, clipped to
+ *    [0, steps): level 0 is the whole ray, and every ambiguous segment splits into 32 children (children that start at
+ *    or past `steps` are not evaluated);
+ *  - a segment is classified by the interval value over its box, with its own tape, as the tile renderers classify
+ *    tiles: upper < 0 proves it inside, and its first sample is a candidate hit (FC_RAY_PROVEN); lower > 0 drops it;
+ *    anything else, NaN included, splits it, and its children take the tape simplified by its choices when that tape is
+ *    shorter (render/mod.rs:96-152);
+ *  - every ambiguous segment of level L - 1 (32 samples) evaluates its samples with its tape: a value < 0 is a
+ *    candidate hit.
+ * The hit is the smallest candidate k.  Segments that start at or past a ray's best candidate so far are skipped, which
+ * changes the speed only: the result depends on the descent alone, not on the launch grid, the passes or the order of
+ * the work.  For tapes of IEEE operations an interval never contradicts a point value in its box, so k is the first
+ * sample whose f32 value is < 0.  For each hit, value and grad are the ROOT tape at pos: value bit for bit what
+ * fc_float_slice_eval gives there, grad (d/dx, d/dy, d/dz) what fc_grad_slice_eval gives.  A miss has k = FC_RAY_MISS
+ * and every other field 0.
+ *  - rays and hits: host or device.  cfg->var_values bind the tape's other inputs (ShapeVars), one binding per call.
+ *  - info (may be NULL): hits, those proven by an interval, the segments evaluated per level, the samples evaluated by
+ *    the leaf launch, the passes run, and with FC_FLAG_TIMING the device time summed over passes.
+ *  - passes: rays run in passes; the first pass holds one ray, later ones are sized from the largest per-ray arena and
+ *    job-list use seen so far, and a pass that overflows anyway is run again in halves: FC_ERR_ARENA or a work-list
+ *    overflow comes back only where one ray alone gives it.
+ *  - Checked before anything is allocated or launched (device rays are first read back, in the order of the context's
+ *    stream): steps of 0 or above FC_RAY_MAX_STEPS, a ray with a non-finite
+ *    origin, dir, t0 or dt, dt <= 0 or a non-finite t at its last sample, a multi-output tape, more than FC_MAX_VARS
+ *    values or a missing value for a bound variable, NULL cfg, rays or hits with n_rays > 0: FC_ERR_INVALID; a tape
+ *    with memory slots: FC_ERR_UNSUPPORTED.  n_rays == 0 launches nothing and returns FC_OK.
+ *  - The cancel flag behaves as in fc_mesh_build.  A cancelled or failed call leaves every hit a miss, and the context
+ *    stays usable. */
+#define FC_RAY_MISS 0xFFFFFFFFu
+#define FC_RAY_PROVEN 1u
+#define FC_RAY_MAX_STEPS 16777216u   /* 2^24 */
+typedef struct fc_ray {
+    float origin[3], dir[3];        /* model space */
+    float t0, dt;                   /* t_k = t0 + k dt, dt > 0 */
+} fc_ray;
+typedef struct fc_ray_hit {
+    uint32_t k;                     /* index of the hit sample, FC_RAY_MISS if none */
+    uint32_t flags;                 /* FC_RAY_PROVEN: the hit is the first sample of an interval-proven-inside segment */
+    float t, pos[3];                /* t_k and x_k */
+    float value, grad[3];           /* the root tape at pos: value, d/dx, d/dy, d/dz */
+} fc_ray_hit;
+typedef struct fc_raycast_cfg {
+    uint32_t steps;                 /* samples per ray, 1 .. FC_RAY_MAX_STEPS */
+    uint32_t flags;                 /* FC_FLAG_TIMING */
+    uint32_t n_var_values;          /* ShapeVars, as fc_octree_cfg */
+    float var_values[FC_MAX_VARS];
+} fc_raycast_cfg;
+typedef struct fc_raycast_info {
+    uint64_t n_hits, n_proven;
+    uint64_t evaluated[8];          /* segments evaluated per interval level */
+    uint64_t leaf_samples;          /* samples evaluated by the leaf launch */
+    uint32_t passes;
+    float device_ms;                /* FC_FLAG_TIMING */
+} fc_raycast_info;
+int32_t fc_raycast(fc_ctx* ctx, const fc_tape* tape, const fc_raycast_cfg* cfg, const fc_ray* rays /* host or device */,
+                   uint64_t n_rays, fc_ray_hit* hits /* host or device */, fc_raycast_info* info /* may be NULL */);
 
 /* ---- 2D contours (libfive's Contours::render, on the quadtree the mesher's octree restricts to) -------------------
  * fc_contour_build extracts the contours of a 2D shape (a sketch, a cut profile, a Z slice of a 3D model) as closed or

@@ -379,12 +379,26 @@ static int32_t bind_frame(const fc_tape* tape, const F& f, float z, Frame2D& out
     return bind_vars(tape, f.var_values, f.n_var_values, out.vb);
 }
 
-// Validation and tile grid shared by fc_render2d and fc_render2d_frames
-static int32_t check_2d(const fc_tape* tape, const fc_render2d_cfg* cfg) {
-    if (cfg->width == 0 || cfg->height == 0) return fail(FC_ERR_INVALID, "empty image");
+// the tapes no renderer takes
+static int32_t check_render_tape(const fc_tape* tape) {
     if (tape->info.mem_count) return fail(FC_ERR_UNSUPPORTED, "renderers need a tape without memory spills (<= 255 registers)");
     if (tape->info.n_outputs != 1) return fail(FC_ERR_INVALID, "ShapeTape has multiple outputs");
     return FC_OK;
+}
+
+// The settings of fc_render2d that the 2D batches refuse; `what` names the batch ("frame batches", "scenes")
+static int32_t check_batch_2d(const fc_render2d_cfg* cfg, const std::string& what) {
+    if (cfg->flags & FC_FLAG_FUSED_TAIL) return fail(FC_ERR_UNSUPPORTED, "FC_FLAG_FUSED_TAIL is not supported by " + what);
+    if (cfg->root_row_begin || cfg->root_row_end) return fail(FC_ERR_UNSUPPORTED, "root row bands are not supported by " + what);
+    if (cfg->root_stride > 1) return fail(FC_ERR_UNSUPPORTED, "the tile interleave is not supported by " + what);
+    if (cfg->out_format > FC_OUT_RGBA8) return fail(FC_ERR_INVALID, "unknown out_format");
+    return FC_OK;
+}
+
+// Validation and tile grid shared by fc_render2d and fc_render2d_frames
+static int32_t check_2d(const fc_tape* tape, const fc_render2d_cfg* cfg) {
+    if (cfg->width == 0 || cfg->height == 0) return fail(FC_ERR_INVALID, "empty image");
+    return check_render_tape(tape);
 }
 static int32_t prepare_2d(fc_ctx* c, const fc_tape* tape, const fc_render2d_cfg* cfg, Tiles2D& g) {
     static const uint32_t DFLT[3] = {128, 32, 8};
@@ -455,6 +469,61 @@ static int32_t abandon_frames(fc_ctx* c, cudaStream_t s, fc_render_stats* stats,
     return rc;
 }
 
+// ---- passes of the 2D batches (fc_render2d_frames: frames; fc_render2d_scene: shapes) ----
+// Items per pass: an item's worst-case lists over its n_roots root tiles, at job_bytes per job, plus its extra_bytes,
+// within FC_FRAMES_PASS_BYTES (at least one item); FIDGET_B200_FRAMES_PER_PASS forces the count
+static int32_t passes_2d(const std::vector<uint32_t>& ts, uint64_t n_roots, uint32_t n_items, uint64_t job_bytes,
+                         uint64_t extra_bytes, uint32_t& per_pass, uint32_t& n_passes) {
+    std::vector<uint64_t> item_tiles;
+    if (int32_t rc = size_lists_2d(ts, n_roots, item_tiles)) return rc;
+    uint64_t per_item = extra_bytes;
+    for (size_t l = 1; l < item_tiles.size(); ++l) per_item += item_tiles[l] * job_bytes;
+    per_pass = uint32_t(std::min<uint64_t>(n_items, std::max<uint64_t>(1, FC_FRAMES_PASS_BYTES / per_item)));
+    if (const int forced = env_int("FIDGET_B200_FRAMES_PER_PASS", 0); forced > 0) per_pass = std::min<uint32_t>(n_items, forced);
+    n_passes = (n_items + per_pass - 1) / per_pass;
+    return FC_OK;
+}
+// a new pass: fresh lists, cursors and arena; error bits accumulate over the call
+static int32_t reset_pass_2d(fc_ctx* c, cudaStream_t s) {
+    CU(cudaMemsetAsync(c->counters.p, 0, offsetof(Counters, error), s));
+    CU(cudaMemsetAsync(&c->counters.as<Counters>()->arena_top, 0, sizeof(unsigned long long), s));
+    return FC_OK;
+}
+// pass k's arena high-water mark, into frame_tops[k] for the call's stats
+static int32_t record_top_2d(fc_ctx* c, cudaStream_t s, uint32_t k) {
+    CU(cudaMemcpyAsync(c->frame_tops.as<unsigned long long>() + k, &c->counters.as<Counters>()->arena_top,
+                       sizeof(unsigned long long), cudaMemcpyDeviceToDevice, s));
+    return FC_OK;
+}
+// With a flag attached, the wait that ends a 2D batch that enqueued passes_run of its n_passes passes: FC_ERR_CANCELLED,
+// stats zeroed, if the flag cancelled it
+static int32_t wait_cancel_2d(fc_ctx* c, cudaStream_t s, const CallCancel& cc, uint32_t passes_run, uint32_t n_passes,
+                              fc_render_stats* stats) {
+    if (!cc.flag) return FC_OK;
+    int32_t rc = wait_call(c, s, cc);
+    // (passes_run < n_passes: the flag stopped the passes, but was cleared before the wait saw it)
+    if (!rc && passes_run < n_passes) rc = fail(FC_ERR_CANCELLED, "cancelled");
+    if (rc && stats) memset(stats, 0, sizeof *stats);
+    return rc;
+}
+// The end of a 2D batch of n_passes passes (L + 3 timing events each): the device's error bits and the stats, with the
+// largest arena high-water mark of frame_tops
+static int32_t finish_2d(fc_ctx* c, cudaStream_t s, int L, uint32_t n_passes, bool timing, uint32_t launches,
+                         fc_render_stats* stats) {
+    CU(cudaStreamSynchronize(s));
+    int32_t rc = check_device_errors(c);
+    if (stats) {
+        Stats h;
+        std::vector<unsigned long long> tops(n_passes);
+        CU(cudaMemcpy(&h, c->stats.p, sizeof h, cudaMemcpyDeviceToHost));
+        CU(cudaMemcpy(tops.data(), c->frame_tops.p, tops.size() * sizeof(unsigned long long), cudaMemcpyDeviceToHost));
+        write_stats(stats, h, false, *std::max_element(tops.begin(), tops.end()), launches);
+        if (timing)
+            for (uint32_t k = 0; k < n_passes; ++k) add_stage_ms_2d(c, size_t(k) * (L + 3), L, false, h, stats->stage_ms);
+    }
+    return rc;
+}
+
 // the small formats, derived on the device from `rows` rows of distance image
 static void derive_format(uint32_t fmt, const float* dimg, uint32_t width, uint32_t rows, uint8_t* dst, cudaStream_t s) {
     if (fmt == FC_OUT_RGBA8) launch_to_rgba(0, dimg, uint64_t(width) * rows, dst, s);
@@ -489,8 +558,13 @@ struct Tiles3D {
 
 static int32_t check_3d(const fc_tape* tape, const fc_render3d_cfg* cfg) {
     if (cfg->width == 0 || cfg->height == 0 || cfg->depth == 0) return fail(FC_ERR_INVALID, "empty volume");
-    if (tape->info.mem_count) return fail(FC_ERR_UNSUPPORTED, "renderers need a tape without memory spills (<= 255 registers)");
-    if (tape->info.n_outputs != 1) return fail(FC_ERR_INVALID, "ShapeTape has multiple outputs");
+    return check_render_tape(tape);
+}
+// The settings of fc_render3d that the 3D batches refuse; `what` names the batch ("frame batches", "scenes")
+static int32_t check_batch_3d(const fc_render3d_cfg* cfg, const std::string& what) {
+    if (cfg->z_begin || cfg->z_end) return fail(FC_ERR_UNSUPPORTED, "Z slabs are not supported by " + what);
+    if (cfg->root_row_begin || cfg->root_row_end) return fail(FC_ERR_UNSUPPORTED, "root row bands are not supported by " + what);
+    if (cfg->root_stride > 1) return fail(FC_ERR_UNSUPPORTED, "the tile interleave is not supported by " + what);
     return FC_OK;
 }
 // tile ladder, launch widths, choice scratch words and the occlusion map's shape
@@ -807,6 +881,13 @@ static int32_t ensure_pass_pin(fc_ctx* c) {
     if (!c->pass_pin) CU(cudaHostAlloc(reinterpret_cast<void**>(&c->pass_pin), 2 * sizeof(PassStatus), cudaHostAllocDefault));
     return FC_OK;
 }
+// the finished pass's counters and (want_stats) stats, into pinned slot `slot` on s
+static int32_t read_pass_status(fc_ctx* c, cudaStream_t s, int slot, bool want_stats) {
+    PassStatus* hs = c->pass_pin + slot;
+    CU(cudaMemcpyAsync(&hs->ctr, c->counters.p, sizeof(Counters), cudaMemcpyDeviceToHost, s));
+    if (want_stats) CU(cudaMemcpyAsync(&hs->st, c->stats.p, sizeof(Stats), cudaMemcpyDeviceToHost, s));
+    return FC_OK;
+}
 
 extern "C" {
 
@@ -923,11 +1004,8 @@ int32_t fc_render2d_frames(fc_ctx* c, const fc_tape* tape, const fc_render2d_cfg
                            uint32_t n_frames, void* out, fc_render_stats* stats) {
     if (!c || !tape || !cfg || !out || (n_frames && !frames)) return fail(FC_ERR_INVALID, "null argument");
     if (int32_t vrc = check_2d(tape, cfg)) return vrc;
-    if (cfg->flags & FC_FLAG_FUSED_TAIL) return fail(FC_ERR_UNSUPPORTED, "FC_FLAG_FUSED_TAIL is not supported by frame batches");
-    if (cfg->root_row_begin || cfg->root_row_end) return fail(FC_ERR_UNSUPPORTED, "root row bands are not supported by frame batches");
-    if (cfg->root_stride > 1) return fail(FC_ERR_UNSUPPORTED, "the tile interleave is not supported by frame batches");
+    if (int32_t vrc = check_batch_2d(cfg, "frame batches")) return vrc;
     const uint32_t fmt = cfg->out_format;
-    if (fmt > FC_OUT_RGBA8) return fail(FC_ERR_INVALID, "unknown out_format");
     // every frame's ShapeVars binding, before anything is allocated or launched
     std::vector<Frame2D> table(n_frames);
     for (uint32_t k = 0; k < n_frames; ++k)
@@ -950,19 +1028,16 @@ int32_t fc_render2d_frames(fc_ctx* c, const fc_tape* tape, const fc_render2d_cfg
     const bool out_dev = is_device_ptr(out);
     cudaStream_t s = c->stream;
 
-    // ---- frames per pass: the worst-case lists of a frame plus its staged images, within FC_FRAMES_PASS_BYTES ----
-    std::vector<uint64_t> frame_tiles;
-    if (int32_t src = size_lists_2d(g.ts, uint64_t(g.roots_x) * roots_y, frame_tiles)) return src;
-    uint64_t per_frame = 0;
-    for (int l = 1; l <= L; ++l) per_frame += frame_tiles[l] * (sizeof(TileJob) + sizeof(FillRec));
+    // ---- frames per pass: the worst-case lists of a frame (jobs and fills) plus its staged images ----
     const size_t img_f32 = size_t(W) * H * 4, img_fmt = format_bytes(fmt, W, H);
     const bool stage_f32 = fmt != FC_OUT_F32 || !out_dev;             // the distance images live in the context
     const int f32_bufs = fmt == FC_OUT_F32 ? 2 : 1;                    // (a host F32 copy-back is double-buffered)
-    if (stage_f32) per_frame += uint64_t(img_f32) * f32_bufs;
-    if (fmt != FC_OUT_F32 && !out_dev) per_frame += 2ull * img_fmt;    // double-buffered derived images
-    uint32_t per_pass = uint32_t(std::min<uint64_t>(n_frames, std::max<uint64_t>(1, FC_FRAMES_PASS_BYTES / per_frame)));
-    if (const int forced = env_int("FIDGET_B200_FRAMES_PER_PASS", 0); forced > 0) per_pass = std::min<uint32_t>(n_frames, forced);
-    const uint32_t n_passes = (n_frames + per_pass - 1) / per_pass;
+    const uint64_t staged = (stage_f32 ? uint64_t(img_f32) * f32_bufs : 0) +
+                            (fmt != FC_OUT_F32 && !out_dev ? 2ull * img_fmt : 0);   // double-buffered derived images
+    uint32_t per_pass, n_passes;
+    if (int32_t prc = passes_2d(g.ts, uint64_t(g.roots_x) * roots_y, n_frames, sizeof(TileJob) + sizeof(FillRec), staged,
+                                per_pass, n_passes))
+        return prc;
 
     g.roots_y = roots_y * per_pass;
     g.n_roots = uint64_t(g.roots_x) * g.roots_y;
@@ -989,30 +1064,28 @@ int32_t fc_render2d_frames(fc_ctx* c, const fc_tape* tape, const fc_render2d_cfg
     if (want_stats) CU(cudaMemsetAsync(c->stats.p, 0, sizeof(Stats), s));
 
     // host `out`: pass k's images go back on the copy stream while pass k + 1 runs (issued after pass k + 1 is
-    // enqueued, so that a copy into pageable memory, which blocks the host, still overlaps the next pass)
+    // enqueued, so that a copy into pageable memory, which blocks the host, still overlaps the next pass).  The work
+    // stream waits for the copy from then on: pass k + 2 reuses staging buffer k & 1, and the call ends with its last copy.
     auto copy_back = [&](uint32_t k) -> int32_t {
         const uint32_t f0 = k * per_pass, n = std::min(per_pass, n_frames - f0);
         const size_t fb = fmt == FC_OUT_F32 ? img_f32 : img_fmt;
         const void* src = fmt == FC_OUT_F32 ? static_cast<const void*>(stage[k & 1]) : static_cast<const void*>(fstage[k & 1]);
         if (int32_t wrc = wait_pass(c, int(k & 1), cc, false)) return wrc;   // (a cancelled pass copies nothing)
-        return copy_pass_back(c, int(k & 1), static_cast<uint8_t*>(out) + size_t(f0) * fb, src, size_t(n) * fb);
+        if (int32_t crc = copy_pass_back(c, int(k & 1), static_cast<uint8_t*>(out) + size_t(f0) * fb, src, size_t(n) * fb))
+            return crc;
+        CU(cudaStreamWaitEvent(s, c->ev_copied[k & 1], 0));
+        return FC_OK;
     };
-    auto abandon = [&](int32_t rc) { return abandon_frames(c, s, stats, rc); };
     VarBind vb0 = table[0].vb;   // (unused by the kernels: every frame comes from the table)
     size_t ev = 0;
-    uint32_t launches = 0, passes_run = 0;
-    for (uint32_t k = 0; k < n_passes; ++k) {
-        if (k && cc.flag && __atomic_load_n(cc.flag, __ATOMIC_ACQUIRE)) break;   // cancelled: enqueue no further pass
+    uint32_t launches = 0;
+    auto enqueue = [&](uint32_t k) -> int32_t {
         const uint32_t f0 = k * per_pass, n = std::min(per_pass, n_frames - f0);
         Tiles2D gp = g;
         gp.roots_y = roots_y * n;
         gp.n_roots = uint64_t(g.roots_x) * gp.roots_y;
         gp.frames = c->frame_table.as<Frame2D>() + f0;
-        if (k) {   // a new pass: fresh lists, cursors and arena; error bits accumulate over the call
-            CU(cudaMemsetAsync(c->counters.p, 0, offsetof(Counters, error), s));
-            CU(cudaMemsetAsync(&c->counters.as<Counters>()->arena_top, 0, sizeof(unsigned long long), s));
-        }
-        if (!out_dev && k >= 2) CU(cudaStreamWaitEvent(s, c->ev_copied[k & 1], 0));   // staging buffer k & 1 is free again
+        if (k) if (int32_t rrc = reset_pass_2d(c, s)) return rrc;
         float* dimg = stage_f32 ? stage[k & 1] : static_cast<float*>(out) + size_t(f0) * W * H;
         bool fused = false;
         if (int32_t erc = enqueue_tiles_2d(c, tape, cfg, gp, vb0, dimg, want_stats, timing, cc, s, ev, launches, fused))
@@ -1023,46 +1096,25 @@ int32_t fc_render2d_frames(fc_ctx* c, const fc_tape* tape, const fc_render2d_cfg
             ++launches;
             CU(cudaGetLastError());
         }
-        if (want_stats)
-            CU(cudaMemcpyAsync(c->frame_tops.as<unsigned long long>() + k, &c->counters.as<Counters>()->arena_top,
-                               sizeof(unsigned long long), cudaMemcpyDeviceToDevice, s));
+        if (want_stats) if (int32_t trc = record_top_2d(c, s, k)) return trc;
+        if (!out_dev) CU(cudaEventRecord(c->ev_pass[k & 1], s));
+        return FC_OK;
+    };
+    auto abandon = [&](int32_t rc) { return abandon_frames(c, s, stats, rc); };
+    uint32_t passes_run = 0;
+    for (uint32_t k = 0; k < n_passes; ++k) {
+        if (k && cc.flag && __atomic_load_n(cc.flag, __ATOMIC_ACQUIRE)) break;   // cancelled: enqueue no further pass
+        if (int32_t erc = enqueue(k)) return abandon(erc);
         ++passes_run;
-        if (!out_dev) {
-            CU(cudaEventRecord(c->ev_pass[k & 1], s));
-            if (k) if (int32_t crc = copy_back(k - 1)) return abandon(crc);
-        }
+        if (!out_dev && k) if (int32_t crc = copy_back(k - 1)) return abandon(crc);
     }
-    if (!out_dev) {
-        if (int32_t crc = copy_back(passes_run - 1)) return abandon(crc);
-        CU(cudaStreamWaitEvent(s, c->ev_copied[(passes_run - 1) & 1], 0));   // the call ends when its last copy does
-    }
-    const bool early_return = async && out_dev && !want_stats;
-    if (early_return) {
+    if (!out_dev) if (int32_t crc = copy_back(passes_run - 1)) return abandon(crc);
+    if (async && out_dev && !want_stats) {
         c->async_call = cc;
         return FC_OK;
     }
-    if (cc.flag) {
-        if (int32_t wrc = wait_call(c, s, cc)) {
-            if (stats) memset(stats, 0, sizeof *stats);
-            return wrc;
-        }
-        if (passes_run < n_passes) {   // the flag stopped the passes, but was cleared before the wait saw it
-            if (stats) memset(stats, 0, sizeof *stats);
-            return fail(FC_ERR_CANCELLED, "cancelled");
-        }
-    }
-    CU(cudaStreamSynchronize(s));
-    int32_t rc = check_device_errors(c);
-    if (stats) {
-        Stats h;
-        std::vector<unsigned long long> tops(n_passes);
-        CU(cudaMemcpy(&h, c->stats.p, sizeof h, cudaMemcpyDeviceToHost));
-        CU(cudaMemcpy(tops.data(), c->frame_tops.p, tops.size() * sizeof(unsigned long long), cudaMemcpyDeviceToHost));
-        write_stats(stats, h, false, *std::max_element(tops.begin(), tops.end()), launches);
-        if (timing)
-            for (uint32_t k = 0; k < n_passes; ++k) add_stage_ms_2d(c, size_t(k) * (L + 3), L, false, h, stats->stage_ms);
-    }
-    return rc;
+    if (int32_t wrc = wait_cancel_2d(c, s, cc, passes_run, n_passes, stats)) return abandon(wrc);
+    return finish_2d(c, s, L, n_passes, timing, launches, stats);
 }
 
 // A 2D scene (kernels.cuh, Scene2D): every placement's tiles go through the tile pipeline of fc_render2d_frames, which
@@ -1076,11 +1128,8 @@ int32_t fc_render2d_scene(fc_ctx* c, const fc_tape* const* tapes, const fc_frame
     static_assert(FC_SCENE_MAX_SHAPES < FC_SCENE2D_NONE, "a shape's index is never FC_SCENE2D_NONE");
     if (!c || !cfg || (!out && !index) || (n_shapes && (!tapes || !placements))) return fail(FC_ERR_INVALID, "null argument");
     if (n_shapes > FC_SCENE_MAX_SHAPES) return fail(FC_ERR_UNSUPPORTED, "more than FC_SCENE_MAX_SHAPES shapes");
-    if (cfg->flags & FC_FLAG_FUSED_TAIL) return fail(FC_ERR_UNSUPPORTED, "FC_FLAG_FUSED_TAIL is not supported by scenes");
-    if (cfg->root_row_begin || cfg->root_row_end) return fail(FC_ERR_UNSUPPORTED, "root row bands are not supported by scenes");
-    if (cfg->root_stride > 1) return fail(FC_ERR_UNSUPPORTED, "the tile interleave is not supported by scenes");
+    if (int32_t vrc = check_batch_2d(cfg, "scenes")) return vrc;
     const uint32_t fmt = cfg->out_format;
-    if (fmt > FC_OUT_RGBA8) return fail(FC_ERR_INVALID, "unknown out_format");
     if (fmt == FC_OUT_F32) return fail(FC_ERR_UNSUPPORTED, "a 2D scene keeps no distances: FC_OUT_F32 is not supported");
     // every placement's tape and ShapeVars binding, before anything is allocated or launched
     std::vector<Frame2D> table(n_shapes);
@@ -1114,15 +1163,10 @@ int32_t fc_render2d_scene(fc_ctx* c, const fc_tape* const* tapes, const fc_frame
     const size_t npix = size_t(W) * H, n_blocks = size_t(g.blocks_x) * g.blocks_y, img_fmt = format_bytes(fmt, W, H);
     cudaStream_t s = c->stream;
 
-    // ---- shapes per pass: their worst-case job lists within FC_FRAMES_PASS_BYTES (the maps are the call's) ----
+    // ---- shapes per pass: their worst-case job lists (the maps are the call's) ----
     const uint64_t shape_roots = uint64_t(g.roots_x) * g.roots_y;
-    std::vector<uint64_t> shape_tiles;
-    if (int32_t src = size_lists_2d(g.ts, shape_roots, shape_tiles)) return src;
-    uint64_t per_shape = 0;
-    for (int l = 1; l <= L; ++l) per_shape += shape_tiles[l] * sizeof(TileJob);
-    uint32_t per_pass = uint32_t(std::min<uint64_t>(n_shapes, std::max<uint64_t>(1, FC_FRAMES_PASS_BYTES / per_shape)));
-    if (const int forced = env_int("FIDGET_B200_FRAMES_PER_PASS", 0); forced > 0) per_pass = std::min<uint32_t>(n_shapes, forced);
-    const uint32_t n_passes = (n_shapes + per_pass - 1) / per_pass;
+    uint32_t per_pass, n_passes;
+    if (int32_t prc = passes_2d(g.ts, shape_roots, n_shapes, sizeof(TileJob), 0, per_pass, n_passes)) return prc;
     auto pass_range = [&](uint32_t k, uint32_t& lo, uint32_t& hi) {   // pass k: shapes [lo, hi), the top pass first
         hi = n_shapes - k * per_pass;
         lo = hi - std::min(hi, per_pass);
@@ -1180,17 +1224,12 @@ int32_t fc_render2d_scene(fc_ctx* c, const fc_tape* const* tapes, const fc_frame
         Tiles2D gp = g;
         gp.n_roots = shape_roots * (hi - lo);
         gp.groups = groups[k];
-        if (k) {   // a new pass: fresh lists, cursors and arena; error bits accumulate over the call
-            CU(cudaMemsetAsync(c->counters.p, 0, offsetof(Counters, error), s));
-            CU(cudaMemsetAsync(&c->counters.as<Counters>()->arena_top, 0, sizeof(unsigned long long), s));
-        }
+        if (k) if (int32_t rrc = reset_pass_2d(c, s)) return rrc;
         bool fused = false;
         if (int32_t erc = enqueue_tiles_2d(c, tapes[hi - 1], cfg, gp, table[hi - 1].vb, nullptr, want_stats, timing, cc, s,
                                            ev, launches, fused))
             return abandon_frames(c, s, stats, erc);
-        if (want_stats)
-            CU(cudaMemcpyAsync(c->frame_tops.as<unsigned long long>() + k, &c->counters.as<Counters>()->arena_top,
-                               sizeof(unsigned long long), cudaMemcpyDeviceToDevice, s));
+        if (want_stats) if (int32_t trc = record_top_2d(c, s, k)) return trc;
         ++passes_run;
     }
     if (passes_run == n_passes) {
@@ -1214,30 +1253,11 @@ int32_t fc_render2d_scene(fc_ctx* c, const fc_tape* const* tapes, const fc_frame
         c->async_call = cc;
         return FC_OK;
     }
-    if (cc.flag) {   // a cancelled call copies nothing to the host
-        if (int32_t wrc = wait_call(c, s, cc)) {
-            if (stats) memset(stats, 0, sizeof *stats);
-            return wrc;
-        }
-        if (passes_run < n_passes) {   // the flag stopped the passes, but was cleared before the wait saw it
-            if (stats) memset(stats, 0, sizeof *stats);
-            return fail(FC_ERR_CANCELLED, "cancelled");
-        }
-    }
+    // a cancelled call copies nothing to the host
+    if (int32_t wrc = wait_cancel_2d(c, s, cc, passes_run, n_passes, stats)) return wrc;
     if (host_out) CU(cudaMemcpyAsync(out, dout, img_fmt, cudaMemcpyDeviceToHost, s));
     if (host_index) CU(cudaMemcpyAsync(index, dindex, npix * 2, cudaMemcpyDeviceToHost, s));
-    CU(cudaStreamSynchronize(s));
-    int32_t rc = check_device_errors(c);
-    if (stats) {
-        Stats h;
-        std::vector<unsigned long long> tops(n_passes);
-        CU(cudaMemcpy(&h, c->stats.p, sizeof h, cudaMemcpyDeviceToHost));
-        CU(cudaMemcpy(tops.data(), c->frame_tops.p, tops.size() * sizeof(unsigned long long), cudaMemcpyDeviceToHost));
-        write_stats(stats, h, false, *std::max_element(tops.begin(), tops.end()), launches);
-        if (timing)
-            for (uint32_t k = 0; k < n_passes; ++k) add_stage_ms_2d(c, size_t(k) * (L + 3), L, false, h, stats->stage_ms);
-    }
-    return rc;
+    return finish_2d(c, s, L, n_passes, timing, launches, stats);
 }
 
 int32_t fc_render3d(fc_ctx* c, const fc_tape* tape, const fc_render3d_cfg* cfg, fc_geometry_pixel* out,
@@ -1342,9 +1362,7 @@ int32_t fc_render3d_frames(fc_ctx* c, const fc_tape* tape, const fc_render3d_cfg
                            uint32_t n_frames, fc_geometry_pixel* out, fc_render_stats* stats) {
     if (!c || !tape || !cfg || !out || (n_frames && !frames)) return fail(FC_ERR_INVALID, "null argument");
     if (int32_t vrc = check_3d(tape, cfg)) return vrc;
-    if (cfg->z_begin || cfg->z_end) return fail(FC_ERR_UNSUPPORTED, "Z slabs are not supported by frame batches");
-    if (cfg->root_row_begin || cfg->root_row_end) return fail(FC_ERR_UNSUPPORTED, "root row bands are not supported by frame batches");
-    if (cfg->root_stride > 1) return fail(FC_ERR_UNSUPPORTED, "the tile interleave is not supported by frame batches");
+    if (int32_t vrc = check_batch_3d(cfg, "frame batches")) return vrc;
     // every frame's ShapeVars binding, before anything is allocated or launched (z is unused in 3D)
     std::vector<Frame2D> table(n_frames);
     for (uint32_t k = 0; k < n_frames; ++k)
@@ -1423,11 +1441,9 @@ int32_t fc_render3d_frames(fc_ctx* c, const fc_tape* tape, const fc_render3d_cfg
         void* dimg = host_out ? static_cast<void*>(stage[b]) : static_cast<void*>(out + size_t(r.f0) * img_px);
         if (int32_t erc = enqueue_tiles_3d(c, tape, cfg, gp, vb0, dimg, 0, r.n * H, want_stats, timing, cc, s, ev, launches))
             return erc;
-        // the pass's counters and stats, into pinned slot b for the host to read while the next pass runs (the slot is
-        // read before buffer b takes another pass)
-        PassStatus* hs = c->pass_pin + b;
-        CU(cudaMemcpyAsync(&hs->ctr, c->counters.p, sizeof(Counters), cudaMemcpyDeviceToHost, s));
-        if (want_stats) CU(cudaMemcpyAsync(&hs->st, c->stats.p, sizeof(Stats), cudaMemcpyDeviceToHost, s));
+        // the pass's status, into pinned slot b for the host to read while the next pass runs (the slot is read before
+        // buffer b takes another pass)
+        if (int32_t src = read_pass_status(c, s, b, want_stats)) return src;
         CU(cudaEventRecord(c->ev_pass[b], s));
         return FC_OK;
     };
@@ -1502,9 +1518,7 @@ int32_t fc_render3d_scene(fc_ctx* c, const fc_tape* const* tapes, const fc_frame
     if (!c || !cfg || !out || (n_shapes && (!tapes || !placements))) return fail(FC_ERR_INVALID, "null argument");
     if (n_shapes > FC_SCENE_MAX_SHAPES) return fail(FC_ERR_UNSUPPORTED, "more than FC_SCENE_MAX_SHAPES shapes");
     if (cfg->flags & FC_FLAG_EXACT_CENSUS) return fail(FC_ERR_UNSUPPORTED, "the exact census is not supported by scenes");
-    if (cfg->z_begin || cfg->z_end) return fail(FC_ERR_UNSUPPORTED, "Z slabs are not supported by scenes");
-    if (cfg->root_row_begin || cfg->root_row_end) return fail(FC_ERR_UNSUPPORTED, "root row bands are not supported by scenes");
-    if (cfg->root_stride > 1) return fail(FC_ERR_UNSUPPORTED, "the tile interleave is not supported by scenes");
+    if (int32_t vrc = check_batch_3d(cfg, "scenes")) return vrc;
     // every placement's tape and ShapeVars binding, and the key's limits, before anything is allocated or launched
     std::vector<Frame2D> table(n_shapes);
     for (uint32_t k = 0; k < n_shapes; ++k) {
@@ -1618,9 +1632,8 @@ int32_t fc_render3d_scene(fc_ctx* c, const fc_tape* const* tapes, const fc_frame
         if (int32_t erc = enqueue_tiles_3d(c, tapes[r.f0], cfg, gp, table[r.f0].vb, dimg, 0, H, want_stats, timing, cc, s, ev,
                                            launches, dindex))
             return abandon(erc);
-        PassStatus* hs = c->pass_pin;
-        CU(cudaMemcpyAsync(&hs->ctr, c->counters.p, sizeof(Counters), cudaMemcpyDeviceToHost, s));
-        if (want_stats) CU(cudaMemcpyAsync(&hs->st, c->stats.p, sizeof(Stats), cudaMemcpyDeviceToHost, s));
+        if (int32_t src = read_pass_status(c, s, 0, want_stats)) return src;
+        const PassStatus* hs = c->pass_pin;
         if (early_return && !plan.more()) {   // FC_FLAG_ASYNC: the last pass is left running
             c->async_call = cc;
             return FC_OK;

@@ -14,7 +14,7 @@ FLAGS="$FLAGS $EXTRA"
 # dev_ops.cuh as a string for the tape compiler (compile.cu): NVRTC compiles the same device arithmetic at run time
 mkdir -p build
 { echo 'extern const char k_dev_ops_source[] = R"FC_DEV_OPS('; cat $SRC/cuda/dev_ops.cuh; echo ')FC_DEV_OPS";'; } > build/dev_ops_src.cc
-$NVCC $FLAGS -o $OUT build/dev_ops_src.cc $SRC/cuda/compile.cu $SRC/cuda/kernels.cu $SRC/cuda/coop.cu $SRC/cuda/bulk.cu $SRC/cuda/tail2d.cu $SRC/cuda/octree.cu $SRC/cuda/effects.cu $SRC/cuda/capi.cu $SRC/cuda/schedule.cu $SRC/cuda/render.cu $SRC/cuda/octree_capi.cu $SRC/cuda/measure.cu $SRC/cuda/ray.cu $SRC/cuda/ray_capi.cu $SRC/cuda/mesh.cu $SRC/cuda/contour.cu $SRC/cuda/effects_capi.cu $SRC/cuda/solve.cu $SRC/cuda/solve_capi.cu $SRC/host/tape.cc $SRC/host/host_capi.cc -ldl
+$NVCC $FLAGS -o $OUT build/dev_ops_src.cc $SRC/cuda/compile.cu $SRC/cuda/kernels.cu $SRC/cuda/coop.cu $SRC/cuda/bulk.cu $SRC/cuda/tail2d.cu $SRC/cuda/octree.cu $SRC/cuda/effects.cu $SRC/cuda/capi.cu $SRC/cuda/schedule.cu $SRC/cuda/render.cu $SRC/cuda/octree_capi.cu $SRC/cuda/measure.cu $SRC/cuda/volume.cu $SRC/cuda/ray.cu $SRC/cuda/ray_capi.cu $SRC/cuda/mesh.cu $SRC/cuda/contour.cu $SRC/cuda/effects_capi.cu $SRC/cuda/solve.cu $SRC/cuda/solve_capi.cu $SRC/host/tape.cc $SRC/host/host_capi.cc -ldl
 make -s -C oracle liboracle.so
 # the solver's CPU oracle (oracle/solve.cc) on top of liboracle's point and gradient VM
 CXX=$([ -x /usr/bin/g++ ] && echo /usr/bin/g++ || echo g++)

@@ -149,6 +149,29 @@ class FcRaycastInfo(_Record):
                 ("leaf_samples", C.c_uint64), ("passes", C.c_uint32), ("device_ms", C.c_float)]
 
 
+class FcVolumeCfg(C.Structure):
+    _fields_ = [("depth", C.c_uint32), ("flags", C.c_uint32), ("band", C.c_float), ("pad", C.c_uint32)]
+
+
+class FcVolumeBrick(C.Structure):
+    _fields_ = [("frame", C.c_uint32), ("ix", C.c_uint16), ("iy", C.c_uint16), ("iz", C.c_uint16), ("pad", C.c_uint16)]
+
+
+class FcVolumeTile(C.Structure):
+    _fields_ = [("frame", C.c_uint32), ("ix", C.c_uint16), ("iy", C.c_uint16), ("iz", C.c_uint16),
+                ("log2_edge", C.c_uint8), ("inside", C.c_uint8)]
+
+
+class FcVolumeInfo(_Record):
+    _fields_ = [(n, C.c_uint64) for n in ("n_bricks", "n_tiles", "n_inside_tiles")] + \
+               [("evaluated", C.c_uint64 * 16), ("brick_edge", C.c_uint32), ("passes", C.c_uint32),
+                ("device_ms", C.c_float), ("level_ms", C.c_float)]
+
+
+class FcVolumeFrameInfo(_Record):
+    _fields_ = [(n, C.c_uint64) for n in ("n_bricks", "n_tiles", "first_brick", "first_tile")]
+
+
 class FcContourCfg(C.Structure):
     _fields_ = [("depth", C.c_uint32), ("has_transform", C.c_uint32), ("world_to_model", C.c_float * 9), ("z", C.c_float),
                 ("flags", C.c_uint32), ("n_var_values", C.c_uint32), ("var_values", C.c_float * 16)]
@@ -193,6 +216,7 @@ FC_FLAG_FUSED_TAIL = 8
 FC_FLAG_EXACT_CENSUS = 16
 FC_FLAG_FULL_LADDER = 32
 FC_FLAG_MESH_COLLAPSE = 64
+FC_FLAG_VOLUME_GRADS = 128
 FC_OUT_F32, FC_OUT_MASK_U8, FC_OUT_BITMAP_1BIT, FC_OUT_RGBA8 = 0, 1, 2, 3
 FC_ERR_CANCELLED = -6
 FC_FRAMES_PASS_BYTES = 512 << 20
@@ -263,6 +287,9 @@ CUDA_API = {
     "fc_mesh_build_frames": (_i32, [_vp, _vp, _P(FcOctreeCfg), _P(FcMeshFrame), _u32, _P(FcMeshInfo),
                                     _P(FcMeshFrameInfo)]),
     "fc_measure": (_i32, [_vp, _vp, _P(FcOctreeCfg), _P(FcMeshFrame), _u32, _vp, _P(C.c_float)]),
+    "fc_volume_build": (_i32, [_vp, _vp, _P(FcVolumeCfg), _P(FcMeshFrame), _u32, _P(FcVolumeInfo),
+                               _P(FcVolumeFrameInfo)]),
+    "fc_volume_read": (_i32, [_vp, _vp, _vp, _vp, _vp]),
     "fc_raycast": (_i32, [_vp, _vp, _P(FcRaycastCfg), _vp, _u64, _vp, _P(FcRaycastInfo)]),
     "fc_contour_build": (_i32, [_vp, _vp, _P(FcContourCfg), _P(FcContourInfo)]),
     "fc_contour_read": (_i32, [_vp, _vp, _vp, _vp]),

@@ -145,6 +145,12 @@ void fc_ctx_destroy(fc_ctx* c) {
     c->contour_offs.release();
     c->contour_flags.release();
     c->contour_slices.release();
+    c->vol_bricks.release();
+    c->vol_values.release();
+    c->vol_grads.release();
+    c->vol_tiles.release();
+    c->vol_list.release();
+    c->vol_scratch.release();
     c->tile_slots.release();
     c->fx_in.release();
     c->fx_out.release();
@@ -239,10 +245,12 @@ static int32_t cancel_site_of(const std::string& name) {
     static_assert(sizeof(solve) / sizeof(solve[0]) == CS_MEASURE_BRICK - CS_SOLVE, "one name per poll site");
     for (int i = 0; i < CS_MEASURE_BRICK - CS_SOLVE; ++i)
         if (name == solve[i]) return CS_SOLVE + i;
-    static_assert(CS_RAY_HITS + 1 == CS_COUNT, "one name per poll site");
+    static_assert(CS_VOLUME_GRADS + 1 == CS_COUNT, "one name per poll site");
     if (name == "k_measure_brick") return CS_MEASURE_BRICK;
     if (name == "k_ray_leaf") return CS_RAY_LEAF;
     if (name == "k_ray_hits") return CS_RAY_HITS;
+    if (name == "k_volume_brick") return CS_VOLUME_BRICK;
+    if (name == "k_volume_grads") return CS_VOLUME_GRADS;
     return -1;
 }
 

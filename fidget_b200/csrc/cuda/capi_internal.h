@@ -126,6 +126,12 @@ struct fc_ctx {
     uint32_t contour_n_verts = 0, contour_n_polys = 0;
     uint32_t* contour_offsets = nullptr;                        // in contour_offs
     uint8_t* contour_closed = nullptr;                          // in contour_flags
+    // fc_volume_build: the volume, resident in HBM until read (brick records, values, gradients, tile records), a pass's
+    // tile list and sort scratch; the counts of the volume (0: none) and its values per brick
+    DevBuf vol_bricks, vol_values, vol_grads, vol_tiles, vol_list, vol_scratch;
+    uint64_t vol_n_bricks = 0, vol_n_tiles = 0;
+    uint32_t vol_cells = 0;
+    bool vol_grads_on = false;
     DevBuf fx_in, fx_out, fx_tmp, fx_tables;  // effects: staged host images, intermediate maps, SSAO tables
     DevBuf solve_meta, solve_vals, solve_res; // the solvers: tape table + slot maps, staged host values / results
     DevBuf solve_work;                        // fc_solve_large_batch: one workspace slice per cluster in flight

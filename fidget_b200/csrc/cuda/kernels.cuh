@@ -29,6 +29,7 @@ enum CancelSite : int32_t {
     CS_SOLVE, CS_SOLVE_LARGE,                             // the solvers: item = problem index (claim and every iteration)
     CS_MEASURE_BRICK,                                     // fc_measure's brick kernel: item = brick
     CS_RAY_LEAF, CS_RAY_HITS,                             // fc_raycast's leaf (item = segment) and hit (item = warp) kernels
+    CS_VOLUME_BRICK, CS_VOLUME_GRADS,                     // fc_volume_build's brick and gradient kernels: item = brick
     CS_COUNT
 };
 struct CancelRef {
@@ -286,6 +287,48 @@ struct MeasureBrickParams {
     MeasureAcc* acc;
     CancelRef cancel;
 };
+
+// fc_volume_build (volume.cu).  Its interval levels (k_tree_level_volume) take the band and the tile list in a kernel
+// argument of their own, so that LevelParams keeps the layout the other level kernels are built with: a cell whose
+// interval lies below -band or above band is proven, appended to `tiles` as its volume_tile_key and not split;
+// *n_tiles counts the proven cells, beyond cap_tiles too (an overflow also sets error bit 1).
+struct VolumeLevel {
+    unsigned long long* tiles;
+    uint32_t* n_tiles;
+    uint32_t cap_tiles;
+    float band;
+};
+// Sort keys of a pass's bricks and tiles: (frame of the pass, iz, iy, ix) of the first cell, 12 bits per coordinate
+// (FC_MAX_OCTREE_DEPTH), so that sorting them gives the canonical order; a tile's key also carries its log2 edge and
+// whether it is inside in its 5 low bits (below the cell, which alone orders the unique tiles of a frame)
+constexpr int VOLUME_TILE_LOW_BITS = 5;
+__host__ __device__ __forceinline__ unsigned long long volume_key(uint32_t f, uint32_t x, uint32_t y, uint32_t z) {
+    return (((((unsigned long long)f << 12) | z) << 12 | y) << 12) | x;
+}
+__host__ __device__ __forceinline__ unsigned long long volume_tile_key(uint32_t f, uint32_t x, uint32_t y, uint32_t z,
+                                                                       uint32_t log2_edge, bool inside) {
+    return (volume_key(f, x, y, z) << VOLUME_TILE_LOW_BITS) | (log2_edge << 1) | (inside ? 1u : 0u);
+}
+// fc_volume_brick and fc_volume_tile
+struct VolumeBrick { uint32_t frame; uint16_t ix, iy, iz, pad; };
+struct VolumeTile { uint32_t frame; uint16_t ix, iy, iz; uint8_t log2_edge, inside; };
+// The brick and gradient kernels: brick r of the pass (r < n) is job order[r] of `jobs` (list `list` of the levels),
+// with sort key keys[r]; its brick^3 values go to values[r], its gradients to grads[r], its record to bricks[r].  frame
+// f of the pass is fc_volume_build's frame f0 + f, and frames[f] its record.
+struct VolumeBrickParams {
+    const TileJob* jobs;
+    const uint32_t* order;
+    const unsigned long long* keys;
+    uint32_t n, f0;
+    uint32_t depth, brick;
+    float* values;
+    float* grads;
+    VolumeBrick* bricks;
+    Counters* ctr;
+    int cursor;
+    CancelRef cancel;
+};
+void launch_tree_level_volume(const LevelParams& p, const MeshFrame* frames, const VolumeLevel& v, int blocks, cudaStream_t s);
 
 // fc_raycast (ray.cu).  A ray and a hit as fc_ray and fc_ray_hit lay them out.  The interval levels take their lists,
 // arena, tape and vars from LevelParams and the pass from RayPass: a job is a segment of ray x starting at sample y,

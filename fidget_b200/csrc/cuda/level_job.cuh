@@ -164,11 +164,14 @@ __device__ __forceinline__ TapeRef simplify_children(const LevelParams& p, const
 // the cell's rows are relative to its slice.  DIM 3 with FRAMES (octree mode 1): the stacked octree of a mesh frame
 // batch, each cell's frame read the same way (its Z is the cell's own).  MEASURE (DIM 3, TREE, FRAMES: fc_measure): the
 // block moments and box of the lanes' proven-inside cells go into their frame's accumulator, p.measure[cell row /
-// frame_rows]; a warp's children share one frame, the root cells of level 0 each have their own.
-template <int DIM, bool FUSED, bool FRAMES = false, bool SCENE = false, bool TREE = false, bool MEASURE = false>
+// frame_rows]; a warp's children share one frame, the root cells of level 0 each have their own.  VOLUME (DIM 3, TREE,
+// FRAMES: fc_volume_build): cells are proven against -vol->band and vol->band instead of 0, and every proven cell is
+// appended to vol's tile list, one atomic per warp.
+template <int DIM, bool FUSED, bool FRAMES = false, bool SCENE = false, bool TREE = false, bool MEASURE = false,
+          bool VOLUME = false>
 __device__ __forceinline__ void level_job(const LevelParams& p, uint32_t j, uint32_t n_roots, itv* slots, uint32_t* cs,
                                           uint32_t (*live)[32], int lane, uint32_t epoch,
-                                          const ContourSlice* slices = nullptr) {
+                                          const ContourSlice* slices = nullptr, const VolumeLevel* vol = nullptr) {
     const uint32_t T = p.tile;
     bool cull_open = false, cull_check = false;
     TapeRef tr;
@@ -270,8 +273,9 @@ __device__ __forceinline__ void level_job(const LevelParams& p, uint32_t j, uint
             [&](uint32_t oi, itv v) { if (oi == 0) r = v; });
         pk.finish();
 
-        const bool fill_in = valid && !p.pixel_perfect && r.y < 0.0f;
-        const bool fill_out = valid && !p.pixel_perfect && !fill_in && r.x > 0.0f;
+        const float band = VOLUME ? vol->band : 0.0f;
+        const bool fill_in = valid && !p.pixel_perfect && r.y < (VOLUME ? -band : 0.0f);
+        const bool fill_out = valid && !p.pixel_perfect && !fill_in && r.x > band;
         const bool amb = valid && !fill_in && !fill_out;
 
         if constexpr (MEASURE) {
@@ -285,6 +289,22 @@ __device__ __forceinline__ void level_job(const LevelParams& p, uint32_t j, uint
                 } else {
                     ms.warp_fold();
                     if (lane == 0) ms.flush(p.measure + cy / p.frame_rows, true, 0);
+                }
+            }
+        }
+        if constexpr (VOLUME) {
+            static_assert(DIM == 3 && TREE && FRAMES, "fc_volume_build's levels are the stacked octree's");
+            const bool proven = fill_in || fill_out;
+            const uint32_t mp = __ballot_sync(FULL, proven);
+            if (mp) {
+                uint32_t base = 0;
+                if (lane == 0) base = atomicAdd(vol->n_tiles, uint32_t(__popc(mp)));
+                base = __shfl_sync(FULL, base, 0);
+                if (proven) {
+                    const uint32_t slot = base + __popc(mp & lanemask_lt());
+                    if (slot < vol->cap_tiles)
+                        vol->tiles[slot] = volume_tile_key(cy / p.frame_rows, cx, cy - fv.y0, cz, uint32_t(__ffs(T) - 1), fill_in);
+                    else atomicOr(&p.ctr->error, 2u);
                 }
             }
         }

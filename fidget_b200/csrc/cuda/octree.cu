@@ -181,6 +181,31 @@ __global__ void __launch_bounds__(WARPS_PER_BLOCK * 32) k_tree_level(const __gri
         level_job<DIM, false, STACK, false, true, MEASURE>(p, j, n_roots, slots, cs, live_s[wib], lane, p.epoch, frames);
     }
 }
+// fc_volume_build's levels: k_tree_level's loop over the stacked octree, proven cells appended to vol's tile list (a
+// kernel of its own, so that the other instantiations keep their machine code)
+__global__ void __launch_bounds__(WARPS_PER_BLOCK * 32) k_tree_level_volume(const __grid_constant__ LevelParams p,
+                                                                            const MeshFrame* frames,
+                                                                            const __grid_constant__ VolumeLevel vol) {
+    __shared__ uint32_t live_s[WARPS_PER_BLOCK][8][32];
+    const int lane = threadIdx.x & 31;
+    const int wib = threadIdx.x >> 5;
+    const uint32_t gw = blockIdx.x * WARPS_PER_BLOCK + wib;
+    uint32_t* cs = p.choice_scratch + size_t(gw) * p.choice_words * 32u + lane;
+    itv slots[REG_SLOTS];
+    const uint32_t n_roots = p.roots_y;
+    const uint32_t n_jobs = p.root_mode ? (n_roots + 31u) / 32u : min(p.ctr->n_jobs[p.level], p.cap_in);
+    for (;;) {
+        uint32_t j = 0;
+        if (lane == 0) {
+            j = atomicAdd(&p.ctr->cursor[p.level], 1u);
+            if (j < n_jobs && cancel_poll(p.cancel, CS_LEVEL0 + p.level, j)) j = ~0u;
+        }
+        j = __shfl_sync(FULL, j, 0);
+        if (j >= n_jobs) break;
+        level_job<3, false, true, false, true, false, true>(p, j, n_roots, slots, cs, live_s[wib], lane, p.epoch, frames,
+                                                            &vol);
+    }
+}
 void launch_tree_level(const LevelParams& p, int dim, const ContourSlice* frames, int blocks, cudaStream_t s) {
     if (dim == 3) k_tree_level<3, true><<<blocks, WARPS_PER_BLOCK * 32, 0, s>>>(p, frames);
     else if (frames) k_tree_level<2, true><<<blocks, WARPS_PER_BLOCK * 32, 0, s>>>(p, frames);
@@ -188,6 +213,9 @@ void launch_tree_level(const LevelParams& p, int dim, const ContourSlice* frames
 }
 void launch_tree_level_measure(const LevelParams& p, const MeshFrame* frames, int blocks, cudaStream_t s) {
     k_tree_level<3, true, true><<<blocks, WARPS_PER_BLOCK * 32, 0, s>>>(p, frames);
+}
+void launch_tree_level_volume(const LevelParams& p, const MeshFrame* frames, const VolumeLevel& v, int blocks, cudaStream_t s) {
+    k_tree_level_volume<<<blocks, WARPS_PER_BLOCK * 32, 0, s>>>(p, frames, v);
 }
 
 }  // namespace fdev

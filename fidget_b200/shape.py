@@ -1111,6 +1111,108 @@ def measure(shape: CudaShape, depth: int, world_to_model=None, var_values=None, 
     return (out, ms.value) if timing else out
 
 
+class Volume:
+    """A sparse narrow-band volume (``fc_volume_build``), in its canonical order:
+
+    - ``bricks``: [n, 4] int32 rows (frame, ix, iy, iz), each brick's first cell;
+    - ``values``: [n, B, B, B] float32, indexed [z, y, x] inside the brick; ``grads``: [n, B, B, B, 3] or None;
+    - ``tiles``: [m, 6] int32 rows (frame, ix, iy, iz, log2_edge, inside) of the proven tiles;
+    - ``per_frame``: dict of [n_frames] int64 arrays n_bricks, n_tiles, first_brick, first_tile; ``info``: a dict.
+
+    numpy arrays, or with ``device=True`` CUDA torch tensors (``per_frame`` and ``info`` stay on the host)."""
+
+    def __init__(self, depth, band, bricks, values, grads, tiles, per_frame, info):
+        self.depth, self.band = depth, band
+        self.brick_edge = info["brick_edge"]
+        self.bricks, self.values, self.grads, self.tiles = bricks, values, grads, tiles
+        self.per_frame, self.info = per_frame, info
+
+
+def _volume_rows(raw, n, words, torch_dev):
+    """fc_volume_brick / fc_volume_tile records (12 bytes each, raw bytes) as [n, 4] / [n, 6] int32 rows"""
+    if torch_dev is not None:
+        import torch
+        u16 = raw[:, 4:10].contiguous().view(torch.int16).to(torch.int32) & 0xFFFF
+        cols = [raw[:, 0:4].contiguous().view(torch.int32), u16]
+        if words == 6:
+            cols.append(raw[:, 10:12].to(torch.int32))
+        return torch.cat(cols, 1)
+    u32 = raw[:, 0:4].copy().view(np.uint32).astype(np.int32)
+    u16 = raw[:, 4:10].copy().view(np.uint16).astype(np.int32)
+    cols = [u32, u16] + ([raw[:, 10:12].astype(np.int32)] if words == 6 else [])
+    return np.concatenate(cols, 1).reshape(n, words)
+
+
+def volume(shape: CudaShape, depth: int, band: float = 0.0, world_to_model=None, var_values=None, grads: bool = False,
+           device: bool = False, cancel: CancelToken | None = None, timing: bool = False):
+    """The shape's field at the cell centres of the depth-``depth`` grid of [-1,1]^3, as 8^3 bricks where the interval
+    octree cannot rule out |v| <= ``band`` and proven inside / outside tiles everywhere else (``fc_volume_build``).
+    ``world_to_model`` / ``var_values`` are per-frame as in ``measure``.  Returns a ``Volume``, None when ``cancel``
+    cancelled the call."""
+    lib = shape._lib
+    if world_to_model is not None and not isinstance(world_to_model, (list, tuple)) and \
+            np.asarray(world_to_model).shape == (4, 4):
+        world_to_model = [world_to_model]
+    if var_values is not None and np.asarray(var_values, dtype=np.float32).ndim == 1:
+        var_values = [var_values]
+    table = mesh_frame_table(world_to_model=world_to_model, var_values=var_values)
+    n = len(table)
+    c = _lib.FcVolumeCfg()
+    c.depth = depth
+    c.band = band
+    c.flags = (_lib.FC_FLAG_TIMING if timing else 0) | (_lib.FC_FLAG_VOLUME_GRADS if grads else 0)
+    info = _lib.FcVolumeInfo()
+    per = (_lib.FcVolumeFrameInfo * max(n, 1))()
+    cuda = shape.cuda
+    rc = cuda._cancellable(cancel, lambda: lib.fc_volume_build(cuda._h, shape._h, C.byref(c), table, n, C.byref(info),
+                                                               per))
+    if rc == _lib.FC_ERR_CANCELLED:
+        return None
+    _ck(rc)
+    d = info.as_dict()
+    B, nb, nt = d["brick_edge"], d["n_bricks"], d["n_tiles"]
+    pf = {k: np.array([getattr(per[i], k) for i in range(n)], dtype=np.int64)
+          for k in ("n_bricks", "n_tiles", "first_brick", "first_tile")}
+    torch_dev = None
+    if device:
+        import torch
+        torch_dev = torch.device("cuda", cuda.device)
+        raw_b = torch.empty((nb, 12), dtype=torch.uint8, device=torch_dev)
+        vals = torch.empty((nb, B, B, B), dtype=torch.float32, device=torch_dev)
+        grd = torch.empty((nb, B, B, B, 3), dtype=torch.float32, device=torch_dev) if grads else None
+        raw_t = torch.empty((nt, 12), dtype=torch.uint8, device=torch_dev)
+    else:
+        raw_b = np.empty((nb, 12), dtype=np.uint8)
+        vals = np.empty((nb, B, B, B), dtype=np.float32)
+        grd = np.empty((nb, B, B, B, 3), dtype=np.float32) if grads else None
+        raw_t = np.empty((nt, 12), dtype=np.uint8)
+    _ck(lib.fc_volume_read(cuda._h, _ptr(raw_b) if nb else None, _ptr(vals) if nb else None,
+                           _ptr(grd) if grads and nb else None, _ptr(raw_t) if nt else None))
+    return Volume(depth, band, _volume_rows(raw_b, nb, 4, torch_dev), vals, grd, _volume_rows(raw_t, nt, 6, torch_dev),
+                  pf, d)
+
+
+def volume_dense(vol: Volume, frame: int = 0, inside: float = -np.inf, outside: float = np.inf):
+    """Frame ``frame`` of a ``Volume`` as a dense [2^D, 2^D, 2^D] float32 array indexed [z, y, x]: the brick values,
+    ``inside`` in inside tiles and ``outside`` in outside tiles (numpy, or torch on the volume's device).  For small
+    depths: the array has 8^D cells."""
+    n, B = 1 << vol.depth, vol.brick_edge
+    if hasattr(vol.values, "data_ptr"):
+        import torch
+        out = torch.full((n, n, n), float("nan"), dtype=torch.float32, device=vol.values.device)
+        tiles, bricks = vol.tiles.cpu().numpy(), vol.bricks.cpu().numpy()
+    else:
+        out = np.full((n, n, n), np.nan, dtype=np.float32)
+        tiles, bricks = vol.tiles, vol.bricks
+    for f, ix, iy, iz, lg, ins in tiles[tiles[:, 0] == frame].tolist():
+        e = 1 << lg
+        out[iz:iz + e, iy:iy + e, ix:ix + e] = inside if ins else outside
+    for r in np.nonzero(bricks[:, 0] == frame)[0].tolist():
+        _, ix, iy, iz = bricks[r].tolist()
+        out[iz:iz + B, iy:iy + B, ix:ix + B] = vol.values[r]
+    return out
+
+
 # ---------------------------------------------------------------------------
 # Ray casts: fc_raycast
 RAY = np.dtype([("origin", np.float32, 3), ("dir", np.float32, 3), ("t0", np.float32), ("dt", np.float32)])

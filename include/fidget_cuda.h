@@ -65,7 +65,7 @@ int32_t fc_ctx_set_arena_bytes(fc_ctx* ctx, uint64_t bytes);
  * layout of Rust's AtomicBool (CancelToken::into_raw() as *const u8): nonzero = cancelled.  The library reads it with
  * an acquire load, from any thread; NULL detaches it.  Context-wide, like fc_ctx_set_stream, and consulted only by
  * fc_render2d, fc_render2d_frames, fc_render2d_scene, fc_render3d, fc_render3d_frames, fc_render3d_scene, fc_octree_sample,
- * fc_mesh_build, fc_mesh_build_frames, fc_contour_build, fc_raycast, fc_solve_batch, fc_solve_large_batch, and
+ * fc_mesh_build, fc_mesh_build_frames, fc_contour_build, fc_raycast, fc_volume_build, fc_solve_batch, fc_solve_large_batch, and
  * fc_ctx_synchronize after the most recent FC_FLAG_ASYNC call of those.  With a flag attached:
  *  - set on entry: the call returns FC_ERR_CANCELLED before it allocates or launches anything;
  *  - set while the call runs: the kernels stop claiming work and the call returns FC_ERR_CANCELLED ("cancelled" in
@@ -603,6 +603,80 @@ typedef struct fc_measure_result {
 int32_t fc_measure(fc_ctx* ctx, const fc_tape* tape, const fc_octree_cfg* cfg /* depth, flags */,
                    const fc_mesh_frame* frames /* host */, uint32_t n_frames, fc_measure_result* out /* host */,
                    float* device_ms /* FC_FLAG_TIMING, may be NULL */);
+
+/* ---- Sparse narrow-band volumes: the field on a voxel grid ---------------------------------------------------------
+ * fc_volume_build samples the field of a shape at the cell centres of the depth-D grid of the world cube [-1,1]^3
+ * (0 <= D <= FC_MAX_OCTREE_DEPTH), densely near the surface and as proven tiles everywhere else, the result staying in
+ * HBM until fc_volume_read copies it out (VDB-style exports, SDF textures, collision lookups, training data):
+ *  - Grid.  Cell (i, j, k) is centred at -1 + (2i + 1) 2^-D on X, likewise on Y and Z (exact in f32).  With
+ *    has_transform the centre is mapped through world_to_model in f32 (Matrix4::transform_point, divided by the
+ *    homogeneous term where that is not zero), as fc_measure maps it; projective matrices are allowed.
+ *  - Band.  cfg->band, 0 <= band < inf.  With B = min(8, 2^D) the brick edge, interval levels run from the root cell
+ *    down to cells of edge B, one octree depth per level, with fc_octree_sample's bounds, transform and tape
+ *    simplification.  A cell whose interval [lo, hi] has hi < -band is an inside tile, lo > band an outside tile; a tile
+ *    is recorded and not split.  Anything else, NaN included, is split; an unsplit cell of edge B is a brick.  With
+ *    band == 0 this is exactly the classification of fc_measure and the octree sampler.
+ *  - Brick values.  Every brick stores its B^3 values, values[brick][(k B + j) B + i] (x fastest): the f32 result of
+ *    the brick's simplified tape at the mapped centre, the evaluation fc_measure makes.
+ *  - Gradients.  With FC_FLAG_VOLUME_GRADS each brick also stores grads[brick][cell][3], the world-space partials
+ *    (d/dx, d/dy, d/dz) of the brick's tape at the cell centre, as fc_octree_leaf.grad gives them.
+ *  - Partition.  The tiles and bricks of a frame partition its cube exactly; every tile has edge 2^log2_edge >= B.
+ *  - Order.  Bricks and tiles are each sorted by (frame, iz, iy, ix) of their first cell: the output is byte for byte
+ *    independent of the launch grid, the order of the work and the passes.
+ *  - Which values are exact.  For tapes of IEEE operations an interval never contradicts a point value in its box, so:
+ *    every centre whose root-tape value v has |v| <= band lies in a brick; every centre in an inside tile has
+ *    v < -band and every centre in an outside tile has v > band; brick values equal fc_float_slice_eval of the root
+ *    tape at the mapped centre, bit for bit.
+ *  - frames (host, n_frames entries): each frame's has_transform, world_to_model and var_values.  Passes: the frames of
+ *    a pass share each launch in one stacked octree; the first pass holds one frame, later ones are sized from the
+ *    largest per-frame arena, job-list and tile-list use seen so far, and a pass that overflows anyway is run again in
+ *    halves: FC_ERR_ARENA or a work-list overflow (the tile list included) comes back only where one frame alone gives
+ *    it.  Once a pass's levels are done its brick and tile counts are known, and the volume grows to hold them before
+ *    its bricks are evaluated: n_bricks B^3 4 (1 + 3 grads) bytes of values and gradients, 12 bytes per brick and per
+ *    tile.  When that would exceed the device's free memory the call returns FC_ERR_UNSUPPORTED ("volume too large")
+ *    and the context stays usable.
+ *  - info (may be NULL): the counts of the whole volume, the cells evaluated per interval level, B, the passes run, and
+ *    with FC_FLAG_TIMING the device time (level_ms: of the interval levels alone) summed over passes.  per_frame (may be
+ *    NULL, n_frames entries): frame k's counts and its first brick and tile in the volume.
+ *  - Checked before anything is allocated or launched: fc_measure's refusals but the projective matrix (depth above
+ *    FC_MAX_OCTREE_DEPTH, a multi-output tape, more than FC_MAX_VARS values, a frame without a value for a bound
+ *    variable, NULL frames with n_frames > 0: FC_ERR_INVALID; a tape with memory slots: FC_ERR_UNSUPPORTED), and a NaN,
+ *    negative or infinite band: FC_ERR_INVALID.  n_frames == 0 launches nothing and leaves an empty volume.
+ *  - The cancel flag behaves as in fc_mesh_build.  A cancelled or failed call leaves no volume: fc_volume_read copies
+ *    nothing and info and per_frame are zeroed.
+ * fc_volume_read copies the volume of the last fc_volume_build into host or device memory; any pointer may be NULL:
+ * bricks (n_bricks), values (n_bricks B^3 floats), grads (n_bricks B^3 3 floats; FC_ERR_INVALID unless the volume was
+ * built with FC_FLAG_VOLUME_GRADS), tiles (n_tiles). */
+#define FC_FLAG_VOLUME_GRADS 128u
+typedef struct fc_volume_cfg {
+    uint32_t depth;
+    uint32_t flags;                 /* FC_FLAG_VOLUME_GRADS, FC_FLAG_TIMING */
+    float band;
+    uint32_t pad;
+} fc_volume_cfg;
+typedef struct fc_volume_brick {
+    uint32_t frame;
+    uint16_t ix, iy, iz, pad;       /* first cell */
+} fc_volume_brick;
+typedef struct fc_volume_tile {
+    uint32_t frame;
+    uint16_t ix, iy, iz;            /* first cell */
+    uint8_t log2_edge;              /* edge 2^log2_edge cells */
+    uint8_t inside;                 /* 1: hi < -band, 0: lo > band */
+} fc_volume_tile;
+typedef struct fc_volume_info {
+    uint64_t n_bricks, n_tiles, n_inside_tiles;
+    uint64_t evaluated[16];         /* cells evaluated per interval level */
+    uint32_t brick_edge, passes;
+    float device_ms, level_ms;      /* FC_FLAG_TIMING */
+} fc_volume_info;
+typedef struct fc_volume_frame_info {
+    uint64_t n_bricks, n_tiles, first_brick, first_tile;
+} fc_volume_frame_info;
+int32_t fc_volume_build(fc_ctx* ctx, const fc_tape* tape, const fc_volume_cfg* cfg, const fc_mesh_frame* frames /* host */,
+                        uint32_t n_frames, fc_volume_info* info /* may be NULL */,
+                        fc_volume_frame_info* per_frame /* may be NULL */);
+int32_t fc_volume_read(fc_ctx* ctx, fc_volume_brick* bricks, float* values, float* grads, fc_volume_tile* tiles);
 
 /* ---- Ray casts: the first inside sample along each ray --------------------------------------------------------------
  * fc_raycast answers, for each of n_rays rays, where the ray first enters the shape (picking, line of sight, depth
